@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — measurement contract of the repo (task statement, "Measurement").
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload W] [--precision P]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload W] [--precision P] [--dump-outputs DIR]
 
 Workloads (one full TRAIN STEP per step unless noted: network forward, criterion, backward, NCCL gradient all-reduce
 for N > 1, division by the global batch, NaN/Inf guard, clipGradNorm, SGD; data parallel by utterance = weak scaling,
@@ -15,17 +15,21 @@ the gradient all-reduce is the only collective — SURVEY.md §8e):
                      B=8 x T=1000 x 80 per GPU, 10 000 word pieces (train_am_500ms_future_context.cfg: batchsize 8).
   asg                configs[4] point: fused ASG forward+backward at T=1500, N=30, B=64 per GPU (no train step).
   asg_sweep          configs[4]: T in {100,500,1500,4000} x B in {1,16,64,256} per GPU, oracle parity on every point.
---precision: f32 (fp32-accurate: error-compensated 3xTF32 tcgen05 GEMMs and time convolutions), tf32, bf16 (bf16 GEMM operands,
+--precision: f32 (fp32-accurate: error-compensated 3xTF32 wgmma GEMMs and time convolutions), tf32, bf16 (bf16 GEMM operands,
 fp32 accumulation / LayerNorm / criterion / optimizer); default = the precision the workload's BASELINE config states.
 
 One JSON line on rank 0.  `value` = frames/s with the batch resident in HBM; `e2e` = the same step through the C ABI
 with HOST (pinned) batches, H2D of features/targets and D2H of the losses inside the timed region; `roofline` = the
-dominant kernel (train steps: gemm_umma_kernel, achieved algorithmic TFLOP/s over all GEMM launches of the timed
+dominant kernel (train steps: gemm_wgmma_kernel, achieved algorithmic TFLOP/s over all GEMM launches of the timed
 steps; asg: asg_chains_kernel GB/s) timed live with CUDA events through w2l_set_profile_event_list against
 MEASURED_PEAKS.json; `cpu_baseline` = the CPU port (oracle/) timed on this box's host cores.  The default workload
 also reports the other precisions of the same step, the TDS+ASG step BASELINE.json's metric names, and the ASG point.
 `--impl reference` times the CPU implementation as the reference arm (the reference's own ArrayFire-CPU backend cannot
 be built here: DESIGN.md §2): same config (B, T, arch) as the GPU arm, all host threads it can use.
+`--dump-outputs DIR` writes, after the timed steps, what the timed path computed in its last step as DIR/<name>.npy
+(float32; arrays above 4 M elements as a fixed, seeded sample of 4 M, named <name>_sample.npy): the per-utterance losses
+and the parameters after the update for the train steps; loss, d_emis and d_trans for the ASG workloads (asg_sweep: the
+T=1500, B=64 point).  The inputs are seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -73,12 +77,12 @@ WORKLOADS = {
                                    "(BASELINE.json configs[3]; recipes/streaming_convnets/librispeech/)"),
 }
 DTYPE_NOTE = {
-    "f32": "f32 storage and fp32-ACCURATE contractions: the tcgen05 GEMMs split every staged operand tile into tf32 hi + lo parts and "
-           "accumulate Al*Bh + Ah*Bl + Ah*Bh in fp32 TMEM (products good to ~2^-21); time convolutions on the mma.sync kernels with the same 3xTF32 split in registers; "
+    "f32": "f32 storage and fp32-ACCURATE contractions: the wgmma GEMMs split every staged operand tile into tf32 hi + lo parts and "
+           "accumulate Al*Bh + Ah*Bl + Ah*Bh in fp32 registers (products good to ~2^-21); time convolutions on the mma.sync kernels with the same 3xTF32 split in registers; "
            "criterion / LayerNorm / optimizer in f32/f64",
     "tf32": "f32 storage; dense contractions multiply TF32 operands on the tensor cores with f32 accumulation (cuDNN / cuBLAS default for "
             "fp32 tensors); criterion, LayerNorm, optimizer in f32/f64",
-    "bf16": "bf16 GEMM operands (activations and weights cast by their producers), fp32 accumulation in TMEM; fp32 master weights, "
+    "bf16": "bf16 GEMM operands (activations and weights cast by their producers), fp32 accumulation in registers; fp32 master weights, "
             "LayerNorm, criterion (fp32 loss) and optimizer: the reference's AMP mode (Train.cpp:211-219) with bf16",
 }
 
@@ -89,7 +93,7 @@ def asg_algorithmic_bytes(B, T, N, L):
 
 
 def arch_gemm_flops(arch_text, B, T, n_feat, n_label):
-    """2*M*N*K summed over every dense contraction that runs on the tcgen05 GEMM (TDS fully-connected layers, Linear layers,
+    """2*M*N*K summed over every dense contraction that runs on the wgmma GEMM (TDS fully-connected layers, Linear layers,
     the WN Conv1D layers of the conv_glu archs as im2col GEMMs), x3 (forward, data gradient, weight gradient).
     Returns (flops per step, output frames)."""
     total, t, pend = 0, T, None
@@ -191,7 +195,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d, "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback (B200_PROFILING.md)"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "fallback: NVIDIA H100 SXM data sheet (700 W), not measured"
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -320,7 +324,7 @@ def train_workload_text(cfg):
 
 
 # ---------------------------------------------------------------------------------------------------------
-# B200 arms
+# GPU arms
 # ---------------------------------------------------------------------------------------------------------
 class Timed:
     def __init__(self, world, local_rank):
@@ -369,6 +373,22 @@ class Timed:
             ms = float(tms.item())
         kern = profile.times_ms(used) if profile is not None else []
         return ms, kern, launches, clocks
+
+
+DUMP_MAX_ELEMENTS = 4 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """DIR/<name>.npy in float32; an array above DUMP_MAX_ELEMENTS is written as a fixed, seeded sample of that many
+    elements (sorted flat indices, DIR/<name>_sample.npy) so the files stay small but comparable run to run"""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy().reshape(-1) if hasattr(t, "detach") else np.asarray(t, dtype=np.float32).reshape(-1)
+        if a.size > DUMP_MAX_ELEMENTS:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, DUMP_MAX_ELEMENTS, replace=False))
+            np.save(os.path.join(out_dir, f"{name}_sample.npy"), a[idx].astype(np.float32))
+        else:
+            np.save(os.path.join(out_dir, f"{name}.npy"), a.astype(np.float32))
 
 
 def asg_point(tm: "Timed", rank, steps, warmup, profile=True, cfg=None, check=False):
@@ -425,10 +445,11 @@ def asg_point(tm: "Timed", rank, steps, warmup, profile=True, cfg=None, check=Fa
         parity = {"loss": rel(loss.cpu().numpy(), ol), "d_emis": rel(d_emis.cpu().numpy(), ode), "d_trans": rel(d_trans.cpu().numpy(), odt)}
     prof = capi.ProfileList(2, 8) if profile else None
     ms, kern, launches, clocks = tm.run(step, steps, warmup, sample_clocks=profile, profile=prof, profile_steps=min(steps, 8))
+    outputs = {"loss": loss.clone(), "d_emis": d_emis.clone(), "d_trans": d_trans.clone()}  # the last timed step's results
     ms_e2e, _, _, _ = tm.run(step_e2e, steps, warmup)
     kavg = sum(kern) / len(kern) if kern else None
     return dict(cfg=cfg, ms=ms / steps, ms_e2e=ms_e2e / steps, kernel_ms=kavg, launches=launches, clocks=clocks,
-                ws_mb=ws.numel() / 1e6, h2d=B * T * N * 4 + B * L * 4, d2h=B * 4, parity=parity)
+                ws_mb=ws.numel() / 1e6, h2d=B * T * N * 4 + B * L * 4, d2h=B * 4, parity=parity, outputs=outputs)
 
 
 def run_asg(args, rank, world, local_rank):
@@ -436,6 +457,8 @@ def run_asg(args, rank, world, local_rank):
     r = asg_point(tm, rank, args.steps, args.warmup, check=True)
     if rank != 0:
         return
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, r["outputs"])
     cfg = r["cfg"]
     B, T, N, L = cfg["B"], cfg["T"], cfg["N"], cfg["L"]
     peaks, src = measured_peaks()
@@ -454,7 +477,7 @@ def run_asg(args, rank, world, local_rank):
         "config": {"workload": "ASG criterion fwd+bwd, T=1500 N=30 B=64 L<=250 per GPU (BASELINE.json configs[4] point)",
                    "criterion": "asg", "scale_mode": cfg["scale_mode"], "sharding": f"utterances, dp{world}",
                    "cold_inputs": f"rotating {cfg['n_input_sets']} input sets ({cfg['n_input_sets'] * B * T * N * 4 / 1e6:.0f} MB) + "
-                                  f"{r['ws_mb']:.0f} MB workspace rewritten per step > 126 MB L2"},
+                                  f"{r['ws_mb']:.0f} MB workspace rewritten per step > 50 MB L2"},
         "asg_fwd_bwd_ms_per_batch": r["ms"], "oracle_parity_rel": r["parity"],
         "clocks": r["clocks"],
         "e2e": {"value": frames / (r["ms_e2e"] * 1e-3), "unit": "frames/s", "ms_per_step": r["ms_e2e"],
@@ -478,8 +501,9 @@ def run_asg_sweep(args, rank, world, local_rank):
     for T in (100, 500, 1500, 4000):
         for B in (1, 16, 64, 256):
             cfg = dict(T=T, N=30, B=B, L=max(2, T // 6), scale_mode="target_sz_sqrt", n_input_sets=max(2, min(16, (160 << 20) // (B * T * 120))))
-            steps = max(5, min(args.steps, 40))
-            r = asg_point(tm, rank, steps, 3, profile=True, cfg=cfg, check=(rank == 0))
+            r = asg_point(tm, rank, args.steps, args.warmup, profile=True, cfg=cfg, check=(rank == 0))
+            if rank == 0 and T == 1500 and B == 64 and args.dump_outputs:
+                dump_outputs(args.dump_outputs, r["outputs"])
             alg = asg_algorithmic_bytes(B, T, 30, cfg["L"])
             if rank == 0:
                 points.append({"T": T, "B": B, "L": cfg["L"], "ms_per_batch": r["ms"], "e2e_ms_per_batch": r["ms_e2e"],
@@ -491,7 +515,7 @@ def run_asg_sweep(args, rank, world, local_rank):
     worst = max(max(p["oracle_parity_rel"].values()) for p in points)
     head = next(p for p in points if p["T"] == 1500 and p["B"] == 64)
     line = {"metric": "frames_per_sec", "value": head["frames_per_sec"], "unit": "frames/s", "n_gpus": world, "steps": args.steps,
-            "warmup": 3, "ms_per_step": head["ms_per_batch"], "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
+            "warmup": args.warmup, "ms_per_step": head["ms_per_batch"], "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "f32", "data": "synthetic",
             "config": {"workload": "ASG criterion fwd+bwd sweep T in {100,500,1500,4000} x B in {1,16,64,256} per GPU, N=30 "
                                    "(BASELINE.json configs[4]); value = the T=1500,B=64 point", "sharding": f"utterances, dp{world}"},
@@ -555,6 +579,8 @@ def run_train(args, rank, world, local_rank):
     gemm_flops, t_out = arch_gemm_flops(cfg["arch"], B, T, F, N)
     prof = capi.ProfileList(1, 400 * prof_steps)
     ms, kern, launches, clocks = tm.run(step, args.steps, args.warmup, sample_clocks=True, profile=prof, profile_steps=prof_steps)
+    if rank == 0 and args.dump_outputs:  # the last timed step's losses and the parameters it updated
+        dump_outputs(args.dump_outputs, {"loss": loss, "params": trainer.get_flat(0)})
     ms_e2e, _, _, _ = tm.run(step_e2e, args.steps, args.warmup)
     final_loss = float(loss.sum().item())
     skipped = trainer.skipped_steps()
@@ -571,8 +597,8 @@ def run_train(args, rank, world, local_rank):
             if prec == precision:
                 continue
             t2 = make_trainer(cfg, prec)
-            k = max(5, min(args.steps, 10))
-            ms2, _, _, _ = tm.run(lambda i: step(i, t2), k, 3)
+            k = args.steps
+            ms2, _, _, _ = tm.run(lambda i: step(i, t2), k, args.warmup)
             sweep[prec] = {"ms_per_step": ms2 / k, "frames_per_sec": B * T * k / (ms2 * 1e-3)}
             t2.close()
         extras["precision_sweep"] = sweep
@@ -581,12 +607,12 @@ def run_train(args, rank, world, local_rank):
         f3, y3 = make_train_inputs(np.random.default_rng(77), c2)
         df3, dy3 = torch.from_numpy(f3).to(tm.dev), torch.from_numpy(y3).to(tm.dev)
         l3 = torch.empty(c2["B"], dtype=torch.float32, device=tm.dev)
-        k = max(5, min(args.steps, 10))
-        ms3, _, _, _ = tm.run(lambda i: t3.step(df3, dy3, True, float(c2["B"]), l3), k, 3)
+        k = args.steps
+        ms3, _, _, _ = tm.run(lambda i: t3.step(df3, dy3, True, float(c2["B"]), l3), k, args.warmup)
         extras["tds_asg_point"] = {"workload": train_workload_text(c2), "precision": c2["precision"], "ms_per_step": ms3 / k,
                                    "frames_per_sec_per_gpu": c2["B"] * c2["T"] * k / (ms3 * 1e-3), "final_loss_sum": float(l3.sum().item())}
         t3.close()
-        asg = asg_point(tm, rank, 10, 3, profile=False)
+        asg = asg_point(tm, rank, args.steps, args.warmup, profile=False)
         alg = asg_algorithmic_bytes(ASG_CFG["B"], ASG_CFG["T"], ASG_CFG["N"], ASG_CFG["L"])
         extras["asg_fwd_bwd_ms_per_batch"] = asg["ms"]
         extras["asg_point"] = {"config": "T=1500 N=30 B=64", "ms_per_batch": asg["ms"], "e2e_ms_per_batch": asg["ms_e2e"],
@@ -607,7 +633,7 @@ def run_train(args, rank, world, local_rank):
     tp = os.path.join(ROOT, "profiles", "gemm_traffic.json")
     if os.path.exists(tp):
         traffic = json.load(open(tp)).get(f"dram_bytes_per_launch_{precision}")
-    kname = {"f32": "gemm_umma_kernel<f32x3>", "tf32": "gemm_umma_kernel<tf32>", "bf16": "gemm_umma_kernel<bf16>"}[precision]
+    kname = {"f32": "gemm_wgmma_kernel<f32x3>", "tf32": "gemm_wgmma_kernel<tf32>", "bf16": "gemm_wgmma_kernel<bf16>"}[precision]
     line = {
         "metric": "frames_per_sec", "value": frames * args.steps / (ms * 1e-3), "unit": "frames/s", "n_gpus": world,
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak",
@@ -616,7 +642,7 @@ def run_train(args, rank, world, local_rank):
                    "parallelism": f"dp{world}", "precision": precision,
                    "optimizer": f"SGD lr={cfg['lr']} lrcrit={cfg['lrcrit']} momentum={cfg['momentum']} maxgradnorm={cfg['maxgradnorm']}",
                    "dropout": "as in the arch file", "params": trainer.num_params(0),
-                   "cold_inputs": f"rotating {nsets} input sets; activations + gradients of a step ({B}x{T} frames) exceed the 126 MB L2"},
+                   "cold_inputs": f"rotating {nsets} input sets; activations + gradients of a step ({B}x{T} frames) exceed the 50 MB L2"},
         "final_loss_sum": final_loss, "skipped_steps_nan_guard": skipped,
         "clocks": clocks,
         "e2e": {"value": frames * args.steps / (ms_e2e * 1e-3), "unit": "frames/s", "ms_per_step": ms_e2e / args.steps,
@@ -624,7 +650,7 @@ def run_train(args, rank, world, local_rank):
         "gpu_launches": launches,
         "roofline": {"bound": "tensor", "kernel": kname, "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
                      "frac": achieved / peak, "traffic": traffic,
-                     "peak_source": src + " bf16_tflops_sustained (tf32 / f32x3 math has 1/2 / 1/6 of the bf16 hardware ceiling)",
+                     "peak_source": src + "; peak = bf16 (tf32 / f32x3 math has 1/2 / 1/6 of the bf16 hardware ceiling)",
                      "gemm_ms_per_step": gemm_ms_per_step, "gemm_launches_per_step": len(kern) / max(1, prof_steps),
                      "algorithmic_flops_per_step": gemm_flops, "gemm_share_of_step": gemm_ms_per_step / (ms / args.steps),
                      "gemm_launch_us_first_step": [round(1e3 * t, 1) for t in kern[:int(len(kern) / max(1, prof_steps))]]},
@@ -646,6 +672,8 @@ def main():
     ap.add_argument("--precision", default="config", choices=["config", "f32", "tf32", "bf16"])
     ap.add_argument("--no-extras", action="store_true", help="skip the precision sweep / TDS+ASG / ASG point of the default workload")
     ap.add_argument("--no-cpu", action="store_true", help="skip the CPU baseline leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the timed path computed in its last step to DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

@@ -1,6 +1,6 @@
 // fl_compat.h — the slice of flashlight 0.3's C++ operator surface that wav2letter's Train.cpp loop
 // touches (SURVEY.md §8b, Appendix F), re-implemented on top of libw2l_b200's C ABI (include/w2l_b200.h)
-// for sm_100a.  Same names, argument meaning and error behaviour as the reference so that the loop at
+// for sm_90a.  Same names, argument meaning and error behaviour as the reference so that the loop at
 // recipes/slimIPL/src/Train.cpp:383-410 (construction), :1430-1804 (step) reads unchanged:
 //
 //   fl::Variable                      device tensor + grad + backward closure (.array() .dims(i) .grad()
@@ -223,7 +223,7 @@ class Conv2D : public UnaryModule {
   void setAsymmetricPad(int left, int right) { padL_ = left; padR_ = right; explicitPad_ = true; }
   // Functional form (used by WeightNorm): the same layer with the weight / bias taken from the given variables.
   Variable forwardWith(const Variable& in, const Variable& weight, const Variable& bias, bool maskByConsumer);
-  // `C cin cout kw 1 pad` of the conv_glu archs: W = 1, hundreds of channels — the convolution is the tcgen05 GEMM on a
+  // `C cin cout kw 1 pad` of the conv_glu archs: W = 1, hundreds of channels — the convolution is the wgmma GEMM on a
   // zero-copy im2col view (w2l_gemm_tf32_view).  Channel counts are carried padded to multiples of 4 (zero channels);
   // with gluSplit the two halves of the output channels are padded separately for the GLU that follows.
   void setGluSplit(bool on) { gluSplit_ = on; }
@@ -412,7 +412,7 @@ class SGDOptimizer : public FirstOrderOptimizer {
 double clipGradNorm(const std::vector<Variable>& params, double maxNorm);  // fl::clipGradNorm (host sync, as upstream)
 
 // Packs the parameters of modules into one contiguous arena (values, gradients) so the optimizer, the
-// gradient all-reduce and the norm are single kernels / one NCCL call (B200-first replacement for
+// gradient all-reduce and the norm are single kernels / one NCCL call (GPU-first replacement for
 // flashlight's per-array JIT kernels and CoalescingReducer's staging copies).
 struct ParameterArena {
   af::array values, grads, velocity;

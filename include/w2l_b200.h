@@ -1,5 +1,5 @@
 /*
- * w2l_b200.h — C ABI of libw2l_b200.so: the B200-native (sm_100a) implementation of
+ * w2l_b200.h — C ABI of libw2l_b200.so: the H100-native (sm_90a) implementation of
  * wav2letter's training hot path.  Every entry point below replaces one piece of the
  * un-vendored flashlight-0.3 backend that the reference's Train.cpp loop reaches through
  * fl::pkg::speech::SequenceCriterion / fl::Module (SURVEY.md §8b).  The binding a
@@ -147,7 +147,7 @@ W2L_API int w2l_linseg_target(void* stream, int B, int T, int L, const int32_t* 
 /* ----------------------------------------------------------------------------------------
  * Dense contraction of the acoustic model (replaces fl::Linear's af::matmul -> cuBLAS and the
  * GEMM inside cuDNN's convolutions; forward at Train.cpp:1470, backward at :1720).
- *   C[m][n] = act( sum_k A(m,k) * B(n,k) + bias[n] ),  fp32 storage, tcgen05 math in the kind the thread's precision
+ *   C[m][n] = act( sum_k A(m,k) * B(n,k) + bias[n] ),  fp32 storage, wgmma math in the kind the thread's precision
  *   setting selects (TF32 by default, F32X3 under W2L_PRECISION_F32), fp32 accumulation.  a_mn_major = 0: A stored [M][K] (lda), 1: A stored [K][M];  b_mn_major = 0:
  *   B stored [N][K] (ldb), 1: B stored [K][N].  forward Y = X W^T : (0,0); dgrad dX = dY W :
  *   (0,1) with B = W; wgrad dW = dY^T X : (1,1) with A = dY, B = X.  bias nullable; act 0 none,
@@ -156,14 +156,14 @@ W2L_API int w2l_linseg_target(void* stream, int B, int T, int L, const int32_t* 
 /* w2l_gemm_tf32 with OVERLAPPING operand rows allowed (lda / ldb may be smaller than the row length; still % 4):
  * the im2col matrix of a stride-1 time convolution over [T][Cin] activations — row t = the kw*Cin contiguous floats
  * starting at frame t, row stride Cin — is then a zero-copy TMA view.  This is how the large-channel `C` convolutions
- * of the conv_glu archs (recipes/conv_glu/librispeech/network.arch) run on the tcgen05 GEMM:
+ * of the conv_glu archs (recipes/conv_glu/librispeech/network.arch) run on the wgmma GEMM:
  *   fwd   Y[t][co]  = sum_k Xview[t][k] Warr[co][k]            (A = Xview K-major, lda = Cin;  B = Warr K-major)
  *   dgrad dX[t][ci] = sum_k dYview[t][k] Wflip[ci][k]          (A = zero-padded dY view, lda = Cout)
  *   wgrad dWarr[co][k] += sum_t dY[t][co] Xview[t][k]          (A = dY MN-major; B = Xview MN-major, ldb = Cin)
  * (the data gradient's kw-1 frames of left context are kw-1 zero rows in front of dY: the caller pads a copy) */
 W2L_API int w2l_gemm_tf32_view(void* stream, int a_mn_major, int b_mn_major, int M, int N, int K, const float* A, int lda,
                                const float* B, int ldb, float* C, int ldc, const float* bias, int act, int accumulate);
-/* Operand kinds of the tcgen05 GEMM (csrc/gemm_umma.cu) and the precision setting that selects among them.
+/* Operand kinds of the wgmma GEMM (csrc/gemm_wgmma.cu) and the precision setting that selects among them.
  *   TF32  : fp32 operands in HBM, TF32 products (10-bit mantissa), fp32 accumulation — what cuDNN/cuBLAS do by default
  *           for fp32 tensors on Ampere+; the default.
  *   F32X3 : fp32 operands in HBM, fp32-ACCURATE contraction: each staged tile is split hi/lo in shared memory and the
@@ -190,8 +190,8 @@ W2L_API int w2l_cast_bf16(void* stream, long long n, const float* x, void* y);
 W2L_API int w2l_cast_bf16_rows(void* stream, long long rows, int cols, int ld_in, int cols_padded, const float* x, void* y);
 /* Pin the GEMM tile width (128 / 160 / 224 / 256; 0 = choose per shape, the default).  Thread-local; for tests and tuning. */
 W2L_API int w2l_gemm_set_tile(int bn);
-/* 1 (default): the persistent kernel — one CTA per SM walking tiles, two TMEM accumulators so a tile's epilogue overlaps the
- * next tile's main loop; 0: one tile per CTA.  Thread-local; for tests (the two must agree) and tuning. */
+/* 1 (default): one CTA per SM walking the tiles, so the producer stages the next tile's operands during an epilogue;
+ * 0: one CTA per tile.  Thread-local; for tests (the two must agree) and tuning. */
 W2L_API int w2l_gemm_set_variant(int variant);
 W2L_API int w2l_gemm_tf32(void* stream, int a_mn_major, int b_mn_major, int M, int N, int K, const float* A, int lda,
                           const float* B, int ldb, float* C, int ldc, const float* bias, int act);
@@ -218,8 +218,8 @@ W2L_API int w2l_gemm_tf32_ex(void* stream, int a_mn_major, int b_mn_major, int M
  * ---------------------------------------------------------------------------------------- */
 W2L_API size_t w2l_conv_time_workspace_size(int B, int Tout, int Cin, int Cout, int K);
 /* 0 (default): the mma.sync tensor-core kernels where the shape allows (TF32, or 3xTF32 under W2L_PRECISION_F32); 1: always the
- * fp32 SIMT kernels (the fallback for widths that are not multiples of 8); 2: mma.sync; 3: the tcgen05 / TMA kernel of
- * conv_umma.cu for forward and stride-1 data gradients (parity-green, measured slower at kw = 21: see DESIGN.md).  Thread-local. */
+ * fp32 SIMT kernels (the fallback for widths that are not multiples of 8); 2: mma.sync; 3: the wgmma / TMA kernel of
+ * conv_wgmma.cu for forward and stride-1 data gradients (parity-green, opt-in: see DESIGN.md).  Thread-local. */
 W2L_API int w2l_conv_set_path(int path);
 W2L_API int w2l_conv_time_fwd(void* stream, int B, int T, int Tout, int W, int Cin, int Cout, int K, int stride,
                               int pad_left, const float* x, const float* wt, const float* bias, const float* add, float* y,

@@ -9,9 +9,12 @@ never does.
 """
 from __future__ import annotations
 
+import atexit
 import ctypes
 import os
+import shutil
 import subprocess
+import tempfile
 
 import numpy as np
 
@@ -31,10 +34,19 @@ def build(force: bool = False) -> str:
     return _SO
 
 
+_native_dir = None
+
+
 def build_native() -> str:
-    """-march=native build for the host it is called on (bench.py's CPU legs; BASELINE.md §4)"""
-    so = os.path.join(_HERE, "libw2l_oracle_native.so")
-    subprocess.check_call(["make", "-C", _HERE, "-s", "-B", "native"])
+    """-march=native build for the host it is called on (bench.py's CPU legs; BASELINE.md §4), compiled into one
+    temporary directory per process (removed at exit) so that a read-only source tree works"""
+    global _native_dir
+    if _native_dir is None:
+        _native_dir = tempfile.mkdtemp(prefix="w2l_oracle_")
+        atexit.register(shutil.rmtree, _native_dir, True)
+    so = os.path.join(_native_dir, "libw2l_oracle_native.so")
+    if not os.path.exists(so):
+        subprocess.check_call(["make", "-C", _HERE, "-s", "-B", "native", f"NATIVE_SO={so}"])
     return so
 
 

@@ -9,7 +9,7 @@
  *   flashlight/lib/sequence/criterion/cpu/{FullConnectionCriterion,ForceAlignmentCriterion,
  *   ViterbiPath,CriterionUtils}.cpp and pkg/speech/criterion/backend/cpu/
  *   ConnectionistTemporalClassificationCriterion.cpp.
- * Those sources are absent from /root/reference, so this file restates their published
+ * Those sources are absent from the reference tree, so this file restates their published
  * algorithm (SURVEY.md Appendix A).  PARITY UNPINNED by the reference's own tests (it has none
  * for this path); the oracle is instead pinned in tests/ by brute-force path enumeration,
  * central finite differences, batching invariance, torch.nn.functional.ctc_loss and the two

@@ -46,4 +46,3 @@ for T in (100, 500, 1500, 4000):
                    ns_per_dependent_step=round(ms * 1e6 / T, 1), rel_err_vs_oracle=err)
         rows.append(row)
         print(json.dumps(row), flush=True)
-json.dump(rows, open(os.path.join("gpurun_out", "asg_sweep_r1.json"), "w"), indent=1)

@@ -1,5 +1,5 @@
-"""Forward / stride-1 data gradient of the TDS time convolution: the tcgen05 kernel (path 0) against the mma.sync kernel
-(path 2) on the shapes of the seq2seq_tds and streaming steps, with and without dropout.  Writes gpurun_out/conv_paths.json."""
+"""Forward / stride-1 data gradient of the TDS time convolution: the wgmma kernel (path 3) against the mma.sync kernel
+(path 2) on the shapes of the seq2seq_tds and streaming steps, with and without dropout.  Prints the timings as JSON."""
 import json
 import os
 import sys
@@ -33,11 +33,10 @@ for (B, T, C, K, pl) in [(16, 600, 10, 21, 10), (16, 300, 14, 21, 10), (16, 150,
     bias = torch.randn(C, device="cuda")
     rec = {"B": B, "T": T, "C": C, "K": K, "MB": round(2 * x.numel() * 4 / 1e6, 1)}
     for p in (0.0, 0.2):
-        rec[f"umma_us_p{p}"] = round(time_fwd(x, wt, bias, T, pl, p, 3), 1)
+        rec[f"wgmma_us_p{p}"] = round(time_fwd(x, wt, bias, T, pl, p, 3), 1)
         rec[f"mma_us_p{p}"] = round(time_fwd(x, wt, bias, T, pl, p, 2), 1)
-    rec["umma_GBps"] = round(rec["MB"] * 1e3 / rec["umma_us_p0.2"], 1)
+    rec["wgmma_GBps"] = round(rec["MB"] * 1e3 / rec["wgmma_us_p0.2"], 1)
     rec["mma_GBps"] = round(rec["MB"] * 1e3 / rec["mma_us_p0.2"], 1)
     out.append(rec)
     print(json.dumps(rec), flush=True)
-os.makedirs("gpurun_out", exist_ok=True)
-json.dump(out, open("gpurun_out/conv_paths.json", "w"), indent=1)
+json.dump(out, sys.stdout, indent=1)

@@ -34,4 +34,4 @@ for name, M, N, K, a_mn, b_mn in shapes:
     capi.gemm_set_tile(0)
     out[f"{name} M={M} N={N} K={K}"] = row
     print(f"{name:11s} M={M:5d} N={N:5d} K={K:5d} " + "  ".join(f"bn{bn}: {v[0]:7.1f}us {v[1]:6.1f}TF" for bn, v in row.items()), flush=True)
-json.dump(out, open(os.path.join("gpurun_out", "gemm_tiles.json"), "w"), indent=1)
+json.dump(out, sys.stdout, indent=1)

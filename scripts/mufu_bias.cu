@@ -1,5 +1,5 @@
 // Error statistics of the MUFU approximations used by the FAC recursion against double precision
-// (nvcc -gencode arch=compute_100a,code=sm_100a scripts/mufu_bias.cu -o build/mufu_bias):
+// (nvcc -gencode arch=compute_90a,code=sm_90a scripts/mufu_bias.cu -o build/mufu_bias):
 //   part 1: lg2.approx(1 + r) on r in [0,1], ex2.approx(d) on d in [-30,0], and the composite lg2(1 + ex2(d))
 //   part 2: the composite the recursion actually evaluates, F(d) = lg2.approx(fma(ex2.approx(d), 1.25, 1.25)) against
 //           log2(1.25 (1 + 2^d)), binned by its argument q' = 1.25 (1 + 2^d) in [1.25, 2.5]

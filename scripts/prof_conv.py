@@ -1,5 +1,5 @@
-"""A few launches of the TDS time convolution (forward / stride-1 data gradient: tcgen05 kernel) at the stage shapes of the
-seq2seq_tds step, for `ncu --set full -k regex:conv_umma_fwd`."""
+"""A few launches of the TDS time convolution (forward / stride-1 data gradient: wgmma kernel) at the stage shapes of the
+seq2seq_tds step, for `ncu --set full -k regex:conv_wgmma_fwd`."""
 import sys
 
 import torch

@@ -1,4 +1,4 @@
-"""A few launches of the tcgen05 GEMM on the stage-1 FC shapes of the seq2seq_tds step, for `ncu --set full -k regex:gemm_umma`."""
+"""A few launches of the wgmma GEMM on the stage-1 FC shapes of the seq2seq_tds step, for `ncu --set full -k regex:gemm_wgmma`."""
 import sys
 
 import torch

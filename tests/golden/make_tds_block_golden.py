@@ -1,7 +1,7 @@
 """Extracts the known-answer vectors of the reference's own TDS-block test
 (recipes/streaming_convnets/inference/inference/module/test/TDSBlockTest.cpp:27-188, TEST(TDSBlock, TestOne):
 T=10, groups=5, 2 channels per group, kernel 3, padding 1/1, tolerance 1e-2) into tests/golden/tds_block_golden.npz.
-Run once in the build container (needs /root/reference); only the numbers are stored (test data).
+Run once with the root of the reference tree as its argument; only the numbers are stored (test data).
 
 Layout of the reference's inference modules (Conv1dTest.cpp:30-104, TDSBlockTest.cpp): activations [T][groups][c]
 (feature index w*C + c), conv weights [cout/g][kw][cin/g] shared by every group, Linear weights W[i*nOut + o],
@@ -14,11 +14,11 @@ import sys
 
 import numpy as np
 
-SRC = "/root/reference/recipes/streaming_convnets/inference/inference/module/test/TDSBlockTest.cpp"
+SRC = "recipes/streaming_convnets/inference/inference/module/test/TDSBlockTest.cpp"  # inside the reference tree
 
 
-def main():
-    text = open(SRC).read()
+def main(ref_root):
+    text = open(os.path.join(ref_root, SRC)).read()
     body = text[text.index("TEST(TDSBlock, TestOne)"):text.index("TEST(TDSBlock, Serialization)")]
     vec = {}
     for m in re.finditer(r"std::vector<float>\s+(\w+)\s*=\s*\{([^}]*)\}", body):
@@ -56,4 +56,4 @@ def main():
 
 
 if __name__ == "__main__":
-    main()
+    main(sys.argv[1])

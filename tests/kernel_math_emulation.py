@@ -199,7 +199,7 @@ def fac_emulate(e, y, tr):
 # normalised by the frame maximum and the global transition maximum, lg2(1.25 * (1 + r)) with the constant folded into the
 # transition scores, P consecutive positions per lane, re-centring every kRc frames either with ONE offset per row (the
 # first version) or with one offset PER LANE (what the kernels do).  exp2 / log2 are exact here (float64, rounded to
-# float32): the MUFU table error is a separate, measured effect (profiles/mufu_bias_r2.txt).
+# float32): the MUFU table error is a separate effect (DESIGN.md, ASG accuracy).
 # ------------------------------------------------------------------------------------------------------------------
 LOG2E = 1.4426950408889634
 NEG = F(-1.0e30)

@@ -1,6 +1,6 @@
 """CPU-side checks of the C ABI: the library loads, exports every symbol include/w2l_b200.h
 declares, reports workspace sizes, and rejects bad arguments with the documented codes —
-no kernel is launched (no GPU in the dev container)."""
+no kernel is launched, so they run without a GPU."""
 import ctypes
 import os
 import re

@@ -1,6 +1,7 @@
-"""The arch generators of wav2letter_b200/archs.py reproduce the reference's arch files token for token (checked whenever
-/root/reference is present, i.e. in the build container; the GPU box has no reference tree and uses the generators)."""
+"""The arch generators of wav2letter_b200/archs.py reproduce the reference's arch files token for token (the reference
+files' token streams are stored in tests/golden/reference_archs.json by tests/golden/make_reference_archs.py)."""
 import importlib.util
+import json
 import os
 
 import pytest
@@ -10,7 +11,8 @@ spec = importlib.util.spec_from_file_location("w2l_archs", os.path.join(ROOT, "w
 archs = importlib.util.module_from_spec(spec)
 spec.loader.exec_module(archs)
 
-REF = "/root/reference"
+with open(os.path.join(ROOT, "tests", "golden", "reference_archs.json")) as _f:
+    GOLDEN = json.load(_f)
 
 
 def tokens(text):
@@ -19,12 +21,10 @@ def tokens(text):
 
 @pytest.mark.parametrize("name", sorted(archs.REFERENCE_FILES))
 def test_generated_arch_matches_reference_file(name):
-    path = os.path.join(REF, archs.REFERENCE_FILES[name])
-    if not os.path.exists(path):
-        pytest.skip("reference tree not present")
+    assert GOLDEN[name]["file"] == archs.REFERENCE_FILES[name]
     gen = archs.BASELINE_ARCHS[name][0]
     text = gen(ctc_head=False) if name == "seq2seq_tds_ctc" else gen()
-    assert tokens(text) == tokens(open(path).read())
+    assert tokens(text) == GOLDEN[name]["tokens"]
 
 
 def test_ctc_head_only_changes_the_last_linear():

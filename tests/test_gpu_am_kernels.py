@@ -183,7 +183,7 @@ def test_colsum_sqnorm_sgd():
 ])
 def test_conv_time_streaming_shapes_all_paths(B, T, Cin, Cout, K, stride, pl, pr, path):
     """the asymmetric paddings of the streaming TDS arch (PD l r + C2, TDS with rightPadding) on the three arithmetic paths:
-    the tcgen05 / TMA kernel (forward, stride-1 data gradient), the mma.sync TF32 kernels, the same in error-compensated
+    the wgmma / TMA kernel (forward, stride-1 data gradient), the mma.sync TF32 kernels, the same in error-compensated
     3xTF32 (W2L_PRECISION_F32), and the fp32 SIMT fallback"""
     from wav2letter_b200 import capi
 
@@ -199,7 +199,7 @@ def test_conv_time_streaming_shapes_all_paths(B, T, Cin, Cout, K, stride, pl, pr
     pre.backward(dy.double())
     try:
         capi.set_precision("f32" if path == "x3" else "tf32")
-        capi._check(capi.lib.w2l_conv_set_path({"simt": 1, "mma": 2, "tf32": 3}.get(path, 0)))  # "tf32" = the tcgen05 kernel
+        capi._check(capi.lib.w2l_conv_set_path({"simt": 1, "mma": 2, "tf32": 3}.get(path, 0)))  # "tf32" = the wgmma kernel
         y = capi.conv_time_fwd(x, wt, bias, Tout, stride, pl)
         dx = capi.conv_time_dgrad(dy, wt, T, stride, pl)
         dwt, dbias = capi.conv_time_wgrad(x, dy, K, stride, pl)
@@ -211,3 +211,27 @@ def test_conv_time_streaming_shapes_all_paths(B, T, Cin, Cout, K, stride, pl, pr
     assert rel(dx, x64.grad) < tol, (path, rel(dx, x64.grad))
     assert rel(dwt, w64.grad) < tol, (path, rel(dwt, w64.grad))
     assert rel(dbias, b64.grad) < tol
+
+
+def test_conv_time_wgmma_path_falls_back_when_the_window_does_not_fit():
+    """w2l_conv_set_path(3) selects the wgmma kernel only where its window and weights fit in shared memory: at 32 channels
+    and kw = 27 they do not (and the mma.sync kernel does not cover kw * C > 512), so the call runs on the SIMT kernels"""
+    from wav2letter_b200 import capi
+
+    B, T, C, K, pl, W = 1, 40, 32, 27, 13, 80
+    g = torch.Generator(device="cuda").manual_seed(27)
+    x = torch.randn((B, T, C, W), device="cuda", generator=g)
+    wt = torch.randn((C, C, K), device="cuda", generator=g) * 0.1
+    bias = torch.randn(C, device="cuda", generator=g)
+    Tout = T + 2 * pl - K + 1
+    x64, w64, b64 = x.double().requires_grad_(True), wt.double().requires_grad_(True), bias.double().requires_grad_(True)
+    pre = ref_conv(x64, w64, b64, 1, pl, Tout)
+    dy = torch.randn((B, Tout, C, W), device="cuda", generator=g)
+    pre.backward(dy.double())
+    try:
+        capi._check(capi.lib.w2l_conv_set_path(3))
+        y = capi.conv_time_fwd(x, wt, bias, Tout, 1, pl)
+        dx = capi.conv_time_dgrad(dy, wt, T, 1, pl)
+    finally:
+        capi._check(capi.lib.w2l_conv_set_path(0))
+    assert rel(y, pre) < 3e-3 and rel(dx, x64.grad) < 3e-3

@@ -1,5 +1,5 @@
 """Conv1D + GLU acoustic-model family (recipes/conv_glu/{wsj,librispeech}/network.arch): WeightNorm-wrapped large-channel
-time convolutions run as tcgen05 GEMMs on zero-copy im2col views, GLU (+dropout), Reorder, WeightNorm Linear head.
+time convolutions run as wgmma GEMMs on zero-copy im2col views, GLU (+dropout), Reorder, WeightNorm Linear head.
 Kernel-level parity against float64 torch, then one whole train step (ASG criterion, 6 letter classes) against a float64
 torch graph built from the same parameters.  Tolerances are the TF32 ones of test_gpu_trainer.py."""
 import numpy as np

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05/TMA GEMM (TF32 math, fp32 accumulate) against a float64 reference of
+"""GPU parity of the wgmma/TMA GEMM (TF32 math, fp32 accumulate) against a float64 reference of
 the same op.  Tolerance: TF32 keeps 10 mantissa bits per operand (TMA rounds on load), so each
 product carries <= 2^-10 relative error: |C - ref| <= 1.5e-3 * (|A| |B|^T) element-wise."""
 import numpy as np
@@ -57,8 +57,8 @@ def test_gemm_rejects_unaligned():
 @pytest.mark.parametrize("M,N,K,a_mn,b_mn", [(1120, 1120, 4800, True, True), (360, 360, 9600, True, True),
                                               (256, 200, 2052, False, False), (128, 128, 16 * 32, False, True)])
 def test_gemm_split_k(M, N, K, a_mn, b_mn, accumulate):
-    """few output tiles + long K (the weight-gradient shape): the k blocks are split over blockIdx.z and summed with
-    vector atomics; same TF32 bound, plus the accumulate-onto-C semantics"""
+    """few output tiles + long K (the weight-gradient shape): the k blocks are split into slices whose partial tiles are
+    summed in slice order; same TF32 bound, plus the accumulate-onto-C semantics"""
     import wav2letter_b200 as w
 
     g = torch.Generator(device="cuda").manual_seed(K)
@@ -135,7 +135,7 @@ def test_gemm_view_data_gradient(T, Cin, Cout, kw):
     assert float((dx.double() - ref).abs().max()) < 3e-3 * float(ref.abs().max()) + 1e-3
 
 
-# ---- operand kinds: fp32-accurate 3xTF32 split and bf16 (csrc/gemm_umma.cu) -----------------------------------------
+# ---- operand kinds: fp32-accurate 3xTF32 split and bf16 (csrc/gemm_wgmma.cu) ----------------------------------------
 def _operands(M, N, K, a_mn, b_mn, seed, dtype=torch.float32):
     g = torch.Generator(device="cuda").manual_seed(seed)
     A = torch.randn((K, M) if a_mn else (M, K), device="cuda", generator=g)
@@ -228,8 +228,8 @@ def test_cast_bf16_matches_torch():
 @pytest.mark.parametrize("M,N,K,a_mn,b_mn", [(9600, 800, 800, False, False), (4800, 1120, 1120, False, True), (1120, 1120, 4800, True, True),
                                               (300, 10000, 1440, False, False), (136, 72, 4000, True, False), (128, 128, 64, False, False)])
 def test_gemm_persistent_and_per_tile_kernels_agree(M, N, K, a_mn, b_mn, kind):
-    """the persistent kernel (two TMEM accumulators, tiles walked per SM) against the one-tile-per-CTA kernel: same tile
-    shape and k order, so results agree to the last bit except under split-K (atomic accumulation order)"""
+    """the persistent kernel (one CTA per SM walking the tiles) against the one-tile-per-CTA kernel: same tile
+    shape, k order and split-K slice order, so results agree to the last bit"""
     import wav2letter_b200 as w
 
     A, B = _operands(M, N, K, a_mn, b_mn, seed=M + N, dtype=torch.bfloat16 if kind == "bf16" else torch.float32)
@@ -254,3 +254,19 @@ def test_gemm_persistent_and_per_tile_kernels_agree(M, N, K, a_mn, b_mn, kind):
     ref = (A.t() if a_mn else A).double() @ (B.t() if b_mn else B).double().t()
     tol = {"tf32": 3e-3, "f32x3": 2e-5, "bf16": 2e-5}[kind]
     assert float((P1.double() - ref).abs().max()) <= tol * float(ref.abs().max()) * (K ** 0.5) / 8 + 1e-4
+
+
+@pytest.mark.parametrize("kind", ["tf32", "f32x3", "bf16"])
+def test_gemm_split_k_is_run_to_run_identical(kind):
+    """split-K partial tiles are summed in slice order, so repeating a weight-gradient-shaped GEMM gives the same bits"""
+    import wav2letter_b200 as w
+
+    A, B = _operands(360, 360, 9600, True, True, seed=5, dtype=torch.bfloat16 if kind == "bf16" else torch.float32)
+    C0 = torch.randn(360, 360, device="cuda")
+    outs = []
+    for _ in range(3):
+        C = C0.clone()
+        w.capi.gemm(A, B, kind, True, True, out=C, accumulate=True)
+        outs.append(C)
+    torch.cuda.synchronize()
+    assert torch.equal(outs[0], outs[1]) and torch.equal(outs[0], outs[2])

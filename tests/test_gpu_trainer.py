@@ -4,7 +4,7 @@ Tolerances: emissions / loss 5e-3 relative, all gradients together 2e-2, any sin
 contractions run in TF32 on the tensor cores (10-bit mantissa operands), and the back-propagated error through
 LayerNorm's mean subtractions is what cuBLAS/cuDNN-TF32 shows too: scripts/diag_trainer.py prints this kernel's
 per-parameter error next to torch's own fp32+TF32 error vs float64 on the same network — they agree to 2-3
-digits (e.g. 3.34e-2 vs 3.35e-2 on the worst FC weight; profiles/tds_train_step_r1.md)."""
+digits."""
 import numpy as np
 import pytest
 import torch

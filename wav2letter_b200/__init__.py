@@ -1,4 +1,4 @@
-"""wav2letter_b200 — B200-native (sm_100a) implementation of wav2letter's training hot path.
+"""wav2letter_b200 — H100-native (sm_90a) implementation of wav2letter's training hot path.
 
 The product is ``libw2l_b200.so`` (hand-written CUDA behind the C ABI in ``include/w2l_b200.h``)
 plus the C++ ``fl_compat`` layer that mirrors the reference's operator surface.  This Python

@@ -1,8 +1,8 @@
 """Architecture files of the four BASELINE.json model configs, generated from their layer tables.
 
 Pure Python, no imports: bench.py's reference arm loads this file by path so that the CUDA library is never mapped
-into the reference process.  tests/test_archs.py checks, whenever /root/reference is present, that every generator
-reproduces the recipe's arch file token for token:
+into the reference process.  tests/test_archs.py checks that every generator reproduces the recipe's arch file
+token for token (stored in tests/golden/reference_archs.json):
 
   conv_glu_wsj()          recipes/conv_glu/wsj/network.arch              (configs[0])
   seq2seq_tds(ctc_head)   recipes/seq2seq_tds/librispeech/network.arch   (configs[1]; ctc_head swaps the encoder's

@@ -329,7 +329,7 @@ def get_precision() -> int:
 
 def gemm(A, B, kind="tf32", a_mn=False, b_mn=False, bias=None, act=0, out=None, out_bf16=False, accumulate=False, aux=None,
          aux_mode=0, aux_scale=1.0, dropout_p=0.0, seed=0, M=None, N=None, K=None, lda=None, ldb=None, allow_overlap=False):
-    """General tcgen05 GEMM (w2l_gemm): A/B fp32 (kinds tf32, f32x3) or bfloat16 (kind bf16); C fp32 or bfloat16."""
+    """General wgmma GEMM (w2l_gemm): A/B fp32 (kinds tf32, f32x3) or bfloat16 (kind bf16); C fp32 or bfloat16."""
     if M is None:
         M, K = (A.shape[1], A.shape[0]) if a_mn else A.shape
         N = B.shape[1] if b_mn else B.shape[0]
@@ -352,7 +352,7 @@ def cast_bf16(x):
 
 
 def gemm_set_variant(v: int = 1):
-    """1: persistent kernel with two TMEM accumulators (default); 0: one tile per CTA"""
+    """1: one CTA per SM walking the tiles (default); 0: one tile per CTA"""
     _check(lib.w2l_gemm_set_variant(int(v)))
 
 

@@ -1,4 +1,4 @@
-// am_kernels.cu — non-GEMM kernels of the acoustic-model forward/backward (sm_100a).
+// am_kernels.cu — non-GEMM kernels of the acoustic-model forward/backward (sm_90a).
 //
 // Activations are fp32 [B][T][C][W] (W = 80 filterbank channels innermost, feature index
 // f = c*W + w — the order flashlight's `V 0 1440 1 0` view produces from [T,W,C,B], so Linear
@@ -11,7 +11,7 @@
 //     and into the LayerNorm backward (the mask is read back from the stored activation sign)
 //   fl::SGDOptimizer / fl::clipGradNorm (Train.cpp:1791-1803) -> w2l_sq_norm / w2l_sgd_step on a flat arena
 // These passes are HBM-bound (the k x 1 convolution has only 10-27 channels: SURVEY.md §7.4-3);
-// the dense contractions live in gemm_umma.cu.
+// the dense contractions live in gemm_wgmma.cu.
 #include <cuda_runtime.h>
 
 #include <cooperative_groups.h>
@@ -21,21 +21,20 @@
 namespace w2l {
 // tensor-core path (conv_mma.cu)
 bool conv_mma_supported(int W, int Cin, int Cout, int K, int stride);
-bool conv_umma_supported(int W, int Cin, int Cout, int K, int stride);
-size_t conv_umma_arranged_floats(int Cin, int Cout, int K);
-int conv_umma_fwd(cudaStream_t stream, int B, int T, int Tout, int W, int Cin, int Cout, int K, int stride, int pad_left, const float* x,
+bool conv_wgmma_supported(int W, int Cin, int Cout, int K, int stride);
+size_t conv_wgmma_arranged_floats(int Cin, int Cout, int K);
+int conv_wgmma_fwd(cudaStream_t stream, int B, int T, int Tout, int W, int Cin, int Cout, int K, int stride, int pad_left, const float* x,
                   const float* wt, int wt_cin, int wt_cout, int flip, const float* bias, const float* add, float* y, int act, float drop_p,
                   unsigned long long seed, float* arranged);
 // the tensor-core path (TF32 products; under W2L_PRECISION_F32 the same kernels run error-compensated 3xTF32); shapes it
 // does not cover fall back to the fp32 SIMT kernels below
-static thread_local int g_conv_path = 0;  // w2l_conv_set_path: 0 auto (= mma.sync where the shape allows), 1 fp32 SIMT kernels, 2 mma.sync, 3 tcgen05 — tests / tuning
+static thread_local int g_conv_path = 0;  // w2l_conv_set_path: 0 auto (= mma.sync where the shape allows), 1 fp32 SIMT kernels, 2 mma.sync, 3 wgmma — tests / tuning
 static bool use_conv_mma(int W, int Cin, int Cout, int K, int stride) { return g_conv_path != 1 && conv_mma_supported(W, Cin, Cout, K, stride); }
-// tcgen05 / TMA forward and stride-1 data gradient (conv_umma.cu): parity-green but MEASURED SLOWER than the mma.sync kernel
-// at kw = 21 (138 vs 56 us on the stage-1 shape, profiles/conv_paths_r2.json): with 10-27 channels every tcgen05.mma is a
-// 128 x 16 x 8 sliver and a window needs kw * Cp/8 of them per 128 positions — the tensor pipe is issue-bound at 5 % use.
-// Kept selectable (w2l_conv_set_path(3)) and tested; the default stays on the mma.sync kernels.
-static bool use_conv_umma(int W, int Cin, int Cout, int K, int stride) {
-  return g_conv_path == 3 && current_precision() != W2L_PRECISION_F32 && conv_umma_supported(W, Cin, Cout, K, stride);
+// wgmma / TMA forward and stride-1 data gradient (conv_wgmma.cu): with 10-27 channels every wgmma is a 64 x 16 x 8 sliver
+// and a window needs kw * Cp/8 of them per 64 positions, so the tensor pipe is issue-bound; selectable
+// (w2l_conv_set_path(3)) and tested, the default stays on the mma.sync kernels.
+static bool use_conv_wgmma(int W, int Cin, int Cout, int K, int stride) {
+  return g_conv_path == 3 && current_precision() != W2L_PRECISION_F32 && conv_wgmma_supported(W, Cin, Cout, K, stride);
 }
 size_t conv_mma_arranged_floats(int Cin, int Cout, int K);
 int conv_mma_fwd(cudaStream_t stream, int B, int T, int Tout, int W, int Cin, int Cout, int K, int stride, int pad_left,
@@ -558,17 +557,12 @@ __global__ void __launch_bounds__(256) ln_bwd_apply_kernel(long long R, int vec,
                                                            const float* __restrict__ r, const float* __restrict__ dy,
                                                            const float* __restrict__ gain, const float* __restrict__ mean_rstd,
                                                            const double* __restrict__ sums, float* __restrict__ d_branch,
-                                                           float* __restrict__ d_res, int branch_mode, float branch_scale,
-                                                           float* __restrict__ dgain, float* __restrict__ dbias) {
+                                                           float* __restrict__ d_res, int branch_mode, float branch_scale) {
   const int b = blockIdx.y;
   const float mu = mean_rstd[2 * b], rstd = mean_rstd[2 * b + 1], g = gain ? *gain : 1.f;
   double S, Q;
   sum_partials(sums + 2 * (size_t)b * gridDim.x, gridDim.x, S, Q);
   const float m1 = (float)(S / (double)R), m2 = (float)(Q / (double)R);
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    if (dbias) atomicAdd(dbias, (float)S);
-    if (dgain) atomicAdd(dgain, (float)Q);
-  }
   const float* ab = a + (size_t)b * R;
   const float* rb = r ? r + (size_t)b * R : nullptr;
   const float* db = dy + (size_t)b * R;
@@ -654,7 +648,7 @@ __global__ void __launch_bounds__(256) ln_row_bwd_kernel(long long G, int R, int
                                                          const float* __restrict__ r, const float* __restrict__ dy,
                                                          const float* __restrict__ gain, const float* __restrict__ mean_rstd,
                                                          float* __restrict__ d_branch, float* __restrict__ d_res, int branch_mode,
-                                                         float branch_scale, float* __restrict__ dgain, float* __restrict__ dbias) {
+                                                         float branch_scale, double* __restrict__ part) {
   const long long grp = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   __shared__ float sh_s[8], sh_q[8];
@@ -710,7 +704,7 @@ __global__ void __launch_bounds__(256) ln_row_bwd_kernel(long long G, int R, int
       }
     }
   }
-  // scalar affine gradients: one atomic per CTA
+  // scalar affine gradients: one partial pair per CTA, summed by ln_scalar_grads_kernel
   if (lane == 0) {
     sh_s[warp] = S;
     sh_q[warp] = Q;
@@ -722,14 +716,42 @@ __global__ void __launch_bounds__(256) ln_row_bwd_kernel(long long G, int R, int
       ts += sh_s[w];
       tq += sh_q[w];
     }
-    if (dbias) atomicAdd(dbias, ts);
-    if (dgain) atomicAdd(dgain, tq);
+    part[2 * blockIdx.x] = ts;
+    part[2 * blockIdx.x + 1] = tq;
   }
 }
 
-// out[n] += sum_m X[m][n]   (bias gradients of Linear)
+// the scalar affine gradients of a LayerNorm backward: dbias += sum of the n (dy, dy * xhat) partial pairs, dgain += ...;
+// one block, fixed summation order (run to run identical)
+__global__ void __launch_bounds__(256) ln_scalar_grads_kernel(int n, const double* __restrict__ part, float* __restrict__ dgain,
+                                                              float* __restrict__ dbias) {
+  double s = 0.0, q = 0.0;
+  for (int i = threadIdx.x; i < n; i += 256) {
+    s += part[2 * i];
+    q += part[2 * i + 1];
+  }
+  s = warp_sum(s);
+  q = warp_sum(q);
+  __shared__ double ss[8], sq[8];
+  if ((threadIdx.x & 31) == 0) {
+    ss[threadIdx.x >> 5] = s;
+    sq[threadIdx.x >> 5] = q;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double S = 0.0, Q = 0.0;
+    for (int w = 0; w < 8; ++w) {
+      S += ss[w];
+      Q += sq[w];
+    }
+    if (dbias) *dbias += (float)S;
+    if (dgain) *dgain += (float)Q;
+  }
+}
+
+// part[blockIdx.y][n] = sum of X[m][n] over this CTA's rows   (bias gradients of Linear; colsum_finish_kernel adds the parts)
 __global__ void __launch_bounds__(256) colsum_kernel(int M, int N, const float* __restrict__ X, int ld, int rows_per_cta,
-                                                     float* __restrict__ out) {
+                                                     float* __restrict__ part) {
   const int n = blockIdx.x * 32 + (threadIdx.x & 31);
   const int m0 = blockIdx.y * rows_per_cta, m1 = min(M, m0 + rows_per_cta);
   float s = 0.f;
@@ -742,13 +764,13 @@ __global__ void __launch_bounds__(256) colsum_kernel(int M, int N, const float* 
     float t = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; ++w) t += red[w][threadIdx.x];
-    atomicAdd(out + n, t);
+    part[(size_t)blockIdx.y * N + n] = t;  // this row block's partial column sums
   }
 }
 
 // float4 variant (N, ld multiples of 4, 16-byte aligned base): a block covers 128 columns x rows_per_cta rows
 __global__ void __launch_bounds__(256) colsum4_kernel(int M, int N, const float* __restrict__ X, int ld, int rows_per_cta,
-                                                      float* __restrict__ out) {
+                                                      float* __restrict__ part) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int n = blockIdx.x * 128 + 4 * lane;
   const int m0 = blockIdx.y * rows_per_cta, m1 = min(M, m0 + rows_per_cta);
@@ -775,15 +797,21 @@ __global__ void __launch_bounds__(256) colsum4_kernel(int M, int N, const float*
       t.z += red[w][lane].z;
       t.w += red[w][lane].w;
     }
-    atomicAdd(out + n, t.x);
-    atomicAdd(out + n + 1, t.y);
-    atomicAdd(out + n + 2, t.z);
-    atomicAdd(out + n + 3, t.w);
+    *reinterpret_cast<float4*>(part + (size_t)blockIdx.y * N + n) = t;  // this row block's partial column sums
   }
 }
 
+// out[n] += sum over the row blocks of part[rb][n], in row-block order (run to run identical)
+__global__ void __launch_bounds__(256) colsum_finish_kernel(int N, int row_blocks, const float* __restrict__ part, float* __restrict__ out) {
+  const int n = blockIdx.x * 256 + threadIdx.x;
+  if (n >= N) return;
+  float t = 0.f;
+  for (int rb = 0; rb < row_blocks; ++rb) t += part[(size_t)rb * N + n];
+  out[n] += t;
+}
+
 // ---- optimizer on a flat parameter arena -------------------------------------------------------
-__global__ void __launch_bounds__(256) sq_norm_kernel(long long n, const float* __restrict__ g, double* __restrict__ out) {
+__global__ void __launch_bounds__(256) sq_norm_kernel(long long n, const float* __restrict__ g, double* __restrict__ part) {
   double s = 0.0;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const float v = g[i];
@@ -796,7 +824,22 @@ __global__ void __launch_bounds__(256) sq_norm_kernel(long long n, const float* 
   if (threadIdx.x == 0) {
     double S = 0;
     for (int w = 0; w < 8; ++w) S += ss[w];
-    atomicAdd(out, S);
+    part[blockIdx.x] = S;
+  }
+}
+
+// *out += sum of the n block partials, fixed order (run to run identical)
+__global__ void __launch_bounds__(256) sq_norm_finish_kernel(int n, const double* __restrict__ part, double* __restrict__ out) {
+  double s = 0.0;
+  for (int i = threadIdx.x; i < n; i += 256) s += part[i];
+  s = warp_sum(s);
+  __shared__ double ss[8];
+  if ((threadIdx.x & 31) == 0) ss[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double S = 0.0;
+    for (int w = 0; w < 8; ++w) S += ss[w];
+    *out += S;
   }
 }
 
@@ -917,7 +960,7 @@ __global__ void act_fwd_kernel(long long n, const float* __restrict__ x, int rel
   }
 }
 
-int blocks_for(long long n, int per_block = 256 * 8) { return (int)std::min<long long>((n + per_block - 1) / per_block, 148 * 8); }
+int blocks_for(long long n, int per_block = 256 * 8) { return (int)std::min<long long>((n + per_block - 1) / per_block, sm_count() * 8); }
 
 }  // namespace
 }  // namespace w2l
@@ -934,13 +977,13 @@ static size_t conv_ws_partial_bytes(int B, int Tout, int Cin, int Cout, int K) {
   return align_up(std::max(simt, std::max(mma, (size_t)B * (size_t)std::max(Tout, 16))) * per, 256);
 }
 extern "C" int w2l_conv_set_path(int path) {
-  if (path < 0 || path > 3) return fail(W2L_ERR_INVALID_ARGUMENT, "conv_set_path: 0 (auto), 1 (fp32 SIMT kernels), 2 (mma.sync kernels) or 3 (tcgen05 kernel)");
+  if (path < 0 || path > 3) return fail(W2L_ERR_INVALID_ARGUMENT, "conv_set_path: 0 (auto), 1 (fp32 SIMT kernels), 2 (mma.sync kernels) or 3 (wgmma kernel)");
   g_conv_path = path;
   return W2L_OK;
 }
 extern "C" size_t w2l_conv_time_workspace_size(int B, int Tout, int Cin, int Cout, int K) {
   const size_t arranged = std::max(std::max((size_t)std::max(Cin, Cout) * K * co_pad(std::max(Cin, Cout)), conv_mma_arranged_floats(Cin, Cout, K)),
-                                   conv_umma_arranged_floats(Cin, Cout, K)) * sizeof(float);
+                                   conv_wgmma_arranged_floats(Cin, Cout, K)) * sizeof(float);
   return conv_ws_partial_bytes(B, Tout, Cin, Cout, K) + align_up(arranged, 256);
 }
 
@@ -974,8 +1017,8 @@ extern "C" int w2l_conv_time_fwd(void* stream_, int B, int T, int Tout, int W, i
   if (ws_bytes < w2l_conv_time_workspace_size(B, Tout, Cin, Cout, K)) return fail(W2L_ERR_WORKSPACE, "conv_time_fwd: workspace too small");
   const int CO = co_pad(Cout);
   float* arranged = reinterpret_cast<float*>(static_cast<char*>(ws) + conv_ws_partial_bytes(B, Tout, Cin, Cout, K));
-  if (use_conv_umma(W, Cin, Cout, K, stride))
-    return conv_umma_fwd(stream, B, T, Tout, W, Cin, Cout, K, stride, pad_left, x, wt, Cin, Cout, 0, bias, add, y, act, dropout_p, seed, arranged);
+  if (use_conv_wgmma(W, Cin, Cout, K, stride))
+    return conv_wgmma_fwd(stream, B, T, Tout, W, Cin, Cout, K, stride, pad_left, x, wt, Cin, Cout, 0, bias, add, y, act, dropout_p, seed, arranged);
   if (use_conv_mma(W, Cin, Cout, K, stride))
     return conv_mma_fwd(stream, B, T, Tout, W, Cin, Cout, K, stride, pad_left, x, wt, Cin, Cout, 0, bias, add, y, act, dropout_p, seed,
                         arranged, K, 1, 0, 1, 0, Tout);
@@ -1001,10 +1044,10 @@ extern "C" int w2l_conv_time_dgrad(void* stream_, int B, int T, int Tout, int W,
   if (int rc = conv_check(B, T, Tout, W, Cin, Cout, K, stride)) return rc;
   if (!dy || !wt || !dx || !ws) return fail(W2L_ERR_INVALID_ARGUMENT, "conv_time_dgrad: null pointer");
   if (ws_bytes < w2l_conv_time_workspace_size(B, Tout, Cin, Cout, K)) return fail(W2L_ERR_WORKSPACE, "conv_time_dgrad: workspace too small");
-  if (stride == 1 && use_conv_umma(W, Cout, Cin, K, 1)) {
-    // dx = conv(dy, flipped weights) with pad_left' = K-1-pad_left, channel roles swapped — tcgen05 path
+  if (stride == 1 && use_conv_wgmma(W, Cout, Cin, K, 1)) {
+    // dx = conv(dy, flipped weights) with pad_left' = K-1-pad_left, channel roles swapped — wgmma path
     float* arranged = reinterpret_cast<float*>(static_cast<char*>(ws) + conv_ws_partial_bytes(B, Tout, Cin, Cout, K));
-    return conv_umma_fwd(stream, B, Tout, T, W, Cout, Cin, K, 1, K - 1 - pad_left, dy, wt, Cin, Cout, 1, nullptr, add, dx, 0, 0.f, 0ull, arranged);
+    return conv_wgmma_fwd(stream, B, Tout, T, W, Cout, Cin, K, 1, K - 1 - pad_left, dy, wt, Cin, Cout, 1, nullptr, add, dx, 0, 0.f, 0ull, arranged);
   }
   if (stride == 1 && use_conv_mma(W, Cout, Cin, K, 1)) {
     // dx = conv(dy, flipped weights) with pad_left' = K-1-pad_left, channel roles swapped — on the tensor-core path
@@ -1087,7 +1130,7 @@ extern "C" int w2l_conv_time_wgrad(void* stream_, int B, int T, int Tout, int W,
 }
 
 // many short groups -> the one-warp-per-group kernels; few long groups -> the two-pass kernels
-static bool ln_use_rows(int B, long long R) { return R <= 8192 && (long long)B * 32 >= 148 * 256; }
+static bool ln_use_rows(int B, long long R) { return R <= 8192 && (long long)B * 32 >= sm_count() * 256; }
 
 extern "C" int w2l_layernorm_fwd(void* stream_, int B, long long R, float eps, const float* a, const float* r,
                                  const float* gain, const float* bias, float* y, float* mean_rstd, double* scratch) {
@@ -1129,9 +1172,9 @@ extern "C" int w2l_layernorm_fwd(void* stream_, int B, long long R, float eps, c
       cudaGetLastError();  // (e.g. the stream is being captured): fall through to the two-kernel path
     }
   }
-  // whole multiples of the 148 SMs at full occupancy (8 CTAs of 256 threads per SM) when the samples are long enough;
+  // whole multiples of the SMs at full occupancy (8 CTAs of 256 threads per SM) when the samples are long enough;
   // at most W2L_LN_MAX_PARTS CTAs per sample (the scratch holds one partial pair per CTA)
-  dim3 grid(std::max(1, std::min(std::min(blocks_for(R, 256 * 4 * 4), W2L_LN_MAX_PARTS), 148 * 8 / std::max(1, std::min(B, 148 * 8)))), B);
+  dim3 grid(std::max(1, std::min(std::min(blocks_for(R, 256 * 4 * 4), W2L_LN_MAX_PARTS), sm_count() * 8 / std::max(1, std::min(B, sm_count() * 8)))), B);
   ln_stats_kernel<<<grid, 256, 0, stream>>>(R, vec, a, r, scratch);
   W2L_LAUNCH_CHECK("ln_stats_kernel");
   ln_apply_kernel<<<grid, 256, 0, stream>>>(R, vec, eps, a, r, gain, bias, scratch, y, mean_rstd);
@@ -1150,19 +1193,26 @@ extern "C" int w2l_layernorm_bwd(void* stream_, int B, long long R, const float*
                                       reinterpret_cast<uintptr_t>(d_branch) | reinterpret_cast<uintptr_t>(d_res)) & 15);
   if (ln_use_rows(B, R)) {
     ln_row_bwd_kernel<<<(B + 7) / 8, 256, 0, stream>>>(B, (int)R, vec, a, r, dy, gain, mean_rstd, d_branch, d_res, branch_mode, branch_scale,
-                                                       dgain, dbias);
+                                                       scratch);
     W2L_LAUNCH_CHECK("ln_row_bwd_kernel");
+    if (dgain || dbias) {
+      ln_scalar_grads_kernel<<<1, 256, 0, stream>>>((B + 7) / 8, scratch, dgain, dbias);
+      W2L_LAUNCH_CHECK("ln_scalar_grads_kernel");
+    }
     return W2L_OK;
   }
   if (B > 65535) return fail(W2L_ERR_UNSUPPORTED, "layernorm_bwd: more than 65535 long groups");
-  // whole multiples of the 148 SMs at full occupancy (8 CTAs of 256 threads per SM) when the samples are long enough;
+  // whole multiples of the SMs at full occupancy (8 CTAs of 256 threads per SM) when the samples are long enough;
   // at most W2L_LN_MAX_PARTS CTAs per sample (the scratch holds one partial pair per CTA)
-  dim3 grid(std::max(1, std::min(std::min(blocks_for(R, 256 * 4 * 4), W2L_LN_MAX_PARTS), 148 * 8 / std::max(1, std::min(B, 148 * 8)))), B);
+  dim3 grid(std::max(1, std::min(std::min(blocks_for(R, 256 * 4 * 4), W2L_LN_MAX_PARTS), sm_count() * 8 / std::max(1, std::min(B, sm_count() * 8)))), B);
   ln_bwd_stats_kernel<<<grid, 256, 0, stream>>>(R, vec, a, r, dy, mean_rstd, scratch);
   W2L_LAUNCH_CHECK("ln_bwd_stats_kernel");
-  ln_bwd_apply_kernel<<<grid, 256, 0, stream>>>(R, vec, a, r, dy, gain, mean_rstd, scratch, d_branch, d_res, branch_mode, branch_scale,
-                                                dgain, dbias);
+  ln_bwd_apply_kernel<<<grid, 256, 0, stream>>>(R, vec, a, r, dy, gain, mean_rstd, scratch, d_branch, d_res, branch_mode, branch_scale);
   W2L_LAUNCH_CHECK("ln_bwd_apply_kernel");
+  if (dgain || dbias) {
+    ln_scalar_grads_kernel<<<1, 256, 0, stream>>>(B * (int)grid.x, scratch, dgain, dbias);
+    W2L_LAUNCH_CHECK("ln_scalar_grads_kernel");
+  }
   return W2L_OK;
 }
 
@@ -1174,22 +1224,53 @@ extern "C" int w2l_colsum_accumulate(void* stream_, int M, int N, const float* X
     // ~4 CTAs per SM: rows per CTA so that col_blocks * row_blocks ~ 600, at least 64 rows each
     const int rows_per_cta = std::max(64, (int)(((long long)M * col_blocks + 599) / 600));
     dim3 grid(col_blocks, (M + rows_per_cta - 1) / rows_per_cta);
-    colsum4_kernel<<<grid, 256, 0, stream>>>(M, N, X, ld, rows_per_cta, out);
-    W2L_LAUNCH_CHECK("colsum_kernel");
+    float* part = nullptr;
+    W2L_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&part), sizeof(float) * (size_t)grid.y * N, stream));
+    colsum4_kernel<<<grid, 256, 0, stream>>>(M, N, X, ld, rows_per_cta, part);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) {
+      count_launch();
+      trace_launch("colsum_kernel");
+      colsum_finish_kernel<<<(N + 255) / 256, 256, 0, stream>>>(N, (int)grid.y, part, out);
+    }
+    cudaFreeAsync(part, stream);
+    if (e != cudaSuccess) return fail(W2L_ERR_CUDA, std::string("launch colsum_kernel: ") + cudaGetErrorString(e));
+    W2L_LAUNCH_CHECK("colsum_finish_kernel");
     return W2L_OK;
   }
   const int rows_per_cta = 256;
   dim3 grid((N + 31) / 32, (M + rows_per_cta - 1) / rows_per_cta);
-  colsum_kernel<<<grid, 256, 0, stream>>>(M, N, X, ld, rows_per_cta, out);
-  W2L_LAUNCH_CHECK("colsum_kernel");
+  float* part = nullptr;
+  W2L_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&part), sizeof(float) * (size_t)grid.y * N, stream));
+  colsum_kernel<<<grid, 256, 0, stream>>>(M, N, X, ld, rows_per_cta, part);
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) {
+    count_launch();
+    trace_launch("colsum_kernel");
+    colsum_finish_kernel<<<(N + 255) / 256, 256, 0, stream>>>(N, (int)grid.y, part, out);
+  }
+  cudaFreeAsync(part, stream);
+  if (e != cudaSuccess) return fail(W2L_ERR_CUDA, std::string("launch colsum_kernel: ") + cudaGetErrorString(e));
+  W2L_LAUNCH_CHECK("colsum_finish_kernel");
   return W2L_OK;
 }
 
 extern "C" int w2l_sq_norm_accumulate(void* stream_, long long n, const float* g, double* out) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (n <= 0 || !g || !out) return fail(W2L_ERR_INVALID_ARGUMENT, "sq_norm: bad arguments");
-  sq_norm_kernel<<<blocks_for(n), 256, 0, stream>>>(n, g, out);
-  W2L_LAUNCH_CHECK("sq_norm_kernel");
+  const int blocks = blocks_for(n);
+  double* part = nullptr;
+  W2L_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&part), sizeof(double) * (size_t)blocks, stream));
+  sq_norm_kernel<<<blocks, 256, 0, stream>>>(n, g, part);
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) {
+    count_launch();
+    trace_launch("sq_norm_kernel");
+    sq_norm_finish_kernel<<<1, 256, 0, stream>>>(blocks, part, out);
+  }
+  cudaFreeAsync(part, stream);
+  if (e != cudaSuccess) return fail(W2L_ERR_CUDA, std::string("launch sq_norm_kernel: ") + cudaGetErrorString(e));
+  W2L_LAUNCH_CHECK("sq_norm_finish_kernel");
   return W2L_OK;
 }
 

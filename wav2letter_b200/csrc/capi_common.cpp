@@ -19,6 +19,14 @@ int fail(int code, const std::string& msg) {
 void count_launch(int n) { g_launches += n; }
 static thread_local int g_precision = W2L_PRECISION_TF32;
 int current_precision() { return g_precision; }
+int sm_count() {
+  static int sms = 0;
+  if (sms == 0) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
+  }
+  return sms;
+}
 void set_precision_value(int p) { g_precision = p; }
 static thread_local cudaEvent_t g_ev_start = nullptr, g_ev_stop = nullptr;
 // event LIST mode: the k-th profiled launch of the selected kind records pair k

@@ -1,4 +1,4 @@
-// common.cuh — shared host/device helpers for libw2l_b200 (sm_100a only).
+// common.cuh — shared host/device helpers for libw2l_b200 (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <math.h>
@@ -16,6 +16,7 @@ void set_error(const std::string& msg);
 int fail(int code, const std::string& msg);
 void count_launch(int n = 1);
 int current_precision();  // W2L_PRECISION_* of the calling thread (w2l_set_precision)
+int sm_count();           // multiprocessors of the current device (132 on an H100 SXM), for grid sizing
 void trace_launch(const char* name);  // trace mode (w2l_trace_begin): one event after every launch, on the trace stream
 // bench hook: events recorded around a call's dominant kernel (nullptr when unset)
 void profile_kind(int kind);  // 1 = GEMM, 2 = criterion chains (set right before profile_start)
@@ -85,9 +86,9 @@ __device__ __forceinline__ float dropout_scale(unsigned long long seed, unsigned
 
 
 __device__ __forceinline__ float warp_max(float v) {
-  float r;
-  asm volatile("redux.sync.max.f32 %0, %1, 0xffffffff;" : "=f"(r) : "f"(v));  // CREDUX.MAX.F32 (sm_100a)
-  return r;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
 }
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

@@ -1,9 +1,9 @@
-// conv_mma.cu — tensor-core time convolution for the TDS family (sm_100a).
+// conv_mma.cu — tensor-core time convolution for the TDS family (sm_90a).
 //
 // A kw x 1 convolution with 10-27 channels over [B][T][C][W=80] activations is, per output frame, the tiny
 // contraction  Y[co][w] = sum_k Wt[co][k] * X[k][w],  k = dk*Cin + ci  (K = kw*Cin = 210..378, M = Cout <= 32,
-// N = W = 80).  tcgen05's minimum tile (M = 128, one CTA-wide accumulator) does not fit that shape; the
-// warp-level tensor path does: mma.sync.m16n8k8 TF32 with fp32 accumulation, one warp per (frame, half of W),
+// N = W = 80).  A warpgroup MMA tile (M = 64 per warpgroup) is mostly padding at that shape; the
+// warp-level tensor path fits it: mma.sync.m16n8k8 TF32 with fp32 accumulation, one warp per (frame, half of W),
 // operands read from a shared-memory window of the input (each input row is staged ONCE per CTA and reused by
 // every tap that touches it — the reuse the SIMT kernels in am_kernels.cu got only through L1).
 //   forward / stride-1 data gradient : A = weights [Mpad][Kpad] (smem), B = input window rows (k -> row
@@ -514,7 +514,7 @@ size_t conv_mma_wgrad_parts(int B, int Tout, int W, int Cin, int Cout, int K, in
   // CTAs per (sample, slice): enough to fill the chip ~twice, never more than there are chunks; the partial buffer
   // is sized for B * max(Tout, 16) parts
   const int chunks = (Tout + TC - 1) / TC;
-  int per_sample = std::max(1, std::min(chunks, (2 * 148 + B * nslices - 1) / (B * nslices)));
+  int per_sample = std::max(1, std::min(chunks, (2 * sm_count() + B * nslices - 1) / (B * nslices)));
   per_sample = std::max(1, std::min(per_sample, std::max(Tout, 16) / nslices));
   if (per_sample_out) *per_sample_out = per_sample;
   return (size_t)B * nslices * per_sample;

@@ -1,5 +1,5 @@
 // criterion_asg.cu — fused ASG (FullConnectionCriterion - ForceAlignmentCriterion) forward +
-// backward for sm_100a.  Replaces flashlight-0.3 lib/sequence/criterion/cuda/
+// backward for sm_90a.  Replaces flashlight-0.3 lib/sequence/criterion/cuda/
 // {FullConnectionCriterion,ForceAlignmentCriterion}.cu as reached from
 // recipes/slimIPL/src/Train.cpp:408-410 (construction), :1675 (forward), :1720 (backward).
 //
@@ -15,15 +15,15 @@
 //                          no inter-warp communication at all.
 //        FCC chains: linear domain, a_t = X_t .* (M' a_{t-1}) * 2^-k, M' = exp(trans - max) in
 //                    registers (row i / column j in lane i / j), the state vector exchanged through
-//                    128 bytes of shared memory (1 STS + 8 broadcast LDS.128), 16 FFMA2 per step,
-//                    power-of-two rescale from the exponent bits of a lagged maximum (one CREDUX,
+//                    128 bytes of shared memory (1 STS + 8 broadcast LDS.128), 32 FFMA per step,
+//                    power-of-two rescale from the exponent bits of a lagged maximum (one warp max,
 //                    exact, off the dependent chain, damped — see pow2_rescale), Z prefetched one
 //                    16-frame block ahead into registers; every a-hat / b-hat vector is stored
 //                    (128 B per frame and direction — the size of the emissions).
 //        FAC chains: log2 domain (the left-to-right band has unbounded dynamic range), lane j owns
 //                    the P = Lp/32 CONSECUTIVE target positions P*j .. P*j+P-1 in registers, so the
 //                    l-1 neighbour is a register except for one SHFL per step; 2 MUFU per state
-//                    (ex2 + lg2), the adds packed two states per instruction (FADD2/FFMA2);
+//                    (ex2 + lg2), the adds written two states at a time (fadd2_rn / ffma2_rn);
 //                    emissions gathered from an 8-frame shared-memory tile; every lane re-centres its
 //                    own positions every 2 frames (two-float offset per lane, lagged, branch-free);
 //                    the row is stored only every 8 frames (a checkpoint: a full FAC lattice would
@@ -42,6 +42,9 @@
 #include "common.cuh"
 
 namespace w2l {
+// float2 lane-wise add / fma, each lane rounded to nearest as a scalar __fadd_rn / __fmaf_rn
+__device__ __forceinline__ float2 fadd2_rn(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 ffma2_rn(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
 namespace {
 
 constexpr int kW = 32;            // padded FCC state width (one lane per state)
@@ -51,10 +54,11 @@ constexpr int kRc = 2;            // FAC chains re-centre every kRc frames
 constexpr float kNeg = -1.0e30f;  // "log zero": finite, absorbing under fp32 addition of ordinary scores
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr double kLn2 = 0.6931471805599453;
-// MUFU.LG2 has a one-signed error: +1.0e-7 (absolute) just above a mantissa of 1, falling to +2e-8 towards 2, and it is
-// exact at 1.0 (scripts/mufu_bias.cu, profiles/mufu_bias_r2.txt).  log2(1 + r) for the small r of a weakly contested
-// state therefore came out 1e-7 too large at every step while an uncontested state (r = 0) got nothing: a differential
-// that grows linearly along the chain (1.4e-4 of the posteriors after 1500 frames).  The recursion evaluates
+// MUFU.LG2 is taken to have a one-signed error: positive just above a mantissa of 1, falling towards 2, exact at 1.0.
+// That was measured on an earlier GPU generation and is assumed, not measured, on sm_90; the workaround below costs
+// nothing either way.
+// log2(1 + r) for the small r of a weakly contested state would then come out slightly too large at every step while
+// an uncontested state (r = 0) got nothing: a differential that grows linearly along the chain.  The recursion evaluates
 // lg2(1.25 * (1 + r)) instead — same instruction count (an FFMA for the FADD): mantissas 1.25 .. 2 for r < 0.6, where
 // the error is small and flat, and the same for r = 0 as for small r — and subtracts the constant log2(1.25) for free by
 // folding it into the transition scores (lse(a - c, b - c) = lse(a, b) - c).
@@ -203,7 +207,7 @@ __device__ __forceinline__ float matvec32(const float (&M)[kW], const float* vsm
   // Eight VOLATILE loads (ptxas keeps their order) whose LAST one feeds the FIRST arithmetic instruction: all eight are
   // in flight, in 32 distinct registers, before any product issues.  Left to itself ptxas recycles one or two register
   // quads and sinks each load behind the consumer of the previous one — two loads in flight, four to eight dependent
-  // ~30-cycle rounds per step (profiles/asg_r2.md).
+  // ~30-cycle rounds per step.
   asm volatile(
       "ld.volatile.shared.v4.f32 {%0, %1, %2, %3}, [%32];\n\t"
       "ld.volatile.shared.v4.f32 {%4, %5, %6, %7}, [%32+16];\n\t"
@@ -227,10 +231,10 @@ __device__ __forceinline__ float matvec32(const float (&M)[kW], const float* vsm
   float2 r[kW / 4];
 #pragma unroll
   for (int q = 0; q < kW / 4; ++q) {
-    const float2 pq = __ffma2_rn(make_float2(M[4 * q], M[4 * q + 1]), make_float2(v[4 * q], v[4 * q + 1]), z2);
-    r[q] = __ffma2_rn(make_float2(M[4 * q + 2], M[4 * q + 3]), make_float2(v[4 * q + 2], v[4 * q + 3]), pq);
+    const float2 pq = ffma2_rn(make_float2(M[4 * q], M[4 * q + 1]), make_float2(v[4 * q], v[4 * q + 1]), z2);
+    r[q] = ffma2_rn(make_float2(M[4 * q + 2], M[4 * q + 3]), make_float2(v[4 * q + 2], v[4 * q + 3]), pq);
   }
-  const float2 s = __fadd2_rn(__fadd2_rn(__fadd2_rn(r[0], r[1]), __fadd2_rn(r[2], r[3])), __fadd2_rn(__fadd2_rn(r[4], r[5]), __fadd2_rn(r[6], r[7])));
+  const float2 s = fadd2_rn(fadd2_rn(fadd2_rn(r[0], r[1]), fadd2_rn(r[2], r[3])), fadd2_rn(fadd2_rn(r[4], r[5]), fadd2_rn(r[6], r[7])));
   return s.x + s.y;
 }
 
@@ -304,7 +308,7 @@ __device__ void fcc_alpha_chain(const AsgParams& p, int b, float* vec /* [2][32]
       const float xs = x * s;
       float* vb = vec + (k & 1) * kW;
       vb[lane] = a;
-      const float mx = warp_max(a);  // max_j a_{t-1}[j]: one CREDUX, off the dependent chain
+      const float mx = warp_max(a);  // max_j a_{t-1}[j]: five shuffles, off the dependent chain
       __syncwarp();
       a = xs * matvec32(M, vb);
       ksum += kcur;
@@ -421,17 +425,17 @@ __device__ __forceinline__ float lds_f(uint32_t a) {
   return v;
 }
 // two states at once: (va, na) / (vb, nb) = (own value, neighbour value) of states a / b; returns the new values.
-// 6 packed adds + 4 FMNMX + 4 MUFU for the pair.
+// 12 FADD + 4 FMNMX + 4 MUFU for the pair.
 __device__ __forceinline__ float2 fac_pair(float va, float na, float s1a, float s2a, float za, float vb, float nb, float s1b,
                                            float s2b, float zb) {
-  const float2 a = __fadd2_rn(make_float2(va, na), make_float2(s1a, s2a));
-  const float2 b = __fadd2_rn(make_float2(vb, nb), make_float2(s1b, s2b));
+  const float2 a = fadd2_rn(make_float2(va, na), make_float2(s1a, s2a));
+  const float2 b = fadd2_rn(make_float2(vb, nb), make_float2(s1b, s2b));
   const float2 mx = make_float2(fmaxf(a.x, a.y), fmaxf(b.x, b.y));
   const float2 mn = make_float2(fminf(a.x, a.y), fminf(b.x, b.y));
-  const float2 d = __ffma2_rn(mx, make_float2(-1.f, -1.f), mn);  // mn - mx (exact)
-  const float2 q = __ffma2_rn(make_float2(ex2f(d.x), ex2f(d.y)), make_float2(kLgScale, kLgScale), make_float2(kLgScale, kLgScale));
-  const float2 base = __fadd2_rn(make_float2(za, zb), mx);
-  return __fadd2_rn(base, make_float2(lg2f(q.x), lg2f(q.y)));
+  const float2 d = ffma2_rn(mx, make_float2(-1.f, -1.f), mn);  // mn - mx (exact)
+  const float2 q = ffma2_rn(make_float2(ex2f(d.x), ex2f(d.y)), make_float2(kLgScale, kLgScale), make_float2(kLgScale, kLgScale));
+  const float2 base = fadd2_rn(make_float2(za, zb), mx);
+  return fadd2_rn(base, make_float2(lg2f(q.x), lg2f(q.y)));
 }
 // one alpha step: row_t[l] = z_t[y_l] + lse(row[l] + s1, row[l-1] + s2); zrow = shared byte address of frame t's Z row
 template <int P>
@@ -510,9 +514,9 @@ __device__ __forceinline__ void twofloat_add(float& hi, float& lo, float m) {
 
 // One warp walks one FAC recursion, P positions per lane.  (A variant that spread a recursion over four warps, two
 // positions per lane, with the boundary value handed from warp to warp through a shared-memory message ring, was built
-// and measured in this round: 186 ns per step against 162 ns for this one — the per-step dependent chain
-// SHFL -> FADD2 -> FMNMX -> FFMA2 -> EX2 -> FADD2 -> LG2 -> FADD2 is ~160 cycles whatever the width, and the ring's
-// bookkeeping cost what the narrower rows saved.  profiles/asg_r2.md.)
+// and found slower than this one — the per-step dependent chain
+// SHFL -> FADD -> FMNMX -> FFMA -> EX2 -> FADD -> LG2 -> FADD is ~160 cycles whatever the width, and the ring's
+// bookkeeping cost what the narrower rows saved.)
 template <int P, bool kBeta>
 __device__ void fac_chain(const AsgParams& p, int b, float* ztile /* [kSeg][32] shared */) {
   const int lane = threadIdx.x & 31;
@@ -527,7 +531,7 @@ __device__ void fac_chain(const AsgParams& p, int b, float* ztile /* [kSeg][32] 
   // their lane's maximum wherever the row's global maximum is.  With one offset per row the states far below the row
   // maximum — which carry the posterior mass when the alignment band is tight (L close to T, the TDS-output regime) —
   // lost absolute precision: 1.8e-4 on the posteriors at T = 700, L = 540 against 4.5e-6 with per-lane offsets in a
-  // float32 emulation (profiles/asg_r2.md).  D is the neighbour's offset minus this lane's, added to the value that crosses
+  // float32 emulation.  D is the neighbour's offset minus this lane's, added to the value that crosses
   // the lane boundary.
   float Chi = 0.f, Clo = 0.f, pend = kNeg, off = 0.f, D = 0.f;
 
@@ -729,18 +733,18 @@ __host__ __device__ inline FacGradLayout fac_grad_layout(int Lp, int warps) {
 __device__ __forceinline__ float2 fac_grad_pair(float va, float na, float s1a, float s2a, float za, float oa,  //
                                                 float vb, float nb, float s1b, float s2b, float zb, float ob,  //
                                                 float2& xsa /* (stay, advance) of a */, float2& xsb) {
-  const float2 a = __fadd2_rn(make_float2(va, na), make_float2(s1a, s2a));
-  const float2 b = __fadd2_rn(make_float2(vb, nb), make_float2(s1b, s2b));
-  const float2 ea = __fadd2_rn(a, make_float2(oa, oa));
-  const float2 eb = __fadd2_rn(b, make_float2(ob, ob));
+  const float2 a = fadd2_rn(make_float2(va, na), make_float2(s1a, s2a));
+  const float2 b = fadd2_rn(make_float2(vb, nb), make_float2(s1b, s2b));
+  const float2 ea = fadd2_rn(a, make_float2(oa, oa));
+  const float2 eb = fadd2_rn(b, make_float2(ob, ob));
   xsa = make_float2(ex2f(ea.x), ex2f(ea.y));
   xsb = make_float2(ex2f(eb.x), ex2f(eb.y));
   const float2 mx = make_float2(fmaxf(a.x, a.y), fmaxf(b.x, b.y));
   const float2 mn = make_float2(fminf(a.x, a.y), fminf(b.x, b.y));
-  const float2 d = __ffma2_rn(mx, make_float2(-1.f, -1.f), mn);
-  const float2 q = __ffma2_rn(make_float2(ex2f(d.x), ex2f(d.y)), make_float2(kLgScale, kLgScale), make_float2(kLgScale, kLgScale));
-  const float2 base = __fadd2_rn(make_float2(za, zb), mx);
-  return __fadd2_rn(base, make_float2(lg2f(q.x), lg2f(q.y)));
+  const float2 d = ffma2_rn(mx, make_float2(-1.f, -1.f), mn);
+  const float2 q = ffma2_rn(make_float2(ex2f(d.x), ex2f(d.y)), make_float2(kLgScale, kLgScale), make_float2(kLgScale, kLgScale));
+  const float2 base = fadd2_rn(make_float2(za, zb), mx);
+  return fadd2_rn(base, make_float2(lg2f(q.x), lg2f(q.y)));
 }
 
 template <int P>
@@ -904,7 +908,7 @@ __global__ void __launch_bounds__(128, P <= 8 ? 4 : 2) asg_fac_grad_kernel(AsgPa
         } else {
 #pragma unroll
           for (int k = P - 2; k >= 0; k -= 2) {  // pairs, descending: v[k-1], v[k] are still alpha_{t-1}
-            const float2 brk = __fadd2_rn(*reinterpret_cast<const float2*>(br + k), K2);
+            const float2 brk = fadd2_rn(*reinterpret_cast<const float2*>(br + k), K2);
             const float2 nv = fac_grad_pair(st.v[k], k ? st.v[k - 1] : up, st.s1[k], st.s2[k], lds_f(zrow + st.y4[k]), brk.x,  //
                                             st.v[k + 1], st.v[k], st.s1[k + 1], st.s2[k + 1], lds_f(zrow + st.y4[k + 1]), brk.y, xv[k], xv[k + 1]);
             *reinterpret_cast<float2*>(grow + lane * P + k) = make_float2(xv[k].x + xv[k].y, xv[k + 1].x + xv[k + 1].y);
@@ -921,7 +925,7 @@ __global__ void __launch_bounds__(128, P <= 8 ? 4 : 2) asg_fac_grad_kernel(AsgPa
         const float inv = gt > 0.f ? __fdividef(1.0f, gt) : 0.f;
         const float2 inv2 = make_float2(inv, inv);
 #pragma unroll
-        for (int k = 0; k < P; ++k) ds[k] = __ffma2_rn(xv[k], inv2, ds[k]);
+        for (int k = 0; k < P; ++k) ds[k] = ffma2_rn(xv[k], inv2, ds[k]);
         __syncwarp();
       }
     }
@@ -1161,7 +1165,7 @@ __global__ void __launch_bounds__(32 * kHaloMaxW) asg_fac_grad_halo_kernel(AsgPa
         float2 xv[P];
 #pragma unroll
         for (int k = P - 2; k >= 0; k -= 2) {
-          const float2 brk = __fadd2_rn(*reinterpret_cast<const float2*>(br + k), K2);
+          const float2 brk = fadd2_rn(*reinterpret_cast<const float2*>(br + k), K2);
           const float2 nv = fac_grad_pair(st.v[k], k ? st.v[k - 1] : up, st.s1[k], st.s2[k], lds_f(zrow + st.y4[k]), brk.x,  //
                                           st.v[k + 1], st.v[k], st.s1[k + 1], st.s2[k + 1], lds_f(zrow + st.y4[k + 1]), brk.y, xv[k], xv[k + 1]);
           *reinterpret_cast<float2*>(grow + lane * P + k) = make_float2(xv[k].x + xv[k].y, xv[k + 1].x + xv[k + 1].y);
@@ -1180,7 +1184,7 @@ __global__ void __launch_bounds__(32 * kHaloMaxW) asg_fac_grad_halo_kernel(AsgPa
         const float inv = gt > 0.f ? __fdividef(1.0f, gt) : 0.f;
         const float2 inv2 = make_float2(inv, inv);
 #pragma unroll
-        for (int k = 0; k < P; ++k) ds[k] = __ffma2_rn(xv[k], inv2, ds[k]);
+        for (int k = 0; k < P; ++k) ds[k] = ffma2_rn(xv[k], inv2, ds[k]);
       }
     }
     cp_async_wait_all();
@@ -1287,8 +1291,8 @@ __global__ void __launch_bounds__(kFccGradWarps * 32, 2) asg_fcc_grad_kernel(Asg
           for (int q = 0; q < kW / 4; ++q) {
             float4 v;
             asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(tile_sa + (k * kW + 4 * q) * 4));
-            acc[2 * q] = __ffma2_rn(w2, make_float2(v.x, v.y), acc[2 * q]);
-            acc[2 * q + 1] = __ffma2_rn(w2, make_float2(v.z, v.w), acc[2 * q + 1]);
+            acc[2 * q] = ffma2_rn(w2, make_float2(v.x, v.y), acc[2 * q]);
+            acc[2 * q + 1] = ffma2_rn(w2, make_float2(v.z, v.w), acc[2 * q + 1]);
           }
         }
       }
@@ -1375,7 +1379,7 @@ int fac_grad_slots(int warps, size_t smem) {
   int per_sm = 0;
   if (smem > 48 * 1024) cudaFuncSetAttribute(asg_fac_grad_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, asg_fac_grad_kernel<P>, warps * 32, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   return per_sm * sms;
 }
@@ -1385,7 +1389,7 @@ int fac_grad_ctas(const AsgParams& p) {
     int per_sm = 0;
     cudaFuncSetAttribute(asg_fac_grad_halo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, asg_fac_grad_halo_kernel, 32 * p.Wg, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     int want = per_sm * sms / p.B;
     if (want < 1) want = 1;
@@ -1483,7 +1487,7 @@ extern "C" int w2l_asg_forward_backward(void* stream_, int terms, int B, int T, 
   if ((d_emis == nullptr) != (d_trans == nullptr))
     return fail(W2L_ERR_INVALID_ARGUMENT, "asg: d_emis and d_trans must be given together");
   if (scale_mode < 0 || scale_mode > 4) return fail(W2L_ERR_INVALID_ARGUMENT, "asg: bad scale mode");
-  if (N > kW) return fail(W2L_ERR_UNSUPPORTED, "asg: N > 32 tokens is not covered by the sm_100a kernels");
+  if (N > kW) return fail(W2L_ERR_UNSUPPORTED, "asg: N > 32 tokens is not covered by these kernels");
   AsgParams p{};
   shape(p, B, T, N, L);  // the workspace is sized for the declared L whether or not a target is given
   if (!target) p.L = 0;
@@ -1515,7 +1519,7 @@ extern "C" int w2l_asg_forward_backward(void* stream_, int terms, int B, int T, 
   p.n_fac_parts = (has_fac && p.need_grad) ? gA * B : 0;
 
   const long long nframes = (long long)B * T;
-  const int frame_blocks = (int)std::min<long long>((nframes + 7) / 8, 148 * 8);
+  const int frame_blocks = (int)std::min<long long>((nframes + 7) / 8, sm_count() * 8);
   const int meta_blocks = (B + 7) / 8;
   asg_prep_kernel<<<frame_blocks + meta_blocks, 256, 0, stream>>>(p, frame_blocks);
   W2L_LAUNCH_CHECK("asg_prep_kernel");

@@ -1,4 +1,4 @@
-// criterion_ctc.cu — CTC forward + backward on raw activations for sm_100a.
+// criterion_ctc.cu — CTC forward + backward on raw activations for sm_90a.
 // Replaces ConnectionistTemporalClassificationCriterion::forward (CTCLoss constructed at
 // recipes/slimIPL/src/Train.cpp:406-407, cpc/Train.cpp:524-525; upstream CUDA backend = warp-ctc).
 // Conventions: internal log-softmax over N, blank = N-1 (Train.cpp:248-251), every sample runs
@@ -30,8 +30,9 @@ constexpr float kNeg = -1.0e30f;  // "log zero": finite, absorbing under fp32 ad
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr double kLn2 = 0.6931471805599453;
 constexpr int kRc = 2;  // frames between re-centrings
-// MUFU.LG2 is one-signed (+1e-7 just above a mantissa of 1, exact at 1.0): the recursion takes lg2(1.25 * sum) and folds
-// the constant log2(1.25) into the emission term (criterion_asg.cu, profiles/mufu_bias_r2.txt)
+// MUFU.LG2's error is taken to be one-signed (positive just above a mantissa of 1, exact at 1.0; assumed, not measured,
+// on sm_90): the recursion takes lg2(1.25 * sum) and folds
+// the constant log2(1.25) into the emission term (criterion_asg.cu)
 constexpr float kLgScale = 1.25f;
 constexpr float kLgShift = 0.32192809488736235f;
 
@@ -381,11 +382,15 @@ __global__ void __launch_bounds__(256) ctc_grad_kernel(CtcParams p) {
 #pragma unroll
   for (int w = 0; w < 8; ++w) tot += wsum_s[w];
   const float inv = tot > 0.f ? coef / tot : 0.f;
-  for (int s = threadIdx.x; s < S; s += blockDim.x) {
-    const float q = post_s[s];
-    if (q != 0.f) {
-      const int zs = (s & 1) ? yg[s >> 1] : N - 1;
-      atomicAdd(de + zs, -q * inv);
+  // occupancy scatter: states sharing a label (the blanks, repeated labels) add to the same entry, so one thread adds
+  // them in state order (run to run identical); the frame row's softmax writes above are visible after the barrier
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < S; ++s) {
+      const float q = post_s[s];
+      if (q != 0.f) {
+        const int zs = (s & 1) ? yg[s >> 1] : N - 1;
+        de[zs] -= q * inv;
+      }
     }
   }
 }
@@ -462,7 +467,7 @@ extern "C" int w2l_ctc_forward_backward(void* stream_, int B, int T, int N, int 
   if (!workspace || workspace_bytes < need)
     return fail(W2L_ERR_WORKSPACE, "ctc: workspace too small (need " + std::to_string(need) + " bytes)");
   const long long nframes = (long long)B * T;
-  const int frame_blocks = (int)std::min<long long>((nframes + 7) / 8, 148 * 8);
+  const int frame_blocks = (int)std::min<long long>((nframes + 7) / 8, sm_count() * 8);
   ctc_prep_kernel<<<frame_blocks + (B + 255) / 256, 256, 0, stream>>>(p, frame_blocks);
   W2L_LAUNCH_CHECK("ctc_prep_kernel");
   const int grid = p.need_grad ? 2 * B : B;  // alpha chains, then beta chains

@@ -1,4 +1,4 @@
-// criterion_viterbi.cu — Viterbi decoders for sm_100a.
+// criterion_viterbi.cu — Viterbi decoders for sm_90a.
 //   w2l_fcc_viterbi : ASGLoss::viterbiPath (recipes/slimIPL/src/Train.cpp:838, :1375) — max-plus
 //                     FullConnection recursion + backtrace (upstream lib/sequence/criterion/
 //                     cuda/ViterbiPath.cu).  Bit-exact contract: fp32 add then compare, j
@@ -297,7 +297,7 @@ extern "C" int w2l_argmax_path(void* stream_, int B, int T, int N, const float* 
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (B <= 0 || T <= 0 || N <= 0 || !emis || !path) return fail(W2L_ERR_INVALID_ARGUMENT, "argmax_path: bad arguments");
   const long long nframes = (long long)B * T;
-  const int blocks = (int)std::min<long long>((nframes + 7) / 8, 148 * 8);
+  const int blocks = (int)std::min<long long>((nframes + 7) / 8, sm_count() * 8);
   argmax_path_kernel<<<blocks, 256, 0, stream>>>(nframes, N, emis, path);
   W2L_LAUNCH_CHECK("argmax_path_kernel");
   return W2L_OK;

@@ -1,4 +1,4 @@
-// glu_wn_kernels.cu — the element-wise / per-row pieces of the Conv1D+GLU acoustic-model family (sm_100a):
+// glu_wn_kernels.cu — the element-wise / per-row pieces of the Conv1D+GLU acoustic-model family (sm_90a):
 //   WeightNorm   w[r][:] = g[r] * v[r][:] / ||v[r][:]||        (fl::WeightNorm around Conv2D (dim 3) and Linear (dim 0):
 //                                                               both normalise per OUTPUT unit, i.e. per contiguous row
 //                                                               of the [cout][cin*kw] / [out][in] weight; arch opcode
@@ -220,9 +220,10 @@ __global__ void __launch_bounds__(256) conv1d_unarrange_kernel(int cin, int cout
 }
 
 // bias gradient of a padded-row output: dbias[co] += sum_rows dy[row][out_row(co)].  Lanes = 32 consecutive output channels
-// (coalesced 128-byte reads of a row), warps and grid.y stride over the rows, one atomic per (CTA, channel).
+// (coalesced 128-byte reads of a row), warps and grid.y stride over the rows; one partial per (CTA, channel) in
+// part[blockIdx.y][co], added in grid.y order by conv1d_bias_grad_finish_kernel (run to run identical).
 __global__ void __launch_bounds__(256) conv1d_bias_grad_kernel(long long rows, int cout, int cout_p, int glu_split,
-                                                               const float* __restrict__ dy, float* __restrict__ dbias) {
+                                                               const float* __restrict__ dy, float* __restrict__ part) {
   __shared__ float red[8][33];
   const int co = blockIdx.x * 32 + threadIdx.x;
   const bool ok = co < cout;
@@ -236,8 +237,16 @@ __global__ void __launch_bounds__(256) conv1d_bias_grad_kernel(long long rows, i
     float t = 0.f;
 #pragma unroll
     for (int k = 0; k < 8; ++k) t += red[k][threadIdx.x];
-    atomicAdd(dbias + co, t);
+    part[(size_t)blockIdx.y * cout + co] = t;
   }
+}
+__global__ void __launch_bounds__(256) conv1d_bias_grad_finish_kernel(int cout, int parts, const float* __restrict__ part,
+                                                                      float* __restrict__ dbias) {
+  const int co = blockIdx.x * 256 + threadIdx.x;
+  if (co >= cout) return;
+  float t = 0.f;
+  for (int k = 0; k < parts; ++k) t += part[(size_t)k * cout + co];
+  dbias[co] += t;
 }
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + __expf(-x)); }
@@ -319,7 +328,7 @@ __global__ void __launch_bounds__(256) glu_bwd_kernel(long long rows, int H, int
   }
 }
 
-int blocks_for_n(long long n) { return (int)std::min<long long>((n + 2047) / 2048, 148 * 8); }
+int blocks_for_n(long long n) { return (int)std::min<long long>((n + 2047) / 2048, sm_count() * 8); }
 
 }  // namespace
 }  // namespace w2l
@@ -385,8 +394,18 @@ extern "C" int w2l_conv1d_unarrange_grad(void* stream_, int cin, int cout, int k
   W2L_LAUNCH_CHECK("conv1d_unarrange_kernel");
   if (dbias && dy && rows > 0) {
     dim3 bgrid((cout + 31) / 32, (unsigned)std::min<long long>((rows + 2047) / 2048, 64));
-    conv1d_bias_grad_kernel<<<bgrid, dim3(32, 8), 0, stream>>>(rows, cout, cout_p, glu_split, dy, dbias);
-    W2L_LAUNCH_CHECK("conv1d_bias_grad_kernel");
+    float* part = nullptr;
+    W2L_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&part), sizeof(float) * (size_t)bgrid.y * cout, stream));
+    conv1d_bias_grad_kernel<<<bgrid, dim3(32, 8), 0, stream>>>(rows, cout, cout_p, glu_split, dy, part);
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) {
+      count_launch();
+      trace_launch("conv1d_bias_grad_kernel");
+      conv1d_bias_grad_finish_kernel<<<(cout + 255) / 256, 256, 0, stream>>>(cout, (int)bgrid.y, part, dbias);
+    }
+    cudaFreeAsync(part, stream);
+    if (e != cudaSuccess) return fail(W2L_ERR_CUDA, std::string("launch conv1d_bias_grad_kernel: ") + cudaGetErrorString(e));
+    W2L_LAUNCH_CHECK("conv1d_bias_grad_finish_kernel");
   }
   return W2L_OK;
 }

@@ -1,5 +1,5 @@
 // fl_compat.cpp — implementation of include/fl_compat/fl_compat.h on top of the C ABI (include/w2l_b200.h).
-// Host code only: every arithmetic operation is a call into libw2l_b200's sm_100a kernels.
+// Host code only: every arithmetic operation is a call into libw2l_b200's sm_90a kernels.
 #include "fl_compat/fl_compat.h"
 
 #include <dlfcn.h>
@@ -561,7 +561,7 @@ Variable Conv2D::forwardWith(const Variable& in, const Variable& weight, const V
 }
 
 // ------------------------------------------------------------------------------------------------
-// Large-channel time convolution (conv_glu archs): one tcgen05 GEMM per sample on a zero-copy im2col view.
+// Large-channel time convolution (conv_glu archs): one wgmma GEMM per sample on a zero-copy im2col view.
 //   activations [B][T][Cp] (Cp = channels padded to a multiple of 4 with zero channels), stride 1
 //   fwd   y_b [Tout][Cout_p]   = Xp_b view [Tout][kw*Cp] (row stride Cp)  x  Warr [Cout_p][kw*Cp]^T + bias
 //   wgrad dWarr               += dY_b^T [Cout_p][Tout]  x  Xp_b view                      (accumulated over b)
@@ -921,7 +921,7 @@ Variable LayerNorm::forwardResidual(const Variable& a, const Variable& r, int br
 }
 
 // ================================================================================================
-// Linear (tcgen05 GEMM)
+// Linear (wgmma GEMM)
 // ================================================================================================
 Linear::Linear(int nIn_, int nOut_, bool bias) : nIn(nIn_), nOut(nOut_), hasBias_(bias) {
   if (nIn <= 0 || nOut <= 0) throw std::invalid_argument("Linear: non-positive size");
@@ -1359,7 +1359,7 @@ void initDistributed(int worldRank, int worldSize, const void* id128) {
   ncclUniqueId id;
   std::memcpy(&id, id128, 128);
   // the all-reduce runs UNDER the backward pass: cap its CTAs so it does not take SMs from the GEMMs it overlaps
-  // (W2L_NCCL_MAX_CTAS overrides; NVLink5 / NVSwitch needs few CTAs to saturate)
+  // (W2L_NCCL_MAX_CTAS overrides; the cap of 8 assumes NVLink / NVSwitch needs few CTAs to saturate — not measured on H100)
   ncclConfig_t config = NCCL_CONFIG_INITIALIZER;
   int maxCtas = 8;
   if (const char* e = std::getenv("W2L_NCCL_MAX_CTAS")) maxCtas = std::atoi(e);

@@ -3,7 +3,7 @@
 // against flashlight:
 //   input -> ntwrk->forward -> criterion->forward -> zeroGrad -> loss.backward() -> reducer (NCCL all-reduce
 //   of every net + criterion gradient) -> grads / (totalBatch) -> clipGradNorm(net U crit) -> critopt/netopt step
-// B200-first differences, all behind the same call sequence: parameters, gradients and momentum live in flat
+// GPU-first differences, all behind the same call sequence: parameters, gradients and momentum live in flat
 // arenas (one NCCL call, one norm kernel, one fused scale+clip+SGD kernel instead of per-array JIT kernels).
 // The Python harness (bench.py, tests) drives it with device pointers; no arithmetic happens on the host.
 #include <cuda_runtime.h>
