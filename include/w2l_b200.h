@@ -196,8 +196,9 @@ W2L_API int w2l_gemm_set_variant(int variant);
 W2L_API int w2l_gemm_tf32(void* stream, int a_mn_major, int b_mn_major, int M, int N, int K, const float* A, int lda,
                           const float* B, int ldb, float* C, int ldc, const float* bias, int act);
 
-/* Extended epilogue: after bias/act, (a) forward dropout with keep-scale 1/(1-p) (Philox4x32-10 keyed by
- * (seed, element index)), (b) backward activation mask read back from a stored activation tensor
+/* Extended epilogue: after bias/act, (a) forward dropout with keep-scale 1/(1-p) (N % 4 == 0): one murmur3-style 32-bit
+ * hash of (seed, (row*N + col) >> 1) per pair of columns, 16 bits per element, kept iff bits >= floor(p * 65536)
+ * (DESIGN.md, "Dropout masks"), (b) backward activation mask read back from a stored activation tensor
  * aux[M][ld_aux]: aux_mode 1 multiplies by (aux > 0) * aux_scale (fused ReLU+dropout backward),
  * 2 by (aux != 0) * aux_scale (dropout backward), (c) accumulate != 0: C += result. */
 W2L_API int w2l_gemm_tf32_ex(void* stream, int a_mn_major, int b_mn_major, int M, int N, int K, const float* A, int lda,

@@ -5,7 +5,9 @@ and EVERY parameter gradient of one train step of the CUDA path against a float6
 The arch text comes from wav2letter_b200/archs.py, whose generators tests/test_archs.py checks token-for-token against
 recipes/conv_glu/{wsj,librispeech}/network.arch, recipes/seq2seq_tds/librispeech/network.arch and
 recipes/streaming_convnets/librispeech/am_500ms_future_context.arch (stored in tests/golden/reference_archs.json).  Dropout probabilities are set to 0 and SpecAugment's mask counts to 0 — random masks cannot be
-compared across implementations; both are covered by their own tests.
+compared across implementations.  tests/test_gpu_dropout.py checks every dropout site bit for bit against the NumPy
+models of tests/dropout_reference.py (whose statistics tests/test_dropout_reference.py checks), the backward passes'
+use of the forward mask, and w2l_mask_bands against NumPy.
 
 Tolerances.  precision "f32" (fp32-accurate contractions: 3xTF32 split GEMMs, fp32 SIMT time convolutions):
 emissions 2e-4 of the largest emission, per-sample loss 2e-4 (both ~2e-5 / 1e-6 measured), all gradients together within

@@ -83,6 +83,9 @@ def _load() -> ctypes.CDLL:
     lib.w2l_conv1d_unarrange_grad.argtypes = [vp, i, i, i, i, i, i, vp, vp, ll, vp, vp]
     lib.w2l_glu_fwd.argtypes = [vp, ll, i, vp, vp, f32, u64]
     lib.w2l_glu_bwd.argtypes = [vp, ll, i, vp, vp, vp, f32, u64]
+    lib.w2l_act_fwd.argtypes = [vp, ll, vp, i, f32, u64, vp]
+    lib.w2l_mask_mul.argtypes = [vp, ll, vp, vp, i, f32, vp]
+    lib.w2l_conv_set_path.argtypes = [i]
     lib.w2l_gemm_tf32_view.argtypes = [vp, i, i, i, i, i, vp, i, vp, i, vp, i, vp, i, i]
     lib.w2l_gemm_tf32_ex.argtypes = [vp, i, i, i, i, i, vp, i, vp, i, vp, i, vp, i, i, vp, i, i, f32, f32, u64]
     lib.w2l_conv_time_workspace_size.restype = sz

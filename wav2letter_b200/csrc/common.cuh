@@ -58,8 +58,8 @@ struct Carver {
 #ifdef __CUDACC__
 constexpr float kNegInf = -INFINITY;
 
-// ---- Philox4x32-10 (counter-based; forward passes are reproducible per (seed, element index); the
-// backward pass regenerates nothing — masks are read back from the stored activations) ----------
+// ---- Philox4x32-10 (counter-based; forward passes are reproducible per (seed, element index); only GLU's
+// backward regenerates its mask, the others read it back from the stored activations) -----------
 __device__ __forceinline__ uint4 philox4x32(uint32_t c0, uint32_t c1, uint32_t k0, uint32_t k1) {
   uint32_t c2 = 0, c3 = 0;
 #pragma unroll
