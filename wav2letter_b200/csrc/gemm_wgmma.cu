@@ -7,9 +7,9 @@
 //
 // Three operand kinds, one kernel template (the "precision" of BASELINE.json's configs):
 //   W2L_GEMM_TF32   fp32 operands in HBM, tf32 products (10-bit mantissas)  — cuDNN/cuBLAS default for fp32
-//   W2L_GEMM_F32X3  fp32 operands in HBM, fp32-ACCURATE: every staged tile is split in shared memory into
-//                   hi = tf32(x) and lo = tf32(x - hi) and the tensor core accumulates Al*Bh + Ah*Bl + Ah*Bh —
-//                   products good to ~2^-21, i.e. SGEMM-grade (configs[1] "fp32")
+//   W2L_GEMM_F32X3  fp32 operands in HBM, fp32-ACCURATE: every staged value is split into hi = tf32(x) and
+//                   lo = tf32(x - hi) (A in registers, B in shared memory) and the tensor core accumulates
+//                   Al*Bh + Ah*Bl + Ah*Bh — products good to ~2^-21, i.e. SGEMM-grade (configs[1] "fp32")
 //   W2L_GEMM_BF16   bf16 operands in HBM — half the operand bytes, twice the MAC rate
 //                   (configs[2]/[3] "bf16 convs / fp32 loss"; the reference's AMP switch, Train.cpp:211-219)
 // C is fp32 or bf16 (c_bf16); bias / ReLU / dropout / mask / accumulate epilogue.
@@ -24,19 +24,25 @@
 //
 // Structure: CTAs walk 128 x BN output tiles (n fastest, so CTAs running together share their A rows in L2); by default
 // one CTA per SM (persistent), w2l_gemm_set_variant(0) launches one CTA per tile.  384 threads:
-//   warpgroup 0, warp 0     TMA producer: 2D boxes into a shared-memory ring, full / empty mbarrier per stage; it runs
-//                           ahead across tile boundaries, so the next tile's operands arrive during an epilogue
-//   warpgroup 0, warps 1-3  operand conversion where wgmma cannot read the staged tile as it is: tf32 wgmma takes
-//                           K-major operands only, so MN-major fp32 tiles are transposed into the K-major 128B-swizzled
-//                           layout (rounded to tf32), and F32X3 writes hi and lo tiles; `ready` barrier per stage
-//   warpgroups 1, 2         64 x BN halves of the tile: wgmma m64nBNk8 (tf32) / m64nBNk16 (bf16; MN-major operands
-//                           through the transpose bits) from shared memory into register accumulators; epilogue straight
-//                           from the accumulator fragment
+//   warpgroup 0, warp 0     TMA producer: 2D boxes into a shared-memory ring of raw [A | B] tiles, full / empty mbarrier
+//                           per stage; it runs ahead across tile boundaries, so the next tile's operands arrive during an
+//                           epilogue
+//   warpgroup 0, warps 1-3  B conversion for the "converted" kinds (F32X3, and TF32 with an MN-major operand): the raw fp32
+//                           B tile is rounded (hi = tf32) or split (hi, lo) into K-major 128B-swizzled tiles of a second
+//                           ring, with a ready / empty mbarrier pair per stage
+//   warpgroups 1, 2         64 x BN halves of the tile into register accumulators; epilogue straight from the accumulator
+//                           fragment.  bf16 and unconverted TF32: wgmma m64nBNk16 / m64nBNk8 with both operands in shared
+//                           memory (MN-major bf16 through the transpose bits).  Converted kinds: each warpgroup reads its
+//                           64 x 32 slice of the raw A tile into the tf32 register-fragment layout, rounds / splits it in
+//                           registers and issues m64n128k8 with A from registers.  It frees the raw stage as soon as its
+//                           fragments are loaded, so TMA, B conversion and MMAs of different k blocks overlap; fragments
+//                           are double-buffered because a register operand must stay intact until its wgmma completes.
 // Shared-memory operand layouts (wgmma canonical, 128B swizzle, tiles 1024-byte aligned):
 //   K-major        rows of 128 B (32 fp32 / 64 bf16 along k), 8-row groups 1024 B apart; a k step is +32 B
 //   MN-major bf16  TMA boxes of [64 k-rows][64 elements along m/n]; lbo = 8192 B between boxes, sbo = 1024 B
 //                  (8 k-rows); a k16 step is +2048 B
-//   MN-major fp32  unswizzled TMA box [32 k-rows][rows along m/n], converted before use
+//   MN-major fp32  A: 16 unswizzled boxes [32 k-rows][8 m], 1 KB apart, so the fragment reads are conflict-free;
+//                  B: one unswizzled box [32 k-rows][BN], converted before use
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -61,19 +67,26 @@ constexpr int kConvThreads = 96;            // warps 1..3
 constexpr int kConsumerThreads = 256;       // warpgroups 1, 2
 enum { kTf32 = W2L_GEMM_TF32, kF32x3 = W2L_GEMM_F32X3, kBf16 = W2L_GEMM_BF16 };
 
-// A stage holds the raw TMA tiles [A | B] and, when the operands are converted, [hi A | hi B] (+ [lo A | lo B] for F32X3).
-// The ring takes as many stages as fit in 227 KB, at most 6.  BN is 128 / 160 / 224 / 256 (F32X3: 128, BF16: 128 / 256).
+// The raw ring's stages hold the TMA tiles [A | B]; the converted kinds add a ring of converted B stages, [hi B] or
+// [hi B | lo B] for F32X3.  Unconverted kinds: as many raw stages as fit in 227 KB, at most 6.  Converted kinds: 4 raw
+// stages, the rest of the 227 KB for converted stages (at most 4).  BN is 128 / 160 / 224 / 256 for unconverted TF32,
+// 128 / 256 for BF16, 128 for the converted kinds (accumulators plus two A fragment sets must fit in registers).
 __host__ __device__ constexpr bool converts(int mode, bool a_mn, bool b_mn) { return mode == kF32x3 || (mode == kTf32 && (a_mn || b_mn)); }
 __host__ __device__ constexpr size_t raw_bytes(int bn) { return (size_t)kTileBytes + (size_t)bn * kRowBytes; }
-__host__ __device__ constexpr size_t stage_bytes(int mode, bool a_mn, bool b_mn, int bn) {
-  return raw_bytes(bn) * (1 + (converts(mode, a_mn, b_mn) ? (mode == kF32x3 ? 2 : 1) : 0));
-}
+__host__ __device__ constexpr size_t cvt_bytes(int mode, int bn) { return (size_t)bn * kRowBytes * (mode == kF32x3 ? 2 : 1); }
 constexpr size_t kSmemTail = 1024 + 256;  // alignment slack + barriers
-__host__ __device__ constexpr int stages_for(int mode, bool a_mn, bool b_mn, int bn) {
-  return (227 * 1024 - kSmemTail) / stage_bytes(mode, a_mn, b_mn, bn) > 6 ? 6 : (int)((227 * 1024 - kSmemTail) / stage_bytes(mode, a_mn, b_mn, bn));
+constexpr size_t kSmemBudget = 227 * 1024 - kSmemTail;
+constexpr int kConvRawStages = 4;
+__host__ __device__ constexpr int raw_stages(int mode, bool a_mn, bool b_mn, int bn) {
+  return converts(mode, a_mn, b_mn) ? kConvRawStages : (kSmemBudget / raw_bytes(bn) > 6 ? 6 : (int)(kSmemBudget / raw_bytes(bn)));
+}
+__host__ __device__ constexpr int cvt_stages(int mode, bool a_mn, bool b_mn, int bn) {
+  return !converts(mode, a_mn, b_mn) ? 0
+         : (kSmemBudget - kConvRawStages * raw_bytes(bn)) / cvt_bytes(mode, bn) > 4 ? 4
+                                                                                     : (int)((kSmemBudget - kConvRawStages * raw_bytes(bn)) / cvt_bytes(mode, bn));
 }
 __host__ __device__ constexpr size_t smem_for(int mode, bool a_mn, bool b_mn, int bn) {
-  return stages_for(mode, a_mn, b_mn, bn) * stage_bytes(mode, a_mn, b_mn, bn) + kSmemTail;
+  return raw_stages(mode, a_mn, b_mn, bn) * raw_bytes(bn) + cvt_stages(mode, a_mn, b_mn, bn) * cvt_bytes(mode, bn) + kSmemTail;
 }
 
 struct GemmParams {
@@ -208,15 +221,18 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   constexpr bool kIsBf16 = kMode == kBf16, kSplit = kMode == kF32x3, kConv = converts(kMode, kAMn, kBMn);
   constexpr int BKE = kRowBytes / (kIsBf16 ? 2 : 4);  // elements of k per stage: 32 fp32 / 64 bf16
-  constexpr int kStages = stages_for(kMode, kAMn, kBMn, BN);
-  constexpr size_t kStage = stage_bytes(kMode, kAMn, kBMn, BN), kRaw = raw_bytes(BN);
+  constexpr int kStages = raw_stages(kMode, kAMn, kBMn, BN), kCvtStages = cvt_stages(kMode, kAMn, kBMn, BN);
+  constexpr size_t kRaw = raw_bytes(BN), kCvt = cvt_bytes(kMode, BN);
   constexpr uint32_t kOperandBytes = (uint32_t)kRaw;
-  static_assert(kStages >= 2, "gemm: at least two pipeline stages");
+  static_assert(kStages >= 2 && (!kConv || kCvtStages >= 2), "gemm: at least two stages per ring");
+  static_assert(!kConv || BN == 128, "gemm: the converted kinds take A from registers at BN = 128");
   static_assert(!kIsBf16 || !kBMn || BN % 64 == 0, "gemm: MN-major bf16 B is staged in boxes of 64 columns");
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * kStage);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + kStages;
-  uint64_t* ready = bars + 2 * kStages;
+  unsigned char* cvt_ring = smem + kStages * kRaw;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(cvt_ring + kCvtStages * kCvt);
+  uint64_t* full = bars;                       // raw stage landed (TMA transaction count)
+  uint64_t* empty = bars + kStages;            // raw stage free: consumers (and the B conversion) are done reading it
+  uint64_t* ready = bars + 2 * kStages;        // converted B stage written
+  uint64_t* cvt_empty = ready + kCvtStages;    // converted B stage free: the MMAs reading it have completed
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
   const int total_kb = (p.K + BKE - 1) / BKE;
@@ -226,8 +242,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   if (tid == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], kConsumerThreads);
+      mbar_init(&empty[s], kConsumerThreads + (kConv ? kConvThreads : 0));
+    }
+    for (int s = 0; s < kCvtStages; ++s) {
       mbar_init(&ready[s], kConvThreads);
+      mbar_init(&cvt_empty[s], kConsumerThreads);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -256,7 +275,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
             const int s = it % kStages;
             mbar_wait(&empty[s], ((it / kStages) & 1) ^ 1);
             mbar_expect_tx(&full[s], kOperandBytes);
-            unsigned char* sa = smem + s * kStage;
+            unsigned char* sa = smem + s * kRaw;
             unsigned char* sb = sa + kTileBytes;
             const int k0 = (kb_begin + kb) * BKE;
             if (!kAMn) {
@@ -265,7 +284,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
 #pragma unroll
               for (int j = 0; j < BM / 64; ++j) tma_load_2d(&map_a, &full[s], sa + j * 8192, m0 + 64 * j, k0);  // box {64 m, 64 k}
             } else {
-              tma_load_2d(&map_a, &full[s], sa, m0, k0);  // box {128 m, 32 k}, unswizzled
+#pragma unroll
+              for (int j = 0; j < BM / 8; ++j) tma_load_2d(&map_a, &full[s], sa + j * 1024, m0 + 8 * j, k0);  // box {8 m, 32 k}
             }
             if (!kBMn) {
               tma_load_2d(&map_b, &full[s], sb, k0, n0);
@@ -278,21 +298,22 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
           }
         }
       }
-    } else if (kConv) {
-      // ===== operand conversion (warps 1..3) =====
+    } else if constexpr (kConv) {
+      // ===== B conversion (warps 1..3) =====
       const int ct = tid - 32;
       uint32_t it = 0;
       for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
         int m0, n0, kb_begin, num_kb;
         tile_coords(t, m0, n0, kb_begin, num_kb);
         for (int kb = 0; kb < num_kb; ++kb, ++it) {
-          const int s = it % kStages;
+          const int s = it % kStages, c = it % kCvtStages;
+          mbar_wait(&cvt_empty[c], ((it / kCvtStages) & 1) ^ 1);
           mbar_wait(&full[s], (it / kStages) & 1);
-          unsigned char* st = smem + s * kStage;
-          convert_tile<kAMn, kSplit, BM>(st, st + kRaw, st + 2 * kRaw, ct);
-          convert_tile<kBMn, kSplit, BN>(st + kTileBytes, st + kRaw + kTileBytes, st + 2 * kRaw + kTileBytes, ct);
+          unsigned char* dst = cvt_ring + c * kCvt;
+          convert_tile<kBMn, kSplit, BN>(smem + s * kRaw + kTileBytes, dst, dst + BN * kRowBytes, ct);
+          mbar_arrive(&empty[s]);
           asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to wgmma
-          mbar_arrive(&ready[s]);
+          mbar_arrive(&ready[c]);
         }
       }
     }
@@ -300,6 +321,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     // ===== consumers: warpgroup wg owns rows 64 (wg - 1) .. + 63 of the tile =====
     const int cw = wg - 1;
     const bool vec_c = (p.ldc % 2) == 0 && (reinterpret_cast<uintptr_t>(p.C) & (p.c_bf16 ? 3 : 7)) == 0;
+    // converted kinds: this thread's A fragment rows fr, fr + 8 (wgmma register layout, wgmma_ptx.cuh) and k offset fq
+    const int fr = 64 * cw + 16 * (warp & 3) + (lane >> 2), fq = lane & 3;
     uint32_t it = 0;
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       int m0, n0, kb_begin, num_kb;
@@ -307,40 +330,97 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
       float acc[BN / 2];
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-      for (int kb = 0; kb < num_kb; ++kb, ++it) {
-        const int s = it % kStages;
-        mbar_wait(kConv ? &ready[s] : &full[s], (it / kStages) & 1);
-        const uint32_t st = smem_u32(smem + s * kStage);
-        const uint32_t a_base = (kConv ? st + (uint32_t)kRaw : st) + (uint32_t)(cw * 8192), b_base = (kConv ? st + (uint32_t)kRaw : st) + kTileBytes;
-        wg::fence_operands(acc);
-        wg::fence();
+      if constexpr (kConv) {
+        // A fragments of one k block: [k8 step][a0..a3], hi = tf32(x) and (F32X3) lo = tf32(x - hi), rounded as convert_tile
+        struct AFrag {
+          uint32_t hi[4][4], lo[4][4];
+        };
+        auto fence_frag = [&](AFrag& f) {
+          wg::fence_operands(f.hi);
+          if constexpr (kSplit) wg::fence_operands(f.lo);
+        };
+        // one k block: A fragments from raw stage s (then free it), MMAs on converted B stage c; on return, the MMAs of the
+        // previous k block (fragments `prev`) have completed and its converted B stage is freed
+        auto step = [&](AFrag& cur, AFrag& prev, int kb) {
+          const int s = it % kStages, c = it % kCvtStages;
+          mbar_wait(&full[s], (it / kStages) & 1);
+          const uint32_t sa = smem_u32(smem + s * kRaw);
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const int sc = (kb | k) != 0;
-          if constexpr (kIsBf16) {
-            const uint64_t da = kAMn ? make_desc_sw128(a_base + k * 2048, 8192, 1024) : make_desc_sw128(a_base + k * 32, 16, 1024);
-            const uint64_t db = kBMn ? make_desc_sw128(b_base + k * 2048, 8192, 1024) : make_desc_sw128(b_base + k * 32, 16, 1024);
-            wg::mma_bf16<BN, kAMn ? 1 : 0, kBMn ? 1 : 0>(acc, da, db, sc);
-          } else {
-            const uint64_t da = make_desc_sw128(a_base + k * 32, 16, 1024), db = make_desc_sw128(b_base + k * 32, 16, 1024);
-            if constexpr (kSplit) {
-              const uint32_t lo = (uint32_t)kRaw;  // lo tiles follow the hi tiles
-              wg::mma_tf32<BN>(acc, make_desc_sw128(a_base + lo + k * 32, 16, 1024), db, sc);  // Al * Bh
-              wg::mma_tf32<BN>(acc, da, make_desc_sw128(b_base + lo + k * 32, 16, 1024), 1);   // Ah * Bl
-              wg::mma_tf32<BN>(acc, da, db, 1);                                                 // Ah * Bh
-            } else {
-              wg::mma_tf32<BN>(acc, da, db, sc);
+          for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {  // a0 (r, k), a1 (r + 8, k), a2 (r, k + 4), a3 (r + 8, k + 4)
+              const int r = fr + 8 * (i & 1), k = 8 * kk + 4 * (i >> 1) + fq;
+              const int off = kAMn ? (r >> 3) * 1024 + k * 32 + (r & 7) * 4 : r * 128 + (((k >> 2) ^ (r & 7)) << 4) + (k & 3) * 4;
+              uint32_t x;
+              asm volatile("ld.shared.b32 %0, [%1];" : "=r"(x) : "r"(sa + off) : "memory");
+              cur.hi[kk][i] = rn_tf32(x);
+              if constexpr (kSplit) cur.lo[kk][i] = rn_tf32(__float_as_uint(__uint_as_float(x) - __uint_as_float(cur.hi[kk][i])));
             }
           }
+          mbar_arrive(&empty[s]);
+          mbar_wait(&ready[c], (it / kCvtStages) & 1);
+          const uint32_t b_base = smem_u32(cvt_ring + c * kCvt);
+          fence_frag(cur);  // the fragments are final before wgmma.fence (a later definition would serialise the MMAs)
+          wg::fence_operands(acc);
+          wg::fence();
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) {
+            const int sc = (kb | kk) != 0;
+            const uint64_t db = make_desc_sw128(b_base + kk * 32, 16, 1024);
+            if constexpr (kSplit) {
+              wg::mma_tf32_rs<BN>(acc, cur.lo[kk], db, sc);                                                  // Al * Bh
+              wg::mma_tf32_rs<BN>(acc, cur.hi[kk], make_desc_sw128(b_base + BN * kRowBytes + kk * 32, 16, 1024), 1);  // Ah * Bl
+              wg::mma_tf32_rs<BN>(acc, cur.hi[kk], db, 1);                                                   // Ah * Bh
+            } else {
+              wg::mma_tf32_rs<BN>(acc, cur.hi[kk], db, sc);
+            }
+          }
+          wg::commit();
+          wg::fence_operands(acc);
+          // F32X3 keeps one k block of MMAs in flight.  TF32 drains them: with in-flight fragments ptxas serialises the single
+          // MMA per k8 step on its operand registers (C7513)
+          if constexpr (kSplit) wg::wait<1>(); else wg::wait<0>();
+          fence_frag(prev);
+          if (kb > 0) mbar_arrive(&cvt_empty[(it - 1) % kCvtStages]);
+          ++it;
+        };
+        AFrag fa, fb;
+        for (int kb = 0; kb < num_kb; kb += 2) {
+          step(fa, fb, kb);
+          if (kb + 1 < num_kb) step(fb, fa, kb + 1);
         }
-        wg::commit();
+        wg::wait<0>();
         wg::fence_operands(acc);
-        wg::wait<1>();  // the previous stage's MMAs are done: release it
-        if (kb > 0) mbar_arrive(&empty[(it - 1) % kStages]);
+        fence_frag(fa);
+        fence_frag(fb);
+        if (num_kb > 0) mbar_arrive(&cvt_empty[(it - 1) % kCvtStages]);
+      } else {
+        for (int kb = 0; kb < num_kb; ++kb, ++it) {
+          const int s = it % kStages;
+          mbar_wait(&full[s], (it / kStages) & 1);
+          const uint32_t a_base = smem_u32(smem + s * kRaw) + (uint32_t)(cw * 8192), b_base = smem_u32(smem + s * kRaw) + kTileBytes;
+          wg::fence_operands(acc);
+          wg::fence();
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const int sc = (kb | k) != 0;
+            if constexpr (kIsBf16) {
+              const uint64_t da = kAMn ? make_desc_sw128(a_base + k * 2048, 8192, 1024) : make_desc_sw128(a_base + k * 32, 16, 1024);
+              const uint64_t db = kBMn ? make_desc_sw128(b_base + k * 2048, 8192, 1024) : make_desc_sw128(b_base + k * 32, 16, 1024);
+              wg::mma_bf16<BN, kAMn ? 1 : 0, kBMn ? 1 : 0>(acc, da, db, sc);
+            } else {
+              wg::mma_tf32<BN>(acc, make_desc_sw128(a_base + k * 32, 16, 1024), make_desc_sw128(b_base + k * 32, 16, 1024), sc);
+            }
+          }
+          wg::commit();
+          wg::fence_operands(acc);
+          wg::wait<1>();  // the previous stage's MMAs are done: release it
+          if (kb > 0) mbar_arrive(&empty[(it - 1) % kStages]);
+        }
+        wg::wait<0>();
+        wg::fence_operands(acc);
+        if (num_kb > 0) mbar_arrive(&empty[(it - 1) % kStages]);
       }
-      wg::wait<0>();
-      wg::fence_operands(acc);
-      if (num_kb > 0) mbar_arrive(&empty[(it - 1) % kStages]);
       const int z = t / tiles_mn;  // split-K slice (an empty slice writes zeros)
       const int row0 = m0 + 64 * cw + 16 * (warp & 3) + (lane >> 2);
       const int col0 = n0 + 2 * (lane & 3);
@@ -416,7 +496,7 @@ int launch_bn(cudaStream_t stream, const CUtensorMap& ma, const CUtensorMap& mb,
 }
 template <int kMode, bool kAMn, bool kBMn>
 int launch_mode(cudaStream_t stream, int bn, const CUtensorMap& ma, const CUtensorMap& mb, const GemmParams& p) {
-  if constexpr (kMode == kF32x3) {
+  if constexpr (converts(kMode, kAMn, kBMn)) {
     return launch_bn<kMode, kAMn, kBMn, 128>(stream, ma, mb, p);
   } else if constexpr (kMode == kBf16) {  // 128 or 256 (MN-major B is staged in 64-wide boxes)
     return bn <= 128 ? launch_bn<kMode, kAMn, kBMn, 128>(stream, ma, mb, p) : launch_bn<kMode, kAMn, kBMn, 256>(stream, ma, mb, p);
@@ -446,9 +526,9 @@ int splits_for(int tiles, int total_kb, bool plain) {
 }
 // tile width: minimise (waves over the SMs) x (operand bytes per tile + epilogue)
 thread_local int g_force_bn = 0;  // w2l_gemm_set_tile: tests pin the tile width
-int choose_bn(int mode, bool b_mn, int M, int N, int total_kb, bool plain, int* splits_out) {
+int choose_bn(int mode, bool a_mn, bool b_mn, int M, int N, int total_kb, bool plain, int* splits_out) {
   auto allowed = [&](int bn) {
-    if (mode == kF32x3) return bn == 128;
+    if (converts(mode, a_mn, b_mn)) return bn == 128;
     if (mode == kBf16) return bn == 128 || bn == 256;
     return true;
   };
@@ -501,17 +581,17 @@ int gemm_impl(void* stream_, int mode, int a_mn_major, int b_mn_major, int M, in
   const int total_kb = (K + bke - 1) / bke;
   const bool plain = act == 0 && aux_mode == 0 && dropout_p == 0.f && bias == nullptr && !c_bf16;
   int splits = 1;
-  const int BN = choose_bn(mode, b_mn_major != 0, M, N, total_kb, plain, &splits);
+  const int BN = choose_bn(mode, a_mn_major != 0, b_mn_major != 0, M, N, total_kb, plain, &splits);
   const bool conv = converts(mode, a_mn_major != 0, b_mn_major != 0);
   const bool bf16 = mode == kBf16;
   CUtensorMap ma, mb;
   int rc;
-  // K-major: box {128 B of k, tile rows}, 128B swizzle.  MN-major bf16: box {64 m/n, 64 k}, 128B swizzle.  MN-major fp32: box
-  // {tile rows, 32 k}, unswizzled (converted in shared memory)
+  // K-major: box {128 B of k, tile rows}, 128B swizzle.  MN-major bf16: box {64 m/n, 64 k}, 128B swizzle.  MN-major fp32:
+  // A in boxes {8 m, 32 k} (read as register fragments), B in one box {BN, 32 k} (converted in shared memory), unswizzled
   if (!a_mn_major)
     rc = make_map(&ma, mode, conv, A, M, K, lda, bke, BM, true);
   else
-    rc = make_map(&ma, mode, conv, A, K, M, lda, bf16 ? 64 : BM, bke, bf16);
+    rc = make_map(&ma, mode, conv, A, K, M, lda, bf16 ? 64 : 8, bke, bf16);
   if (rc) return rc;
   if (!b_mn_major)
     rc = make_map(&mb, mode, conv, B, N, K, ldb, bke, BN, true);
