@@ -93,6 +93,7 @@ class Tensor {
   void copyFrom(const Tensor& src) const;  // device-to-device, same byte size
 
  private:
+  friend void readOnGradStream(const Tensor& t);
   std::shared_ptr<Storage> st_;
   size_t off_ = 0;
   Dims dims_;
@@ -104,6 +105,18 @@ void* currentStream();            // cudaStream_t used by every fl_compat call o
 void copyRows(void* dst, size_t dstPitch, const void* src, size_t srcPitch, size_t width, size_t height);
 void setCurrentStream(void* s);   // (the Python harness passes torch's current stream)
 void sync();                      // af::sync()
+
+// The gradient stream (null: none, the default).  Parameter-gradient work whose only consumer is the gradient arena (the
+// Linear weight-gradient GEMM and bias column sum) runs on it, beside the data-gradient chain on the current stream.
+// forkGradStream(): the gradient stream waits for the work queued so far on the current stream.
+// readOnGradStream(t): gradient-stream work reads t; when t's storage is released, the free is queued on the gradient
+//   stream behind the work queued so far on both streams, so neither stream waits for the other.
+// joinGradStream(): the current stream waits for the work queued so far on the gradient stream.
+void setGradStream(void* s, int delayUs = 0);  // delayUs: tests, a w2l_delay before each fork's work
+void* gradStream();
+void forkGradStream();
+void readOnGradStream(const Tensor& t);
+void joinGradStream();
 
 }  // namespace w2l
 

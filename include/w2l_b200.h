@@ -298,6 +298,8 @@ W2L_API int w2l_mask_bands(void* stream, int B, int T, int C, int W, const float
 W2L_API int w2l_transpose_input(void* stream, int B, int F, int T, const float* in, float* out);
 W2L_API int w2l_axpy(void* stream, long long n, float a, const float* x, float* y);
 W2L_API int w2l_fill(void* stream, long long n, float v, float* y);
+/* one single-thread kernel that sleeps about `us` microseconds (at most 1e6); tests use it to hold a stream back */
+W2L_API int w2l_delay(void* stream, int us);
 W2L_API int w2l_act_fwd(void* stream, long long n, const float* x, int relu, float dropout_p, unsigned long long seed, float* y);
 W2L_API int w2l_mask_mul(void* stream, long long n, const float* g, const float* ref, int mode, float scale, float* out);
 
@@ -317,6 +319,12 @@ W2L_API int w2l_trainer_step(void* trainer, void* stream, int B, int T, const fl
                              float* loss_out, int train, float total_batch);
 W2L_API int w2l_trainer_forward(void* trainer, void* stream, int B, int T, const float* features, float* emissions_out,
                                 long long capacity, int* t_out);
+/* 1 (default): the backward pass computes the Linear layers' weight and bias gradients on a second stream of the
+ * trainer, beside the data-gradient chain; 0: everything on the caller's stream.  Results are bit-identical either way. */
+W2L_API int w2l_trainer_set_grad_stream(void* trainer, int on);
+/* tests: queue a w2l_delay of `us` microseconds on the gradient stream before each piece of work handed to it, so a
+ * missing wait or an early free shows up as a changed result (0, the default: none) */
+W2L_API int w2l_trainer_set_grad_stream_delay(void* trainer, int us);
 /* precision of the trainer's dense contractions (W2L_PRECISION_*; default: the creating thread's w2l_set_precision) */
 W2L_API int w2l_trainer_set_precision(void* trainer, int precision);
 /* steps whose update was skipped on the device because the loss or a gradient was NaN / Inf (Train.cpp:1686-1698,

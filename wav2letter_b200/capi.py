@@ -25,7 +25,7 @@ EXPORTS = [
     "w2l_fac_viterbi_workspace_size", "w2l_fac_viterbi",
     "w2l_ctc_workspace_size", "w2l_ctc_forward_backward", "w2l_argmax_path", "w2l_linseg_target",
     "w2l_set_precision", "w2l_get_precision", "w2l_gemm", "w2l_cast_bf16", "w2l_cast_bf16_rows", "w2l_sgd_step_ex", "w2l_finite_guard",
-    "w2l_mask_bands", "w2l_trainer_set_precision", "w2l_trainer_status", "w2l_trainer_save", "w2l_trainer_load", "w2l_trainer_export_streaming",
+    "w2l_mask_bands", "w2l_trainer_set_precision", "w2l_trainer_set_grad_stream", "w2l_trainer_set_grad_stream_delay", "w2l_delay", "w2l_trainer_status", "w2l_trainer_save", "w2l_trainer_load", "w2l_trainer_export_streaming",
     "w2l_text_create", "w2l_text_destroy", "w2l_text_num_classes", "w2l_text_encode", "w2l_text_prediction2ltr", "w2l_text_target2ltr",
     "w2l_text_ltr2wrd", "w2l_edit_distance",
     "w2l_gemm_set_variant", "w2l_gemm_set_tile", "w2l_gemm_tf32", "w2l_gemm_tf32_ex", "w2l_gemm_tf32_view", "w2l_conv_set_path", "w2l_conv_time_workspace_size", "w2l_conv_time_fwd", "w2l_conv_time_dgrad",
@@ -106,6 +106,9 @@ def _load() -> ctypes.CDLL:
     lib.w2l_finite_guard.argtypes = [vp, i, vp, vp, vp]
     lib.w2l_mask_bands.argtypes = [vp, i, i, i, i, vp, vp, i, vp, vp, i, vp, vp, f32]
     lib.w2l_trainer_set_precision.argtypes = [vp, i]
+    lib.w2l_trainer_set_grad_stream.argtypes = [vp, i]
+    lib.w2l_trainer_set_grad_stream_delay.argtypes = [vp, i]
+    lib.w2l_delay.argtypes = [vp, i]
     lib.w2l_trainer_status.argtypes = [vp, vp, vp]
     cp = ctypes.c_char_p
     lib.w2l_trainer_save.argtypes = [vp, vp, cp]

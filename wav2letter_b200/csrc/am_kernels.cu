@@ -1334,6 +1334,16 @@ extern "C" int w2l_axpy(void* stream_, long long n, float a, const float* x, flo
   W2L_LAUNCH_CHECK("axpy_kernel");
   return W2L_OK;
 }
+// one thread sleeping about `us` microseconds in 1 us naps (tests: holds a stream back by a known amount)
+__global__ void delay_kernel(int us) {
+  for (int i = 0; i < us; ++i) __nanosleep(1000);
+}
+extern "C" int w2l_delay(void* stream_, int us) {
+  if (us < 0 || us > 1000000) return fail(W2L_ERR_INVALID_ARGUMENT, "delay: microseconds must be in [0, 1e6]");
+  delay_kernel<<<1, 1, 0, static_cast<cudaStream_t>(stream_)>>>(us);
+  W2L_LAUNCH_CHECK("delay_kernel");
+  return W2L_OK;
+}
 extern "C" int w2l_fill(void* stream_, long long n, float v, float* y) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (n <= 0 || !y) return fail(W2L_ERR_INVALID_ARGUMENT, "fill: bad arguments");

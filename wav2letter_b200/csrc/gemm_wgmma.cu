@@ -23,10 +23,13 @@
 // without any transposition pass in global memory.
 //
 // Structure: CTAs walk 128 x BN output tiles (n fastest, so CTAs running together share their A rows in L2); by default
-// one CTA per SM (persistent), w2l_gemm_set_variant(0) launches one CTA per tile.  384 threads:
-//   warpgroup 0, warp 0     TMA producer: 2D boxes into a shared-memory ring of raw [A | B] tiles, full / empty mbarrier
-//                           per stage; it runs ahead across tile boundaries, so the next tile's operands arrive during an
-//                           epilogue
+// one CTA per SM (persistent), w2l_gemm_set_variant(0) launches one CTA per tile.  The persistent CTAs schedule their
+// work dynamically: CTA b starts on work item b, then claims the next unstarted item (tile, split-K slice) from a global
+// counter, so a launch that shares the SMs with a kernel on another stream finishes when the work does.  384 threads:
+//   warpgroup 0, warp 0     TMA producer: claims the work items and passes each id to the other roles through a small
+//                           shared-memory ring (full / empty mbarrier per slot, so every role walks the same sequence);
+//                           2D boxes into a shared-memory ring of raw [A | B] tiles, full / empty mbarrier per stage; it
+//                           runs ahead across tile boundaries, so the next tile's operands arrive during an epilogue
 //   warpgroup 0, warps 1-3  B conversion for the "converted" kinds (F32X3, and TF32 with an MN-major operand): the raw fp32
 //                           B tile is rounded (hi = tf32) or split (hi, lo) into K-major 128B-swizzled tiles of a second
 //                           ring, with a ready / empty mbarrier pair per stage
@@ -50,6 +53,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
+#include <mutex>
 
 #include "common.cuh"
 #include "tma_ptx.cuh"
@@ -74,9 +78,10 @@ enum { kTf32 = W2L_GEMM_TF32, kF32x3 = W2L_GEMM_F32X3, kBf16 = W2L_GEMM_BF16 };
 __host__ __device__ constexpr bool converts(int mode, bool a_mn, bool b_mn) { return mode == kF32x3 || (mode == kTf32 && (a_mn || b_mn)); }
 __host__ __device__ constexpr size_t raw_bytes(int bn) { return (size_t)kTileBytes + (size_t)bn * kRowBytes; }
 __host__ __device__ constexpr size_t cvt_bytes(int mode, int bn) { return (size_t)bn * kRowBytes * (mode == kF32x3 ? 2 : 1); }
-constexpr size_t kSmemTail = 1024 + 256;  // alignment slack + barriers
+constexpr size_t kSmemTail = 1024 + 256;  // alignment slack + barriers + the work-item id ring
 constexpr size_t kSmemBudget = 227 * 1024 - kSmemTail;
 constexpr int kConvRawStages = 4;
+constexpr int kIdSlots = 4;  // work-item ids the producer may publish ahead of the tile the consumers are on
 __host__ __device__ constexpr int raw_stages(int mode, bool a_mn, bool b_mn, int bn) {
   return converts(mode, a_mn, b_mn) ? kConvRawStages : (kSmemBudget / raw_bytes(bn) > 6 ? 6 : (int)(kSmemBudget / raw_bytes(bn)));
 }
@@ -216,7 +221,8 @@ __device__ __forceinline__ void epilogue_pair(const GemmParams& p, int z, int ro
 
 template <int kMode, bool kAMn, bool kBMn, int BN>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, GemmParams p, int tiles_m, int tiles_n) {
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, GemmParams p, int tiles_m, int tiles_n,
+                  unsigned int* sched) {  // [claimed, finished CTAs] counters of the dynamic schedule; null: CTA b walks b, b + grid, ...
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   constexpr bool kIsBf16 = kMode == kBf16, kSplit = kMode == kF32x3, kConv = converts(kMode, kAMn, kBMn);
@@ -233,6 +239,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
   uint64_t* empty = bars + kStages;            // raw stage free: consumers (and the B conversion) are done reading it
   uint64_t* ready = bars + 2 * kStages;        // converted B stage written
   uint64_t* cvt_empty = ready + kCvtStages;    // converted B stage free: the MMAs reading it have completed
+  uint64_t* id_full = cvt_empty + kCvtStages;  // work-item id published by the producer
+  uint64_t* id_empty = id_full + kIdSlots;     // work-item id read by every other role
+  int* id_ring = reinterpret_cast<int*>(id_empty + kIdSlots);
+  static_assert((2 * (kStages + kCvtStages + kIdSlots)) * 8 + kIdSlots * 4 <= kSmemTail - 1024, "gemm: barrier space");
+  constexpr uint32_t kIdReaders = kConsumerThreads + (kConv ? kConvThreads : 0);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
   const int total_kb = (p.K + BKE - 1) / BKE;
@@ -248,11 +259,25 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
       mbar_init(&ready[s], kConvThreads);
       mbar_init(&cvt_empty[s], kConsumerThreads);
     }
+    for (int s = 0; s < kIdSlots; ++s) {
+      mbar_init(&id_full[s], 1);
+      mbar_init(&id_empty[s], kIdReaders);
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
 
-  // every role walks the same tile sequence with the same k-block counts, so the ring phases agree
+  // every role walks the same work-item sequence with the same k-block counts, so the ring phases agree: the first item is
+  // blockIdx.x, the producer claims each later one and publishes it in id_ring (an id >= total_tiles ends the walk)
+  uint32_t id_it = 0;
+  auto next_item = [&]() {
+    const int s = id_it % kIdSlots;
+    mbar_wait(&id_full[s], (id_it / kIdSlots) & 1);
+    const int t = id_ring[s];
+    mbar_arrive(&id_empty[s]);
+    ++id_it;
+    return t;
+  };
   auto tile_coords = [&](int t, int& m0, int& n0, int& kb_begin, int& num_kb) {
     const int z = t / tiles_mn, r = t - z * tiles_mn;
     m0 = (r / tiles_n) * BM;
@@ -268,7 +293,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
         uint32_t it = 0;
-        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+        for (int t = blockIdx.x; t < total_tiles;) {
           int m0, n0, kb_begin, num_kb;
           tile_coords(t, m0, n0, kb_begin, num_kb);
           for (int kb = 0; kb < num_kb; ++kb, ++it) {
@@ -296,13 +321,28 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
               tma_load_2d(&map_b, &full[s], sb, n0, k0);
             }
           }
+          // items 0 .. grid-1 are the CTAs' first ones; the counter hands out the rest in the order they are asked for
+          t = sched ? (int)gridDim.x + (int)atomicAdd(sched, 1u) : t + (int)gridDim.x;
+          const int s = id_it % kIdSlots;
+          mbar_wait(&id_empty[s], ((id_it / kIdSlots) & 1) ^ 1);
+          id_ring[s] = t;
+          mbar_arrive(&id_full[s]);
+          ++id_it;
+        }
+        // the last CTA to finish claiming resets the counters for the next launch on this stream
+        if (sched) {
+          __threadfence();
+          if (atomicAdd(sched + 1, 1u) == gridDim.x - 1) {
+            atomicExch(sched, 0u);
+            atomicExch(sched + 1, 0u);
+          }
         }
       }
     } else if constexpr (kConv) {
       // ===== B conversion (warps 1..3) =====
       const int ct = tid - 32;
       uint32_t it = 0;
-      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+      for (int t = blockIdx.x; t < total_tiles; t = next_item()) {
         int m0, n0, kb_begin, num_kb;
         tile_coords(t, m0, n0, kb_begin, num_kb);
         for (int kb = 0; kb < num_kb; ++kb, ++it) {
@@ -324,7 +364,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     // converted kinds: this thread's A fragment rows fr, fr + 8 (wgmma register layout, wgmma_ptx.cuh) and k offset fq
     const int fr = 64 * cw + 16 * (warp & 3) + (lane >> 2), fq = lane & 3;
     uint32_t it = 0;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+    for (int t = blockIdx.x; t < total_tiles; t = next_item()) {
       int m0, n0, kb_begin, num_kb;
       tile_coords(t, m0, n0, kb_begin, num_kb);
       float acc[BN / 2];
@@ -475,6 +515,30 @@ const char* kernel_name(int mode) { return mode == kBf16 ? "gemm_wgmma_kernel<bf
 
 thread_local int g_variant = 1;  // 1: one CTA per SM walking tiles (default), 0: one CTA per tile (w2l_gemm_set_variant; tests compare the two)
 
+// Counters of the dynamic schedule, [claimed, finished CTAs], one pair per stream: launches on one stream run one after
+// another, so the last CTA of a launch can zero its pair for the next, and launches on two streams never share a pair.
+// Past kSchedSlots distinct streams a launch walks its tiles statically (same results, no load balancing).
+constexpr int kSchedSlots = 64;
+__device__ unsigned int g_sched[kSchedSlots][2];
+unsigned int* sched_slot(cudaStream_t stream) {
+  static std::mutex mu;
+  static cudaStream_t owner[kSchedSlots];
+  static int used = 0;
+  int slot = -1;
+  {
+    std::lock_guard<std::mutex> lock(mu);
+    for (int i = 0; i < used && slot < 0; ++i)
+      if (owner[i] == stream) slot = i;
+    if (slot < 0 && used < kSchedSlots) {
+      owner[used] = stream;
+      slot = used++;
+    }
+  }
+  void* base = nullptr;
+  if (slot < 0 || cudaGetSymbolAddress(&base, g_sched) != cudaSuccess) return nullptr;
+  return static_cast<unsigned int*>(base) + 2 * slot;
+}
+
 template <int kMode, bool kAMn, bool kBMn, int BN>
 int launch_bn(cudaStream_t stream, const CUtensorMap& ma, const CUtensorMap& mb, const GemmParams& p) {
   constexpr size_t smem = smem_for(kMode, kAMn, kBMn, BN);
@@ -487,9 +551,10 @@ int launch_bn(cudaStream_t stream, const CUtensorMap& ma, const CUtensorMap& mb,
   const int tiles_m = (p.M + BM - 1) / BM, tiles_n = (p.N + BN - 1) / BN;
   const int total = tiles_m * tiles_n * p.k_splits;
   const int grid = g_variant == 1 ? std::min(total, sm_count()) : total;
+  unsigned int* sched = g_variant == 1 && grid < total ? sched_slot(stream) : nullptr;
   profile_kind(1);
   profile_start(stream);
-  gemm_wgmma_kernel<kMode, kAMn, kBMn, BN><<<grid, kGemmThreads, smem, stream>>>(ma, mb, p, tiles_m, tiles_n);
+  gemm_wgmma_kernel<kMode, kAMn, kBMn, BN><<<grid, kGemmThreads, smem, stream>>>(ma, mb, p, tiles_m, tiles_n, sched);
   profile_stop(stream);
   W2L_LAUNCH_CHECK(kernel_name(kMode));
   return W2L_OK;

@@ -45,6 +45,29 @@ void copyRows(void* dst, size_t dstPitch, const void* src, size_t srcPitch, size
 void setCurrentStream(void* s) { g_stream = static_cast<cudaStream_t>(s); }
 void sync() { cudaCheck(cudaStreamSynchronize(g_stream), "af::sync"); }
 
+namespace {
+thread_local cudaStream_t g_grad_stream = nullptr;
+thread_local int g_grad_delay_us = 0;
+// `to` waits for the work queued so far on `from` (one event serves every hand-over: a wait binds to the record before it)
+cudaError_t handOver(cudaStream_t from, cudaStream_t to) {
+  static thread_local cudaEvent_t ev = nullptr;
+  cudaError_t e = ev ? cudaSuccess : cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaEventRecord(ev, from);
+  if (e == cudaSuccess) e = cudaStreamWaitEvent(to, ev, 0);
+  return e;
+}
+}  // namespace
+void setGradStream(void* s, int delayUs) {
+  g_grad_stream = static_cast<cudaStream_t>(s);
+  g_grad_delay_us = s ? delayUs : 0;
+}
+void* gradStream() { return g_grad_stream; }
+void forkGradStream() {
+  cudaCheck(handOver(g_stream, g_grad_stream), "gradient stream fork");
+  if (g_grad_delay_us) check(w2l_delay(g_grad_stream, g_grad_delay_us));
+}
+void joinGradStream() { cudaCheck(handOver(g_grad_stream, g_stream), "gradient stream join"); }
+
 size_t dtypeSize(DType t) {
   switch (t) {
     case DType::f32:
@@ -70,12 +93,24 @@ struct Storage {
   size_t bytes = 0;
   cudaStream_t stream = nullptr;
   bool owner = true;
+  bool gradRead = false;  // read by gradient-stream work (readOnGradStream)
   ~Storage() {
     // stream-ordered free on the stream the thread is working on NOW (every C-ABI call sets it): that orders the free
     // after the buffer's last use even when a cached buffer (workspaces, arenas) was allocated under another stream
-    if (ptr && owner) cudaFreeAsync(ptr, g_stream ? g_stream : stream);
+    if (!ptr || !owner) return;
+    cudaStream_t s = g_stream ? g_stream : stream;
+    // a buffer the gradient stream reads is freed there, behind its last use on both streams (once the gradient stream
+    // has been joined and cleared, the current stream's order already covers that work)
+    if (gradRead && g_grad_stream && g_grad_stream != s) {
+      handOver(s, g_grad_stream);
+      s = g_grad_stream;
+    }
+    cudaFreeAsync(ptr, s);
   }
 };
+void readOnGradStream(const Tensor& t) {
+  if (!t.isEmpty()) t.st_->gradRead = true;
+}
 
 namespace {
 // Stream-ordered allocation comes from the device's default pool.  By default that pool returns its memory
@@ -163,6 +198,9 @@ namespace fl {
 using w2l::check;
 using w2l::currentStream;
 using w2l::DType;
+using w2l::forkGradStream;
+using w2l::gradStream;
+using w2l::readOnGradStream;
 
 // ================================================================================================
 // Variable / autograd
@@ -998,11 +1036,22 @@ Variable Linear::forwardWith(const Variable& in, const Variable& weight, const V
     }
     const GemmOperand dyop = gemmOperand(dy, M, nout, nout);  // zero-padded columns when nout is not a TMA row length
     if (ins[1].isCalcGrad()) {  // dW[nout][Kp] = dy^T x  (both operands MN-major, no transposition pass)
+      // gradients that go straight into arena slots, read by nothing before the optimizer, are computed on the gradient
+      // stream (when the trainer has one), overlapping the data-gradient chain that follows
+      void* wstream = currentStream();
+      if (gradStream() && Kp == nin && !ins[1].gradStorage().isEmpty() && (!hasBias || !ins[2].gradStorage().isEmpty())) {
+        wstream = gradStream();
+        forkGradStream();
+        readOnGradStream(dy);
+        readOnGradStream(dyop.a);
+        readOnGradStream(xop.a);
+      }
       if (Kp == nin) {
         af::array dw = ins[1].gradStorage();
         const int accumulate = dw.isEmpty() ? 0 : 1;  // arena slot (zeroed by zeroGrad): C += in the GEMM epilogue
         if (!accumulate) dw = af::array::empty(ins[1].dims());
-        check(gemmP(1, 1, nout, nin, M, dyop, xop, dw.f32(), nin, nullptr, 0, accumulate));
+        check(w2l_gemm(wstream, gemmKind(), 1, 1, nout, nin, M, dyop.a.ptr(), dyop.ld, xop.a.ptr(), xop.ld, dw.f32(), nin, 0, nullptr, 0, accumulate,
+                       nullptr, 0, 0, 0, 1.f, 0.f, 0ull, 0));
         ins[1].addGrad(Variable(dw, false));
       } else {  // padded K: the gradient of the zero columns is dropped
         af::array dwp = af::array::empty(af::dim4(Kp, nout));
@@ -1014,7 +1063,7 @@ Variable Linear::forwardWith(const Variable& in, const Variable& weight, const V
       if (hasBias) {
         af::array db = ins[2].gradStorage();
         if (db.isEmpty()) db = af::array::zeros(ins[2].dims());
-        check(w2l_colsum_accumulate(currentStream(), M, nout, dy.f32(), nout, db.f32()));
+        check(w2l_colsum_accumulate(wstream, M, nout, dy.f32(), nout, db.f32()));
         ins[2].addGrad(Variable(db, false));
       }
     }
@@ -1308,6 +1357,9 @@ void OverlappedArenaReducer::launch(Bucket& b) {
   cudaStream_t compute = static_cast<cudaStream_t>(currentStream()), comm = static_cast<cudaStream_t>(comm_stream_);
   cudaEvent_t e = static_cast<cudaEvent_t>(b.event);
   if (cudaEventRecord(e, compute) != cudaSuccess || cudaStreamWaitEvent(comm, e, 0) != cudaSuccess)
+    throw std::runtime_error("OverlappedArenaReducer: event record/wait failed");
+  // the bucket's weight gradients may have been written on the gradient stream
+  if (gradStream() && (cudaEventRecord(e, static_cast<cudaStream_t>(gradStream())) != cudaSuccess || cudaStreamWaitEvent(comm, e, 0) != cudaSuccess))
     throw std::runtime_error("OverlappedArenaReducer: event record/wait failed");
   float* ptr = grads_.f32() + b.offset;
   ncclCheck(ncclAllReduce(ptr, ptr, b.count, ncclFloat32, ncclSum, g_comm, comm), "ncclAllReduce (bucket)");

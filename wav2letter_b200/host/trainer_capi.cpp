@@ -46,6 +46,35 @@ struct Trainer {
   std::string archText, critName;
   int scaleMode = 0;
   float transdiag = 0.f;
+  // the gradient stream (fl_compat.h): the weight gradients of the Linear layers run on it, beside the data-gradient
+  // chain; created at the first training step, at the device's lowest stream priority so the chain goes first
+  bool useGradStream = true;
+  int gradStreamDelayUs = 0;  // tests (w2l_trainer_set_grad_stream_delay)
+  cudaStream_t gradStream = nullptr;
+  ~Trainer() {
+    if (gradStream) {
+      cudaStreamSynchronize(gradStream);
+      cudaStreamDestroy(gradStream);
+    }
+  }
+};
+
+// the trainer's gradient stream for the backward pass of one step; on exit the caller's stream waits for its work
+struct GradStreamScope {
+  bool on;
+  GradStreamScope(cudaStream_t s, int delayUs) : on(s != nullptr) { w2l::setGradStream(s, delayUs); }
+  void join() {
+    if (on) w2l::joinGradStream();
+    on = false;
+    w2l::setGradStream(nullptr);
+  }
+  ~GradStreamScope() {
+    try {
+      join();
+    } catch (...) {
+      w2l::setGradStream(nullptr);
+    }
+  }
 };
 
 struct PrecisionScope {  // the trainer's precision for the duration of one call; the thread's own setting is restored
@@ -236,9 +265,17 @@ W2L_API int w2l_trainer_step(void* h, void* stream, int B, int T, const float* f
       t->reducer->setNormAccumulator(t->sqnorm.f64());  // per-bucket sum(g^2) behind each all-reduce, off the critical path
     }
     t->sqnorm.zero();  // before any bucket can be launched
+    if (t->useGradStream && !t->gradStream) {
+      int least = 0, greatest = 0;
+      if (cudaDeviceGetStreamPriorityRange(&least, &greatest) != cudaSuccess ||
+          cudaStreamCreateWithPriority(&t->gradStream, cudaStreamNonBlocking, least) != cudaSuccess)
+        throw std::runtime_error("trainer: cannot create the gradient stream");
+    }
+    GradStreamScope grads(t->useGradStream ? t->gradStream : nullptr, t->gradStreamDelayUs);
     if (t->reducer) t->reducer->arm();
     loss.backward();
     if (t->reducer) t->reducer->finalize();
+    grads.join();  // the weight gradients are complete before the norm, the clip and the update read them
     if (fl::isDistributedInit() && t->critArena.elements) fl::allReduce(t->critArena.grads);
     // [opt]  grads /= totalBatch (Train.cpp:1752,1783), clipGradNorm(net U crit) (:1791-1798), step (:1801-1802).
     // The reference's numerical guards — LOG(FATAL) on a NaN / Inf loss (:1686-1698), skip-and-retry on non-finite
@@ -260,6 +297,15 @@ W2L_API int w2l_trainer_step(void* h, void* stream, int B, int T, const float* f
   });
 }
 
+W2L_API int w2l_trainer_set_grad_stream(void* h, int on) {
+  static_cast<Trainer*>(h)->useGradStream = on != 0;
+  return W2L_OK;
+}
+W2L_API int w2l_trainer_set_grad_stream_delay(void* h, int us) {
+  if (us < 0 || us > 1000000) return w2l::fail(W2L_ERR_INVALID_ARGUMENT, "trainer_set_grad_stream_delay: microseconds must be in [0, 1e6]");
+  static_cast<Trainer*>(h)->gradStreamDelayUs = us;
+  return W2L_OK;
+}
 W2L_API int w2l_trainer_set_precision(void* h, int precision) {
   if (precision != W2L_PRECISION_TF32 && precision != W2L_PRECISION_F32 && precision != W2L_PRECISION_BF16)
     return w2l::fail(W2L_ERR_INVALID_ARGUMENT, "trainer_set_precision: unknown precision");

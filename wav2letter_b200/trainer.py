@@ -32,6 +32,14 @@ class Trainer:
     def set_precision(self, precision):
         _check(lib.w2l_trainer_set_precision(self.h, capi.PRECISIONS[precision] if isinstance(precision, str) else int(precision)))
 
+    def set_grad_stream(self, on: bool):
+        """True (default): the Linear layers' weight gradients run on a second stream beside the data-gradient chain"""
+        _check(lib.w2l_trainer_set_grad_stream(self.h, int(on)))
+
+    def set_grad_stream_delay(self, us: int):
+        """tests: hold the gradient stream back by `us` microseconds before each piece of work handed to it"""
+        _check(lib.w2l_trainer_set_grad_stream_delay(self.h, int(us)))
+
     def skipped_steps(self) -> int:
         """steps whose update the device-side guard skipped (NaN / Inf loss or gradient); synchronises"""
         n = ctypes.c_longlong(0)
