@@ -35,6 +35,7 @@ EXPORTS = [
     "w2l_trainer_create", "w2l_trainer_destroy", "w2l_trainer_step", "w2l_trainer_forward", "w2l_trainer_num_params",
     "w2l_trainer_param_layout", "w2l_trainer_get_flat", "w2l_trainer_set_flat", "w2l_trainer_sync_parameters",
     "w2l_trainer_describe", "w2l_nccl_unique_id", "w2l_init_distributed",
+    "w2l_mfsc_num_frames", "w2l_mfsc_workspace_size", "w2l_mfsc",
 ]
 
 
@@ -143,6 +144,10 @@ def _load() -> ctypes.CDLL:
     lib.w2l_trainer_describe.argtypes = [vp]
     lib.w2l_nccl_unique_id.argtypes = [vp]
     lib.w2l_init_distributed.argtypes = [i, i, vp]
+    lib.w2l_mfsc_num_frames.argtypes = [i, i, i, i]
+    lib.w2l_mfsc_workspace_size.restype = sz
+    lib.w2l_mfsc_workspace_size.argtypes = [i, i, i, i, i, i]
+    lib.w2l_mfsc.argtypes = [vp, i, i, vp, vp, i, i, i, i, i, vp, i, vp, sz]
     return lib
 
 
