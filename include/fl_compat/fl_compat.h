@@ -531,6 +531,12 @@ class SequenceCriterion : public fl::Module {
  public:
   // per-frame token ids [T] (single sample) or [T,B]
   virtual af::array viterbiPath(const af::array& input, const af::array& inputSize = af::array()) = 0;
+  // forced alignment: the best path that spells `target` ([L,B] int32, -1 padded), per-frame token ids [T,B] (-1 over
+  // a sample that cannot be aligned).  index (nullable) receives [T,B] int32: the target position per frame (ASG,
+  // LinSeg) or the extended-target state (CTC).  Upstream's name; its signature, recalled (flashlight is not
+  // vendored), also takes input / target sizes, which the criteria here do not use (every sample runs the padded T).
+  // A criterion that does not override it (a user's own, e.g. cpc/CPCCriterion.h) throws std::logic_error.
+  virtual af::array viterbiPathWithTarget(const af::array& input, const af::array& target, af::array* index = nullptr);
 };
 
 // ASGLoss(numClasses, scalemode, transdiag)  — Train.cpp:408-410
@@ -539,6 +545,7 @@ class AutoSegmentationCriterion : public SequenceCriterion {
   AutoSegmentationCriterion(int N, CriterionScaleMode scalemode = CriterionScaleMode::NONE, double transdiag = 0.0);
   std::vector<Variable> forward(const std::vector<Variable>& inputs) override;  // {emissions [N,T,B], target [L,B]} -> {loss [B]}
   af::array viterbiPath(const af::array& input, const af::array& inputSize = af::array()) override;
+  af::array viterbiPathWithTarget(const af::array& input, const af::array& target, af::array* index = nullptr) override;
   std::string prettyString() const override;
 
  private:
@@ -554,6 +561,7 @@ class ConnectionistTemporalClassificationCriterion : public SequenceCriterion {
   explicit ConnectionistTemporalClassificationCriterion(CriterionScaleMode scalemode = CriterionScaleMode::NONE);
   std::vector<Variable> forward(const std::vector<Variable>& inputs) override;
   af::array viterbiPath(const af::array& input, const af::array& inputSize = af::array()) override;
+  af::array viterbiPathWithTarget(const af::array& input, const af::array& target, af::array* index = nullptr) override;
   std::string prettyString() const override;
 
  private:
@@ -569,6 +577,7 @@ class LinearSegmentationCriterion : public SequenceCriterion {
   LinearSegmentationCriterion(int N, CriterionScaleMode scalemode = CriterionScaleMode::NONE);
   std::vector<Variable> forward(const std::vector<Variable>& inputs) override;
   af::array viterbiPath(const af::array& input, const af::array& inputSize = af::array()) override;
+  af::array viterbiPathWithTarget(const af::array& input, const af::array& target, af::array* index = nullptr) override;
   std::string prettyString() const override;
 
  private:

@@ -106,6 +106,11 @@ std::vector<std::string> tknPrediction2Ltr(std::vector<int> tokens, const lib::t
 std::vector<std::string> tknTarget2Ltr(std::vector<int> tokens, const lib::text::Dictionary& tokenDict, const std::string& criterion,
                                        const std::string& surround, bool eosToken, int replabel, bool useWordPiece, const std::string& wordSep);
 std::vector<std::string> tkn2Wrd(const std::vector<std::string>& input, const std::string& wordSep);
+// Word timings of one forced alignment (w2l_text_align_words in w2l_b200.h): target tokens, the aligned index of every
+// frame (extended-target state when ctcStates, else target position) -> one `.align` line, segments
+// "uttId 1 <begin s> <duration s> <word>" joined by a literal backslash-n, silence as "$"
+std::string alignWords(const std::vector<int>& target, const std::vector<int>& frameIdx, bool ctcStates, const lib::text::Dictionary& dict,
+                       const std::string& surround, int replabel, const std::string& wordSep, double msPerFrame, const std::string& uttId);
 
 }  // namespace speech
 }  // namespace pkg

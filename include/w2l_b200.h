@@ -140,6 +140,31 @@ W2L_API int w2l_ctc_forward_backward(void* stream, int B, int T, int N, int L, i
                                      void* workspace, size_t workspace_bytes);
 W2L_API int w2l_argmax_path(void* stream, int B, int T, int N, const float* emis, int32_t* path);
 
+/* ----------------------------------------------------------------------------------------
+ * CTC Viterbi with target: the forced alignment of a CTC model (upstream SequenceCriterion::viterbiPathWithTarget of
+ * CTCLoss).  Contract, bit for bit:
+ *   - inputs are raw activations emis[B][T][N], blank = N-1 as in w2l_ctc_forward_backward, and target[B][L], -1
+ *     padded (L_b = index of the last non-negative entry + 1).  The extended target is z of length S = 2 L_b + 1,
+ *     blanks interleaved: z_s = blank for even s, y_{(s-1)/2} for odd s.
+ *   - scores are the raw activations, not the log-softmax: every path takes exactly one state per frame, so the
+ *     per-frame log-partition adds the same constant to every path and the argmax is the same.
+ *   - alpha_0[0] = e_0[blank], alpha_0[1] = e_0[z_1], others -inf;
+ *     alpha_t[s] = fp32(max(alpha_{t-1}[s], alpha_{t-1}[s-1], alpha_{t-1}[s-2] if z_s != blank and z_s != z_{s-2})
+ *                       + e_t[z_s]) — one add, no FMA, no reassociation.
+ *   - ties: predecessors are taken in the order s, s-1, s-2, and a later one replaces the current one only if it is
+ *     strictly greater.  The end state is S-1 unless alpha_{T-1}[S-2] > alpha_{T-1}[S-1].
+ *   - path[b][t] = z of the state the path occupies at frame t (a label, or N-1 for blank); state[b][t] (nullable) = s.
+ *   - every sample runs over the full padded T, like every criterion call here.  An empty target gives all blanks.
+ *   - a target that needs more frames than T (L_b + adjacent repeats > T), or that holds a label outside [0, N-1),
+ *     gives path = state = -1 for the whole utterance (the loss would truncate it; an alignment that drops words is
+ *     worse than none).
+ * Limits: those of the CTC loss, min(L, T) <= 1023 (S <= 2047), any N >= 2; W2L_ERR_UNSUPPORTED beyond.  target may be
+ * NULL when L = 0.  The workspace holds the gathered scores [B][T][Sp] (Sp = 32 P >= S) and 2-bit backpointers.
+ * ---------------------------------------------------------------------------------------- */
+W2L_API size_t w2l_ctc_viterbi_workspace_size(int B, int T, int N, int L);
+W2L_API int w2l_ctc_viterbi_target(void* stream, int B, int T, int N, int L, const float* emis, const int32_t* target,
+                                   int32_t* path, int32_t* state, void* workspace, size_t workspace_bytes);
+
 /* LinearSegmentationCriterion's target stretch (Train.cpp:589-617, --linseg): out[b][t] =
  * target[b][floor(t * L_b / T)]; LinSeg = w2l_asg_forward_backward(W2L_TERM_ASG, L = T) on it (loss FCC - FAC). */
 W2L_API int w2l_linseg_target(void* stream, int B, int T, int L, const int32_t* target, int32_t* out);
@@ -341,6 +366,14 @@ W2L_API int w2l_trainer_step(void* trainer, void* stream, int B, int T, const fl
                              float* loss_out, int train, float total_batch);
 W2L_API int w2l_trainer_forward(void* trainer, void* stream, int B, int T, const float* features, float* emissions_out,
                                 long long capacity, int* t_out);
+/* Forced alignment: the eval-mode network forward of w2l_trainer_forward, then the criterion's viterbiPathWithTarget on
+ * its emissions.  path / idx: device int32 [B][T'] (capacity elements each; idx nullable), T' through t_out.  CTC:
+ * w2l_ctc_viterbi_target, idx = extended-target state.  ASG / LinSeg: w2l_fac_viterbi with the criterion's transitions,
+ * idx = target position.  A target that cannot be aligned gives -1 over its whole row. */
+W2L_API int w2l_trainer_align(void* trainer, void* stream, int B, int T, const float* features, int L, const int32_t* target,
+                              int32_t* path, int32_t* idx, long long capacity, int* t_out);
+/* input frames per output frame: the product of the time strides of the network's convolutions */
+W2L_API int w2l_trainer_time_stride(void* trainer);
 /* 1 (default): the backward pass computes the Linear layers' weight and bias gradients on a second stream of the
  * trainer, beside the data-gradient chain; 0: everything on the caller's stream.  Results are bit-identical either way. */
 W2L_API int w2l_trainer_set_grad_stream(void* trainer, int on);
@@ -390,6 +423,18 @@ W2L_API long long w2l_text_encode(void* text, const char* transcript, int32_t* o
 W2L_API long long w2l_text_prediction2ltr(void* text, const int32_t* path, int n, char* out, long long cap);
 W2L_API long long w2l_text_target2ltr(void* text, const int32_t* target, int len, char* out, long long cap);
 W2L_API long long w2l_text_ltr2wrd(void* text, const char* letters, char* out, long long cap);
+/* Word timings of one aligned utterance (host pointers): target[len] (-1 padded) and idx[n_frames] from
+ * w2l_trainer_align (CTC: extended-target state, ASG: target position).  Writes one `.align` line without its newline,
+ * NUL-terminated (returns the bytes needed, terminator included; -1 on error):
+ *   utt_id TAB seg \n seg \n ... (segments joined by the two characters backslash, n)
+ * with seg = "utt_id 1 <begin s> <duration s> <word>", a silence segment having the word "$".  A target position
+ * belongs to a word or to silence: the word separator and --surround tokens are silence and end the word, a token that
+ * starts with the word separator (word pieces) starts a word, a replabel belongs to the token before it.  A word runs
+ * from the first to the last frame whose state maps into it (CTC blanks inside it included); the frames before, between
+ * and after words are "$" segments, and the line always starts with one (of zero duration when the first word starts
+ * at frame 0).  Time = frame * ms_per_frame / 1000.  An idx of -1 (no alignment) is an error. */
+W2L_API long long w2l_text_align_words(void* text, const int32_t* target, int len, const int32_t* idx, int n_frames,
+                                       double ms_per_frame, const char* utt_id, char* out, long long cap);
 /* out4 += {reference length, deletions, insertions, substitutions} of one (hypothesis, reference) pair */
 W2L_API int w2l_edit_distance(const char* hyp, const char* ref, long long* out4);
 

@@ -16,6 +16,7 @@ from .capi import (  # noqa: F401
     argmax_path,
     asg_forward_backward,
     ctc_forward_backward,
+    ctc_viterbi_target,
     fac_viterbi,
     fcc_viterbi,
     launch_count,

@@ -24,17 +24,18 @@ EXPORTS = [
     "w2l_fcc_viterbi_workspace_size", "w2l_fcc_viterbi",
     "w2l_fac_viterbi_workspace_size", "w2l_fac_viterbi",
     "w2l_ctc_workspace_size", "w2l_ctc_forward_backward", "w2l_argmax_path", "w2l_linseg_target",
+    "w2l_ctc_viterbi_workspace_size", "w2l_ctc_viterbi_target",
     "w2l_set_precision", "w2l_get_precision", "w2l_gemm", "w2l_cast_bf16", "w2l_cast_bf16_rows", "w2l_sgd_step_ex", "w2l_finite_guard",
     "w2l_mask_bands", "w2l_trainer_set_precision", "w2l_trainer_set_grad_stream", "w2l_trainer_set_grad_stream_delay", "w2l_delay", "w2l_trainer_status", "w2l_trainer_save", "w2l_trainer_load", "w2l_trainer_export_streaming",
     "w2l_text_create", "w2l_text_destroy", "w2l_text_num_classes", "w2l_text_encode", "w2l_text_prediction2ltr", "w2l_text_target2ltr",
-    "w2l_text_ltr2wrd", "w2l_edit_distance",
+    "w2l_text_ltr2wrd", "w2l_text_align_words", "w2l_edit_distance",
     "w2l_gemm_set_variant", "w2l_gemm_set_tile", "w2l_gemm_tf32", "w2l_gemm_tf32_ex", "w2l_gemm_tf32_view", "w2l_conv_set_path", "w2l_conv_time_workspace_size", "w2l_conv_time_fwd", "w2l_conv_time_dgrad",
     "w2l_conv_time_wgrad", "w2l_layernorm_fwd", "w2l_layernorm_bwd", "w2l_colsum_accumulate", "w2l_sq_norm_accumulate",
     "w2l_sgd_step", "w2l_weightnorm_fwd", "w2l_weightnorm_bwd", "w2l_conv1d_arrange", "w2l_conv1d_arrange_ex", "w2l_conv1d_unarrange_grad",
     "w2l_glu_fwd", "w2l_glu_bwd", "w2l_transpose_input", "w2l_axpy", "w2l_fill", "w2l_act_fwd", "w2l_mask_mul",
     "w2l_trainer_create", "w2l_trainer_destroy", "w2l_trainer_step", "w2l_trainer_forward", "w2l_trainer_num_params",
     "w2l_trainer_param_layout", "w2l_trainer_get_flat", "w2l_trainer_set_flat", "w2l_trainer_sync_parameters",
-    "w2l_trainer_describe", "w2l_nccl_unique_id", "w2l_init_distributed",
+    "w2l_trainer_describe", "w2l_nccl_unique_id", "w2l_init_distributed", "w2l_trainer_align", "w2l_trainer_time_stride",
     "w2l_mfsc_num_frames", "w2l_mfsc_workspace_size", "w2l_mfsc",
 ]
 
@@ -75,6 +76,9 @@ def _load() -> ctypes.CDLL:
     lib.w2l_ctc_forward_backward.argtypes = [vp, i, i, i, i, i, vp, vp, vp, vp, vp, vp, sz]
     lib.w2l_argmax_path.argtypes = [vp, i, i, i, vp, vp]
     lib.w2l_linseg_target.argtypes = [vp, i, i, i, vp, vp]
+    lib.w2l_ctc_viterbi_workspace_size.restype = sz
+    lib.w2l_ctc_viterbi_workspace_size.argtypes = [i, i, i, i]
+    lib.w2l_ctc_viterbi_target.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, vp, sz]
     lib.w2l_gemm_tf32.argtypes = [vp, i, i, i, i, i, vp, i, vp, i, vp, i, vp, i]
     f32, u64, ll = ctypes.c_float, ctypes.c_ulonglong, ctypes.c_longlong
     ll = ctypes.c_longlong
@@ -127,6 +131,8 @@ def _load() -> ctypes.CDLL:
     lib.w2l_text_prediction2ltr.argtypes = [vp, vp, i, vp, ll]
     lib.w2l_text_target2ltr.argtypes = [vp, vp, i, vp, ll]
     lib.w2l_text_ltr2wrd.argtypes = [vp, cp, vp, ll]
+    lib.w2l_text_align_words.restype = ll
+    lib.w2l_text_align_words.argtypes = [vp, vp, i, vp, i, ctypes.c_double, cp, vp, ll]
     lib.w2l_edit_distance.argtypes = [cp, cp, vp]
     lib.w2l_trainer_create.restype = vp
     lib.w2l_trainer_create.argtypes = [vp, ctypes.c_char_p, i, i, ctypes.c_char_p, i, f32, f32, f32, f32, f32]
@@ -134,6 +140,8 @@ def _load() -> ctypes.CDLL:
     lib.w2l_trainer_destroy.restype = None
     lib.w2l_trainer_step.argtypes = [vp, vp, i, i, vp, i, vp, vp, i, f32]
     lib.w2l_trainer_forward.argtypes = [vp, vp, i, i, vp, vp, ll, vp]
+    lib.w2l_trainer_align.argtypes = [vp, vp, i, i, vp, i, vp, vp, vp, ll, vp]
+    lib.w2l_trainer_time_stride.argtypes = [vp]
     lib.w2l_trainer_num_params.restype = ll
     lib.w2l_trainer_num_params.argtypes = [vp, i]
     lib.w2l_trainer_param_layout.argtypes = [vp, i, i, vp, vp]
@@ -284,6 +292,21 @@ def argmax_path(emis):
     path = torch.empty((B, T), dtype=torch.int32, device=emis.device)
     _check(lib.w2l_argmax_path(_stream(), B, T, N, _ptr(emis), _ptr(path)))
     return path
+
+
+def ctc_viterbi_target(emis, target, return_state=False):
+    """CTC forced alignment on raw activations (blank = N-1): path [B,T] int32 (label or blank per frame, -1 for a
+    target that cannot be aligned) and, with return_state, the extended-target state per frame."""
+    emis = _req(emis, torch.float32, "emis")
+    target = _req(target, torch.int32, "target")
+    B, T, N = emis.shape
+    L = target.shape[1]
+    path = torch.empty((B, T), dtype=torch.int32, device=emis.device)
+    state = torch.empty((B, T), dtype=torch.int32, device=emis.device) if return_state else None
+    ws = workspace(lib.w2l_ctc_viterbi_workspace_size(B, T, N, L), emis.device)
+    _check(lib.w2l_ctc_viterbi_target(_stream(), B, T, N, L, _ptr(emis), _ptr(target), _ptr(path), _ptr(state), _ptr(ws),
+                                      ws.numel()))
+    return (path, state) if return_state else path
 
 
 def linseg_target(target, T: int):

@@ -1712,6 +1712,30 @@ af::array AutoSegmentationCriterion::viterbiPath(const af::array& input, const a
   return path;
 }
 
+af::array SequenceCriterion::viterbiPathWithTarget(const af::array&, const af::array&, af::array*) {
+  throw std::logic_error(prettyString() + ": viterbiPathWithTarget is not implemented");
+}
+
+namespace {
+// ASG and LinSeg: the forced alignment of ForceAlignmentCriterion (w2l_fac_viterbi) under the criterion's transitions
+af::array facAlign(int N, const Variable& trans, const af::array& input, const af::array& target, af::array* index) {
+  const int T = (int)input.dims(1), B = (int)input.dims(2), L = (int)target.dims(0);
+  if (input.dims(0) != N) throw std::invalid_argument("viterbiPathWithTarget: class count mismatch");
+  if (target.type() != DType::i32 || target.dims(1) != B) throw std::invalid_argument("viterbiPathWithTarget: target must be s32 [L,B]");
+  af::array path = af::array::empty(af::dim4(T, B), DType::i32);
+  af::array idx = index ? af::array::empty(af::dim4(T, B), DType::i32) : af::array();
+  af::array ws = af::array::empty(af::dim4((long long)std::max<size_t>(w2l_fac_viterbi_workspace_size(B, T, N, L), 256)), DType::u8);
+  check(w2l_fac_viterbi(currentStream(), B, T, N, L, input.f32(), target.i32(), trans.array().f32(), path.i32(), index ? idx.i32() : nullptr,
+                        ws.ptr(), ws.bytes()));
+  if (index) *index = idx;
+  return path;
+}
+}  // namespace
+
+af::array AutoSegmentationCriterion::viterbiPathWithTarget(const af::array& input, const af::array& target, af::array* index) {
+  return facAlign(N_, params_[0], input, target, index);
+}
+
 ConnectionistTemporalClassificationCriterion::ConnectionistTemporalClassificationCriterion(CriterionScaleMode scalemode) : scaleMode_(scalemode) {}
 std::string ConnectionistTemporalClassificationCriterion::prettyString() const { return "ConnectionistTemporalClassificationCriterion"; }
 std::vector<Variable> ConnectionistTemporalClassificationCriterion::forward(const std::vector<Variable>& inputs) {
@@ -1750,6 +1774,19 @@ af::array ConnectionistTemporalClassificationCriterion::viterbiPath(const af::ar
   return path;
 }
 
+af::array ConnectionistTemporalClassificationCriterion::viterbiPathWithTarget(const af::array& input, const af::array& target,
+                                                                             af::array* index) {
+  const int N = (int)input.dims(0), T = (int)input.dims(1), B = (int)input.dims(2), L = (int)target.dims(0);
+  if (target.type() != DType::i32 || target.dims(1) != B) throw std::invalid_argument("viterbiPathWithTarget: target must be s32 [L,B]");
+  af::array path = af::array::empty(af::dim4(T, B), DType::i32);
+  af::array state = index ? af::array::empty(af::dim4(T, B), DType::i32) : af::array();
+  af::array ws = workspaceFor(ws_, w2l_ctc_viterbi_workspace_size(B, T, N, L));
+  check(w2l_ctc_viterbi_target(currentStream(), B, T, N, L, input.f32(), target.i32(), path.i32(), index ? state.i32() : nullptr, ws.ptr(),
+                               ws.bytes()));
+  if (index) *index = state;
+  return path;
+}
+
 LinearSegmentationCriterion::LinearSegmentationCriterion(int N, CriterionScaleMode scalemode) : N_(N), scaleMode_(scalemode) {
   params_.push_back(Variable(af::array::zeros(af::dim4(N, N)), true));
 }
@@ -1769,6 +1806,10 @@ af::array LinearSegmentationCriterion::viterbiPath(const af::array& input, const
   af::array ws = af::array::empty(af::dim4((long long)std::max<size_t>(w2l_fcc_viterbi_workspace_size(B, T, N), 256)), DType::u8);
   check(w2l_fcc_viterbi(currentStream(), B, T, N, input.f32(), params_[0].array().f32(), path.i32(), ws.ptr(), ws.bytes()));
   return path;
+}
+
+af::array LinearSegmentationCriterion::viterbiPathWithTarget(const af::array& input, const af::array& target, af::array* index) {
+  return facAlign(N_, params_[0], input, target, index);
 }
 
 }  // namespace speech

@@ -5,6 +5,7 @@
 #include "fl_compat/text.h"
 
 #include <algorithm>
+#include <cstdio>
 #include <cstring>
 #include <fstream>
 #include <memory>
@@ -309,6 +310,75 @@ std::vector<std::string> tkn2Wrd(const std::vector<std::string>& input, const st
   return words;
 }
 
+std::string alignWords(const std::vector<int>& target, const std::vector<int>& frameIdx, bool ctcStates, const Dictionary& dict,
+                       const std::string& surround, int replabel, const std::string& wordSep, double msPerFrame, const std::string& uttId) {
+  // the word of every target position (-1: silence), following the target transform of targetFeatures: the word
+  // separator and surround tokens are silence and close the word, a token that starts with the separator (word pieces)
+  // opens one, a replabel repeats the token before it inside that token's word
+  std::unordered_map<int, int> repValue;
+  for (int r = 1; r <= replabel; ++r) repValue[dict.getIndex("<" + std::to_string(r) + ">")] = r;
+  const int n = (int)target.size();
+  std::vector<int> wordOf((size_t)n, -1);
+  std::vector<std::string> words;
+  bool open = false;
+  std::string prev;
+  for (int p = 0; p < n; ++p) {
+    const std::string tok = dict.getEntry(target[(size_t)p]);
+    auto rep = repValue.find(target[(size_t)p]);
+    if (rep != repValue.end()) {
+      wordOf[(size_t)p] = p > 0 ? wordOf[(size_t)p - 1] : -1;
+      if (wordOf[(size_t)p] >= 0)
+        for (int r = 0; r < rep->second; ++r) words[(size_t)wordOf[(size_t)p]] += prev;
+      continue;
+    }
+    if ((!surround.empty() && tok == surround) || (!wordSep.empty() && tok == wordSep)) {
+      open = false;
+    } else {
+      if (!open || (!wordSep.empty() && tok.compare(0, wordSep.size(), wordSep) == 0)) {
+        words.emplace_back();
+        open = true;
+      }
+      wordOf[(size_t)p] = (int)words.size() - 1;
+      words.back() += tok;
+    }
+    prev = tok;
+  }
+  // frames -> first / last frame of every word
+  const int frames = (int)frameIdx.size();
+  const int nIdx = ctcStates ? 2 * n + 1 : n;
+  std::vector<int> first(words.size(), -1), last(words.size(), -1);
+  for (int f = 0; f < frames; ++f) {
+    const int i = frameIdx[(size_t)f];
+    if (i < 0 || i >= nIdx) throw std::invalid_argument("alignWords: frame " + std::to_string(f) + " is not aligned to the target");
+    const int pos = ctcStates ? ((i & 1) ? i >> 1 : -1) : i;
+    if (pos >= 0 && wordOf[(size_t)pos] >= 0) {
+      const size_t w = (size_t)wordOf[(size_t)pos];
+      if (first[w] < 0) first[w] = f;
+      last[w] = f;
+    }
+  }
+  const int end = frames > 0 ? frameIdx[(size_t)frames - 1] : -1;
+  if (n > 0 && (ctcStates ? end < nIdx - 2 : end != n - 1)) throw std::invalid_argument("alignWords: the alignment does not reach the end of the target");
+  std::string line = uttId + "\t";
+  int cursor = 0, segs = 0;
+  auto seg = [&](int from, int to, const std::string& word) {
+    char buf[64];
+    std::snprintf(buf, sizeof(buf), " 1 %.3f %.3f ", from * msPerFrame / 1000.0, (to - from) * msPerFrame / 1000.0);
+    line += (segs++ ? "\\n" : "") + uttId + buf + word;
+  };
+  for (size_t w = 0; w < words.size(); ++w) {
+    if (first[w] < 0 || first[w] < cursor) throw std::invalid_argument("alignWords: word " + std::to_string(w) + " has no frames of its own");
+    if (w == 0 || first[w] > cursor) seg(cursor, first[w], "$");
+    std::string text = words[w];
+    if (!wordSep.empty())
+      for (size_t at; (at = text.find(wordSep)) != std::string::npos;) text.erase(at, wordSep.size());
+    seg(first[w], last[w] + 1, text);
+    cursor = last[w] + 1;
+  }
+  if (words.empty() || cursor < frames) seg(cursor, frames, "$");
+  return line;
+}
+
 }  // namespace speech
 }  // namespace pkg
 
@@ -459,6 +529,22 @@ W2L_API long long w2l_text_ltr2wrd(void* h, const char* letters, char* out, long
   return guardedText([&]() -> long long {
     auto* t = static_cast<TextPipeline*>(h);
     return putJoined(fl::pkg::speech::tkn2Wrd(splitSpace(letters), t->wordsep), out, cap);
+  });
+}
+// forced alignment of one utterance (target row, index per frame) -> its `.align` line
+W2L_API long long w2l_text_align_words(void* h, const int32_t* target, int len, const int32_t* idx, int n_frames, double ms_per_frame,
+                                       const char* utt_id, char* out, long long cap) {
+  return guardedText([&]() -> long long {
+    auto* t = static_cast<TextPipeline*>(h);
+    if (len < 0 || n_frames < 0 || (len > 0 && !target) || (n_frames > 0 && !idx) || !(ms_per_frame > 0))
+      throw std::invalid_argument("text_align_words: bad arguments");
+    const int n = fl::pkg::speech::getTargetSize(target, len);
+    const std::string line = fl::pkg::speech::alignWords(std::vector<int>(target, target + n), std::vector<int>(idx, idx + n_frames),
+                                                         t->criterion == fl::pkg::speech::kCtcCriterion, t->dict, t->surround, t->replabel,
+                                                         t->wordsep, ms_per_frame, utt_id ? utt_id : "");
+    const long long need = (long long)line.size() + 1;
+    if (out && cap >= need) std::memcpy(out, line.c_str(), (size_t)need);
+    return need;
   });
 }
 // EditDistanceMeter::add on one (hypothesis, reference) pair of space-joined token strings: out4 += {n, ndel, nins, nsub}

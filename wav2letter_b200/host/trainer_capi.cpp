@@ -135,6 +135,17 @@ void getArena(std::istream& i, const af::array& a, long long n, void* stream) {
       cudaStreamSynchronize(static_cast<cudaStream_t>(stream)) != cudaSuccess)
     throw std::runtime_error("checkpoint: upload failed");
 }
+// input frames per output frame: the time strides of the convolutions, through Sequential and WeightNorm containers
+int timeStride(const std::shared_ptr<fl::Module>& m) {
+  if (auto s = std::dynamic_pointer_cast<fl::Sequential>(m)) {
+    int r = 1;
+    for (const auto& c : s->modules()) r *= timeStride(c);
+    return r;
+  }
+  if (auto w = std::dynamic_pointer_cast<fl::WeightNorm>(m)) return timeStride(w->module());
+  if (auto c = std::dynamic_pointer_cast<fl::Conv2D>(m)) return c->stride;
+  return 1;
+}
 constexpr char kMagic[8] = {'W', '2', 'L', 'B', '2', '0', '0', '\0'};
 }  // namespace
 
@@ -336,6 +347,28 @@ W2L_API int w2l_trainer_forward(void* h, void* stream, int B, int T, const float
     if (t_out) *t_out = (int)(out.elements() / ((long long)B * t->nLabel));  // frames of nLabel values per sample
   });
 }
+
+// network forward (eval mode) + the criterion's forced alignment: path / idx device [T',B] (idx nullable)
+W2L_API int w2l_trainer_align(void* h, void* stream, int B, int T, const float* features, int L, const int32_t* target, int32_t* path,
+                              int32_t* idx, long long capacity, int* t_out) {
+  return guarded([&] {
+    w2l::setCurrentStream(stream);
+    auto* t = static_cast<Trainer*>(h);
+    if (B <= 0 || T <= 0 || L <= 0 || !features || !target || !path) throw std::invalid_argument("trainer_align: bad arguments");
+    PrecisionScope scope(t->precision);
+    t->net->eval();
+    Variable out = t->net->forward(std::vector<Variable>{fl::input(af::array::wrap(const_cast<float*>(features), af::dim4(T, t->nFeat, 1, B)))}).front();
+    const af::array tgt = af::array::wrap(const_cast<int32_t*>(target), af::dim4(L, B), w2l::DType::i32);
+    af::array index;
+    const af::array p = t->crit->viterbiPathWithTarget(out.array(), tgt, idx ? &index : nullptr);
+    if (p.elements() > capacity) throw std::invalid_argument("trainer_align: output buffer too small");
+    af::array::wrap(path, p.dims(), w2l::DType::i32).copyFrom(p);
+    if (idx) af::array::wrap(idx, index.dims(), w2l::DType::i32).copyFrom(index);
+    if (t_out) *t_out = (int)p.dims(0);
+  });
+}
+
+W2L_API int w2l_trainer_time_stride(void* h) { return timeStride(static_cast<Trainer*>(h)->net); }
 
 W2L_API int w2l_nccl_unique_id(void* out128) {
   return guarded([&] { fl::pkg::runtime::createUniqueId(out128); });

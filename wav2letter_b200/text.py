@@ -71,6 +71,18 @@ class TextPipeline:
         lib.w2l_text_ltr2wrd(self.h, s, buf, n)
         return buf.value.decode().split()
 
+    def align_words(self, target_row, idx, ms_per_frame: float, utt_id: str) -> str:
+        """one `.align` line (no newline) from a forced alignment: target_row the padded target, idx the aligned index of
+        every frame (Trainer.align; CTC: extended-target state, ASG: target position)"""
+        tgt = np.ascontiguousarray(target_row, dtype=np.int32)
+        ix = np.ascontiguousarray(idx, dtype=np.int32)
+        args = (self.h, tgt.ctypes.data_as(ctypes.c_void_p), tgt.size, ix.ctypes.data_as(ctypes.c_void_p), ix.size,
+                float(ms_per_frame), utt_id.encode())
+        n = self._need(lib.w2l_text_align_words(*args, None, 0))
+        buf = ctypes.create_string_buffer(n)
+        lib.w2l_text_align_words(*args, buf, n)
+        return buf.value.decode()
+
 
 class EditDistanceMeter:
     """fl::EditDistanceMeter: add(hypothesis tokens, reference tokens); value() = [error %, n, ins %, del %, sub %]"""

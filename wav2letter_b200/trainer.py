@@ -118,6 +118,26 @@ class Trainer:
         _check(lib.w2l_trainer_forward(self.h, _stream(), B, T, _ptr(features), _ptr(out), cap, ctypes.byref(tout)))
         return out[: B * tout.value * self.n_label].view(B, tout.value, self.n_label)
 
+    def align(self, features: torch.Tensor, target: torch.Tensor):
+        """Forced alignment: eval-mode forward, then the criterion's viterbiPathWithTarget.  features CUDA float
+        [B,1,F,T], target CUDA int32 [B,L] (-1 padded).  Returns (path, idx), CUDA int32 [B,T']: the token per output
+        frame and, for CTC, the extended-target state, for ASG, the target position (-1 over a row that cannot be
+        aligned)."""
+        B, _, F, T = features.shape
+        L = target.shape[1]
+        cap = B * (2 * T + 64)  # as in forward: SAME-padded even kernels grow the frame count by one each
+        path = torch.empty(cap, dtype=torch.int32, device=features.device)
+        idx = torch.empty(cap, dtype=torch.int32, device=features.device)
+        tout = ctypes.c_int(0)
+        _check(lib.w2l_trainer_align(self.h, _stream(), B, T, _ptr(features), L, _ptr(target), _ptr(path), _ptr(idx), cap,
+                                     ctypes.byref(tout)))
+        n = B * tout.value
+        return path[:n].view(B, tout.value), idx[:n].view(B, tout.value)
+
+    def time_stride(self) -> int:
+        """input frames per output frame (the product of the network's time strides)"""
+        return int(lib.w2l_trainer_time_stride(self.h))
+
     def sync_parameters(self):
         _check(lib.w2l_trainer_sync_parameters(self.h, _stream()))
 
