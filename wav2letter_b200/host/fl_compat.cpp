@@ -424,6 +424,7 @@ af::array workspaceFor(af::array& cache, size_t bytes) {
   return cache;
 }
 thread_local af::array g_conv_ws;
+thread_local af::array g_conv_grad_ws;  // time-convolution weight gradients on the gradient stream
 
 // ---- precision of the dense contractions (w2l_set_precision; DESIGN.md §4) ----------------------------------
 bool bf16Mode() { return w2l_get_precision() == W2L_PRECISION_BF16; }
@@ -572,21 +573,8 @@ Variable Conv2D::forwardWith(const Variable& in, const Variable& weight, const V
       check(w2l_mask_mul(currentStream(), y.elements(), dy.f32(), y.f32(), relu ? 1 : 2, dp > 0.f ? 1.0f / (1.0f - dp) : 1.0f, m.f32()));
       dy = m;
     }
-    af::array ws2 = workspaceFor(g_conv_ws, w2l_conv_time_workspace_size(B, Tout, cin, cout, k));
-    if (ins[1].isCalcGrad()) {
-      // accumulate straight into the gradient arena slots when the parameters are arena-backed
-      af::array dw = ins[1].gradStorage();
-      if (dw.isEmpty()) dw = af::array::zeros(ins[1].dims());
-      af::array db;
-      if (hasBias) {
-        db = ins[2].gradStorage();
-        if (db.isEmpty()) db = af::array::zeros(ins[2].dims());
-      }
-      check(w2l_conv_time_wgrad(currentStream(), B, T, Tout, W, cin, cout, k, s, pl, ins[0].array().f32(), dy.f32(), dw.f32(),
-                                hasBias ? db.f32() : nullptr, ws2.ptr(), ws2.bytes()));
-      ins[1].addGrad(Variable(dw, false));
-      if (hasBias) ins[2].addGrad(Variable(db, false));
-    }
+    const size_t wsb2 = w2l_conv_time_workspace_size(B, Tout, cin, cout, k);
+    af::array ws2 = workspaceFor(g_conv_ws, wsb2);
     if (ins[0].isCalcGrad()) {
       // a gradient already sitting on the input (the residual path of a TDS block) is summed in the kernel's epilogue
       af::array acc = ins[0].accumulableGrad();
@@ -594,6 +582,30 @@ Variable Conv2D::forwardWith(const Variable& in, const Variable& weight, const V
       check(w2l_conv_time_dgrad(currentStream(), B, T, Tout, W, cin, cout, k, s, pl, dy.f32(), ins[1].array().f32(),
                                 acc.isEmpty() ? nullptr : acc.f32(), dx.f32(), ws2.ptr(), ws2.bytes()));
       if (acc.isEmpty()) ins[0].addGrad(Variable(dx, false), true);
+    }
+    if (ins[1].isCalcGrad()) {
+      // accumulate straight into the gradient arena slots when the parameters are arena-backed; such gradients are read
+      // by nothing before the optimizer, so they are computed on the gradient stream (when the trainer has one), beside
+      // the data-gradient chain.  Their CTA partials then go to a workspace of their own: the next convolutions on the
+      // compute stream reuse g_conv_ws while the gradient stream may still be reading it.
+      af::array dw = ins[1].gradStorage();
+      af::array db = hasBias ? ins[2].gradStorage() : af::array();
+      void* wstream = currentStream();
+      af::array wws = ws2;
+      if (gradStream() && !dw.isEmpty() && (!hasBias || !db.isEmpty())) {
+        wstream = gradStream();
+        wws = workspaceFor(g_conv_grad_ws, wsb2);
+        readOnGradStream(wws);
+        readOnGradStream(dy);
+        readOnGradStream(ins[0].array());
+        forkGradStream();
+      }
+      if (dw.isEmpty()) dw = af::array::zeros(ins[1].dims());
+      if (hasBias && db.isEmpty()) db = af::array::zeros(ins[2].dims());
+      check(w2l_conv_time_wgrad(wstream, B, T, Tout, W, cin, cout, k, s, pl, ins[0].array().f32(), dy.f32(), dw.f32(),
+                                hasBias ? db.f32() : nullptr, wws.ptr(), wws.bytes()));
+      ins[1].addGrad(Variable(dw, false));
+      if (hasBias) ins[2].addGrad(Variable(db, false));
     }
   });
 }
