@@ -193,7 +193,8 @@ W2L_API int w2l_gemm_tf32_view(void* stream, int a_mn_major, int b_mn_major, int
  *           for fp32 tensors on Ampere+; the default.
  *   F32X3 : fp32 operands in HBM, fp32-ACCURATE contraction: each staged tile is split hi/lo in shared memory and the
  *           tensor core accumulates Al*Bh + Ah*Bl + Ah*Bh (error-compensated 3xTF32, products good to ~2^-21) — the
- *           precision BASELINE.json configs[1] ("fp32") states; the time convolutions use the fp32 SIMT kernels.
+ *           precision BASELINE.json configs[1] ("fp32") states; the time convolutions run their mma.sync kernels in
+ *           3xTF32 the same way.
  *   BF16  : bf16 operands in HBM (activations / weights cast by their producers), fp32 accumulation — the AMP mode of
  *           the reference (recipes/slimIPL/src/Train.cpp:211-219) with bf16 instead of fp16, configs[2]/[3].
  * w2l_set_precision is thread-local and selects the kind used by the fp32-operand entry points (w2l_gemm_tf32*,
@@ -240,13 +241,12 @@ W2L_API int w2l_gemm_tf32_ex(void* stream, int a_mn_major, int b_mn_major, int M
  *   dgrad : dx = conv^T(dy) (+ add)                           add may be dx itself (in-place accumulation;
  *                                                            likewise add == y in fwd)
  *   wgrad : dwt += ..., dbias += ...  (deterministic two-stage reduction)
+ * The shape alone selects the kernels: where W % 8 == 0, stride <= kw and kw * max(Cin, Cout) <= 512 (for a strided
+ * data gradient, ceil(kw / stride) taps per phase), the mma.sync tensor-core kernels (TF32 products, 3xTF32 under
+ * W2L_PRECISION_F32); otherwise the fp32 SIMT kernels.
  * The workspace size call covers all three.
  * ---------------------------------------------------------------------------------------- */
 W2L_API size_t w2l_conv_time_workspace_size(int B, int Tout, int Cin, int Cout, int K);
-/* 0 (default): the mma.sync tensor-core kernels where the shape allows (TF32, or 3xTF32 under W2L_PRECISION_F32); 1: always the
- * fp32 SIMT kernels (the fallback for widths that are not multiples of 8); 2: mma.sync; 3: the wgmma / TMA kernel of
- * conv_wgmma.cu for forward and stride-1 data gradients (parity-green, opt-in: see DESIGN.md).  Thread-local. */
-W2L_API int w2l_conv_set_path(int path);
 W2L_API int w2l_conv_time_fwd(void* stream, int B, int T, int Tout, int W, int Cin, int Cout, int K, int stride,
                               int pad_left, const float* x, const float* wt, const float* bias, const float* add, float* y,
                               int act, float dropout_p, unsigned long long seed, void* ws, size_t ws_bytes);

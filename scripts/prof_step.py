@@ -17,7 +17,7 @@ import bench  # noqa: E402
 from wav2letter_b200 import capi  # noqa: E402
 from wav2letter_b200.trainer import Trainer  # noqa: E402
 
-CONV_PREFIXES = ("conv_mma_", "conv_time_", "conv_wgrad_", "conv_arrange_", "conv_wgmma_")
+CONV_PREFIXES = ("conv_mma_", "conv_time_", "conv_wgrad_", "conv_arrange_")
 
 
 def card():

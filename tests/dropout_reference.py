@@ -8,7 +8,6 @@ are flat indices into the tensor the kernel writes ([B][T][C][W] for the time co
   simt_scale        dropout_scale (common.cuh): SIMT conv forward, w2l_act_fwd, GLU scalar path
   conv_mma_scale    mma.sync conv forward (TF32 and 3xTF32): the same bits, rebuilt by lane pairs
   glu_vec_scale     GLU float4 path (keep4): the same bits, one Philox block per 4 channels
-  conv_wgmma_scale  wgmma conv forward: one Philox block per (b, frame, column, 8 channels), 16 bits per element
   gemm_scale        GEMM epilogue: one 32-bit murmur3-style hash per pair of columns, 16 bits per element
 """
 import numpy as np
@@ -66,7 +65,7 @@ def _keep24(v, p):
 
 
 def thresh16(p):
-    """the 16-bit threshold uint32(float32(p) * 65536) of the wgmma conv and GEMM masks"""
+    """the 16-bit threshold uint32(float32(p) * 65536) of the GEMM mask"""
     return np.uint32(int(np.float32(p) * np.float32(65536.0)))
 
 
@@ -104,20 +103,6 @@ def glu_vec_scale(seed, e, p, H):
     k0, k1 = _key(seed)
     r = philox4x32_10(q & MASK32, (np.uint64(4) * q) >> np.uint64(34), 0, 0, k0, k1)
     return _scale(_keep24(_word(r, e - np.uint64(4) * q), p), p)
-
-
-def conv_wgmma_scale(seed, e, p, C, W):
-    """wgmma conv epilogue, y [B][T][C][W]: element (b, t, c, w) draws block counter (i0, i0 >> 32) with
-    i0 = the element index of channel 8 (c // 8) at (b, t, w); word (c % 8) // 2, 16-bit half c % 2; keep iff the
-    16 bits >= uint32(float32(p) * 65536)"""
-    e = _u64(e)
-    c = (e // np.uint64(W)) % np.uint64(C)
-    i0 = e - (c % np.uint64(8)) * np.uint64(W)
-    k0, k1 = _key(seed)
-    r = philox4x32_10(i0 & MASK32, i0 >> np.uint64(32), 0, 0, k0, k1)
-    v = _word(r, (c % np.uint64(8)) // np.uint64(2)).astype(np.uint64)
-    bits = (v >> (np.uint64(16) * (c % np.uint64(2)))) & np.uint64(0xFFFF)
-    return _scale(bits >= np.uint64(thresh16(p)), p)
 
 
 def gemm_scale(seed, e, p):

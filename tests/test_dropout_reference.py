@@ -18,11 +18,9 @@ MODELS = {
     "simt": lambda s, e, p: R.simt_scale(s, e, p),
     "conv_mma": lambda s, e, p: R.conv_mma_scale(s, e, p, W),
     "glu_vec": lambda s, e, p: R.glu_vec_scale(s, e, p, W),
-    "conv_wgmma": lambda s, e, p: R.conv_wgmma_scale(s, e, p, C, W),
     "gemm": lambda s, e, p: R.gemm_scale(s, e, p),  # C [B*T*C rows][W columns]
 }
-BASE_MODEL = {"simt": R.simt_scale, "conv_mma": R.conv_mma_scale, "glu_vec": R.glu_vec_scale, "conv_wgmma": R.conv_wgmma_scale,
-              "gemm": R.gemm_scale}
+BASE_MODEL = {"simt": R.simt_scale, "conv_mma": R.conv_mma_scale, "glu_vec": R.glu_vec_scale, "gemm": R.gemm_scale}
 SEED = R.host_seed(3)
 
 

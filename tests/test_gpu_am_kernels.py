@@ -154,18 +154,18 @@ def test_colsum_sqnorm_sgd():
     assert rel(v, ve) < 1e-5 and rel(p, p0 - lr * ve) < 1e-5
 
 
-@pytest.mark.parametrize("path", ["tf32", "mma", "x3", "simt"])
+@pytest.mark.parametrize("path", ["mma", "x3", "simt"])
 @pytest.mark.parametrize("B,T,Cin,Cout,K,stride,pl,pr", [
     (2, 40, 23, 23, 11, 1, 10, 0), (2, 40, 15, 15, 9, 1, 7, 1), (2, 46, 19, 23, 12, 2, 9, 1), (2, 40, 23, 27, 11, 1, 10, 0),
     (2, 52, 1, 15, 10, 2, 5, 3), (2, 36, 27, 27, 11, 1, 10, 0), (1, 24, 18, 18, 21, 1, 10, 10),
 ])
 def test_conv_time_streaming_shapes_all_paths(B, T, Cin, Cout, K, stride, pl, pr, path):
     """the asymmetric paddings of the streaming TDS arch (PD l r + C2, TDS with rightPadding) on the three arithmetic paths:
-    the wgmma / TMA kernel (forward, stride-1 data gradient), the mma.sync TF32 kernels, the same in error-compensated
-    3xTF32 (W2L_PRECISION_F32), and the fp32 SIMT fallback"""
+    the mma.sync TF32 kernels, the same in error-compensated 3xTF32 (W2L_PRECISION_F32), both at W = 80, and the fp32
+    SIMT kernels, which a width that is not a multiple of 8 selects"""
     from wav2letter_b200 import capi
 
-    W = 80
+    W = 76 if path == "simt" else 80
     g = torch.Generator(device="cuda").manual_seed(T * 7 + Cin)
     x = torch.randn((B, T, Cin, W), device="cuda", generator=g)
     wt = torch.randn((Cout, Cin, K), device="cuda", generator=g) * 0.1
@@ -175,25 +175,33 @@ def test_conv_time_streaming_shapes_all_paths(B, T, Cin, Cout, K, stride, pl, pr
     pre = ref_conv(x64, w64, b64, stride, pl, Tout)
     dy = torch.randn((B, Tout, Cout, W), device="cuda", generator=g)
     pre.backward(dy.double())
+    out = {}
+
+    def run():
+        out["y"] = capi.conv_time_fwd(x, wt, bias, Tout, stride, pl)
+        out["dx"] = capi.conv_time_dgrad(dy, wt, T, stride, pl)
+        out["dwt"], out["dbias"] = capi.conv_time_wgrad(x, dy, K, stride, pl)
+
     try:
         capi.set_precision("f32" if path == "x3" else "tf32")
-        capi._check(capi.lib.w2l_conv_set_path({"simt": 1, "mma": 2, "tf32": 3}.get(path, 0)))  # "tf32" = the wgmma kernel
-        y = capi.conv_time_fwd(x, wt, bias, Tout, stride, pl)
-        dx = capi.conv_time_dgrad(dy, wt, T, stride, pl)
-        dwt, dbias = capi.conv_time_wgrad(x, dy, K, stride, pl)
+        ran = capi.trace(run)
     finally:
         capi.set_precision("tf32")
-        capi._check(capi.lib.w2l_conv_set_path(0))
-    tol = 3e-3 if path in ("tf32", "mma") else 2e-5
+    y, dx, dwt, dbias = out["y"], out["dx"], out["dwt"], out["dbias"]
+    if path == "simt":
+        assert not any(k.startswith("conv_mma_") for k in ran), ran
+    else:
+        assert {"conv_mma_fwd_kernel", "conv_mma_wgrad_kernel"} <= set(ran), ran
+    tol = 3e-3 if path == "mma" else 2e-5
     assert rel(y, pre) < tol, (path, rel(y, pre))
     assert rel(dx, x64.grad) < tol, (path, rel(dx, x64.grad))
     assert rel(dwt, w64.grad) < tol, (path, rel(dwt, w64.grad))
     assert rel(dbias, b64.grad) < tol
 
 
-def test_conv_time_wgmma_path_falls_back_when_the_window_does_not_fit():
-    """w2l_conv_set_path(3) selects the wgmma kernel only where its window and weights fit in shared memory: at 32 channels
-    and kw = 27 they do not (and the mma.sync kernel does not cover kw * C > 512), so the call runs on the SIMT kernels"""
+def test_conv_time_runs_simt_when_the_window_exceeds_the_mma_kernels():
+    """the mma.sync kernels cover kw * C <= 512: at 32 channels and kw = 27 the forward and the data gradient run on the
+    fp32 SIMT kernels in either precision (the SIMT weight gradient's register tiles do not cover this filter)"""
     from wav2letter_b200 import capi
 
     B, T, C, K, pl, W = 1, 40, 32, 27, 13, 80
@@ -206,10 +214,14 @@ def test_conv_time_wgmma_path_falls_back_when_the_window_does_not_fit():
     pre = ref_conv(x64, w64, b64, 1, pl, Tout)
     dy = torch.randn((B, Tout, C, W), device="cuda", generator=g)
     pre.backward(dy.double())
-    try:
-        capi._check(capi.lib.w2l_conv_set_path(3))
-        y = capi.conv_time_fwd(x, wt, bias, Tout, 1, pl)
-        dx = capi.conv_time_dgrad(dy, wt, T, 1, pl)
-    finally:
-        capi._check(capi.lib.w2l_conv_set_path(0))
-    assert rel(y, pre) < 3e-3 and rel(dx, x64.grad) < 3e-3
+    for precision in ("tf32", "f32"):
+        out = {}
+        try:
+            capi.set_precision(precision)
+            ran_fwd = capi.trace(lambda: out.setdefault("y", capi.conv_time_fwd(x, wt, bias, Tout, 1, pl)))
+            ran_dgrad = capi.trace(lambda: out.setdefault("dx", capi.conv_time_dgrad(dy, wt, T, 1, pl)))
+        finally:
+            capi.set_precision("tf32")
+        assert "conv_time_fwd_kernel" in ran_fwd and "conv_time_fwd_kernel(dgrad)" in ran_dgrad, (precision, ran_fwd, ran_dgrad)
+        assert not any(k.startswith("conv_mma_") for k in {**ran_fwd, **ran_dgrad}), precision
+        assert rel(out["y"], pre) < 2e-5 and rel(out["dx"], x64.grad) < 2e-5, precision

@@ -9,7 +9,7 @@ compared across implementations.  tests/test_gpu_dropout.py checks every dropout
 models of tests/dropout_reference.py (whose statistics tests/test_dropout_reference.py checks), the backward passes'
 use of the forward mask, and w2l_mask_bands against NumPy.
 
-Tolerances.  precision "f32" (fp32-accurate contractions: 3xTF32 split GEMMs, fp32 SIMT time convolutions):
+Tolerances.  precision "f32" (fp32-accurate contractions: 3xTF32 split GEMMs and time convolutions):
 emissions 2e-4 of the largest emission, per-sample loss 2e-4 (both ~2e-5 / 1e-6 measured), all gradients together within
 1e-2 of the largest entry, and every single parameter's gradient within 5e-2 RELATIVE L2 error (floor: 1e-2 of the net's
 largest entry) OR within 8x of the error stock fp32 torch (TF32 off) makes on that same parameter against float64.  Two fp32 effects set that floor: the

@@ -55,15 +55,16 @@ def kernels_run(fn):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# time convolution forward: SIMT (path 1), mma.sync TF32 (2) and 3xTF32 (2 under W2L_PRECISION_F32), wgmma (3)
+# time convolution forward: SIMT (W % 8 != 0), mma.sync TF32 and 3xTF32 (W2L_PRECISION_F32)
 # ---------------------------------------------------------------------------------------------------------------------
-CONV_KERNEL = {"simt": "conv_time_fwd_kernel", "mma": "conv_mma_fwd_kernel", "x3": "conv_mma_fwd_kernel", "wgmma": "conv_wgmma_fwd_kernel"}
+CONV_KERNEL = {"simt": "conv_time_fwd_kernel", "mma": "conv_mma_fwd_kernel", "x3": "conv_mma_fwd_kernel"}
 CONV_CASES = [  # path, B, T, Cin, Cout, K, stride, W
-    ("simt", 2, 23, 5, 7, 3, 1, 20), ("simt", 3, 30, 4, 13, 5, 2, 36), ("simt", 2, 19, 6, 27, 3, 1, 80),
+    ("simt", 2, 23, 5, 7, 3, 1, 20), ("simt", 3, 30, 4, 13, 5, 2, 36), ("simt", 2, 19, 6, 27, 3, 1, 76),
     ("mma", 2, 21, 5, 7, 3, 1, 8), ("mma", 2, 26, 6, 13, 5, 2, 16), ("mma", 3, 19, 4, 9, 3, 1, 24), ("mma", 2, 20, 5, 27, 3, 1, 32),
     ("mma", 2, 33, 7, 17, 5, 2, 40), ("mma", 2, 30, 10, 10, 5, 1, 80),
     ("x3", 2, 21, 5, 13, 3, 1, 24), ("x3", 2, 30, 6, 27, 5, 2, 80),
-    ("wgmma", 2, 23, 5, 5, 3, 1, 20), ("wgmma", 2, 30, 10, 13, 5, 1, 80), ("wgmma", 3, 27, 6, 27, 3, 2, 40), ("wgmma", 2, 18, 8, 16, 3, 1, 8),
+    ("mma", 2, 35, 9, 18, 5, 1, 8), ("mma", 2, 35, 9, 18, 5, 2, 24), ("mma", 2, 35, 9, 18, 5, 1, 40), ("mma", 2, 35, 9, 18, 5, 2, 80),
+    ("x3", 2, 35, 9, 18, 5, 1, 8), ("x3", 2, 35, 9, 18, 5, 2, 24), ("x3", 2, 35, 9, 18, 5, 1, 40), ("x3", 2, 35, 9, 18, 5, 2, 80),
 ]
 
 
@@ -71,13 +72,11 @@ def run_conv(path, *args, **kw):
     c = capi()
     try:
         c.set_precision("f32" if path == "x3" else "tf32")
-        c._check(c.lib.w2l_conv_set_path({"simt": 1, "mma": 2, "x3": 2, "wgmma": 3}[path]))
         out = {}
         ran = kernels_run(lambda: out.setdefault("y", c.conv_time_fwd(*args, **kw)))
         return out["y"], ran
     finally:
         c.set_precision("tf32")
-        c._check(c.lib.w2l_conv_set_path(0))
 
 
 @pytest.mark.parametrize("path,B,T,Cin,Cout,K,stride,W", CONV_CASES)
@@ -90,8 +89,7 @@ def test_conv_time_fwd_dropout_matches_model(path, B, T, Cin, Cout, K, stride, W
     Tout = (T + 2 * pl - K) // stride + 1
     pre = ref_conv64(x, wt, bias, stride, pl, Tout).float()  # exact integers
     add = ints((B, Tout, Cout, W), -8, 8, g)
-    fn, kw = {"simt": (R.simt_scale, {}), "mma": (R.conv_mma_scale, dict(W=W)), "x3": (R.conv_mma_scale, dict(W=W)),
-              "wgmma": (R.conv_wgmma_scale, dict(C=Cout, W=W))}[path]
+    fn, kw = {"simt": (R.simt_scale, {}), "mma": (R.conv_mma_scale, dict(W=W)), "x3": (R.conv_mma_scale, dict(W=W))}[path]
     seed = R.host_seed(W + Cout)
     for act, p, residual in ((0, 0.2, False), (1, P_ODD, False), (0, 0.5, True), (1, 0.75, True)):
         y, ran = run_conv(path, x, wt, bias, Tout, stride, pl, act=act, dropout_p=p, seed=seed, add=add if residual else None)
@@ -104,20 +102,6 @@ def test_conv_time_fwd_dropout_matches_model(path, B, T, Cin, Cout, K, stride, W
         assert torch.equal(y, y2)
     y3, _ = run_conv(path, x, wt, bias, Tout, stride, pl, act=1, dropout_p=0.75, seed=seed + 1, add=add)
     assert not torch.equal(y, y3)
-
-
-@pytest.mark.parametrize("W,stride", [(8, 1), (24, 2), (40, 1), (80, 2)])
-def test_conv_time_fwd_simt_and_mma_masks_agree(W, stride):
-    """the mma.sync epilogue rebuilds dropout_scale's mask from lane-pair shuffles: same seed, same output as SIMT"""
-    g = torch.Generator(device="cuda").manual_seed(W)
-    B, T, Cin, Cout, K = 2, 35, 9, 18, 5
-    x = ints((B, T, Cin, W), -8, 8, g)
-    wt = ints((Cout, Cin, K), -1, 1, g)
-    bias = ints((Cout,), -3, 3, g)
-    Tout = (T + 4 - K) // stride + 1
-    ys = [run_conv(path, x, wt, bias, Tout, stride, 2, act=0, dropout_p=0.25, seed=0xD00D)[0] for path in ("simt", "mma", "x3")]
-    assert torch.equal(ys[0], ys[1]) and torch.equal(ys[0], ys[2])
-    assert float((ys[0] == 0).float().mean()) > 0.2
 
 
 # ---------------------------------------------------------------------------------------------------------------------

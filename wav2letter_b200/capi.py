@@ -29,7 +29,7 @@ EXPORTS = [
     "w2l_mask_bands", "w2l_trainer_set_precision", "w2l_trainer_set_grad_stream", "w2l_trainer_set_grad_stream_delay", "w2l_delay", "w2l_trainer_status", "w2l_trainer_save", "w2l_trainer_load", "w2l_trainer_export_streaming",
     "w2l_text_create", "w2l_text_destroy", "w2l_text_num_classes", "w2l_text_encode", "w2l_text_prediction2ltr", "w2l_text_target2ltr",
     "w2l_text_ltr2wrd", "w2l_text_align_words", "w2l_edit_distance",
-    "w2l_gemm_set_variant", "w2l_gemm_set_tile", "w2l_gemm_tf32", "w2l_gemm_tf32_ex", "w2l_gemm_tf32_view", "w2l_conv_set_path", "w2l_conv_time_workspace_size", "w2l_conv_time_fwd", "w2l_conv_time_dgrad",
+    "w2l_gemm_set_variant", "w2l_gemm_set_tile", "w2l_gemm_tf32", "w2l_gemm_tf32_ex", "w2l_gemm_tf32_view", "w2l_conv_time_workspace_size", "w2l_conv_time_fwd", "w2l_conv_time_dgrad",
     "w2l_conv_time_wgrad", "w2l_layernorm_fwd", "w2l_layernorm_bwd", "w2l_colsum_accumulate", "w2l_sq_norm_accumulate",
     "w2l_sgd_step", "w2l_weightnorm_fwd", "w2l_weightnorm_bwd", "w2l_conv1d_arrange", "w2l_conv1d_arrange_ex", "w2l_conv1d_unarrange_grad",
     "w2l_glu_fwd", "w2l_glu_bwd", "w2l_transpose_input", "w2l_axpy", "w2l_fill", "w2l_act_fwd", "w2l_mask_mul",
@@ -90,7 +90,6 @@ def _load() -> ctypes.CDLL:
     lib.w2l_glu_bwd.argtypes = [vp, ll, i, vp, vp, vp, f32, u64]
     lib.w2l_act_fwd.argtypes = [vp, ll, vp, i, f32, u64, vp]
     lib.w2l_mask_mul.argtypes = [vp, ll, vp, vp, i, f32, vp]
-    lib.w2l_conv_set_path.argtypes = [i]
     lib.w2l_gemm_tf32_view.argtypes = [vp, i, i, i, i, i, vp, i, vp, i, vp, i, vp, i, i]
     lib.w2l_gemm_tf32_ex.argtypes = [vp, i, i, i, i, i, vp, i, vp, i, vp, i, vp, i, i, vp, i, i, f32, f32, u64]
     lib.w2l_conv_time_workspace_size.restype = sz
@@ -353,7 +352,7 @@ GEMM_KINDS = {"tf32": 0, "f32x3": 1, "bf16": 2}
 
 
 def set_precision(p) -> None:
-    """tf32 (default) | f32 (fp32-accurate 3xTF32 GEMMs + fp32 SIMT time convolutions) | bf16 (bf16 GEMM operands)."""
+    """tf32 (default) | f32 (fp32-accurate 3xTF32 GEMMs and mma.sync time convolutions) | bf16 (bf16 GEMM operands)."""
     _check(lib.w2l_set_precision(PRECISIONS[p] if isinstance(p, str) else int(p)))
 
 

@@ -19,23 +19,9 @@
 #include "common.cuh"
 
 namespace w2l {
-// tensor-core path (conv_mma.cu)
+// the tensor-core path (conv_mma.cu: TF32 products; under W2L_PRECISION_F32 the same kernels run error-compensated
+// 3xTF32); shapes it does not cover run on the fp32 SIMT kernels below
 bool conv_mma_supported(int W, int Cin, int Cout, int K, int stride);
-bool conv_wgmma_supported(int W, int Cin, int Cout, int K, int stride);
-size_t conv_wgmma_arranged_floats(int Cin, int Cout, int K);
-int conv_wgmma_fwd(cudaStream_t stream, int B, int T, int Tout, int W, int Cin, int Cout, int K, int stride, int pad_left, const float* x,
-                  const float* wt, int wt_cin, int wt_cout, int flip, const float* bias, const float* add, float* y, int act, float drop_p,
-                  unsigned long long seed, float* arranged);
-// the tensor-core path (TF32 products; under W2L_PRECISION_F32 the same kernels run error-compensated 3xTF32); shapes it
-// does not cover fall back to the fp32 SIMT kernels below
-static thread_local int g_conv_path = 0;  // w2l_conv_set_path: 0 auto (= mma.sync where the shape allows), 1 fp32 SIMT kernels, 2 mma.sync, 3 wgmma — tests / tuning
-static bool use_conv_mma(int W, int Cin, int Cout, int K, int stride) { return g_conv_path != 1 && conv_mma_supported(W, Cin, Cout, K, stride); }
-// wgmma / TMA forward and stride-1 data gradient (conv_wgmma.cu): with 10-27 channels every wgmma is a 64 x 16 x 8 sliver
-// and a window needs kw * Cp/8 of them per 64 positions, so the tensor pipe is issue-bound; selectable
-// (w2l_conv_set_path(3)) and tested, the default stays on the mma.sync kernels.
-static bool use_conv_wgmma(int W, int Cin, int Cout, int K, int stride) {
-  return g_conv_path == 3 && current_precision() != W2L_PRECISION_F32 && conv_wgmma_supported(W, Cin, Cout, K, stride);
-}
 size_t conv_mma_arranged_floats(int Cin, int Cout, int K);
 int conv_mma_fwd(cudaStream_t stream, int B, int T, int Tout, int W, int Cin, int Cout, int K, int stride, int pad_left,
                  const float* x, const float* wt, int wt_cin, int wt_cout, int flip, const float* bias, const float* add, float* y,
@@ -976,14 +962,9 @@ static size_t conv_ws_partial_bytes(int B, int Tout, int Cin, int Cout, int K) {
   const size_t mma = conv_mma_wgrad_parts(B, Tout, 0, Cin, Cout, K, 1, nullptr, nullptr);  // W unknown here: ten slices
   return align_up(std::max(simt, std::max(mma, (size_t)B * (size_t)std::max(Tout, 16))) * per, 256);
 }
-extern "C" int w2l_conv_set_path(int path) {
-  if (path < 0 || path > 3) return fail(W2L_ERR_INVALID_ARGUMENT, "conv_set_path: 0 (auto), 1 (fp32 SIMT kernels), 2 (mma.sync kernels) or 3 (wgmma kernel)");
-  g_conv_path = path;
-  return W2L_OK;
-}
 extern "C" size_t w2l_conv_time_workspace_size(int B, int Tout, int Cin, int Cout, int K) {
-  const size_t arranged = std::max(std::max((size_t)std::max(Cin, Cout) * K * co_pad(std::max(Cin, Cout)), conv_mma_arranged_floats(Cin, Cout, K)),
-                                   conv_wgmma_arranged_floats(Cin, Cout, K)) * sizeof(float);
+  const size_t arranged =
+      std::max((size_t)std::max(Cin, Cout) * K * co_pad(std::max(Cin, Cout)), conv_mma_arranged_floats(Cin, Cout, K)) * sizeof(float);
   return conv_ws_partial_bytes(B, Tout, Cin, Cout, K) + align_up(arranged, 256);
 }
 
@@ -1017,9 +998,7 @@ extern "C" int w2l_conv_time_fwd(void* stream_, int B, int T, int Tout, int W, i
   if (ws_bytes < w2l_conv_time_workspace_size(B, Tout, Cin, Cout, K)) return fail(W2L_ERR_WORKSPACE, "conv_time_fwd: workspace too small");
   const int CO = co_pad(Cout);
   float* arranged = reinterpret_cast<float*>(static_cast<char*>(ws) + conv_ws_partial_bytes(B, Tout, Cin, Cout, K));
-  if (use_conv_wgmma(W, Cin, Cout, K, stride))
-    return conv_wgmma_fwd(stream, B, T, Tout, W, Cin, Cout, K, stride, pad_left, x, wt, Cin, Cout, 0, bias, add, y, act, dropout_p, seed, arranged);
-  if (use_conv_mma(W, Cin, Cout, K, stride))
+  if (conv_mma_supported(W, Cin, Cout, K, stride))
     return conv_mma_fwd(stream, B, T, Tout, W, Cin, Cout, K, stride, pad_left, x, wt, Cin, Cout, 0, bias, add, y, act, dropout_p, seed,
                         arranged, K, 1, 0, 1, 0, Tout);
   conv_arrange_weights_kernel<<<8, 256, 0, stream>>>(Cin, Cout, K, CO, wt, arranged, 0);
@@ -1044,18 +1023,13 @@ extern "C" int w2l_conv_time_dgrad(void* stream_, int B, int T, int Tout, int W,
   if (int rc = conv_check(B, T, Tout, W, Cin, Cout, K, stride)) return rc;
   if (!dy || !wt || !dx || !ws) return fail(W2L_ERR_INVALID_ARGUMENT, "conv_time_dgrad: null pointer");
   if (ws_bytes < w2l_conv_time_workspace_size(B, Tout, Cin, Cout, K)) return fail(W2L_ERR_WORKSPACE, "conv_time_dgrad: workspace too small");
-  if (stride == 1 && use_conv_wgmma(W, Cout, Cin, K, 1)) {
-    // dx = conv(dy, flipped weights) with pad_left' = K-1-pad_left, channel roles swapped — wgmma path
-    float* arranged = reinterpret_cast<float*>(static_cast<char*>(ws) + conv_ws_partial_bytes(B, Tout, Cin, Cout, K));
-    return conv_wgmma_fwd(stream, B, Tout, T, W, Cout, Cin, K, 1, K - 1 - pad_left, dy, wt, Cin, Cout, 1, nullptr, add, dx, 0, 0.f, 0ull, arranged);
-  }
-  if (stride == 1 && use_conv_mma(W, Cout, Cin, K, 1)) {
+  if (stride == 1 && conv_mma_supported(W, Cout, Cin, K, 1)) {
     // dx = conv(dy, flipped weights) with pad_left' = K-1-pad_left, channel roles swapped — on the tensor-core path
     float* arranged = reinterpret_cast<float*>(static_cast<char*>(ws) + conv_ws_partial_bytes(B, Tout, Cin, Cout, K));
     return conv_mma_fwd(stream, B, Tout, T, W, Cout, Cin, K, 1, K - 1 - pad_left, dy, wt, Cin, Cout, 1, nullptr, add, dx, 0, 0.f, 0ull,
                         arranged, K, 1, 0, 1, 0, T);
   }
-  if (stride > 1 && stride <= K && use_conv_mma(W, Cout, Cin, (K + stride - 1) / stride, 1)) {
+  if (stride > 1 && stride <= K && conv_mma_supported(W, Cout, Cin, (K + stride - 1) / stride, 1)) {
     // polyphase: input frames t with (t + pad_left) % stride == p only see taps p, p + stride, ...; each phase is a
     // stride-1 correlation of dy with those taps reversed, written to every stride-th frame of dx
     float* arranged = reinterpret_cast<float*>(static_cast<char*>(ws) + conv_ws_partial_bytes(B, Tout, Cin, Cout, K));
@@ -1110,7 +1084,7 @@ extern "C" int w2l_conv_time_wgrad(void* stream_, int B, int T, int Tout, int W,
   if (!x || !dy || !dwt || !ws) return fail(W2L_ERR_INVALID_ARGUMENT, "conv_time_wgrad: null pointer");
   if (ws_bytes < w2l_conv_time_workspace_size(B, Tout, Cin, Cout, K)) return fail(W2L_ERR_WORKSPACE, "conv_time_wgrad: workspace too small");
   if (stride > K) return fail(W2L_ERR_UNSUPPORTED, "conv_time_wgrad: stride > kernel width");
-  if (use_conv_mma(W, Cin, Cout, K, stride))
+  if (conv_mma_supported(W, Cin, Cout, K, stride))
     return conv_mma_wgrad(stream, B, T, Tout, W, Cin, Cout, K, stride, pad_left, x, dy, dwt, dbias, static_cast<float*>(ws));
   const int ntiles = ((Cout + 1) / 2) * ((Cin * K + 3) / 4);
   if (ntiles > kWgMaxTiles * kWgThreads) return fail(W2L_ERR_UNSUPPORTED, "conv_time_wgrad: filter too large for the register tiles");

@@ -1,5 +1,5 @@
 // tma_ptx.cuh — the sm_90a PTX the tensor-core kernels are fed by: mbarrier, TMA (cp.async.bulk.tensor) and the wgmma
-// shared-memory matrix descriptor.  Shared by the GEMM (gemm_wgmma.cu) and the time convolution (conv_wgmma.cu).
+// shared-memory matrix descriptor, as the GEMM (gemm_wgmma.cu) uses them.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -37,13 +37,6 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* ba
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
           smem_u32(smem_dst)),
       "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(const CUtensorMap* map, uint64_t* bar, void* smem_dst, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(
-          smem_u32(smem_dst)),
-      "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
 // wgmma descriptor of a 128B-swizzled operand tile (1024-byte aligned atoms of 8 rows x 128 B):
