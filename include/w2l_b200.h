@@ -197,9 +197,14 @@ W2L_API int w2l_gemm_tf32_view(void* stream, int a_mn_major, int b_mn_major, int
  *           3xTF32 the same way.
  *   BF16  : bf16 operands in HBM (activations / weights cast by their producers), fp32 accumulation — the AMP mode of
  *           the reference (recipes/slimIPL/src/Train.cpp:211-219) with bf16 instead of fp16, configs[2]/[3].
+ *   F32X3_SPLIT_B : F32X3 with B split ahead of the call by w2l_split_tf32: B is K-major only and points at
+ *           [2][N][ldb] fp32, the tf32 hi plane then the lo plane (ldb % 4 == 0, ldb >= K).  Results are bit-identical
+ *           to F32X3 on the unsplit B; the kernel loads both planes by TMA and converts nothing, which pays when B (a
+ *           weight) is reused by many rows of output tiles.
  * w2l_set_precision is thread-local and selects the kind used by the fp32-operand entry points (w2l_gemm_tf32*,
- * w2l_conv_time_*) and by the fl_compat modules (which cast their GEMM operands in BF16 mode). */
-enum { W2L_GEMM_TF32 = 0, W2L_GEMM_F32X3 = 1, W2L_GEMM_BF16 = 2 };
+ * w2l_conv_time_*) and by the fl_compat modules (which cast their GEMM operands in BF16 mode and pre-split their
+ * weights in F32 mode). */
+enum { W2L_GEMM_TF32 = 0, W2L_GEMM_F32X3 = 1, W2L_GEMM_BF16 = 2, W2L_GEMM_F32X3_SPLIT_B = 3 };
 enum { W2L_PRECISION_TF32 = 0, W2L_PRECISION_F32 = 1, W2L_PRECISION_BF16 = 2 };
 W2L_API int w2l_set_precision(int precision);
 W2L_API int w2l_get_precision(void);
@@ -214,6 +219,12 @@ W2L_API int w2l_gemm(void* stream, int kind, int a_mn_major, int b_mn_major, int
  * ld_in, to rows of cols_padded bf16) */
 W2L_API int w2l_cast_bf16(void* stream, long long n, const float* x, void* y);
 W2L_API int w2l_cast_bf16_rows(void* stream, long long rows, int cols, int ld_in, int cols_padded, const float* x, void* y);
+/* x [rows][cols] fp32 (row stride ld) -> the B planes of W2L_GEMM_F32X3_SPLIT_B, hi = tf32(x), lo = tf32(x - hi) (round to
+ * nearest, ties away, as the F32X3 kernel rounds):
+ *   transpose = 0: planes [2][rows][cols_padded], plane[r][c] from x[r][c]  (B = x K-major: the forward's weight)
+ *   transpose = 1: planes [2][cols][cols_padded], plane[c][r] from x[r][c]  (B = x^T K-major: the data gradient's weight)
+ * the columns of a plane past the source (c >= cols, resp. r >= rows) are zero. */
+W2L_API int w2l_split_tf32(void* stream, int transpose, int rows, int cols, int ld, int cols_padded, const float* x, float* planes);
 /* Pin the GEMM tile width (128 / 160 / 224 / 256; 0 = choose per shape, the default).  Thread-local; for tests and tuning. */
 W2L_API int w2l_gemm_set_tile(int bn);
 /* 1 (default): one CTA per SM walking the tiles, so the producer stages the next tile's operands during an epilogue;

@@ -25,7 +25,7 @@ EXPORTS = [
     "w2l_fac_viterbi_workspace_size", "w2l_fac_viterbi",
     "w2l_ctc_workspace_size", "w2l_ctc_forward_backward", "w2l_argmax_path", "w2l_linseg_target",
     "w2l_ctc_viterbi_workspace_size", "w2l_ctc_viterbi_target",
-    "w2l_set_precision", "w2l_get_precision", "w2l_gemm", "w2l_cast_bf16", "w2l_cast_bf16_rows", "w2l_sgd_step_ex", "w2l_finite_guard",
+    "w2l_set_precision", "w2l_get_precision", "w2l_gemm", "w2l_cast_bf16", "w2l_cast_bf16_rows", "w2l_split_tf32", "w2l_sgd_step_ex", "w2l_finite_guard",
     "w2l_mask_bands", "w2l_trainer_set_precision", "w2l_trainer_set_grad_stream", "w2l_trainer_set_grad_stream_delay", "w2l_delay", "w2l_trainer_status", "w2l_trainer_save", "w2l_trainer_load", "w2l_trainer_export_streaming",
     "w2l_text_create", "w2l_text_destroy", "w2l_text_num_classes", "w2l_text_encode", "w2l_text_prediction2ltr", "w2l_text_target2ltr",
     "w2l_text_ltr2wrd", "w2l_text_align_words", "w2l_edit_distance",
@@ -106,6 +106,7 @@ def _load() -> ctypes.CDLL:
     lib.w2l_gemm.argtypes = [vp, i, i, i, i, i, i, vp, i, vp, i, vp, i, i, vp, i, i, vp, i, i, i, f32, f32, u64, i]
     lib.w2l_cast_bf16.argtypes = [vp, ll, vp, vp]
     lib.w2l_cast_bf16_rows.argtypes = [vp, ll, i, i, i, vp, vp]
+    lib.w2l_split_tf32.argtypes = [vp, i, i, i, i, i, vp, vp]
     lib.w2l_sgd_step_ex.argtypes = [vp, ll, vp, vp, vp, f32, f32, f32, f32, f32, vp, i, vp]
     lib.w2l_finite_guard.argtypes = [vp, i, vp, vp, vp]
     lib.w2l_mask_bands.argtypes = [vp, i, i, i, i, vp, vp, i, vp, vp, i, vp, vp, f32]
@@ -348,7 +349,7 @@ def trace_list() -> list:
 
 
 PRECISIONS = {"tf32": 0, "f32": 1, "fp32": 1, "bf16": 2}
-GEMM_KINDS = {"tf32": 0, "f32x3": 1, "bf16": 2}
+GEMM_KINDS = {"tf32": 0, "f32x3": 1, "bf16": 2, "f32x3_split_b": 3}
 
 
 def set_precision(p) -> None:
@@ -362,12 +363,13 @@ def get_precision() -> int:
 
 def gemm(A, B, kind="tf32", a_mn=False, b_mn=False, bias=None, act=0, out=None, out_bf16=False, accumulate=False, aux=None,
          aux_mode=0, aux_scale=1.0, dropout_p=0.0, seed=0, M=None, N=None, K=None, lda=None, ldb=None, allow_overlap=False):
-    """General wgmma GEMM (w2l_gemm): A/B fp32 (kinds tf32, f32x3) or bfloat16 (kind bf16); C fp32 or bfloat16."""
+    """General wgmma GEMM (w2l_gemm): A/B fp32 (kinds tf32, f32x3) or bfloat16 (kind bf16); C fp32 or bfloat16.
+    Kind f32x3_split_b: B is the [2][N][ldb] planes of split_tf32 (K is taken from A)."""
     if M is None:
         M, K = (A.shape[1], A.shape[0]) if a_mn else A.shape
-        N = B.shape[1] if b_mn else B.shape[0]
+        N = B.shape[-2] if B.dim() == 3 else (B.shape[1] if b_mn else B.shape[0])
     lda = A.stride(0) if lda is None else lda
-    ldb = B.stride(0) if ldb is None else ldb
+    ldb = B.stride(-2) if ldb is None else ldb
     if out is None:
         out = torch.empty((M, N), dtype=torch.bfloat16 if out_bf16 else torch.float32, device=A.device)
     _check(lib.w2l_gemm(_stream(), GEMM_KINDS[kind], int(a_mn), int(b_mn), M, N, K, _ptr(A), lda, _ptr(B), ldb, _ptr(out),
@@ -381,6 +383,20 @@ def cast_bf16(x):
     x = _req(x, torch.float32, "x")
     y = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
     _check(lib.w2l_cast_bf16(_stream(), x.numel(), _ptr(x), _ptr(y)))
+    return y
+
+
+def split_tf32(x, transpose=False, cols_padded=None):
+    """B planes of kind f32x3_split_b from a 2-D fp32 tensor x (rows contiguous): [2][rows][cols_padded] tf32 hi / lo,
+    or with transpose those of x^T, [2][cols][cols_padded]; cols_padded defaults to the source row length rounded up
+    to 4 (a TMA row)"""
+    if x.dtype != torch.float32 or not x.is_cuda or x.dim() != 2 or x.stride(1) != 1:
+        raise TypeError("split_tf32: x must be a 2-D CUDA float32 tensor with contiguous rows")
+    rows, cols = x.shape
+    k = rows if transpose else cols
+    cols_padded = (k + 3) // 4 * 4 if cols_padded is None else cols_padded
+    y = torch.empty((2, cols if transpose else rows, cols_padded), dtype=torch.float32, device=x.device)
+    _check(lib.w2l_split_tf32(_stream(), int(transpose), rows, cols, x.stride(0), cols_padded, _ptr(x), _ptr(y)))
     return y
 
 

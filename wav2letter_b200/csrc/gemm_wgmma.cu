@@ -5,11 +5,14 @@
 //
 //   C[m][n] = act( sum_k A(m,k) * B(n,k) + bias[n] )        fp32 accumulation in registers
 //
-// Three operand kinds, one kernel template (the "precision" of BASELINE.json's configs):
+// Four operand kinds, one kernel template (the "precision" of BASELINE.json's configs):
 //   W2L_GEMM_TF32   fp32 operands in HBM, tf32 products (10-bit mantissas)  — cuDNN/cuBLAS default for fp32
 //   W2L_GEMM_F32X3  fp32 operands in HBM, fp32-ACCURATE: every staged value is split into hi = tf32(x) and
 //                   lo = tf32(x - hi) (A in registers, B in shared memory) and the tensor core accumulates
 //                   Al*Bh + Ah*Bl + Ah*Bh — products good to ~2^-21, i.e. SGEMM-grade (configs[1] "fp32")
+//   W2L_GEMM_F32X3_SPLIT_B  the same products with B already split in HBM (w2l_split_tf32: K-major hi plane, then lo
+//                   plane), loaded by TMA next to the raw A tile: no conversion warps, bit-identical to F32X3.  For a
+//                   weight B that would otherwise be converted once per row of output tiles
 //   W2L_GEMM_BF16   bf16 operands in HBM — half the operand bytes, twice the MAC rate
 //                   (configs[2]/[3] "bf16 convs / fp32 loss"; the reference's AMP switch, Train.cpp:211-219)
 // C is fp32 or bf16 (c_bf16); bias / ReLU / dropout / mask / accumulate epilogue.
@@ -35,7 +38,8 @@
 //                           ring, with a ready / empty mbarrier pair per stage
 //   warpgroups 1, 2         64 x BN halves of the tile into register accumulators; epilogue straight from the accumulator
 //                           fragment.  bf16 and unconverted TF32: wgmma m64nBNk16 / m64nBNk8 with both operands in shared
-//                           memory (MN-major bf16 through the transpose bits).  Converted kinds: each warpgroup reads its
+//                           memory (MN-major bf16 through the transpose bits).  Converted kinds and F32X3_SPLIT_B (whose
+//                           raw stage is [A | B hi | B lo], B read in place, freed when its MMAs complete): each warpgroup reads its
 //                           64 x 32 slice of the raw A tile into the tf32 register-fragment layout, rounds / splits it in
 //                           registers and issues m64n128k8 with A from registers.  It frees the raw stage as soon as its
 //                           fragments are loaded, so TMA, B conversion and MMAs of different k blocks overlap; fragments
@@ -69,29 +73,33 @@ constexpr int kTileBytes = BM * kRowBytes;  // 16 KB of A per stage
 constexpr int kGemmThreads = 384;
 constexpr int kConvThreads = 96;            // warps 1..3
 constexpr int kConsumerThreads = 256;       // warpgroups 1, 2
-enum { kTf32 = W2L_GEMM_TF32, kF32x3 = W2L_GEMM_F32X3, kBf16 = W2L_GEMM_BF16 };
+enum { kTf32 = W2L_GEMM_TF32, kF32x3 = W2L_GEMM_F32X3, kBf16 = W2L_GEMM_BF16, kF32x3SplitB = W2L_GEMM_F32X3_SPLIT_B };
 
-// The raw ring's stages hold the TMA tiles [A | B]; the converted kinds add a ring of converted B stages, [hi B] or
-// [hi B | lo B] for F32X3.  Unconverted kinds: as many raw stages as fit in 227 KB, at most 6.  Converted kinds: 4 raw
-// stages, the rest of the 227 KB for converted stages (at most 4).  BN is 128 / 160 / 224 / 256 for unconverted TF32,
-// 128 / 256 for BF16, 128 for the converted kinds (accumulators plus two A fragment sets must fit in registers).
+// The raw ring's stages hold the TMA tiles [A | B] ([A | B hi | B lo] for F32X3_SPLIT_B); the converted kinds add a ring
+// of converted B stages, [hi B] or [hi B | lo B] for F32X3.  Unconverted kinds: as many raw stages as fit in 227 KB, at
+// most 6 (4 for F32X3_SPLIT_B).  Converted kinds: 4 raw stages, the rest of the 227 KB for converted stages (at most 4).
+// BN is 128 / 160 / 224 / 256 for unconverted TF32, 128 / 256 for BF16, 128 for the kinds that take A from registers
+// (accumulators plus two A fragment sets must fit in registers).
 __host__ __device__ constexpr bool converts(int mode, bool a_mn, bool b_mn) { return mode == kF32x3 || (mode == kTf32 && (a_mn || b_mn)); }
-__host__ __device__ constexpr size_t raw_bytes(int bn) { return (size_t)kTileBytes + (size_t)bn * kRowBytes; }
+__host__ __device__ constexpr bool a_in_regs(int mode, bool a_mn, bool b_mn) { return converts(mode, a_mn, b_mn) || mode == kF32x3SplitB; }
+__host__ __device__ constexpr size_t raw_bytes(int mode, int bn) { return (size_t)kTileBytes + (size_t)bn * kRowBytes * (mode == kF32x3SplitB ? 2 : 1); }
 __host__ __device__ constexpr size_t cvt_bytes(int mode, int bn) { return (size_t)bn * kRowBytes * (mode == kF32x3 ? 2 : 1); }
 constexpr size_t kSmemTail = 1024 + 256;  // alignment slack + barriers + the work-item id ring
 constexpr size_t kSmemBudget = 227 * 1024 - kSmemTail;
 constexpr int kConvRawStages = 4;
 constexpr int kIdSlots = 4;  // work-item ids the producer may publish ahead of the tile the consumers are on
 __host__ __device__ constexpr int raw_stages(int mode, bool a_mn, bool b_mn, int bn) {
-  return converts(mode, a_mn, b_mn) ? kConvRawStages : (kSmemBudget / raw_bytes(bn) > 6 ? 6 : (int)(kSmemBudget / raw_bytes(bn)));
+  return converts(mode, a_mn, b_mn) ? kConvRawStages
+                                    : (kSmemBudget / raw_bytes(mode, bn) > 6 ? 6 : (int)(kSmemBudget / raw_bytes(mode, bn)));
 }
 __host__ __device__ constexpr int cvt_stages(int mode, bool a_mn, bool b_mn, int bn) {
   return !converts(mode, a_mn, b_mn) ? 0
-         : (kSmemBudget - kConvRawStages * raw_bytes(bn)) / cvt_bytes(mode, bn) > 4 ? 4
-                                                                                     : (int)((kSmemBudget - kConvRawStages * raw_bytes(bn)) / cvt_bytes(mode, bn));
+         : (kSmemBudget - kConvRawStages * raw_bytes(mode, bn)) / cvt_bytes(mode, bn) > 4
+             ? 4
+             : (int)((kSmemBudget - kConvRawStages * raw_bytes(mode, bn)) / cvt_bytes(mode, bn));
 }
 __host__ __device__ constexpr size_t smem_for(int mode, bool a_mn, bool b_mn, int bn) {
-  return raw_stages(mode, a_mn, b_mn, bn) * raw_bytes(bn) + cvt_stages(mode, a_mn, b_mn, bn) * cvt_bytes(mode, bn) + kSmemTail;
+  return raw_stages(mode, a_mn, b_mn, bn) * raw_bytes(mode, bn) + cvt_stages(mode, a_mn, b_mn, bn) * cvt_bytes(mode, bn) + kSmemTail;
 }
 
 struct GemmParams {
@@ -225,13 +233,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
                   unsigned int* sched) {  // [claimed, finished CTAs] counters of the dynamic schedule; null: CTA b walks b, b + grid, ...
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  constexpr bool kIsBf16 = kMode == kBf16, kSplit = kMode == kF32x3, kConv = converts(kMode, kAMn, kBMn);
+  constexpr bool kIsBf16 = kMode == kBf16, kPreSplit = kMode == kF32x3SplitB, kSplit = kMode == kF32x3 || kPreSplit;
+  constexpr bool kConv = converts(kMode, kAMn, kBMn), kRegA = a_in_regs(kMode, kAMn, kBMn);
   constexpr int BKE = kRowBytes / (kIsBf16 ? 2 : 4);  // elements of k per stage: 32 fp32 / 64 bf16
   constexpr int kStages = raw_stages(kMode, kAMn, kBMn, BN), kCvtStages = cvt_stages(kMode, kAMn, kBMn, BN);
-  constexpr size_t kRaw = raw_bytes(BN), kCvt = cvt_bytes(kMode, BN);
+  constexpr size_t kRaw = raw_bytes(kMode, BN), kCvt = cvt_bytes(kMode, BN);
   constexpr uint32_t kOperandBytes = (uint32_t)kRaw;
   static_assert(kStages >= 2 && (!kConv || kCvtStages >= 2), "gemm: at least two stages per ring");
-  static_assert(!kConv || BN == 128, "gemm: the converted kinds take A from registers at BN = 128");
+  static_assert(!kRegA || BN == 128, "gemm: the kinds that take A from registers run at BN = 128");
+  static_assert(!kPreSplit || !kBMn, "gemm: pre-split B planes are K-major");
   static_assert(!kIsBf16 || !kBMn || BN % 64 == 0, "gemm: MN-major bf16 B is staged in boxes of 64 columns");
   unsigned char* cvt_ring = smem + kStages * kRaw;
   uint64_t* bars = reinterpret_cast<uint64_t*>(cvt_ring + kCvtStages * kCvt);
@@ -283,7 +293,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
     m0 = (r / tiles_n) * BM;
     n0 = (r % tiles_n) * BN;
     kb_begin = z * kb_per;
-    num_kb = max(0, min(total_kb, kb_begin + kb_per) - kb_begin);
+    int total = total_kb;
+    if constexpr (kPreSplit) {  // re-derived from the kernel parameter (an opaque copy): held in a register for the whole walk, it spilled
+      int k = p.K;
+      asm volatile("" : "+r"(k));
+      total = (k + BKE - 1) / BKE;
+    }
+    num_kb = max(0, min(total, kb_begin + kb_per) - kb_begin);
   };
 
   if (wg == 0) {
@@ -312,7 +328,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
 #pragma unroll
               for (int j = 0; j < BM / 8; ++j) tma_load_2d(&map_a, &full[s], sa + j * 1024, m0 + 8 * j, k0);  // box {8 m, 32 k}
             }
-            if (!kBMn) {
+            if (kPreSplit) {  // box {128 B of k, BN rows} of plane 0 (hi), then plane 1 (lo)
+              tma_load_3d(&map_b, &full[s], sb, k0, n0, 0);
+              tma_load_3d(&map_b, &full[s], sb + BN * kRowBytes, k0, n0, 1);
+            } else if (!kBMn) {
               tma_load_2d(&map_b, &full[s], sb, k0, n0);
             } else if (kIsBf16) {
 #pragma unroll
@@ -370,7 +389,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
       float acc[BN / 2];
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-      if constexpr (kConv) {
+      if constexpr (kRegA) {
         // A fragments of one k block: [k8 step][a0..a3], hi = tf32(x) and (F32X3) lo = tf32(x - hi), rounded as convert_tile
         struct AFrag {
           uint32_t hi[4][4], lo[4][4];
@@ -379,10 +398,17 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
           wg::fence_operands(f.hi);
           if constexpr (kSplit) wg::fence_operands(f.lo);
         };
-        // one k block: A fragments from raw stage s (then free it), MMAs on converted B stage c; on return, the MMAs of the
-        // previous k block (fragments `prev`) have completed and its converted B stage is freed
+        // the stage holding B of k block i is free once its MMAs have completed: the converted B stage, or for
+        // F32X3_SPLIT_B the raw stage itself
+        auto release_b = [&](uint32_t i) {
+          if constexpr (kConv) mbar_arrive(&cvt_empty[i % kCvtStages]);
+          else mbar_arrive(&empty[i % kStages]);
+        };
+        // one k block: A fragments from raw stage s (then free it, unless B is read from it too), MMAs on converted B
+        // stage c or on the B planes of raw stage s; on return, the MMAs of the previous k block (fragments `prev`) have
+        // completed and its B stage is freed
         auto step = [&](AFrag& cur, AFrag& prev, int kb) {
-          const int s = it % kStages, c = it % kCvtStages;
+          const int s = it % kStages;
           mbar_wait(&full[s], (it / kStages) & 1);
           const uint32_t sa = smem_u32(smem + s * kRaw);
 #pragma unroll
@@ -397,9 +423,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
               if constexpr (kSplit) cur.lo[kk][i] = rn_tf32(__float_as_uint(__uint_as_float(x) - __uint_as_float(cur.hi[kk][i])));
             }
           }
-          mbar_arrive(&empty[s]);
-          mbar_wait(&ready[c], (it / kCvtStages) & 1);
-          const uint32_t b_base = smem_u32(cvt_ring + c * kCvt);
+          uint32_t b_base;
+          if constexpr (kConv) {
+            const int c = it % kCvtStages;
+            mbar_arrive(&empty[s]);
+            mbar_wait(&ready[c], (it / kCvtStages) & 1);
+            b_base = smem_u32(cvt_ring + c * kCvt);
+          } else {
+            b_base = sa + kTileBytes;
+          }
           fence_frag(cur);  // the fragments are final before wgmma.fence (a later definition would serialise the MMAs)
           wg::fence_operands(acc);
           wg::fence();
@@ -421,7 +453,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
           // MMA per k8 step on its operand registers (C7513)
           if constexpr (kSplit) wg::wait<1>(); else wg::wait<0>();
           fence_frag(prev);
-          if (kb > 0) mbar_arrive(&cvt_empty[(it - 1) % kCvtStages]);
+          if (kb > 0) release_b(it - 1);
           ++it;
         };
         AFrag fa, fb;
@@ -433,7 +465,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         wg::fence_operands(acc);
         fence_frag(fa);
         fence_frag(fb);
-        if (num_kb > 0) mbar_arrive(&cvt_empty[(it - 1) % kCvtStages]);
+        if (num_kb > 0) release_b(it - 1);
       } else {
         for (int kb = 0; kb < num_kb; ++kb, ++it) {
           const int s = it % kStages;
@@ -491,27 +523,64 @@ __global__ void __launch_bounds__(256) splitk_reduce_kernel(int M, int N, int sp
   }
 }
 
+// Split pass of F32X3_SPLIT_B: [rows][cols] fp32 (row stride ld) -> planes [2][R][ld_out], hi = tf32(x) then
+// lo = tf32(x - hi), rounded exactly as convert_tile.  kT = false: R = rows, plane[r][c] = x[r][c]; kT = true: R = cols,
+// plane[c][r] = x[r][c] (through a shared-memory tile, so reads and writes are both row-contiguous).  Entries past the
+// source along the plane rows (c >= cols, or r >= rows when transposed) are zero.  32 x 32 tiles of the planes.
+template <bool kT>
+__global__ void __launch_bounds__(256) split_tf32_kernel(int rows, int cols, int ld, int R, int ld_out, const float* __restrict__ x,
+                                                         float* __restrict__ y) {
+  __shared__ float tile[32][33];
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const int r0 = blockIdx.x * 32, c0 = blockIdx.y * 32;  // tile origin in plane coordinates
+  if (kT) {
+    for (int i = ty; i < 32; i += 8) {  // source row c0 + i, source column r0 + tx
+      const int sr = c0 + i, sc = r0 + tx;
+      tile[i][tx] = (sr < rows && sc < cols) ? x[(size_t)sr * ld + sc] : 0.f;
+    }
+    __syncthreads();
+  }
+  const size_t plane = (size_t)R * ld_out;
+  for (int i = ty; i < 32; i += 8) {
+    const int r = r0 + i, c = c0 + tx;
+    if (r >= R || c >= ld_out) continue;
+    const float v = kT ? tile[tx][i] : (c < cols ? x[(size_t)r * ld + c] : 0.f);
+    const uint32_t h = rn_tf32(__float_as_uint(v));
+    const uint32_t l = rn_tf32(__float_as_uint(v - __uint_as_float(h)));
+    y[(size_t)r * ld_out + c] = __uint_as_float(h);
+    y[plane + (size_t)r * ld_out + c] = __uint_as_float(l);
+  }
+}
+
 // ---- host side -----------------------------------------------------------------------------------
-// 2D map over a row-major matrix [rows][cols] (row stride ld elements); box {box_cols, box_rows}
-int make_map(CUtensorMap* map, int mode, bool conv, const void* ptr, long long rows, long long cols, long long ld, int box_cols, int box_rows,
-             bool swizzle) {
+// Row-major matrix [rows][cols] (row stride ld elements), box {box_cols, box_rows}; planes > 1: that many such
+// matrices one after another (rows * ld elements apart), a 3D map with a box of one plane
+int make_map(CUtensorMap* map, int mode, bool raw, const void* ptr, long long rows, long long cols, long long ld, int box_cols, int box_rows,
+             bool swizzle, int planes = 1) {
   EncodeTiledFn fn = encode_fn();
   if (!fn) return fail(W2L_ERR_CUDA, "gemm: cuTensorMapEncodeTiled entry point not found");
   const int es = mode == kBf16 ? 2 : 4;
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * es};
-  cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  // TF32 read directly by wgmma: rounded on load; converted operands: the raw fp32 bits (rounded by the conversion)
-  const CUtensorMapDataType dt = mode == kBf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : (conv ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_TFLOAT32);
-  CUresult r = fn(map, dt, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+  cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)planes};
+  cuuint64_t strides[2] = {(cuuint64_t)ld * es, (cuuint64_t)(rows * ld * es)};
+  cuuint32_t box[3] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  // TF32 read directly by wgmma: rounded on load; operands split or converted on chip: the raw fp32 bits
+  const CUtensorMapDataType dt = mode == kBf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : (raw ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_TFLOAT32);
+  CUresult r = fn(map, dt, planes > 1 ? 3 : 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(W2L_ERR_CUDA, "gemm: cuTensorMapEncodeTiled failed with code " + std::to_string((int)r));
   return W2L_OK;
 }
 
-const char* kernel_name(int mode) { return mode == kBf16 ? "gemm_wgmma_kernel<bf16>" : (mode == kF32x3 ? "gemm_wgmma_kernel<f32x3>" : "gemm_wgmma_kernel<tf32>"); }
+const char* kernel_name(int mode) {
+  switch (mode) {
+    case kBf16: return "gemm_wgmma_kernel<bf16>";
+    case kF32x3: return "gemm_wgmma_kernel<f32x3>";
+    case kF32x3SplitB: return "gemm_wgmma_kernel<f32x3_split_b>";
+    default: return "gemm_wgmma_kernel<tf32>";
+  }
+}
 
 thread_local int g_variant = 1;  // 1: one CTA per SM walking tiles (default), 0: one CTA per tile (w2l_gemm_set_variant; tests compare the two)
 
@@ -561,7 +630,7 @@ int launch_bn(cudaStream_t stream, const CUtensorMap& ma, const CUtensorMap& mb,
 }
 template <int kMode, bool kAMn, bool kBMn>
 int launch_mode(cudaStream_t stream, int bn, const CUtensorMap& ma, const CUtensorMap& mb, const GemmParams& p) {
-  if constexpr (converts(kMode, kAMn, kBMn)) {
+  if constexpr (a_in_regs(kMode, kAMn, kBMn)) {
     return launch_bn<kMode, kAMn, kBMn, 128>(stream, ma, mb, p);
   } else if constexpr (kMode == kBf16) {  // 128 or 256 (MN-major B is staged in 64-wide boxes)
     return bn <= 128 ? launch_bn<kMode, kAMn, kBMn, 128>(stream, ma, mb, p) : launch_bn<kMode, kAMn, kBMn, 256>(stream, ma, mb, p);
@@ -576,10 +645,14 @@ int launch_mode(cudaStream_t stream, int bn, const CUtensorMap& ma, const CUtens
 }
 template <int kMode>
 int launch(cudaStream_t stream, bool a_mn, bool b_mn, int bn, const CUtensorMap& ma, const CUtensorMap& mb, const GemmParams& p) {
-  if (!a_mn && !b_mn) return launch_mode<kMode, false, false>(stream, bn, ma, mb, p);
-  if (!a_mn && b_mn) return launch_mode<kMode, false, true>(stream, bn, ma, mb, p);
-  if (a_mn && b_mn) return launch_mode<kMode, true, true>(stream, bn, ma, mb, p);
-  return launch_mode<kMode, true, false>(stream, bn, ma, mb, p);
+  if constexpr (kMode == kF32x3SplitB) {  // B planes are K-major (gemm_impl rejects b_mn)
+    return a_mn ? launch_mode<kMode, true, false>(stream, bn, ma, mb, p) : launch_mode<kMode, false, false>(stream, bn, ma, mb, p);
+  } else {
+    if (!a_mn && !b_mn) return launch_mode<kMode, false, false>(stream, bn, ma, mb, p);
+    if (!a_mn && b_mn) return launch_mode<kMode, false, true>(stream, bn, ma, mb, p);
+    if (a_mn && b_mn) return launch_mode<kMode, true, true>(stream, bn, ma, mb, p);
+    return launch_mode<kMode, true, false>(stream, bn, ma, mb, p);
+  }
 }
 
 // split-K factor for a tile count: when the tiles alone under-fill the chip and K is long (weight gradients),
@@ -593,7 +666,7 @@ int splits_for(int tiles, int total_kb, bool plain) {
 thread_local int g_force_bn = 0;  // w2l_gemm_set_tile: tests pin the tile width
 int choose_bn(int mode, bool a_mn, bool b_mn, int M, int N, int total_kb, bool plain, int* splits_out) {
   auto allowed = [&](int bn) {
-    if (converts(mode, a_mn, b_mn)) return bn == 128;
+    if (a_in_regs(mode, a_mn, b_mn)) return bn == 128;
     if (mode == kBf16) return bn == 128 || bn == 256;
     return true;
   };
@@ -627,7 +700,8 @@ int gemm_impl(void* stream_, int mode, int a_mn_major, int b_mn_major, int M, in
               void* C, int ldc, int c_bf16, const float* bias, int act, int accumulate, const void* aux, int ld_aux, int aux_bf16,
               int aux_mode, float aux_scale, float dropout_p, unsigned long long seed, bool allow_overlap) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (mode != kTf32 && mode != kF32x3 && mode != kBf16) return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: unknown operand kind");
+  if (mode != kTf32 && mode != kF32x3 && mode != kBf16 && mode != kF32x3SplitB) return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: unknown operand kind");
+  if (mode == kF32x3SplitB && b_mn_major) return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: F32X3_SPLIT_B takes K-major B planes");
   if (M <= 0 || N <= 0 || K <= 0) return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: M, N, K must be positive");
   if (!A || !B || !C) return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: null pointer");
   if (act < 0 || act > 1) return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: act must be 0 (none) or 1 (relu)");
@@ -647,27 +721,32 @@ int gemm_impl(void* stream_, int mode, int a_mn_major, int b_mn_major, int M, in
   const bool plain = act == 0 && aux_mode == 0 && dropout_p == 0.f && bias == nullptr && !c_bf16;
   int splits = 1;
   const int BN = choose_bn(mode, a_mn_major != 0, b_mn_major != 0, M, N, total_kb, plain, &splits);
-  const bool conv = converts(mode, a_mn_major != 0, b_mn_major != 0);
+  const bool raw = a_in_regs(mode, a_mn_major != 0, b_mn_major != 0);
   const bool bf16 = mode == kBf16;
   CUtensorMap ma, mb;
   int rc;
   // K-major: box {128 B of k, tile rows}, 128B swizzle.  MN-major bf16: box {64 m/n, 64 k}, 128B swizzle.  MN-major fp32:
-  // A in boxes {8 m, 32 k} (read as register fragments), B in one box {BN, 32 k} (converted in shared memory), unswizzled
+  // A in boxes {8 m, 32 k} (read as register fragments), B in one box {BN, 32 k} (converted in shared memory), unswizzled.
+  // Pre-split B: the K-major box of each plane
   if (!a_mn_major)
-    rc = make_map(&ma, mode, conv, A, M, K, lda, bke, BM, true);
+    rc = make_map(&ma, mode, raw, A, M, K, lda, bke, BM, true);
   else
-    rc = make_map(&ma, mode, conv, A, K, M, lda, bf16 ? 64 : 8, bke, bf16);
+    rc = make_map(&ma, mode, raw, A, K, M, lda, bf16 ? 64 : 8, bke, bf16);
   if (rc) return rc;
   if (!b_mn_major)
-    rc = make_map(&mb, mode, conv, B, N, K, ldb, bke, BN, true);
+    rc = make_map(&mb, mode, raw, B, N, K, ldb, bke, BN, true, mode == kF32x3SplitB ? 2 : 1);
   else
-    rc = make_map(&mb, mode, conv, B, K, N, ldb, bf16 ? 64 : BN, bke, bf16);
+    rc = make_map(&mb, mode, raw, B, K, N, ldb, bf16 ? 64 : BN, bke, bf16);
   if (rc) return rc;
   GemmParams p{M, N, K, ldc, act, C, bias, accumulate, aux_mode, ld_aux, aux, aux_scale, dropout_p, seed, splits, c_bf16, aux_bf16, nullptr};
   // split-K: partial tiles in stream-ordered scratch (at most about one tile per SM of partials), then a fixed-order sum
   if (splits > 1) W2L_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&p.ws), sizeof(float) * (size_t)splits * M * N, stream));
-  rc = mode == kBf16 ? launch<kBf16>(stream, a_mn_major, b_mn_major, BN, ma, mb, p)
-                     : (mode == kF32x3 ? launch<kF32x3>(stream, a_mn_major, b_mn_major, BN, ma, mb, p) : launch<kTf32>(stream, a_mn_major, b_mn_major, BN, ma, mb, p));
+  switch (mode) {
+    case kBf16: rc = launch<kBf16>(stream, a_mn_major, b_mn_major, BN, ma, mb, p); break;
+    case kF32x3: rc = launch<kF32x3>(stream, a_mn_major, b_mn_major, BN, ma, mb, p); break;
+    case kF32x3SplitB: rc = launch<kF32x3SplitB>(stream, a_mn_major, b_mn_major, BN, ma, mb, p); break;
+    default: rc = launch<kTf32>(stream, a_mn_major, b_mn_major, BN, ma, mb, p);
+  }
   if (splits > 1) {
     if (rc == W2L_OK) {
       const long long mn = (long long)M * N;
@@ -775,5 +854,20 @@ extern "C" int w2l_cast_bf16_rows(void* stream_, long long rows, int cols, int l
   const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, (long long)sm_count() * 16);
   cast_bf16_rows_kernel<<<grid, 256, 0, stream>>>(rows, cols, ld_in, cols_padded, x, static_cast<__nv_bfloat16*>(y));
   W2L_LAUNCH_CHECK("cast_bf16_rows_kernel");
+  return W2L_OK;
+}
+extern "C" int w2l_split_tf32(void* stream_, int transpose, int rows, int cols, int ld, int cols_padded, const float* x, float* planes) {
+  if (rows <= 0 || cols <= 0) return W2L_OK;
+  if (!x || !planes || ld < cols) return fail(W2L_ERR_INVALID_ARGUMENT, "split_tf32: bad arguments");
+  const int R = transpose ? cols : rows;
+  if (cols_padded < (transpose ? rows : cols) || (cols_padded + 31) / 32 > 65535)
+    return fail(W2L_ERR_INVALID_ARGUMENT, "split_tf32: bad plane size");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const dim3 grid((unsigned)((R + 31) / 32), (unsigned)((cols_padded + 31) / 32));
+  if (transpose)
+    split_tf32_kernel<true><<<grid, 256, 0, stream>>>(rows, cols, ld, R, cols_padded, x, planes);
+  else
+    split_tf32_kernel<false><<<grid, 256, 0, stream>>>(rows, cols, ld, R, cols_padded, x, planes);
+  W2L_LAUNCH_CHECK("split_tf32_kernel");
   return W2L_OK;
 }

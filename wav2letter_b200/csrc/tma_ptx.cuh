@@ -39,6 +39,13 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* ba
       "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
+__device__ __forceinline__ void tma_load_3d(const CUtensorMap* map, uint64_t* bar, void* smem_dst, int c0, int c1, int c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(
+          smem_u32(smem_dst)),
+      "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
 // wgmma descriptor of a 128B-swizzled operand tile (1024-byte aligned atoms of 8 rows x 128 B):
 //   K-major : rows of 128 B of k, 8-row groups sbo = 1024 B apart, lbo unused
 //   MN-major: (16-bit operands only) atoms of 64 elements along m/n x 8 k-rows; lbo = stride between 64-element atoms

@@ -472,6 +472,25 @@ int gemmP(int a_mn, int b_mn, int M, int N, int K, const GemmOperand& A, const G
   return w2l_gemm(currentStream(), gemmKind(), a_mn, b_mn, M, N, K, A.a.ptr(), A.ld, B.a.ptr(), B.ld, C, ldc, 0, bias, act, accumulate, aux, ld_aux, 0,
                   aux_mode, aux_scale, dropP, seed, allowOverlap);
 }
+// A weight W as the B operand of gemmWeight: b_mn = 0, B = W [N][K] (forward); b_mn = 1, B = W^T with W [K][N] (data
+// gradient).  In F32 mode the weight is split once per call into tf32 hi / lo planes ([2][N][K padded to 4]), which the
+// kernel reads instead of converting W in every row of output tiles; in the other modes nothing is made (empty).
+GemmOperand weightPlanes(int b_mn, int N, int K, const GemmOperand& W) {
+  GemmOperand planes;
+  if (gemmKind() != W2L_GEMM_F32X3) return planes;
+  planes.ld = (int)padUp(K, 4);
+  planes.a = af::array::empty(af::dim4(planes.ld, N, 2));
+  check(w2l_split_tf32(currentStream(), b_mn, b_mn ? K : N, b_mn ? N : K, W.ld, planes.ld, W.a.f32(), planes.a.f32()));
+  return planes;
+}
+// gemmP with a weight as B (K-major A), from its planes when there are any: results are bit-identical either way
+int gemmWeight(int b_mn, int M, int N, int K, const GemmOperand& A, const GemmOperand& W, const GemmOperand& planes, float* C, int ldc,
+               const float* bias, int act, int accumulate, const float* aux = nullptr, int ld_aux = 0, int aux_mode = 0, float aux_scale = 1.f,
+               float dropP = 0.f, unsigned long long seed = 0) {
+  if (planes.a.isEmpty()) return gemmP(0, b_mn, M, N, K, A, W, C, ldc, bias, act, accumulate, aux, ld_aux, aux_mode, aux_scale, dropP, seed);
+  return w2l_gemm(currentStream(), W2L_GEMM_F32X3_SPLIT_B, 0, 0, M, N, K, A.a.ptr(), A.ld, planes.a.ptr(), planes.ld, C, ldc, 0, bias, act, accumulate,
+                  aux, ld_aux, 0, aux_mode, aux_scale, dropP, seed, 0);
+}
 }  // namespace
 
 // ================================================================================================
@@ -1034,12 +1053,16 @@ Variable Linear::forwardWith(const Variable& in, const Variable& weight, const V
     wop.ld = Kp;
     wop.a = padRowsF32(wv.array().f32(), nOut, nIn, nIn, Kp);
   }
-  check(gemmP(0, 0, M, nOut, Kp, xop, wop, y.f32(), nOut, hasBias_ ? bv.array().f32() : nullptr, relu ? 1 : 0, 0, nullptr, 0, 0, 1.f, dp, nextSeed()));
+  check(gemmWeight(0, M, nOut, Kp, xop, wop, weightPlanes(0, nOut, Kp, wop), y.f32(), nOut, hasBias_ ? bv.array().f32() : nullptr, relu ? 1 : 0, 0,
+                   nullptr, 0, 0, 1.f, dp, nextSeed()));
   const int nin = nIn, nout = nOut;
   const bool hasBias = hasBias_;
   std::vector<Variable> inputs{in, wv};
   if (hasBias) inputs.push_back(bv);
   return Variable(y, inputs, [=](std::vector<Variable>& ins, const Variable& gout) {
+    // the data gradient's weight planes come first: split after the weight gradient is forked to the gradient stream, they
+    // would wait for the SMs that GEMM holds, and the data-gradient chain behind them with them
+    const GemmOperand wtPlanes = ins[0].isCalcGrad() ? weightPlanes(1, Kp, nout, wop) : GemmOperand();
     af::array dy = gout.array();
     if (!maskByConsumer && (relu || dp > 0.f)) {
       af::array m = af::array::empty(y.dims());
@@ -1083,12 +1106,12 @@ Variable Linear::forwardWith(const Variable& in, const Variable& weight, const V
       if (Kp == inCols) {
         af::array acc = ins[0].accumulableGrad();  // e.g. LN2's residual gradient: C += in the GEMM epilogue
         af::array dx = acc.isEmpty() ? af::array::empty(ins[0].dims()) : acc;
-        check(gemmP(0, 1, M, Kp, nout, dyop, wop, dx.f32(), Kp, nullptr, 0, acc.isEmpty() ? 0 : 1, inMaskMode ? ins[0].array().f32() : nullptr, Kp,
-                    inMaskMode, inMaskScale));
+        check(gemmWeight(1, M, Kp, nout, dyop, wop, wtPlanes, dx.f32(), Kp, nullptr, 0, acc.isEmpty() ? 0 : 1, inMaskMode ? ins[0].array().f32() : nullptr,
+                         Kp, inMaskMode, inMaskScale));
         if (acc.isEmpty()) ins[0].addGrad(Variable(dx, false), true);
       } else {  // the input rows were padded for the GEMM: drop the pad columns again
         af::array dxp = af::array::empty(af::dim4(Kp, M));
-        check(gemmP(0, 1, M, Kp, nout, dyop, wop, dxp.f32(), Kp, nullptr, 0, 0));
+        check(gemmWeight(1, M, Kp, nout, dyop, wop, wtPlanes, dxp.f32(), Kp, nullptr, 0, 0));
         af::array dx = af::array::empty(ins[0].dims());
         w2l::copyRows(dx.f32(), sizeof(float) * (size_t)inCols, dxp.f32(), sizeof(float) * (size_t)Kp, sizeof(float) * (size_t)inCols, (size_t)M);
         if (inMaskMode) {
