@@ -305,6 +305,12 @@ W2L_API int w2l_glu_bwd(void* stream, long long rows, int half, const float* x, 
 #define W2L_LN_SCRATCH_DOUBLES(B) (2 * W2L_LN_MAX_PARTS * (size_t)(B))
 W2L_API int w2l_layernorm_fwd(void* stream, int B, long long R, float eps, const float* a, const float* r,
                               const float* gain, const float* bias, float* y, float* mean_rstd, double* scratch);
+/* The forward of w2l_layernorm_fwd always on its one-warp-per-group kernel (G groups of R floats, no scratch).
+ * w2l_layernorm_fwd picks between that kernel and a two-pass one by the group count, and their mean / rstd round
+ * differently; here a group's result depends on its own R values only, whatever G is.  The streaming acoustic model
+ * relies on that: its per-frame LayerNorms see batches whose row count depends on the other streams in the call. */
+W2L_API int w2l_layernorm_rows_fwd(void* stream, long long G, int R, float eps, const float* a, const float* r, const float* gain,
+                                   const float* bias, float* y, float* mean_rstd);
 W2L_API int w2l_layernorm_bwd(void* stream, int B, long long R, const float* a, const float* r, const float* dy,
                               const float* gain, const float* mean_rstd, float* d_branch, float* d_res, int branch_mode,
                               float branch_scale, float* dgain, float* dbias, double* scratch);
@@ -411,6 +417,50 @@ W2L_API void* w2l_trainer_load(void* stream, const char* path);
  * library's layouts (acoustic_model.json + acoustic_model.bin), transitions.bin (ASG; the cereal std::vector<float> the
  * inference examples read, :310-326) and tokens.txt (tokens_text nullable).  Streaming TDS archs only (LN 1 2), like the converter. */
 W2L_API int w2l_trainer_export_streaming(void* trainer, void* stream, const char* outdir, const char* tokens_text);
+/* ----------------------------------------------------------------------------------------
+ * Streaming acoustic model: a trained streaming TDS network run chunk by chunk over many concurrent streams, with the
+ * semantics of the in-tree inference library (recipes/streaming_convnets/inference/inference/module/nn: Sequential,
+ * Conv1dFbGemm start / run / finish, TDSBlock, Residual, LayerNorm, Linear, Relu).  Per stream, the emissions of all
+ * run calls and the finishing one, put end to end, have the frame count of the eval-mode w2l_trainer_forward on the
+ * whole utterance and its values up to the rounding of the LayerNorm statistics (the runtime always takes the
+ * one-warp-per-frame kernel, w2l_layernorm_rows_fwd).  They are the same bits whatever the split into chunks and
+ * whatever other streams share the calls (DESIGN.md §4).  Only the convolutions keep state, per stream slot:
+ *   start  holds pad_left zero frames;
+ *   run    appends the new frames; with avail frames held, nOut = (avail - kw) / stride + 1 frames come out when
+ *          avail >= kw, and nOut * stride are consumed (at most kw - 1 stay);
+ *   finish appends pad_right zero frames, then runs.
+ * The padding of every convolution is the export's (w2l_trainer_export_streaming).  Frame counts are integer arithmetic
+ * on the host: a run call neither reads from the device nor synchronises, and returns the output frame counts at once.
+ * Calls on one handle must be ordered (one CUDA stream, or the caller's synchronisation).
+ *
+ *   w2l_stream_create   snapshots the trainer's network parameters (training may go on), takes the calling thread's
+ *                       w2l_set_precision, and allocates all state and per-call buffers for max_streams slots (at most
+ *                       1024) and chunks of at most max_chunk frames.  Accepts exactly the archs the export accepts,
+ *                       with its error text.  NULL on failure (w2l_last_error).
+ *   w2l_stream_state_bytes   device bytes of carried state per slot (two planes of the held frames of every convolution)
+ *   w2l_stream_max_frames_out  the most output frames one call can give a stream (sizes the emission buffer)
+ *   w2l_stream_start    resets the n slots (host int slots[n]) and holds their left padding; a running slot forgets its past
+ *   w2l_stream_run      slots[n], frames_in[n] (host ints, each <= Tc <= max_chunk), features device [n][1][nFeat][Tc]
+ *                       (ArrayFire [Tc,nFeat,1,n], the trainer's layout); emissions device [n][T'max][nLabel] with
+ *                       T'max = max frames_out, rows t >= frames_out[i] of stream i unspecified; capacity in floats;
+ *                       frames_out[n] host.  finish = 1 appends every layer's right padding after the chunk, and the
+ *                       slot stays finished until the next start.  Errors (W2L_ERR_INVALID_ARGUMENT): a slot out of range
+ *                       or listed twice, a slot not started or already finished, a chunk longer than Tc, Tc > max_chunk,
+ *                       too small a capacity.
+ *   w2l_stream_plan     host only: the frame bookkeeping of one stream over n_calls calls of frames_host[k] frames (the
+ *                       last one finishing when finish_last), for every convolution c of the arch: conv_spec_host
+ *                       [c][4] = {kw, stride, pad_left, pad_right}, frames_out_host[k][max_convs] and tails_host
+ *                       [k][max_convs] (frames held after call k); n_convs gets the convolution count.
+ * ---------------------------------------------------------------------------------------- */
+W2L_API void* w2l_stream_create(void* trainer, void* stream, int max_streams, int max_chunk);
+W2L_API void w2l_stream_destroy(void* s);
+W2L_API long long w2l_stream_state_bytes(void* s);
+W2L_API int w2l_stream_max_frames_out(void* s);
+W2L_API int w2l_stream_start(void* s, void* stream, int n, const int* slots);
+W2L_API int w2l_stream_run(void* s, void* stream, int n, const int* slots, const int* frames_in, const float* features, int Tc, int finish,
+                           float* emissions, long long capacity, int* frames_out);
+W2L_API int w2l_stream_plan(const char* arch_text, int n_feat, int n_label, int n_calls, const int* frames_host, int finish_last,
+                            int max_convs, int* n_convs, int* conv_spec_host, int* frames_out_host, int* tails_host);
 /* data-parallel rendezvous: rank 0 creates the 128-byte NCCL id, the launcher ships it to every rank */
 W2L_API int w2l_nccl_unique_id(void* out128);
 W2L_API int w2l_init_distributed(int rank, int world, const void* id128);

@@ -30,13 +30,15 @@ EXPORTS = [
     "w2l_text_create", "w2l_text_destroy", "w2l_text_num_classes", "w2l_text_encode", "w2l_text_prediction2ltr", "w2l_text_target2ltr",
     "w2l_text_ltr2wrd", "w2l_text_align_words", "w2l_edit_distance",
     "w2l_gemm_set_variant", "w2l_gemm_set_tile", "w2l_gemm_tf32", "w2l_gemm_tf32_ex", "w2l_gemm_tf32_view", "w2l_conv_time_workspace_size", "w2l_conv_time_fwd", "w2l_conv_time_dgrad",
-    "w2l_conv_time_wgrad", "w2l_layernorm_fwd", "w2l_layernorm_bwd", "w2l_colsum_accumulate", "w2l_sq_norm_accumulate",
+    "w2l_conv_time_wgrad", "w2l_layernorm_fwd", "w2l_layernorm_rows_fwd", "w2l_layernorm_bwd", "w2l_colsum_accumulate", "w2l_sq_norm_accumulate",
     "w2l_sgd_step", "w2l_weightnorm_fwd", "w2l_weightnorm_bwd", "w2l_conv1d_arrange", "w2l_conv1d_arrange_ex", "w2l_conv1d_unarrange_grad",
     "w2l_glu_fwd", "w2l_glu_bwd", "w2l_transpose_input", "w2l_axpy", "w2l_fill", "w2l_act_fwd", "w2l_mask_mul",
     "w2l_trainer_create", "w2l_trainer_destroy", "w2l_trainer_step", "w2l_trainer_forward", "w2l_trainer_num_params",
     "w2l_trainer_param_layout", "w2l_trainer_get_flat", "w2l_trainer_set_flat", "w2l_trainer_sync_parameters",
     "w2l_trainer_describe", "w2l_nccl_unique_id", "w2l_init_distributed", "w2l_trainer_align", "w2l_trainer_time_stride",
     "w2l_mfsc_num_frames", "w2l_mfsc_workspace_size", "w2l_mfsc",
+    "w2l_stream_create", "w2l_stream_destroy", "w2l_stream_state_bytes", "w2l_stream_max_frames_out", "w2l_stream_start",
+    "w2l_stream_run", "w2l_stream_plan",
 ]
 
 
@@ -98,6 +100,7 @@ def _load() -> ctypes.CDLL:
     lib.w2l_conv_time_dgrad.argtypes = [vp, i, i, i, i, i, i, i, i, i, vp, vp, vp, vp, vp, sz]
     lib.w2l_conv_time_wgrad.argtypes = [vp, i, i, i, i, i, i, i, i, i, vp, vp, vp, vp, vp, sz]
     lib.w2l_layernorm_fwd.argtypes = [vp, i, ll, f32, vp, vp, vp, vp, vp, vp, vp]
+    lib.w2l_layernorm_rows_fwd.argtypes = [vp, ll, i, f32, vp, vp, vp, vp, vp, vp]
     lib.w2l_layernorm_bwd.argtypes = [vp, i, ll, vp, vp, vp, vp, vp, vp, vp, i, f32, vp, vp, vp]
     lib.w2l_colsum_accumulate.argtypes = [vp, i, i, vp, i, vp]
     lib.w2l_sq_norm_accumulate.argtypes = [vp, ll, vp, vp]
@@ -156,6 +159,16 @@ def _load() -> ctypes.CDLL:
     lib.w2l_mfsc_workspace_size.restype = sz
     lib.w2l_mfsc_workspace_size.argtypes = [i, i, i, i, i, i]
     lib.w2l_mfsc.argtypes = [vp, i, i, vp, vp, i, i, i, i, i, vp, i, vp, sz]
+    lib.w2l_stream_create.restype = vp
+    lib.w2l_stream_create.argtypes = [vp, vp, i, i]
+    lib.w2l_stream_destroy.argtypes = [vp]
+    lib.w2l_stream_destroy.restype = None
+    lib.w2l_stream_state_bytes.restype = ctypes.c_longlong
+    lib.w2l_stream_state_bytes.argtypes = [vp]
+    lib.w2l_stream_max_frames_out.argtypes = [vp]
+    lib.w2l_stream_start.argtypes = [vp, vp, i, vp]
+    lib.w2l_stream_run.argtypes = [vp, vp, i, vp, vp, vp, i, i, vp, ctypes.c_longlong, vp]
+    lib.w2l_stream_plan.argtypes = [ctypes.c_char_p, i, i, i, vp, i, i, vp, vp, vp, vp]
     return lib
 
 

@@ -1156,6 +1156,17 @@ extern "C" int w2l_layernorm_fwd(void* stream_, int B, long long R, float eps, c
   return W2L_OK;
 }
 
+// always the one-warp-per-group kernel, whatever the group count: a group's result depends on its own R values only
+extern "C" int w2l_layernorm_rows_fwd(void* stream_, long long G, int R, float eps, const float* a, const float* r, const float* gain,
+                                      const float* bias, float* y, float* mean_rstd) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (G <= 0 || R <= 0 || !a || !y || !mean_rstd) return fail(W2L_ERR_INVALID_ARGUMENT, "layernorm_rows_fwd: bad arguments");
+  const int vec = (R % 4 == 0) && !((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(r) | reinterpret_cast<uintptr_t>(y)) & 15);
+  ln_row_fwd_kernel<<<(unsigned)((G + 7) / 8), 256, 0, stream>>>(G, R, vec, eps, a, r, gain, bias, y, mean_rstd);
+  W2L_LAUNCH_CHECK("ln_row_fwd_kernel");
+  return W2L_OK;
+}
+
 extern "C" int w2l_layernorm_bwd(void* stream_, int B, long long R, const float* a, const float* r, const float* dy,
                                  const float* gain, const float* mean_rstd, float* d_branch, float* d_res, int branch_mode,
                                  float branch_scale, float* dgain, float* dbias, double* scratch) {

@@ -1,0 +1,603 @@
+// stream_capi.cpp — the streaming acoustic model: a trained streaming TDS network run chunk by chunk over many
+// concurrent streams with the semantics of the in-tree inference library (recipes/streaming_convnets/inference/
+// inference/module/nn: Sequential, Conv1dFbGemm start / run / finish, TDSBlock, Residual, LayerNorm, Linear, Relu).
+//
+// Only the convolutions keep state.  For every call and every convolution the state kernel (csrc/stream_kernels.cu)
+// builds each stream's window [held tail | new frames | right padding on finish] in a batch padded to the longest
+// window, and keeps the unconsumed frames as the stream's next tail; the convolution, the GEMMs and the per-frame
+// LayerNorms then run once over that batch, with the kernels and operands of the training network's eval forward, except
+// that the LayerNorm is always its one-warp-per-frame kernel (the forward chooses by row count; here the row count
+// depends on the other streams in the call, and a stream's emissions must not).  Rows past a
+// stream's valid frames are slack: computed, finite, never read as data (every layer after a convolution is per
+// frame).  All frame counts follow from integer arithmetic on the host, so a call neither reads from the device nor
+// synchronises.  DESIGN.md §4.
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <cstdint>
+#include <cstring>
+#include <memory>
+#include <sstream>
+#include <stdexcept>
+#include <string>
+#include <vector>
+
+#include "stream_internal.h"
+#include "w2l_b200.h"
+
+namespace w2l {
+int fail(int code, const std::string& msg);
+void check(int rc);
+
+namespace streaming {
+
+Arch parseArch(const std::string& archText, int nFeat, int nLabel) {
+  Arch a;
+  a.W = nFeat;
+  std::istringstream in(archText);
+  std::string line;
+  int curC = 1, padL = -1, padR = -1;
+  while (std::getline(in, line)) {
+    const auto hash = line.find('#');
+    if (hash != std::string::npos) line = line.substr(0, hash);
+    for (const char* key : {"NFEAT", "NLABEL"}) {
+      size_t pos;
+      const std::string val = std::to_string(std::string(key) == "NFEAT" ? nFeat : nLabel);
+      while ((pos = line.find(key)) != std::string::npos) line.replace(pos, std::strlen(key), val);
+    }
+    std::istringstream ls(line);
+    std::vector<std::string> c;
+    std::string tok;
+    while (ls >> tok) c.push_back(tok);
+    if (c.empty()) continue;
+    const std::string& op = c[0];
+    Layer l;
+    l.curC = curC;
+    if (op == "PD") {
+      if (c.size() != 4) throw std::invalid_argument("export: padding is supported only along the time axis");
+      padL = std::stoi(c[2]);
+      padR = std::stoi(c[3]);
+      continue;
+    } else if (op == "C2") {
+      if (c.size() < 8) throw std::invalid_argument("export: invalid arch specified for C2");
+      l.op = Op::Conv;
+      l.cin = std::stoi(c[1]);
+      l.cout = std::stoi(c[2]);
+      l.kw = std::stoi(c[3]);
+      l.stride = std::stoi(c[5]);
+      l.padL = padL;
+      l.padR = padR;
+      if (l.padL == -1 && l.padR == -1) l.padL = l.padR = (l.kw - l.stride + 1) / 2;
+      l.nParams = 2;
+      padL = padR = -1;
+      curC = l.cout;
+    } else if (op == "R") {
+      l.op = Op::Relu;
+    } else if (op == "LN") {
+      if (c.size() != 3 || c[1] != "1" || c[2] != "2") throw std::invalid_argument("export: unsupported LayerNorm axis: must be {1, 2} for streaming");
+      l.op = Op::LayerNorm;
+      l.nParams = 2;
+    } else if (op == "L") {
+      l.op = Op::Linear;
+      l.nin = std::stoi(c[1]);
+      l.nout = std::stoi(c[2]);
+      if (l.nin != curC * nFeat) throw std::invalid_argument("export: the Linear head does not take a whole frame");
+      l.nParams = 2;
+    } else if (op == "TDS") {
+      const int ch = std::stoi(c[1]), kw = std::stoi(c[2]), w = std::stoi(c[3]);
+      const int inner = c.size() > 5 && std::stoi(c[5]) > 0 ? std::stoi(c[5]) : ch * w;
+      const int rpad = c.size() > 6 ? std::stoi(c[6]) : -1;
+      if (w != nFeat) throw std::invalid_argument("export: the TDS width must be the filterbank count");
+      if (c.size() > 7 && std::stoi(c[7]) != 0) throw std::invalid_argument("export: streaming TDS blocks normalise per frame (lNormIncludeTime = 0)");
+      l.op = Op::Tds;
+      l.cin = l.cout = ch;
+      l.kw = kw;
+      l.padR = rpad >= 0 ? rpad : (kw - 1 + 1) / 2;
+      l.padL = rpad >= 0 ? kw - 1 - rpad : (kw - 1 + 1) / 2;
+      l.inner = inner;
+      l.nParams = 10;
+      curC = ch;
+    } else if (op == "V" || op == "RO" || op == "DO" || op == "SAUG") {
+      continue;  // skipped, as the converter does
+    } else {
+      throw std::logic_error("export: unrecognized/unparsable line " + line);
+    }
+    a.layers.push_back(l);
+  }
+  return a;
+}
+
+}  // namespace streaming
+}  // namespace w2l
+
+using namespace w2l::streaming;
+
+namespace {
+template <typename F>
+int guarded(F&& f) {
+  try {
+    f();
+    return W2L_OK;
+  } catch (const std::invalid_argument& e) {
+    return w2l::fail(W2L_ERR_INVALID_ARGUMENT, e.what());
+  } catch (const std::exception& e) {
+    return w2l::fail(W2L_ERR_CUDA, e.what());
+  }
+}
+void cuda(cudaError_t e, const char* what) {
+  if (e != cudaSuccess) throw std::runtime_error(std::string(what) + ": " + cudaGetErrorString(e));
+}
+long long up4(long long n) { return (n + 3) / 4 * 4; }
+long long up8(long long n) { return (n + 7) / 8 * 8; }
+
+struct PrecisionScope {  // the runtime's precision for the duration of one call; the thread's own setting is restored
+  int saved;
+  explicit PrecisionScope(int p) : saved(w2l_get_precision()) { w2l_set_precision(p); }
+  ~PrecisionScope() { w2l_set_precision(saved); }
+};
+
+// a Linear layer's weight as the B operand of the forward GEMM in the runtime's precision, made once at create exactly
+// as fl::Linear makes it per call: TF32 the fp32 rows ([nout][K], K = nin padded to 4 floats), F32 the pre-split
+// tf32 hi / lo planes of those rows, BF16 the rows cast to bf16 ([nout][nin padded to 8])
+struct DenseWeight {
+  int nin = 0, nout = 0, K = 0, kind = W2L_GEMM_TF32;
+  const void* B = nullptr;
+  const float* bias = nullptr;
+};
+
+struct Slot {
+  int status = 0;  // 0 never started, 1 running, 2 finished
+  int plane = 0;   // the state plane holding the current tails
+  std::vector<int> tails;  // per convolution
+};
+
+struct Stream {
+  Arch arch;
+  int nFeat = 0, nLabel = 0, precision = 0, maxStreams = 0, maxChunk = 0;
+  std::vector<int> convOf;         // layer -> index among the convolutions (-1 for other layers)
+  std::vector<size_t> paramBase;   // layer -> index of its first parameter
+  std::vector<int> padL;           // per convolution: the zero frames start puts in front
+  std::vector<long long> stateOff;  // per convolution: offset of its region inside a plane
+  long long planeFloats = 0;
+  std::vector<char*> blocks;  // cudaMalloc'd
+  float* snapshot = nullptr;  // parameter copy
+  std::vector<const float*> params;  // per parameter, into snapshot
+  std::vector<DenseWeight> dense;    // per Linear (TDS blocks: two)
+  std::vector<int> denseOf;          // layer -> first index into dense (-1)
+  float* state = nullptr;
+  float* xT = nullptr;  // [n][Tc][nFeat]
+  float* win = nullptr;
+  float* act[4] = {nullptr, nullptr, nullptr, nullptr};
+  float* hidden = nullptr;
+  void* opA = nullptr;  // padded fp32 / bf16 copy of a GEMM's A operand
+  float* meanRstd = nullptr;
+  void* convWs = nullptr;
+  size_t convWsBytes = 0;
+  int maxOut = 0;  // bound on the output frames of one call
+  std::vector<Slot> slots;
+
+  ~Stream() {
+    for (char* b : blocks) cudaFree(b);
+  }
+  template <typename T>
+  T* alloc(size_t n) {
+    char* p = nullptr;
+    cuda(cudaMalloc(&p, std::max<size_t>(n * sizeof(T), 256)), "stream: cudaMalloc");
+    blocks.push_back(p);
+    return reinterpret_cast<T*>(p);
+  }
+  long long slotFloats() const { return 2 * planeFloats; }
+};
+
+// frames of every layer of one call: per convolution and stream the buffer rule, per layer the padded batch
+struct Plan {
+  std::vector<std::vector<int>> fresh, out, tails;  // [conv][stream]
+  std::vector<int> winFrames, outFrames;            // [conv]: longest window, longest output (the padded batch)
+  std::vector<int> framesOut;                       // [stream]
+  int tOutMax = 0;
+};
+Plan plan(const Arch& arch, int n, const std::vector<std::vector<int>>& tails, const int* framesIn, bool finish) {
+  Plan p;
+  std::vector<int> cur(framesIn, framesIn + n);
+  int ci = 0;
+  for (const Layer& l : arch.layers) {
+    if (l.op != Op::Conv && l.op != Op::Tds) continue;
+    p.fresh.push_back(cur);
+    std::vector<int> o(n), t(n);
+    int wmax = 0, omax = 0;
+    for (int i = 0; i < n; ++i) {
+      const ConvStep s = convStep(tails[ci][i], cur[i], finish ? l.padR : 0, l.kw, l.stride);
+      o[i] = s.nOut;
+      t[i] = s.tail;
+      wmax = std::max(wmax, s.avail);
+      omax = std::max(omax, s.nOut);
+    }
+    p.out.push_back(o);
+    p.tails.push_back(t);
+    p.winFrames.push_back(wmax);
+    p.outFrames.push_back(omax);
+    cur = o;
+    ++ci;
+  }
+  p.framesOut = cur;
+  p.tOutMax = n ? *std::max_element(cur.begin(), cur.end()) : 0;
+  return p;
+}
+
+Stream* asStream(void* h) {
+  if (!h) throw std::invalid_argument("stream: null handle");
+  return static_cast<Stream*>(h);
+}
+
+void checkSlots(const Stream* s, int n, const int* slots, bool forRun) {
+  if (n <= 0 || n > s->maxStreams) throw std::invalid_argument("stream: n must be in [1, max_streams]");
+  if (!slots) throw std::invalid_argument("stream: null slot list");
+  std::vector<char> seen(s->maxStreams, 0);
+  for (int i = 0; i < n; ++i) {
+    const int k = slots[i];
+    if (k < 0 || k >= s->maxStreams) throw std::invalid_argument("stream: slot " + std::to_string(k) + " out of range [0, max_streams)");
+    if (seen[k]) throw std::invalid_argument("stream: slot " + std::to_string(k) + " listed twice in one call");
+    seen[k] = 1;
+    if (forRun && s->slots[k].status == 0) throw std::invalid_argument("stream: run on slot " + std::to_string(k) + ", which is not started");
+    if (forRun && s->slots[k].status == 2) throw std::invalid_argument("stream: run on slot " + std::to_string(k) + ", which is finished (start it again)");
+  }
+}
+
+// C[M][nout] = act(A[M][nin] W^T + bias) on the GEMM, A prepared as fl::Linear prepares it
+void dense(Stream* s, cudaStream_t st, const DenseWeight& w, long long M, const float* A, float* C, int act) {
+  const void* a = A;
+  if (w.kind == W2L_GEMM_BF16) {
+    if (w.K == w.nin)
+      w2l::check(w2l_cast_bf16(st, M * w.nin, A, s->opA));
+    else
+      w2l::check(w2l_cast_bf16_rows(st, M, w.nin, w.nin, w.K, A, s->opA));
+    a = s->opA;
+  } else if (w.K != w.nin) {
+    cuda(cudaMemsetAsync(s->opA, 0, sizeof(float) * (size_t)(M * w.K), st), "stream: pad");
+    cuda(cudaMemcpy2DAsync(s->opA, sizeof(float) * w.K, A, sizeof(float) * w.nin, sizeof(float) * w.nin, (size_t)M, cudaMemcpyDeviceToDevice, st),
+         "stream: pad");
+    a = s->opA;
+  }
+  w2l::check(w2l_gemm(st, w.kind, 0, 0, (int)M, w.nout, w.K, a, w.K, w.B, w.K, C, w.nout, 0, w.bias, act, 0, nullptr, 0, 0, 0, 1.f, 0.f, 0ull, 0));
+}
+
+// the per-frame LayerNorm always on its one-warp-per-frame kernel: w2l_layernorm_fwd would choose its kernel by the row
+// count, which depends on the other streams in the call, and the two kernels round mean / rstd differently
+void layerNorm(Stream* s, cudaStream_t st, long long rows, int F, const float* a, const float* r, const float* gain, const float* bias, float* y) {
+  w2l::check(w2l_layernorm_rows_fwd(st, rows, F, 1e-5f, a, r, gain, bias, y, s->meanRstd));
+}
+}  // namespace
+
+extern "C" {
+
+W2L_API int w2l_stream_plan(const char* arch_text, int n_feat, int n_label, int n_calls, const int* frames_host, int finish_last, int max_convs,
+                            int* n_convs, int* conv_spec_host, int* frames_out_host, int* tails_host) {
+  return guarded([&] {
+    if (!arch_text || n_feat <= 0 || n_label <= 0 || n_calls < 0 || (n_calls && !frames_host) || !n_convs)
+      throw std::invalid_argument("stream_plan: bad arguments");
+    const Arch arch = parseArch(arch_text, n_feat, n_label);
+    std::vector<const Layer*> convs;
+    for (const Layer& l : arch.layers)
+      if (l.op == Op::Conv || l.op == Op::Tds) convs.push_back(&l);
+    *n_convs = (int)convs.size();
+    if ((int)convs.size() > max_convs) throw std::invalid_argument("stream_plan: more convolutions than max_convs");
+    for (size_t c = 0; c < convs.size() && conv_spec_host; ++c) {
+      conv_spec_host[4 * c] = convs[c]->kw;
+      conv_spec_host[4 * c + 1] = convs[c]->stride;
+      conv_spec_host[4 * c + 2] = convs[c]->padL;
+      conv_spec_host[4 * c + 3] = convs[c]->padR;
+    }
+    std::vector<std::vector<int>> tails(convs.size(), std::vector<int>(1));
+    for (size_t c = 0; c < convs.size(); ++c) tails[c][0] = convs[c]->padL;
+    for (int k = 0; k < n_calls; ++k) {
+      if (frames_host[k] < 0) throw std::invalid_argument("stream_plan: negative frame count");
+      const Plan p = plan(arch, 1, tails, frames_host + k, finish_last && k == n_calls - 1);
+      for (size_t c = 0; c < convs.size(); ++c) {
+        if (frames_out_host) frames_out_host[(size_t)k * max_convs + c] = p.out[c][0];
+        if (tails_host) tails_host[(size_t)k * max_convs + c] = p.tails[c][0];
+        tails[c][0] = p.tails[c][0];
+      }
+    }
+  });
+}
+
+W2L_API void* w2l_stream_create(void* trainer, void* stream, int max_streams, int max_chunk) {
+  Stream* out = nullptr;
+  guarded([&] {
+    if (!trainer) throw std::invalid_argument("stream_create: null trainer");
+    if (max_streams <= 0 || max_streams > kMaxCallStreams)
+      throw std::invalid_argument("stream_create: max_streams must be in [1, " + std::to_string(kMaxCallStreams) + "]");
+    if (max_chunk <= 0 || max_chunk > 32767) throw std::invalid_argument("stream_create: max_chunk must be in [1, 32767] frames");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const TrainerSnapshotSource src = trainerSnapshotSource(trainer);
+    auto s = std::make_unique<Stream>();
+    s->arch = parseArch(src.arch, src.nFeat, src.nLabel);
+    s->nFeat = src.nFeat;
+    s->nLabel = src.nLabel;
+    s->precision = w2l_get_precision();  // the creating thread's setting, as for the trainer
+    s->maxStreams = max_streams;
+    s->maxChunk = max_chunk;
+    const int W = src.nFeat;
+    // parameters: one copy, so training can go on while streams run
+    long long total = 0;
+    for (const auto& p : src.params) total += up4(p.second);
+    s->snapshot = s->alloc<float>((size_t)total);
+    {
+      long long off = 0;
+      for (const auto& p : src.params) {
+        cuda(cudaMemcpyAsync(s->snapshot + off, p.first, sizeof(float) * (size_t)p.second, cudaMemcpyDeviceToDevice, st), "stream: snapshot");
+        s->params.push_back(s->snapshot + off);
+        off += up4(p.second);
+      }
+    }
+    // walk the layers: shapes, parameter use and the largest buffer of every kind
+    size_t pi = 0;
+    auto next = [&](long long expect) {
+      if (pi >= src.params.size()) throw std::runtime_error("export: not enough parameters for the arch");
+      if (expect >= 0 && src.params[pi].second != expect) throw std::invalid_argument("stream_create: a parameter does not have the arch's shape");
+      return s->params[pi++];
+    };
+    const int kind = s->precision == W2L_PRECISION_BF16 ? W2L_GEMM_BF16 : s->precision == W2L_PRECISION_F32 ? W2L_GEMM_F32X3_SPLIT_B : W2L_GEMM_TF32;
+    auto makeDense = [&](int nin, int nout, const float* w, const float* b) {
+      DenseWeight d;
+      d.nin = nin;
+      d.nout = nout;
+      d.kind = kind;
+      d.bias = b;
+      if (kind == W2L_GEMM_BF16) {
+        d.K = (int)up8(nin);
+        void* wb = s->alloc<uint16_t>((size_t)nout * d.K);
+        if (d.K == nin)
+          w2l::check(w2l_cast_bf16(st, (long long)nout * nin, w, wb));
+        else
+          w2l::check(w2l_cast_bf16_rows(st, nout, nin, nin, d.K, w, wb));
+        d.B = wb;
+      } else {
+        d.K = (int)up4(nin);
+        const float* rows = w;
+        if (d.K != nin) {
+          float* p = s->alloc<float>((size_t)nout * d.K);
+          cuda(cudaMemsetAsync(p, 0, sizeof(float) * (size_t)nout * d.K, st), "stream: pad weight");
+          cuda(cudaMemcpy2DAsync(p, sizeof(float) * d.K, w, sizeof(float) * nin, sizeof(float) * nin, (size_t)nout, cudaMemcpyDeviceToDevice, st),
+               "stream: pad weight");
+          rows = p;
+        }
+        if (kind == W2L_GEMM_F32X3_SPLIT_B) {
+          float* planes = s->alloc<float>((size_t)2 * nout * d.K);
+          w2l::check(w2l_split_tf32(st, 0, nout, d.K, d.K, d.K, rows, planes));
+          d.B = planes;
+        } else {
+          d.B = rows;
+        }
+      }
+      s->dense.push_back(d);
+    };
+    int fresh = max_chunk, feat = W;  // most new frames a layer can receive; floats per frame
+    long long maxAct = 1, maxWin = 1, maxHidden = 1, maxOpA = 1, maxFrames = 1;  // per stream
+    size_t ws = 0;
+    for (size_t li = 0; li < s->arch.layers.size(); ++li) {
+      const Layer& l = s->arch.layers[li];
+      s->convOf.push_back(-1);
+      s->denseOf.push_back(-1);
+      s->paramBase.push_back(pi);
+      if (l.op == Op::Conv || l.op == Op::Tds) {
+        if (feat != l.cin * W) throw std::invalid_argument("stream_create: a convolution does not take the frames the layer before it makes");
+        s->convOf.back() = (int)s->stateOff.size();
+        s->stateOff.push_back(s->planeFloats);
+        s->padL.push_back(l.padL);
+        s->planeFloats += up4((long long)maxTail(l) * feat);
+        const int win = maxTail(l) + fresh + l.padR;
+        const int outF = win >= l.kw ? (win - l.kw) / l.stride + 1 : 0;
+        maxWin = std::max(maxWin, (long long)win * feat);
+        ws = std::max(ws, w2l_conv_time_workspace_size(max_streams, std::max(outF, 1), l.cin, l.cout, l.kw));
+        next((long long)l.cout * l.cin * l.kw);
+        next(l.cout);
+        fresh = outF;
+        feat = l.cout * W;
+        maxFrames = std::max(maxFrames, (long long)fresh);
+        if (l.op == Op::Tds) {
+          next(1);
+          next(1);
+          const float* w1 = next((long long)feat * l.inner);
+          const float* b1 = next(l.inner);
+          const float* w2 = next((long long)l.inner * feat);
+          const float* b2 = next(feat);
+          next(1);
+          next(1);
+          s->denseOf.back() = (int)s->dense.size();
+          makeDense(feat, l.inner, w1, b1);
+          makeDense(l.inner, feat, w2, b2);
+          maxHidden = std::max(maxHidden, (long long)fresh * l.inner);
+          maxOpA = std::max(maxOpA, (long long)fresh * up8(std::max(feat, l.inner)));
+        }
+      } else if (l.op == Op::LayerNorm) {
+        next(1);
+        next(1);
+      } else if (l.op == Op::Linear) {
+        if (feat != l.nin) throw std::invalid_argument("stream_create: the Linear layer does not take the frames the layer before it makes");
+        const float* w = next((long long)l.nin * l.nout);
+        const float* b = next(l.nout);
+        s->denseOf.back() = (int)s->dense.size();
+        makeDense(l.nin, l.nout, w, b);
+        maxOpA = std::max(maxOpA, (long long)fresh * up8(l.nin));
+        feat = l.nout;
+      }
+      maxAct = std::max(maxAct, (long long)fresh * feat);
+    }
+    if (pi != src.params.size()) throw std::runtime_error("export: parameters left over after walking the arch");
+    if (s->stateOff.empty()) throw std::invalid_argument("stream_create: the arch has no convolution, nothing to stream");
+    if (feat != src.nLabel) throw std::invalid_argument("stream_create: the last layer does not produce NLABEL values per frame");
+    s->maxOut = fresh;
+    // state and per-call buffers, all up front
+    s->state = s->alloc<float>((size_t)max_streams * (size_t)s->slotFloats());
+    s->xT = s->alloc<float>((size_t)max_streams * max_chunk * W);
+    s->win = s->alloc<float>((size_t)max_streams * maxWin);
+    for (auto& a : s->act) a = s->alloc<float>((size_t)max_streams * maxAct);
+    s->hidden = s->alloc<float>((size_t)max_streams * maxHidden);
+    s->opA = s->alloc<float>((size_t)max_streams * maxOpA);
+    const long long rows = (long long)max_streams * maxFrames;
+    s->meanRstd = s->alloc<float>((size_t)(2 * rows));
+    s->convWsBytes = std::max<size_t>(ws, 256);
+    s->convWs = s->alloc<char>(s->convWsBytes);
+    s->slots.resize(max_streams);
+    for (auto& sl : s->slots) sl.tails.assign(s->stateOff.size(), 0);
+    cuda(cudaMemsetAsync(s->state, 0, sizeof(float) * (size_t)max_streams * (size_t)s->slotFloats(), st), "stream: state");
+    cuda(cudaStreamSynchronize(st), "stream_create");
+    out = s.release();
+  });
+  return out;
+}
+
+W2L_API void w2l_stream_destroy(void* h) { delete static_cast<Stream*>(h); }
+
+W2L_API long long w2l_stream_state_bytes(void* h) {
+  if (!h) return -1;
+  return (long long)sizeof(float) * static_cast<Stream*>(h)->slotFloats();
+}
+
+W2L_API int w2l_stream_max_frames_out(void* h) {
+  if (!h) return -1;
+  return static_cast<Stream*>(h)->maxOut;
+}
+
+W2L_API int w2l_stream_start(void* h, void* stream, int n, const int* slots) {
+  return guarded([&] {
+    Stream* s = asStream(h);
+    checkSlots(s, n, slots, false);
+    w2l::check(launchZeroSlots(stream, s->state, s->slotFloats(), n, slots));
+    for (int i = 0; i < n; ++i) {
+      Slot& sl = s->slots[slots[i]];
+      sl.status = 1;
+      sl.plane = 0;
+      sl.tails = s->padL;  // left padding: zero frames held before the first input frame
+    }
+  });
+}
+
+W2L_API int w2l_stream_run(void* h, void* stream, int n, const int* slots, const int* frames_in, const float* features, int Tc, int finish,
+                           float* emissions, long long capacity, int* frames_out) {
+  return guarded([&] {
+    Stream* s = asStream(h);
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    checkSlots(s, n, slots, true);
+    if (!frames_in || !frames_out) throw std::invalid_argument("stream_run: null frame-count array");
+    if (Tc < 0 || Tc > s->maxChunk) throw std::invalid_argument("stream_run: Tc must be in [0, max_chunk]");
+    int most = 0;
+    for (int i = 0; i < n; ++i) {
+      if (frames_in[i] < 0 || frames_in[i] > Tc)
+        throw std::invalid_argument("stream_run: the chunk of slot " + std::to_string(slots[i]) + " is longer than Tc (or negative)");
+      most = std::max(most, frames_in[i]);
+    }
+    if (most > 0 && !features) throw std::invalid_argument("stream_run: null features");
+    const int W = s->nFeat;
+    const size_t nc = s->stateOff.size();
+    std::vector<std::vector<int>> tails(nc, std::vector<int>(n));
+    for (size_t c = 0; c < nc; ++c)
+      for (int i = 0; i < n; ++i) tails[c][i] = s->slots[slots[i]].tails[c];
+    const Plan p = plan(s->arch, n, tails, frames_in, finish != 0);
+    if ((long long)n * p.tOutMax * s->nLabel > capacity) throw std::invalid_argument("stream_run: emission buffer too small (capacity)");
+    if (p.tOutMax > 0 && !emissions) throw std::invalid_argument("stream_run: null emissions");
+    PrecisionScope scope(s->precision);
+    // [n][1][F][Tc] (ArrayFire [Tc,F,1,n]) -> [n][Tc][F]: frames of W groups of one channel
+    if (most > 0) w2l::check(w2l_transpose_input(st, n, W, Tc, features, s->xT));
+    const float* cur = s->xT;
+    int curFrames = Tc;  // frame stride of every stream in `cur`
+    bool live = true;    // the padded batch has frames
+    auto pick = [&](std::initializer_list<const float*> busy) {
+      for (float* a : s->act)
+        if (std::find(busy.begin(), busy.end(), a) == busy.end()) return a;
+      throw std::logic_error("stream: no free activation buffer");
+    };
+    const auto& layers = s->arch.layers;
+    for (size_t li = 0; li < layers.size(); ++li) {
+      const Layer& l = layers[li];
+      const int feat = l.curC * W;
+      if (l.op == Op::Conv || l.op == Op::Tds) {
+        const int c = s->convOf[li];
+        const int win = p.winFrames[c], tout = p.outFrames[c];
+        if (win > 0) {
+          WindowArgs a;
+          a.in = cur;
+          a.win = s->win;
+          a.state = s->state + s->stateOff[c];
+          a.slotFloats = s->slotFloats();
+          a.planeFloats = s->planeFloats;
+          a.inFrames = curFrames;
+          a.winFrames = win;
+          a.F = feat;
+          a.kw = l.kw;
+          a.stride = l.stride;
+          a.padR = finish ? l.padR : 0;
+          a.n = n;
+          for (int i = 0; i < n; ++i) {
+            a.code[i] = slots[i] << 1 | s->slots[slots[i]].plane;
+            a.cnt[i] = tails[c][i] << 16 | p.fresh[c][i];
+          }
+          w2l::check(launchWindow(st, a));
+        }
+        live = tout > 0;
+        curFrames = tout;
+        if (!live) continue;
+        const size_t pidx = s->paramBase[li];
+        const float* w = s->params[pidx];
+        const float* b = s->params[pidx + 1];
+        const long long rows = (long long)n * tout;
+        const int fout = l.cout * W;
+        if (l.op == Op::Conv) {
+          // a ReLU right after the convolution runs in its epilogue, as in the training network
+          const bool relu = li + 1 < layers.size() && layers[li + 1].op == Op::Relu;
+          float* y = pick({cur});
+          w2l::check(w2l_conv_time_fwd(st, n, win, tout, W, l.cin, l.cout, l.kw, l.stride, 0, s->win, w, b, nullptr, y, relu ? 1 : 0, 0.f, 0ull,
+                                       s->convWs, s->convWsBytes));
+          cur = y;
+          if (relu) ++li;
+          continue;
+        }
+        // TDS: LN1(x + relu(conv x)) -> LN2(z + W2 relu(W1 z + b1) + b2); the residual x of output frame j is window
+        // frame j + padL (the convolution reads frames j .. j + kw - 1 of the window)
+        float* y1 = pick({cur});
+        w2l::check(w2l_conv_time_fwd(st, n, win, tout, W, l.cin, l.cout, l.kw, 1, 0, s->win, w, b, nullptr, y1, 1, 0.f, 0ull, s->convWs, s->convWsBytes));
+        float* res = pick({cur, y1});
+        cuda(cudaMemcpy2DAsync(res, sizeof(float) * (size_t)tout * feat, s->win + (size_t)l.padL * feat, sizeof(float) * (size_t)win * feat,
+                               sizeof(float) * (size_t)tout * feat, (size_t)n, cudaMemcpyDeviceToDevice, st),
+             "stream: residual");
+        float* z = pick({cur, y1, res});
+        layerNorm(s, st, rows, fout, y1, res, s->params[pidx + 2], s->params[pidx + 3], z);
+        const DenseWeight& d1 = s->dense[s->denseOf[li]];
+        const DenseWeight& d2 = s->dense[s->denseOf[li] + 1];
+        dense(s, st, d1, rows, z, s->hidden, 1);
+        dense(s, st, d2, rows, s->hidden, y1, 0);
+        layerNorm(s, st, rows, fout, y1, z, s->params[pidx + 8], s->params[pidx + 9], res);
+        cur = res;
+        continue;
+      }
+      if (!live) continue;
+      const long long rows = (long long)n * curFrames;
+      const size_t pidx = s->paramBase[li];
+      if (l.op == Op::Relu) {
+        float* y = pick({cur});
+        w2l::check(w2l_act_fwd(st, rows * feat, cur, 1, 0.f, 0ull, y));
+        cur = y;
+      } else if (l.op == Op::LayerNorm) {
+        float* y = pick({cur});
+        layerNorm(s, st, rows, feat, cur, nullptr, s->params[pidx], s->params[pidx + 1], y);
+        cur = y;
+      } else if (l.op == Op::Linear) {
+        float* y = li + 1 == layers.size() ? emissions : pick({cur});
+        dense(s, st, s->dense[s->denseOf[li]], rows, cur, y, 0);
+        cur = y;
+      }
+    }
+    if (live && cur != emissions)
+      cuda(cudaMemcpyAsync(emissions, cur, sizeof(float) * (size_t)n * p.tOutMax * s->nLabel, cudaMemcpyDeviceToDevice, st), "stream: emissions");
+    for (int i = 0; i < n; ++i) {
+      Slot& sl = s->slots[slots[i]];
+      for (size_t c = 0; c < nc; ++c) sl.tails[c] = p.tails[c][i];
+      sl.plane ^= 1;
+      if (finish) sl.status = 2;
+      frames_out[i] = p.framesOut[i];
+    }
+  });
+}
+
+}  // extern "C"

@@ -19,6 +19,7 @@
 #include <vector>
 
 #include "fl_compat/fl_compat.h"
+#include "stream_internal.h"
 #include "w2l_b200.h"
 
 namespace w2l {
@@ -148,6 +149,18 @@ int timeStride(const std::shared_ptr<fl::Module>& m) {
 }
 constexpr char kMagic[8] = {'W', '2', 'L', 'B', '2', '0', '0', '\0'};
 }  // namespace
+
+// the streaming runtime's view of a trainer (stream_capi.cpp): what it copies at w2l_stream_create
+w2l::streaming::TrainerSnapshotSource w2l::streaming::trainerSnapshotSource(void* h) {
+  auto* t = static_cast<Trainer*>(h);
+  TrainerSnapshotSource s;
+  s.arch = t->archText;
+  s.nFeat = t->nFeat;
+  s.nLabel = t->nLabel;
+  s.precision = t->precision;
+  for (auto& p : t->net->params()) s.params.emplace_back(p.array().f32(), p.elements());
+  return s;
+}
 
 extern "C" {
 
@@ -513,60 +526,28 @@ W2L_API int w2l_trainer_export_streaming(void* h, void* stream, const char* outd
       for (size_t f = 0; f < b.size(); ++f) o[c ? ((int)f % W) * c + (int)f / W : f] = b[f];
       return o;
     };
-    std::istringstream in(t->archText);
-    std::string line;
-    int curC = 1, padL = -1, padR = -1;
-    while (std::getline(in, line)) {
-      const auto hash = line.find('#');
-      if (hash != std::string::npos) line = line.substr(0, hash);
-      for (const char* key : {"NFEAT", "NLABEL"}) {
-        size_t pos;
-        const std::string val = std::to_string(std::string(key) == "NFEAT" ? t->nFeat : t->nLabel);
-        while ((pos = line.find(key)) != std::string::npos) line.replace(pos, std::strlen(key), val);
-      }
-      std::istringstream ls(line);
-      std::vector<std::string> c;
-      std::string tok;
-      while (ls >> tok) c.push_back(tok);
-      if (c.empty()) continue;
-      const std::string& op = c[0];
+    const w2l::streaming::Arch arch = w2l::streaming::parseArch(t->archText, t->nFeat, t->nLabel);
+    using w2l::streaming::Op;
+    for (const w2l::streaming::Layer& l : arch.layers) {
       std::ostringstream o;
-      if (op == "PD") {
-        if (c.size() != 4) throw std::invalid_argument("export: padding is supported only along the time axis");
-        padL = std::stoi(c[2]);
-        padR = std::stoi(c[3]);
-      } else if (op == "C2") {
-        if (c.size() < 8) throw std::invalid_argument("export: invalid arch specified for C2");
-        const int cin = std::stoi(c[1]), cout = std::stoi(c[2]), kw = std::stoi(c[3]), dw = std::stoi(c[5]);
-        int pl = padL, pr = padR;
-        if (pl == -1 && pr == -1) pl = pr = (kw - dw + 1) / 2;
-        const size_t wo = push(convLayout(next(), cout, cin, kw)), bo = push(next());
-        o << "{\"type\": \"conv1d\", \"cin\": " << cin * W << ", \"cout\": " << cout * W << ", \"kw\": " << kw << ", \"stride\": " << dw
-          << ", \"pad_left\": " << pl << ", \"pad_right\": " << pr << ", \"groups\": " << W << ", \"weight\": " << wo << ", \"bias\": " << bo << "}";
+      if (l.op == Op::Conv) {
+        const size_t wo = push(convLayout(next(), l.cout, l.cin, l.kw)), bo = push(next());
+        o << "{\"type\": \"conv1d\", \"cin\": " << l.cin * W << ", \"cout\": " << l.cout * W << ", \"kw\": " << l.kw << ", \"stride\": " << l.stride
+          << ", \"pad_left\": " << l.padL << ", \"pad_right\": " << l.padR << ", \"groups\": " << W << ", \"weight\": " << wo << ", \"bias\": " << bo << "}";
         emit(o.str());
-        padL = padR = -1;
-        curC = cout;
-      } else if (op == "R") {
+      } else if (l.op == Op::Relu) {
         emit("{\"type\": \"relu\"}");
-      } else if (op == "LN") {
-        if (c.size() != 3 || c[1] != "1" || c[2] != "2") throw std::invalid_argument("export: unsupported LayerNorm axis: must be {1, 2} for streaming");
+      } else if (l.op == Op::LayerNorm) {
         const float g = next()[0], b = next()[0];
-        o << "{\"type\": \"layernorm\", \"feat\": " << curC * W << ", \"gain\": " << g << ", \"bias\": " << b << "}";
+        o << "{\"type\": \"layernorm\", \"feat\": " << l.curC * W << ", \"gain\": " << g << ", \"bias\": " << b << "}";
         emit(o.str());
-      } else if (op == "L") {
-        const int nin = std::stoi(c[1]), nout = std::stoi(c[2]);
-        if (nin != curC * W) throw std::invalid_argument("export: the Linear head does not take a whole frame");
-        const size_t wo = push(linLayout(next(), nin, nout, curC, 0));
+      } else if (l.op == Op::Linear) {
+        const size_t wo = push(linLayout(next(), l.nin, l.nout, l.curC, 0));
         const size_t bo = push(next());
-        o << "{\"type\": \"linear\", \"nin\": " << nin << ", \"nout\": " << nout << ", \"weight\": " << wo << ", \"bias\": " << bo << "}";
+        o << "{\"type\": \"linear\", \"nin\": " << l.nin << ", \"nout\": " << l.nout << ", \"weight\": " << wo << ", \"bias\": " << bo << "}";
         emit(o.str());
-      } else if (op == "TDS") {
-        const int ch = std::stoi(c[1]), kw = std::stoi(c[2]), w = std::stoi(c[3]);
-        const int inner = c.size() > 5 && std::stoi(c[5]) > 0 ? std::stoi(c[5]) : ch * w;
-        const int rpad = c.size() > 6 ? std::stoi(c[6]) : -1;
-        if (w != W) throw std::invalid_argument("export: the TDS width must be the filterbank count");
-        if (c.size() > 7 && std::stoi(c[7]) != 0) throw std::invalid_argument("export: streaming TDS blocks normalise per frame (lNormIncludeTime = 0)");
-        const int pr = rpad >= 0 ? rpad : (kw - 1 + 1) / 2, pl = rpad >= 0 ? kw - 1 - rpad : (kw - 1 + 1) / 2;
+      } else {  // TDS
+        const int ch = l.cin, kw = l.kw, w = W, inner = l.inner;
         const size_t cw = push(convLayout(next(), ch, ch, kw)), cb = push(next());
         const float g1 = next()[0], b1 = next()[0];
         const size_t w1 = push(linLayout(next(), ch * w, inner, ch, 0)), bb1 = push(next());
@@ -574,15 +555,10 @@ W2L_API int w2l_trainer_export_streaming(void* h, void* stream, const char* outd
         const size_t bb2 = push(vecLayout(next(), ch));
         const float g2 = next()[0], b2 = next()[0];
         o << "{\"type\": \"tds\", \"channels\": " << ch << ", \"kw\": " << kw << ", \"feat\": " << ch * w << ", \"inner\": " << inner
-          << ", \"pad_left\": " << pl << ", \"pad_right\": " << pr << ", \"groups\": " << W << ", \"conv_weight\": " << cw << ", \"conv_bias\": " << cb
+          << ", \"pad_left\": " << l.padL << ", \"pad_right\": " << l.padR << ", \"groups\": " << W << ", \"conv_weight\": " << cw << ", \"conv_bias\": " << cb
           << ", \"ln1\": [" << g1 << ", " << b1 << "], \"lin1_weight\": " << w1 << ", \"lin1_bias\": " << bb1 << ", \"lin2_weight\": " << w2
           << ", \"lin2_bias\": " << bb2 << ", \"ln2\": [" << g2 << ", " << b2 << "]}";
         emit(o.str());
-        curC = ch;
-      } else if (op == "V" || op == "RO" || op == "DO" || op == "SAUG") {
-        // skipped, as the converter does
-      } else {
-        throw std::logic_error("export: unrecognized/unparsable line " + line);
       }
     }
     if (pi != params.size()) throw std::runtime_error("export: parameters left over after walking the arch");
