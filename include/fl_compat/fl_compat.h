@@ -333,6 +333,22 @@ class GatedLinearUnit : public UnaryModule {
   float dropP_ = 0.f;
 };
 
+// fl::PReLU(numParams = 1, init = 0.25) — arch opcode `PR [numParams] [init]` (cpc/SequentialBuilder.cpp:437-444):
+// y = x >= 0 ? x : a x, with one learned scalar a, a [1] network parameter in module order.  (Upstream tiles a weight of
+// numParams values along ArrayFire dim 0, which is time in these archs; no arch uses numParams != 1 and it is refused.
+// The semantics are recalled from flashlight 0.3, which is not vendored.)  A following Dropout is fused (fuseDropout).
+// Element-wise: valid frames pass through, as in GatedLinearUnit.
+class PReLU : public UnaryModule {
+ public:
+  PReLU(int numParams, double init);
+  Variable forward(const Variable& in) override;
+  void fuseDropout(float p) { dropP_ = p; }
+  std::string prettyString() const override;
+
+ private:
+  float dropP_ = 0.f;
+};
+
 // fl::WeightNorm(module, dim): w = g * v / ||v|| with the norm taken per output unit (dim 3 of a Conv2D weight
 // [kw,1,cin,cout], dim 0 of flashlight's Linear weight [out,in]).  params(): v, g, then the wrapped layer's bias.
 class WeightNorm : public UnaryModule {

@@ -103,12 +103,23 @@ W2L_API long long w2l_trace_list(char* out, long long out_bytes);
  * Supported: N <= 32 (token sets of the ASG recipes are ~30: conv_glu/.../train.cfg) and
  * targets of at most 1024 positions after the clamp to T (min(L, T) <= 1024: a warp walks a
  * recursion with up to 32 positions per lane); W2L_ERR_UNSUPPORTED beyond.
+ *
+ * w2l_asg64_*: the same signature, layouts, scale modes, terms, target rules and error codes
+ * for 1 <= N <= 64 (the 39 folded phones of the TIMIT recipe, learnable_frontend), from the
+ * same kernels at twice the state width (two states per lane).  It is a separate call because
+ * the N <= 32 contract above, W2L_ERR_UNSUPPORTED for N > 32 included, is published and
+ * tested; callers pick the call from N (the trainer does).  N > 64: W2L_ERR_UNSUPPORTED.
  * ---------------------------------------------------------------------------------------- */
 W2L_API size_t w2l_asg_workspace_size(int B, int T, int N, int L);
 W2L_API int w2l_asg_forward_backward(void* stream, int terms, int B, int T, int N, int L, int scale_mode,
                                      const float* emis, const int32_t* target, const float* trans,
                                      const float* dloss, float* loss, float* d_emis, float* d_trans,
                                      void* workspace, size_t workspace_bytes);
+W2L_API size_t w2l_asg64_workspace_size(int B, int T, int N, int L);
+W2L_API int w2l_asg64_forward_backward(void* stream, int terms, int B, int T, int N, int L, int scale_mode,
+                                       const float* emis, const int32_t* target, const float* trans,
+                                       const float* dloss, float* loss, float* d_emis, float* d_trans,
+                                       void* workspace, size_t workspace_bytes);
 
 /* ----------------------------------------------------------------------------------------
  * Viterbi decoding.  w2l_fcc_viterbi replaces ASGLoss::viterbiPath (Train.cpp:838, :1375):
@@ -116,10 +127,15 @@ W2L_API int w2l_asg_forward_backward(void* stream, int terms, int B, int T, int 
  * bit-exact with upstream ViterbiPath.  w2l_fac_viterbi is the forced alignment
  * (upstream ForceAlignmentCriterion::viterbiPath / fl_asr_align): path = label per frame,
  * path_idx (nullable) = position in the target per frame.
+ * w2l_fcc_viterbi covers N <= 32 (W2L_ERR_UNSUPPORTED beyond, as published);
+ * w2l_fcc_viterbi64 is the same contract, bit-exactness included, for 1 <= N <= 64.
  * ---------------------------------------------------------------------------------------- */
 W2L_API size_t w2l_fcc_viterbi_workspace_size(int B, int T, int N);
 W2L_API int w2l_fcc_viterbi(void* stream, int B, int T, int N, const float* emis, const float* trans,
                             int32_t* path, void* workspace, size_t workspace_bytes);
+W2L_API size_t w2l_fcc_viterbi64_workspace_size(int B, int T, int N);
+W2L_API int w2l_fcc_viterbi64(void* stream, int B, int T, int N, const float* emis, const float* trans,
+                              int32_t* path, void* workspace, size_t workspace_bytes);
 W2L_API size_t w2l_fac_viterbi_workspace_size(int B, int T, int N, int L);
 W2L_API int w2l_fac_viterbi(void* stream, int B, int T, int N, int L, const float* emis, const int32_t* target,
                             const float* trans, int32_t* path, int32_t* path_idx, void* workspace,
@@ -294,6 +310,14 @@ W2L_API int w2l_glu_fwd(void* stream, long long rows, int half, const float* x, 
                         unsigned long long seed);
 W2L_API int w2l_glu_bwd(void* stream, long long rows, int half, const float* x, const float* dy, float* dx, float dropout_p,
                         unsigned long long seed);
+/* PReLU with one parameter (arch opcode `PR`, fl::PReLU): y[i] = (x[i] >= 0 ? x[i] : a[0] x[i]) * mask(i), the following
+ * Dropout fused (mask = dropout_scale's Philox rule, regenerated from `seed` in the backward).  The backward writes
+ * dx[i] = mask(i) dy[i] (x[i] >= 0 ? 1 : a[0]) and da[0] = sum_{x[i] < 0} x[i] mask(i) dy[i] (per-CTA partials and one
+ * fixed-order sum: the same bits every run).  `a` stays on the device: no host sync. */
+W2L_API int w2l_prelu_fwd(void* stream, long long n, const float* x, const float* a, float* y, float dropout_p,
+                          unsigned long long seed);
+W2L_API int w2l_prelu_bwd(void* stream, long long n, const float* x, const float* dy, const float* a, float* dx, float* da,
+                          float dropout_p, unsigned long long seed);
 
 /* fl::LayerNorm over a whole sample (R = T*C*W elements; `LN 0 1 2` / TDSBlock with lnIncludeTime)
  * with scalar gain/bias (device scalars, nullable = 1/0) and a fused residual: y = LN(a + r).

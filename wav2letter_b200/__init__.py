@@ -14,11 +14,13 @@ from .capi import (  # noqa: F401
     TERM_FCC,
     W2LError,
     argmax_path,
+    asg64_forward_backward,
     asg_forward_backward,
     ctc_forward_backward,
     ctc_viterbi_target,
     fac_viterbi,
     fcc_viterbi,
+    fcc_viterbi64,
     launch_count,
     linseg_target,
     reset_launch_count,

@@ -9,6 +9,11 @@ token for token (stored in tests/golden/reference_archs.json):
                                                                            `L 1440 1024` for `L 1440 NLABEL`)
   conv_glu_librispeech()  recipes/conv_glu/librispeech/network.arch      (configs[2])
   streaming_tds()         recipes/streaming_convnets/librispeech/am_500ms_future_context.arch   (configs[3])
+
+and, outside the BASELINE configs (so outside BASELINE_ARCHS / REFERENCE_FILES, which bench.py and test_archs.py walk):
+
+  learnable_frontend_timit()  recipes/learnable_frontend/am_baseline_conv_relu.arch  (TIMIT phones; checked against
+                              tests/golden/learnable_frontend_arch.json)
 """
 
 
@@ -63,6 +68,20 @@ def streaming_tds():
         cin = c
     out += ["RO 2 1 0 3", "V 2160 -1 1 0", "L 2160 NLABEL", "V NLABEL 0 -1 1"]
     return "\n".join(out) + "\n"
+
+
+def learnable_frontend_timit():
+    """7 x (C2 over features-as-channels, kernel 5, SAME padding; PReLU; dropout 0.7), then the Linear head"""
+    out = ["V -1 1 NFEAT 0"]
+    cin = "NFEAT"
+    for _ in range(7):
+        out += [f"C2 {cin} 1000 5 1 1 1 -1 0", "PR", "DO 0.7"]
+        cin = 1000
+    out += ["RO 2 0 3 1", "L 1000 NLABEL"]
+    return "\n".join(out) + "\n"
+
+
+LEARNABLE_FRONTEND_FILE = "recipes/learnable_frontend/am_baseline_conv_relu.arch"
 
 
 # BASELINE.json configs[i] -> (generator, criterion, filterbanks, default label count)

@@ -21,7 +21,9 @@ TERM_FCC, TERM_FAC, TERM_ASG = 1, 2, 3
 EXPORTS = [
     "w2l_version", "w2l_last_error", "w2l_launch_count", "w2l_reset_launch_count", "w2l_set_profile_events", "w2l_set_profile_event_list", "w2l_profile_events_used", "w2l_trace_begin", "w2l_trace_end", "w2l_trace_list",
     "w2l_asg_workspace_size", "w2l_asg_forward_backward",
+    "w2l_asg64_workspace_size", "w2l_asg64_forward_backward",
     "w2l_fcc_viterbi_workspace_size", "w2l_fcc_viterbi",
+    "w2l_fcc_viterbi64_workspace_size", "w2l_fcc_viterbi64",
     "w2l_fac_viterbi_workspace_size", "w2l_fac_viterbi",
     "w2l_ctc_workspace_size", "w2l_ctc_forward_backward", "w2l_argmax_path", "w2l_linseg_target",
     "w2l_ctc_viterbi_workspace_size", "w2l_ctc_viterbi_target",
@@ -32,7 +34,7 @@ EXPORTS = [
     "w2l_gemm_set_variant", "w2l_gemm_set_tile", "w2l_gemm_tf32", "w2l_gemm_tf32_ex", "w2l_gemm_tf32_view", "w2l_conv_time_workspace_size", "w2l_conv_time_fwd", "w2l_conv_time_dgrad",
     "w2l_conv_time_wgrad", "w2l_layernorm_fwd", "w2l_layernorm_rows_fwd", "w2l_layernorm_bwd", "w2l_colsum_accumulate", "w2l_sq_norm_accumulate",
     "w2l_sgd_step", "w2l_weightnorm_fwd", "w2l_weightnorm_bwd", "w2l_conv1d_arrange", "w2l_conv1d_arrange_ex", "w2l_conv1d_unarrange_grad",
-    "w2l_glu_fwd", "w2l_glu_bwd", "w2l_transpose_input", "w2l_axpy", "w2l_fill", "w2l_act_fwd", "w2l_mask_mul",
+    "w2l_glu_fwd", "w2l_glu_bwd", "w2l_prelu_fwd", "w2l_prelu_bwd", "w2l_transpose_input", "w2l_axpy", "w2l_fill", "w2l_act_fwd", "w2l_mask_mul",
     "w2l_trainer_create", "w2l_trainer_destroy", "w2l_trainer_step", "w2l_trainer_forward", "w2l_trainer_num_params",
     "w2l_trainer_param_layout", "w2l_trainer_get_flat", "w2l_trainer_set_flat", "w2l_trainer_sync_parameters",
     "w2l_trainer_describe", "w2l_nccl_unique_id", "w2l_init_distributed", "w2l_trainer_align", "w2l_trainer_time_stride",
@@ -70,6 +72,12 @@ def _load() -> ctypes.CDLL:
     lib.w2l_fcc_viterbi_workspace_size.restype = sz
     lib.w2l_fcc_viterbi_workspace_size.argtypes = [i, i, i]
     lib.w2l_fcc_viterbi.argtypes = [vp, i, i, i, vp, vp, vp, vp, sz]
+    lib.w2l_asg64_workspace_size.restype = sz
+    lib.w2l_asg64_workspace_size.argtypes = [i, i, i, i]
+    lib.w2l_asg64_forward_backward.argtypes = [vp, i, i, i, i, i, i, vp, vp, vp, vp, vp, vp, vp, vp, sz]
+    lib.w2l_fcc_viterbi64_workspace_size.restype = sz
+    lib.w2l_fcc_viterbi64_workspace_size.argtypes = [i, i, i]
+    lib.w2l_fcc_viterbi64.argtypes = [vp, i, i, i, vp, vp, vp, vp, sz]
     lib.w2l_fac_viterbi_workspace_size.restype = sz
     lib.w2l_fac_viterbi_workspace_size.argtypes = [i, i, i, i]
     lib.w2l_fac_viterbi.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, vp, vp, sz]
@@ -90,6 +98,8 @@ def _load() -> ctypes.CDLL:
     lib.w2l_conv1d_unarrange_grad.argtypes = [vp, i, i, i, i, i, i, vp, vp, ll, vp, vp]
     lib.w2l_glu_fwd.argtypes = [vp, ll, i, vp, vp, f32, u64]
     lib.w2l_glu_bwd.argtypes = [vp, ll, i, vp, vp, vp, f32, u64]
+    lib.w2l_prelu_fwd.argtypes = [vp, ll, vp, vp, vp, f32, u64]
+    lib.w2l_prelu_bwd.argtypes = [vp, ll, vp, vp, vp, vp, vp, f32, u64]
     lib.w2l_act_fwd.argtypes = [vp, ll, vp, i, f32, u64, vp]
     lib.w2l_mask_mul.argtypes = [vp, ll, vp, vp, i, f32, vp]
     lib.w2l_gemm_tf32_view.argtypes = [vp, i, i, i, i, i, vp, i, vp, i, vp, i, vp, i, i]
@@ -233,7 +243,19 @@ def set_profile_events(start=None, stop=None) -> None:
 def asg_forward_backward(emis, target, trans, scale_mode="none", dloss=None, terms=TERM_ASG, need_grad=True,
                          out=None, ws=None):
     """Fused ASG (FCC - FAC) forward+backward.  emis [B,T,N] f32, target [B,L] i32 (-1 padded),
-    trans [N,N] f32.  Returns (loss[B], d_emis[B,T,N] | None, d_trans[N,N] | None)."""
+    trans [N,N] f32.  Returns (loss[B], d_emis[B,T,N] | None, d_trans[N,N] | None).  N <= 32."""
+    return _asg(lib.w2l_asg_workspace_size, lib.w2l_asg_forward_backward, emis, target, trans, scale_mode, dloss,
+                terms, need_grad, out, ws)
+
+
+def asg64_forward_backward(emis, target, trans, scale_mode="none", dloss=None, terms=TERM_ASG, need_grad=True,
+                           out=None, ws=None):
+    """asg_forward_backward for 1 <= N <= 64 (w2l_asg64_forward_backward)."""
+    return _asg(lib.w2l_asg64_workspace_size, lib.w2l_asg64_forward_backward, emis, target, trans, scale_mode, dloss,
+                terms, need_grad, out, ws)
+
+
+def _asg(ws_size, call, emis, target, trans, scale_mode, dloss, terms, need_grad, out, ws):
     emis = _req(emis, torch.float32, "emis")
     trans = _req(trans, torch.float32, "trans")
     target = _req(target, torch.int32, "target")
@@ -246,22 +268,52 @@ def asg_forward_backward(emis, target, trans, scale_mode="none", dloss=None, ter
         d_trans = torch.empty_like(trans) if need_grad else None
     else:
         loss, d_emis, d_trans = out
-    need = lib.w2l_asg_workspace_size(B, T, N, L)
+    need = ws_size(B, T, N, L)
     if ws is None:
         ws = workspace(need, emis.device)
-    _check(lib.w2l_asg_forward_backward(_stream(), terms, B, T, N, L, _mode(scale_mode), _ptr(emis), _ptr(target),
-                                        _ptr(trans), _ptr(dloss), _ptr(loss), _ptr(d_emis), _ptr(d_trans),
-                                        _ptr(ws), ws.numel()))
+    _check(call(_stream(), terms, B, T, N, L, _mode(scale_mode), _ptr(emis), _ptr(target),
+                _ptr(trans), _ptr(dloss), _ptr(loss), _ptr(d_emis), _ptr(d_trans),
+                _ptr(ws), ws.numel()))
     return loss, d_emis, d_trans
 
 
+def prelu_fwd(x, a, dropout_p=0.0, seed=0):
+    """PReLU with one parameter and the fused dropout (the `PR` opcode's kernel): x CUDA float32, a CUDA float32 [1]."""
+    x = _req(x, torch.float32, "x")
+    a = _req(a, torch.float32, "a")
+    y = torch.empty_like(x)
+    _check(lib.w2l_prelu_fwd(_stream(), x.numel(), _ptr(x), _ptr(a), _ptr(y), float(dropout_p), int(seed)))
+    return y
+
+
+def prelu_bwd(x, dy, a, dropout_p=0.0, seed=0):
+    """(dx, da [1]) of prelu_fwd for the upstream gradient dy; the dropout mask is regenerated from seed."""
+    x = _req(x, torch.float32, "x")
+    dy = _req(dy, torch.float32, "dy")
+    a = _req(a, torch.float32, "a")
+    dx = torch.empty_like(x)
+    da = torch.empty(1, dtype=torch.float32, device=x.device)
+    _check(lib.w2l_prelu_bwd(_stream(), x.numel(), _ptr(x), _ptr(dy), _ptr(a), _ptr(dx), _ptr(da), float(dropout_p), int(seed)))
+    return dx, da
+
+
 def fcc_viterbi(emis, trans):
+    """Max-plus FCC Viterbi path [B,T] i32, N <= 32."""
+    return _fcc_viterbi(lib.w2l_fcc_viterbi_workspace_size, lib.w2l_fcc_viterbi, emis, trans)
+
+
+def fcc_viterbi64(emis, trans):
+    """fcc_viterbi for 1 <= N <= 64 (w2l_fcc_viterbi64), bit-exact like it."""
+    return _fcc_viterbi(lib.w2l_fcc_viterbi64_workspace_size, lib.w2l_fcc_viterbi64, emis, trans)
+
+
+def _fcc_viterbi(ws_size, call, emis, trans):
     emis = _req(emis, torch.float32, "emis")
     trans = _req(trans, torch.float32, "trans")
     B, T, N = emis.shape
     path = torch.empty((B, T), dtype=torch.int32, device=emis.device)
-    ws = workspace(lib.w2l_fcc_viterbi_workspace_size(B, T, N), emis.device)
-    _check(lib.w2l_fcc_viterbi(_stream(), B, T, N, _ptr(emis), _ptr(trans), _ptr(path), _ptr(ws), ws.numel()))
+    ws = workspace(ws_size(B, T, N), emis.device)
+    _check(call(_stream(), B, T, N, _ptr(emis), _ptr(trans), _ptr(path), _ptr(ws), ws.numel()))
     return path
 
 

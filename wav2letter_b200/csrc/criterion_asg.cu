@@ -37,6 +37,14 @@
 //   4. asg_fcc_grad_kernel parallel over frames, from the stored FCC vectors:
 //                          d_emis = coef*(gamma_fcc - gamma_fac), d_trans partials.
 //   5. asg_parts_reduce_kernel (x2)  deterministic tree sum of the d_trans partials (no atomics).
+//
+// Two widths.  Every kernel is a template over the padded FCC state width NW (S = NW/32 states per lane, lane i owning
+// states i and i+32 when NW = 64).  w2l_asg_forward_backward instantiates NW = 32 (N <= 32, the published contract);
+// w2l_asg64_forward_backward instantiates NW = 64 (N <= 64: the 39 folded phones of TIMIT).  At NW = 64 the FCC chains
+// keep both M' rows of a lane in registers (128 floats) with a half-depth Z prefetch, and the FCC grad kernel runs 4 warps
+// of 8 frames with a 64 x 65 slab per warp in opt-in dynamic shared memory.  The FAC chains are unchanged but for the
+// width of the Z tile; the FAC grad kernels sum occupancies for two labels per lane.  The FAC chain lanes (and with them
+// the per-lane re-centring offsets ckCA / ckCB) stay 32 wide at both widths.
 #include <cuda_runtime.h>
 
 #include "common.cuh"
@@ -47,8 +55,8 @@ __device__ __forceinline__ float2 fadd2_rn(float2 a, float2 b) { return make_flo
 __device__ __forceinline__ float2 ffma2_rn(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
 namespace {
 
-constexpr int kW = 32;            // padded FCC state width (one lane per state)
-constexpr int kBlk = 16;          // frames per register-prefetch block of the FCC chains
+constexpr int kW = 32;            // lanes per warp: FAC chain lanes, and the padded FCC state width of the 32-wide kernels
+constexpr int kBlk = 16;          // frames per register-prefetch block of the FCC chains (NW = 64: half)
 constexpr int kSeg = 8;           // frames per FAC checkpoint segment (= shared-memory tile of the FAC chains)
 constexpr int kRc = 2;            // FAC chains re-centre every kRc frames
 constexpr float kNeg = -1.0e30f;  // "log zero": finite, absorbing under fp32 addition of ordinary scores
@@ -64,8 +72,10 @@ constexpr double kLn2 = 0.6931471805599453;
 // folding it into the transition scores (lse(a - c, b - c) = lse(a, b) - c).
 constexpr float kLgScale = 1.25f;
 constexpr float kLgShift = 0.32192809488736235f;  // log2(1.25)
-constexpr int kFccGradWarps = 8;  // warps per CTA in the FCC grad kernel
-constexpr int kFccGradFrames = 16;  // frames per warp in the FCC grad kernel
+constexpr int kFccGradWarps = 8;  // warps per CTA in the FCC grad kernel (NW = 64: fcc_grad_warps)
+constexpr int kFccGradFrames = 16;  // frames per warp in the FCC grad kernel (NW = 64: fcc_grad_frames)
+template <int NW> __host__ __device__ constexpr int fcc_grad_warps() { return NW == 32 ? kFccGradWarps : 4; }
+template <int NW> __host__ __device__ constexpr int fcc_grad_frames() { return NW == 32 ? kFccGradFrames : 8; }
 constexpr int kFlushRegs = 16;    // positions per label kept in registers by the label-sum
 constexpr int kRedGroup = 32;     // partials summed per thread in the first stage of the d_trans reduction
 
@@ -83,25 +93,25 @@ struct AsgParams {
   float* loss;
   float* d_emis;
   float* d_trans;
-  // workspace
-  float* Z;         // [B][T][32]  (e - m_t) * log2(e); lanes >= N hold kNeg
+  // workspace (NW: the padded state width of the instantiation, 32 or 64)
+  float* Z;         // [B][T][NW]  (e - m_t) * log2(e); lanes >= N hold kNeg
   float* mrow;      // [B][T]
-  float* A;         // [B][T][32] FCC alpha-hat
-  float* Bh;        // [B][T][32] FCC beta-hat
+  float* A;         // [B][T][NW] FCC alpha-hat
+  float* Bh;        // [B][T][NW] FCC beta-hat
   float* sA;        // [B][T] power-of-two scale applied at step t of the alpha chain
   float* ckAa;      // [B][nC][Lp] FAC alpha-tilde row of frame c*kSeg-1 (c >= 1), log2 units
   float* ckBa;      // [B][nC][Lp] FAC beta-tilde  row of frame (c+1)*kSeg (when < T)
   double* ckCA;     // [B][nC][32] per-lane offsets of the stored alpha row (true = tilde + C[lane] + t * tmax2)
   double* ckCB;     // [B][nC][32]
-  float* G;         // [B][T][32] FAC occupancy per label, normalised per frame
+  float* G;         // [B][T][NW] FAC occupancy per label, normalised per frame
   double* fccLogZ;  // [B] natural log, without sum_t m_t
   double* facLogZ2; // [B] log2 units, without sum_t m_t and without (T-1) * tmax * log2e (what the grad kernel subtracts)
   double* facLogZ;  // [B] natural log, without sum_t m_t
   double* msum;     // [B] sum_t m_t
-  float* parts;     // [n_fcc_parts + n_fac_parts][32*32] d_trans partial sums
-  float* parts2;    // [ceil(parts / kRedGroup)][32*32]
+  float* parts;     // [n_fcc_parts + n_fac_parts][NW*NW] d_trans partial sums
+  float* parts2;    // [ceil(parts / kRedGroup)][NW*NW]
   int* order;       // [B][Lp] target positions sorted by label (stable)
-  int* start;       // [B][36] first index of label n in `order` (start[32] = tsz)
+  int* start;       // [B][NW+4] first index of label n in `order` (start[NW] = tsz)
   int* tsz;         // [B]
   int* valid;       // [B]
   float* scale;     // [B]
@@ -127,18 +137,32 @@ __device__ __forceinline__ float lse2_log2(float a, float b) {
 // ------------------------------------------------------------------------------------------
 // 1. prep
 // ------------------------------------------------------------------------------------------
+template <int NW>
 __global__ void __launch_bounds__(256) asg_prep_kernel(AsgParams p, int frame_blocks) {
+  constexpr int S = NW / 32;
   const int lane = threadIdx.x & 31;
   const int wpb = blockDim.x >> 5;
   if ((int)blockIdx.x < frame_blocks) {
     const long long nframes = (long long)p.B * p.T;
     const long long warps = (long long)frame_blocks * wpb;
     for (long long f = (long long)blockIdx.x * wpb + (threadIdx.x >> 5); f < nframes; f += warps) {
-      const float e = lane < p.N ? __ldg(p.emis + f * p.N + lane) : kNegInf;
-      float m = warp_max(e);
-      if (__any_sync(0xffffffffu, e != e)) m = NAN;  // a NaN emission poisons the frame maximum -> the loss
-      float z = lane < p.N ? fmaxf((e - m) * kLog2e, kNeg) : kNeg;  // fmaxf drops NaN: the chains stay finite
-      p.Z[f * kW + lane] = z;
+      float e[S];
+#pragma unroll
+      for (int s = 0; s < S; ++s) e[s] = lane + 32 * s < p.N ? __ldg(p.emis + f * p.N + lane + 32 * s) : kNegInf;
+      float em = e[0];
+      bool nan = e[0] != e[0];
+#pragma unroll
+      for (int s = 1; s < S; ++s) {
+        em = fmaxf(em, e[s]);
+        nan = nan || e[s] != e[s];
+      }
+      float m = warp_max(em);
+      if (__any_sync(0xffffffffu, nan)) m = NAN;  // a NaN emission poisons the frame maximum -> the loss
+#pragma unroll
+      for (int s = 0; s < S; ++s) {
+        float z = lane + 32 * s < p.N ? fmaxf((e[s] - m) * kLog2e, kNeg) : kNeg;  // fmaxf drops NaN: the chains stay finite
+        p.Z[f * NW + lane + 32 * s] = z;
+      }
       if (lane == 0) p.mrow[f] = m;
     }
     return;
@@ -175,23 +199,41 @@ __global__ void __launch_bounds__(256) asg_prep_kernel(AsgParams p, int frame_bl
     p.scale[b] = sc;
     p.coef[b] = ok ? sc * (p.dloss ? p.dloss[b] : 1.0f) : 0.0f;
   }
-  // label-sorted index of the target positions (stable): lane n lists the positions with y_l == n
+  // label-sorted index of the target positions (stable): lane n lists the positions with y_l == n (and n + 32)
   if ((p.terms & W2L_TERM_FAC) && p.need_grad && ok) {
-    int cnt = 0;
-    for (int l = 0; l < tsz; ++l) cnt += (__ldg(y + l) == lane);
-    int pre = cnt;
+    int cnt[S];
 #pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int v = __shfl_up_sync(0xffffffffu, pre, o);
-      if (lane >= o) pre += v;
+    for (int s = 0; s < S; ++s) cnt[s] = 0;
+    for (int l = 0; l < tsz; ++l) {
+      const int v = __ldg(y + l);
+#pragma unroll
+      for (int s = 0; s < S; ++s) cnt[s] += (v == lane + 32 * s);
     }
-    int w0 = pre - cnt;
-    int* st = p.start + (size_t)b * 36;
+    int* st = p.start + (size_t)b * (NW + 4);
     int* od = p.order + (size_t)b * p.Lp;
-    st[lane] = w0;
-    if (lane == 31) st[32] = pre;
-    for (int l = 0; l < tsz; ++l)
-      if (__ldg(y + l) == lane) od[w0++] = l;
+    int w0[S], below = 0;
+#pragma unroll
+    for (int s = 0; s < S; ++s) {
+      int pre = cnt[s];
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int v = __shfl_up_sync(0xffffffffu, pre, o);
+        if (lane >= o) pre += v;
+      }
+      w0[s] = below + pre - cnt[s];
+      st[lane + 32 * s] = w0[s];
+      if (s == S - 1) {
+        if (lane == 31) st[NW] = below + pre;
+      } else {
+        below += __shfl_sync(0xffffffffu, pre, 31);
+      }
+    }
+    for (int l = 0; l < tsz; ++l) {
+      const int v = __ldg(y + l);
+#pragma unroll
+      for (int s = 0; s < S; ++s)
+        if (v == lane + 32 * s) od[w0[s]++] = l;
+    }
   }
 }
 
@@ -237,6 +279,37 @@ __device__ __forceinline__ float matvec32(const float (&M)[kW], const float* vsm
   const float2 s = fadd2_rn(fadd2_rn(fadd2_rn(r[0], r[1]), fadd2_rn(r[2], r[3])), fadd2_rn(fadd2_rn(r[4], r[5]), fadd2_rn(r[6], r[7])));
   return s.x + s.y;
 }
+// out[s] = sum_j M[s][j] * v[j] over the 64 shared-memory entries, for the two states of a lane: 16 broadcast LDS.128,
+// each feeding four independent float2 accumulator chains per state (128 FFMA per step)
+__device__ __forceinline__ void matvec64(const float (&M)[2][64], const float* vsm, float (&out)[2]) {
+  const float4* v4 = reinterpret_cast<const float4*>(vsm);
+  float2 r[2][4];
+#pragma unroll
+  for (int s = 0; s < 2; ++s)
+#pragma unroll
+    for (int u = 0; u < 4; ++u) r[s][u] = make_float2(0.f, 0.f);
+#pragma unroll
+  for (int q = 0; q < 16; ++q) {
+    const float4 v = v4[q];
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+      r[s][(2 * q) & 3] = ffma2_rn(make_float2(M[s][4 * q], M[s][4 * q + 1]), make_float2(v.x, v.y), r[s][(2 * q) & 3]);
+      r[s][(2 * q + 1) & 3] = ffma2_rn(make_float2(M[s][4 * q + 2], M[s][4 * q + 3]), make_float2(v.z, v.w), r[s][(2 * q + 1) & 3]);
+    }
+  }
+#pragma unroll
+  for (int s = 0; s < 2; ++s) {
+    const float2 t = fadd2_rn(fadd2_rn(r[s][0], r[s][1]), fadd2_rn(r[s][2], r[s][3]));
+    out[s] = t.x + t.y;
+  }
+}
+template <int NW>
+__device__ __forceinline__ void matvec(const float (&M)[NW / 32][NW], const float* vsm, float (&out)[NW / 32]) {
+  if constexpr (NW == 32)
+    out[0] = matvec32(M[0], vsm);
+  else
+    matvec64(M, vsm, out);
+}
 
 // 2^-k with k = (unbiased exponent of mx) >> kDamp; returns k through kout.  Exact.
 // kDamp = 1 for the alpha chain: its rescale acts with a lag of two steps (A_t = A_{t-1} + rho_t
@@ -263,8 +336,11 @@ __device__ __forceinline__ float trans_max(const float* trans, int N, int lane) 
   return warp_max(tmax);
 }
 
+// The 32-wide FCC chains, one state per lane.  They are kept apart from the width template below (which computes the
+// same recursion at any NW) because the template, instantiated at NW = 32, orders a few register moves differently:
+// the NW = 32 kernels compile to exactly the instructions they always had.
 // alpha chain: a_t = (X_t * s_t) .* (M' a_{t-1})
-__device__ void fcc_alpha_chain(const AsgParams& p, int b, float* vec /* [2][32] shared */) {
+__device__ void fcc_alpha_chain32(const AsgParams& p, int b, float* vec /* [2][32] shared */) {
   const int lane = threadIdx.x & 31;
   const int T = p.T, N = p.N;
   const float tmax = trans_max(p.trans, N, lane);
@@ -326,7 +402,7 @@ __device__ void fcc_alpha_chain(const AsgParams& p, int b, float* vec /* [2][32]
 }
 
 // beta chain: b_t = M'^T (X_{t+1} .* b_{t+1} * s)
-__device__ void fcc_beta_chain(const AsgParams& p, int b, float* vec) {
+__device__ void fcc_beta_chain32(const AsgParams& p, int b, float* vec) {
   const int lane = threadIdx.x & 31;
   const int T = p.T, N = p.N;
   const float tmax = trans_max(p.trans, N, lane);
@@ -370,6 +446,170 @@ __device__ void fcc_beta_chain(const AsgParams& p, int b, float* vec) {
       bh = matvec32(M, vb);
       Bp -= kW;  // (running pointer: frame t)
       *Bp = bh;
+      s = pow2_rescale<0>(mx, kdummy);
+    }
+  }
+}
+
+// alpha chain: a_t = (X_t * s_t) .* (M' a_{t-1}); lane i holds the states i + 32 s (rows i + 32 s of M')
+template <int NW>
+__device__ void fcc_alpha_chain(const AsgParams& p, int b, float* vec /* [2][NW] shared */) {
+  constexpr int S = NW / 32, kB = NW == 32 ? kBlk : kBlk / 2;  // (NW = 64: half the prefetch depth for the registers)
+  const int lane = threadIdx.x & 31;
+  const int T = p.T, N = p.N;
+  const float tmax = trans_max(p.trans, N, lane);
+  float M[S][NW];
+#pragma unroll
+  for (int q = 0; q < S; ++q) {
+    const int i = lane + 32 * q;
+#pragma unroll
+    for (int j = 0; j < NW; ++j) M[q][j] = (i < N && j < N) ? __expf(__ldg(p.trans + i * N + j) - tmax) : 0.f;
+  }
+  const float* Zl = p.Z + (size_t)b * T * NW + lane;
+  float* Al = p.A + (size_t)b * T * NW + lane;
+  float* sAb = p.sA + (size_t)b * T;
+  const bool store = p.need_grad != 0;
+  const int nblk = (T + kB - 1) / kB;
+  float zn[S][kB];
+#pragma unroll
+  for (int k = 0; k < kB; ++k)
+#pragma unroll
+    for (int q = 0; q < S; ++q) zn[q][k] = k < T ? __ldg(Zl + (size_t)k * NW + 32 * q) : 0.f;
+  float a[S];
+#pragma unroll
+  for (int q = 0; q < S; ++q) a[q] = 0.f;
+  float s = 1.0f;
+  int ksum = 0, kcur = 0;
+  float* Ap = Al;
+  float* sp = sAb;
+  for (int c = 0; c < nblk; ++c) {
+    float zc[S][kB];
+    const int tb = c * kB;
+#pragma unroll
+    for (int k = 0; k < kB; ++k) {
+      const int tn = tb + kB + k;
+#pragma unroll
+      for (int q = 0; q < S; ++q) {
+        zc[q][k] = zn[q][k];
+        zn[q][k] = tn < T ? __ldg(Zl + (size_t)tn * NW + 32 * q) : 0.f;
+      }
+    }
+#pragma unroll
+    for (int k = 0; k < kB; ++k) {
+      const int t = tb + k;
+      if (t >= T) break;
+      float x[S];
+#pragma unroll
+      for (int q = 0; q < S; ++q) x[q] = ex2f(zc[q][k]);
+      if (t == 0) {
+#pragma unroll
+        for (int q = 0; q < S; ++q) a[q] = x[q];
+        if (store) {
+#pragma unroll
+          for (int q = 0; q < S; ++q) Al[32 * q] = a[q];
+          if (lane == 0) sAb[0] = 1.0f;
+        }
+        continue;
+      }
+      float xs[S];
+#pragma unroll
+      for (int q = 0; q < S; ++q) xs[q] = x[q] * s;
+      float* vb = vec + (k & 1) * NW;
+      float am = a[0];
+#pragma unroll
+      for (int q = 0; q < S; ++q) {
+        vb[lane + 32 * q] = a[q];
+        if (q) am = fmaxf(am, a[q]);
+      }
+      const float mx = warp_max(am);  // max_j a_{t-1}[j]: five shuffles, off the dependent chain
+      __syncwarp();
+      float mv[S];
+      matvec<NW>(M, vb, mv);
+#pragma unroll
+      for (int q = 0; q < S; ++q) a[q] = xs[q] * mv[q];
+      ksum += kcur;
+      if (store) {
+        Ap += NW;  // (running pointers: frame t)
+        sp += 1;
+#pragma unroll
+        for (int q = 0; q < S; ++q) Ap[32 * q] = a[q];
+        if (lane == 0) *sp = s;
+      }
+      s = pow2_rescale<1>(mx, kcur);  // applied at t+1 from |a_{t-1}| (lag two): damped
+    }
+  }
+  float as = a[0];
+#pragma unroll
+  for (int q = 1; q < S; ++q) as += a[q];
+  const float tot = warp_sum(as);
+  if (lane == 0) p.fccLogZ[b] = (double)(T - 1) * (double)tmax + kLn2 * (double)ksum + log((double)tot);
+}
+
+// beta chain: b_t = M'^T (X_{t+1} .* b_{t+1} * s); lane j holds the states j + 32 s (columns j + 32 s of M')
+template <int NW>
+__device__ void fcc_beta_chain(const AsgParams& p, int b, float* vec) {
+  constexpr int S = NW / 32, kB = NW == 32 ? kBlk : kBlk / 2;
+  const int lane = threadIdx.x & 31;
+  const int T = p.T, N = p.N;
+  const float tmax = trans_max(p.trans, N, lane);
+  float M[S][NW];
+#pragma unroll
+  for (int q = 0; q < S; ++q) {
+    const int j = lane + 32 * q;
+#pragma unroll
+    for (int i = 0; i < NW; ++i) M[q][i] = (j < N && i < N) ? __expf(__ldg(p.trans + i * N + j) - tmax) : 0.f;
+  }
+  const float* Zl = p.Z + (size_t)b * T * NW + lane;
+  float* Bl = p.Bh + (size_t)b * T * NW + lane;
+  float bh[S];  // b_{T-1}
+#pragma unroll
+  for (int q = 0; q < S; ++q) {
+    bh[q] = lane + 32 * q < N ? 1.0f : 0.0f;
+    Bl[(size_t)(T - 1) * NW + 32 * q] = bh[q];
+  }
+  if (T < 2) return;
+  // step t (T-2 .. 0) consumes X_{t+1}; block c covers t in [c*kB, c*kB + kB) and reads frames t+1
+  const int ctop = (T - 2) / kB;
+  float zn[S][kB];
+#pragma unroll
+  for (int k = 0; k < kB; ++k) {
+    const int f = ctop * kB + k + 1;
+#pragma unroll
+    for (int q = 0; q < S; ++q) zn[q][k] = f < T ? __ldg(Zl + (size_t)f * NW + 32 * q) : 0.f;
+  }
+  float s = 1.0f;
+  int kdummy;
+  float* Bp = Bl + (size_t)(T - 1) * NW;
+  for (int c = ctop; c >= 0; --c) {
+    float zc[S][kB];
+    const int tb = c * kB;
+#pragma unroll
+    for (int k = 0; k < kB; ++k) {
+      const int f = tb - kB + k + 1;
+#pragma unroll
+      for (int q = 0; q < S; ++q) {
+        zc[q][k] = zn[q][k];
+        zn[q][k] = f >= 1 ? __ldg(Zl + (size_t)f * NW + 32 * q) : 0.f;
+      }
+    }
+#pragma unroll
+    for (int k = kB - 1; k >= 0; --k) {
+      const int t = tb + k;
+      if (t > T - 2) continue;
+      float* vb = vec + (k & 1) * NW;
+      float um = 0.f;
+#pragma unroll
+      for (int q = 0; q < S; ++q) {
+        const float u = bh[q] * (ex2f(zc[q][k]) * s);
+        vb[lane + 32 * q] = u;
+        um = q ? fmaxf(um, u) : u;
+      }
+      const float mx = warp_max(um);
+      __syncwarp();
+      matvec<NW>(M, vb, bh);
+      Bp -= NW;  // (running pointer: frame t)
+#pragma unroll
+      for (int q = 0; q < S; ++q) Bp[32 * q] = bh[q];
       s = pow2_rescale<0>(mx, kdummy);
     }
   }
@@ -517,14 +757,15 @@ __device__ __forceinline__ void twofloat_add(float& hi, float& lo, float m) {
 // and found slower than this one — the per-step dependent chain
 // SHFL -> FADD -> FMNMX -> FFMA -> EX2 -> FADD -> LG2 -> FADD is ~160 cycles whatever the width, and the ring's
 // bookkeeping cost what the narrower rows saved.)
-template <int P, bool kBeta>
-__device__ void fac_chain(const AsgParams& p, int b, float* ztile /* [kSeg][32] shared */) {
+template <int P, bool kBeta, int NW>
+__device__ void fac_chain(const AsgParams& p, int b, float* ztile /* [kSeg][NW] shared */) {
+  constexpr int S = NW / 32;
   const int lane = threadIdx.x & 31;
   const int T = p.T, L = p.tsz[b];
   const float tmax = trans_max(p.trans, p.N, lane);
   FacState<P> st;
   fac_load_target<P>(st, p, b, L, lane, kBeta, tmax);
-  const float* Zl = p.Z + (size_t)b * T * kW + lane;
+  const float* Zl = p.Z + (size_t)b * T * NW + lane;
   const uint32_t zt = (uint32_t)__cvta_generic_to_shared(ztile);
   const bool store = p.need_grad != 0;
   // Every LANE keeps its P positions relative to its own offset (two-float Chi + Clo): values stay within a few tens of
@@ -537,9 +778,9 @@ __device__ void fac_chain(const AsgParams& p, int b, float* ztile /* [kSeg][32] 
 
   auto step = [&](int t, int krow) {
     if (!kBeta)
-      fac_alpha_step<P>(st, zt + krow * (4 * kW), lane, D);
+      fac_alpha_step<P>(st, zt + krow * (4 * NW), lane, D);
     else
-      fac_beta_step<P>(st, st.s2, zt + krow * (4 * kW), lane, D);
+      fac_beta_step<P>(st, st.s2, zt + krow * (4 * NW), lane, D);
     // lagged, branch-free re-centring: the lane maximum taken at one step is subtracted after the next one
     if ((t & (kRc - 1)) == (kBeta ? kRc - 1 : 0)) {
       // the lane maximum is put at +off, half of what it lost over the last period, so that the live states straddle
@@ -574,17 +815,22 @@ __device__ void fac_chain(const AsgParams& p, int b, float* ztile /* [kSeg][32] 
 
   if (!kBeta) {
     // ---- alpha: frames 0 .. T-1; checkpoint c+1 = row of frame (c+1)*kSeg - 1 ----------------------------------------
-    float zn[kSeg];
+    float zn[S][kSeg];
 #pragma unroll
-    for (int k = 0; k < kSeg; ++k) zn[k] = k < T ? __ldg(Zl + (size_t)k * kW) : 0.f;
+    for (int k = 0; k < kSeg; ++k)
+#pragma unroll
+      for (int q = 0; q < S; ++q) zn[q][k] = k < T ? __ldg(Zl + (size_t)k * NW + 32 * q) : 0.f;
     for (int c = 0; c < p.nC; ++c) {
       const int tb = c * kSeg;
       __syncwarp();
 #pragma unroll
       for (int k = 0; k < kSeg; ++k) {
-        ztile[k * kW + lane] = zn[k];
         const int tn = tb + kSeg + k;
-        zn[k] = tn < T ? __ldg(Zl + (size_t)tn * kW) : 0.f;
+#pragma unroll
+        for (int q = 0; q < S; ++q) {
+          ztile[k * NW + lane + 32 * q] = zn[q][k];
+          zn[q][k] = tn < T ? __ldg(Zl + (size_t)tn * NW + 32 * q) : 0.f;
+        }
       }
       __syncwarp();
       int k0 = 0;
@@ -615,20 +861,24 @@ __device__ void fac_chain(const AsgParams& p, int b, float* ztile /* [kSeg][32] 
   } else {
     // ---- beta: frames T-1 .. 0; checkpoint c-1 = row of frame c*kSeg -------------------------------------------------
     const int ctop = (T - 1) / kSeg;
-    float zn[kSeg];
+    float zn[S][kSeg];
 #pragma unroll
     for (int k = 0; k < kSeg; ++k) {
       const int f = ctop * kSeg + k;
-      zn[k] = f < T ? __ldg(Zl + (size_t)f * kW) : 0.f;
+#pragma unroll
+      for (int q = 0; q < S; ++q) zn[q][k] = f < T ? __ldg(Zl + (size_t)f * NW + 32 * q) : 0.f;
     }
     for (int c = ctop; c >= 0; --c) {
       const int tb = c * kSeg;
       __syncwarp();
 #pragma unroll
       for (int k = 0; k < kSeg; ++k) {
-        ztile[k * kW + lane] = zn[k];
         const int f = tb - kSeg + k;
-        zn[k] = f >= 0 ? __ldg(Zl + (size_t)f * kW) : 0.f;
+#pragma unroll
+        for (int q = 0; q < S; ++q) {
+          ztile[k * NW + lane + 32 * q] = zn[q][k];
+          zn[q][k] = f >= 0 ? __ldg(Zl + (size_t)f * NW + 32 * q) : 0.f;
+        }
       }
       __syncwarp();
       int khi = kSeg - 1;
@@ -636,7 +886,7 @@ __device__ void fac_chain(const AsgParams& p, int b, float* ztile /* [kSeg][32] 
         const int kl = T - 1 - tb;
 #pragma unroll
         for (int k = 0; k < P; ++k)
-          if (lane * P + k == L - 1) st.v[k] = ztile[kl * kW + (st.y4[k] >> 2)];
+          if (lane * P + k == L - 1) st.v[k] = ztile[kl * NW + (st.y4[k] >> 2)];
         khi = kl - 1;
       }
       if (khi == kSeg - 1) {
@@ -653,9 +903,9 @@ __device__ void fac_chain(const AsgParams& p, int b, float* ztile /* [kSeg][32] 
   }
 }
 
-template <int P>
+template <int P, int NW>
 __global__ void __launch_bounds__(32) asg_chains_kernel(AsgParams p) {
-  __shared__ __align__(16) float sm[kSeg * kW];
+  __shared__ __align__(16) float sm[kSeg * NW];
   const int role = p.roles[blockIdx.x / p.B];
   const int b = blockIdx.x % p.B;
   const int lane = threadIdx.x;
@@ -668,13 +918,13 @@ __global__ void __launch_bounds__(32) asg_chains_kernel(AsgParams p) {
   }
   if (!p.valid[b]) return;
   if (role == kRoleFacAlpha)
-    fac_chain<P, false>(p, b, sm);
+    fac_chain<P, false, NW>(p, b, sm);
   else if (role == kRoleFacBeta)
-    fac_chain<P, true>(p, b, sm);
+    fac_chain<P, true, NW>(p, b, sm);
   else if (role == kRoleFccAlpha)
-    fcc_alpha_chain(p, b, sm);
+    if constexpr (NW == 32) fcc_alpha_chain32(p, b, sm); else fcc_alpha_chain<NW>(p, b, sm);
   else
-    fcc_beta_chain(p, b, sm);
+    if constexpr (NW == 32) fcc_beta_chain32(p, b, sm); else fcc_beta_chain<NW>(p, b, sm);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -713,16 +963,17 @@ __device__ __forceinline__ float label_sum(uint32_t row_sa, const float* row, co
 struct FacGradLayout {
   int start, ztile, bnext, brow, grow, dsum, dtr, per_warp, total;
 };
+template <int NW>
 __host__ __device__ inline FacGradLayout fac_grad_layout(int Lp, int warps) {
   FacGradLayout f;
   int o = 0;
-  f.start = o;  o += 36;
+  f.start = o;  o += NW + 4;
   f.dsum = o;   o += 2 * Lp;
-  f.dtr = o;    o += kW * (kW + 1);
+  f.dtr = o;    o += NW * (NW + 1);
   o = (o + 3) & ~3;
-  f.per_warp = 2 * kSeg * kW + Lp + kSeg * Lp + Lp + 4;  // two Z tiles, next beta row, beta rows, gamma row (+ a zero slot)
+  f.per_warp = 2 * kSeg * NW + Lp + kSeg * Lp + Lp + 4;  // two Z tiles, next beta row, beta rows, gamma row (+ a zero slot)
   f.ztile = o;
-  f.bnext = o + 2 * kSeg * kW;
+  f.bnext = o + 2 * kSeg * NW;
   f.brow = f.bnext + Lp;
   f.grow = f.brow + kSeg * Lp;
   f.total = o + warps * f.per_warp;
@@ -747,16 +998,18 @@ __device__ __forceinline__ float2 fac_grad_pair(float va, float na, float s1a, f
   return fadd2_rn(base, make_float2(lg2f(q.x), lg2f(q.y)));
 }
 
-template <int P>
-__global__ void __launch_bounds__(128, P <= 8 ? 4 : 2) asg_fac_grad_kernel(AsgParams p) {
+// (NW = 64: the second label's flush index costs 16 registers, so P = 8 runs at 2 CTAs per SM instead of spilling)
+template <int P, int NW>
+__global__ void __launch_bounds__(128, P <= 8 * 32 / NW ? 4 : 2) asg_fac_grad_kernel(AsgParams p) {
+  constexpr int S = NW / 32;
   extern __shared__ __align__(16) float smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
   const int b = blockIdx.y;
   const int T = p.T, Lp = p.Lp;
-  const FacGradLayout lay = fac_grad_layout(Lp, nw);
-  float* part = p.parts + ((size_t)p.n_fcc_parts + (size_t)b * gridDim.x + blockIdx.x) * (kW * kW);
+  const FacGradLayout lay = fac_grad_layout<NW>(Lp, nw);
+  float* part = p.parts + ((size_t)p.n_fcc_parts + (size_t)b * gridDim.x + blockIdx.x) * (NW * NW);
   if (!p.valid[b]) {
-    for (int k = threadIdx.x; k < kW * kW; k += blockDim.x) part[k] = 0.f;
+    for (int k = threadIdx.x; k < NW * NW; k += blockDim.x) part[k] = 0.f;
     return;  // the FCC grad kernel writes the zero gradient rows
   }
   const int L = p.tsz[b];
@@ -771,8 +1024,8 @@ __global__ void __launch_bounds__(128, P <= 8 ? 4 : 2) asg_fac_grad_kernel(AsgPa
     dsum_s[l] = 0.f;
     dsum_s[Lp + l] = 0.f;
   }
-  for (int k = threadIdx.x; k < 33; k += blockDim.x) start_s[k] = p.start[(size_t)b * 36 + k];
-  for (int k = threadIdx.x; k < kW * (kW + 1); k += blockDim.x) dtr_s[k] = 0.f;
+  for (int k = threadIdx.x; k < NW + 1; k += blockDim.x) start_s[k] = p.start[(size_t)b * (NW + 4) + k];
+  for (int k = threadIdx.x; k < NW * (NW + 1); k += blockDim.x) dtr_s[k] = 0.f;
   __syncthreads();
 
   float2 ds[P];  // (stay, advance) transition statistics of the owned positions
@@ -787,8 +1040,8 @@ __global__ void __launch_bounds__(128, P <= 8 ? 4 : 2) asg_fac_grad_kernel(AsgPa
     const uint32_t bnext_sa = (uint32_t)__cvta_generic_to_shared(bnext);
     const uint32_t grow_sa = (uint32_t)__cvta_generic_to_shared(grow);
     const float tmax = trans_max(p.trans, p.N, lane);
-    const float* Zb = p.Z + (size_t)b * T * kW;
-    float* Gb = p.G + (size_t)b * T * kW;
+    const float* Zb = p.Z + (size_t)b * T * NW;
+    float* Gb = p.G + (size_t)b * T * NW;
     const double logZ2 = p.facLogZ2[b];
     FacState<P> st;  // s2 = the alpha walk's advance scores; the beta walk's live in s2b
     float s2b[P];
@@ -796,18 +1049,19 @@ __global__ void __launch_bounds__(128, P <= 8 ? 4 : 2) asg_fac_grad_kernel(AsgPa
 #pragma unroll
     for (int k = 0; k < P; ++k) s2b[k] = st.s2[k];
     fac_load_target<P>(st, p, b, L, lane, false, tmax);
-    FlushIndex fx;
-    fx.load(order_s, start_s, lane, Lp);
+    FlushIndex fx[S];  // labels lane + 32 s
+#pragma unroll
+    for (int q = 0; q < S; ++q) fx[q].load(order_s, start_s, lane + 32 * q, Lp);
     if (lane == 0) grow[Lp] = 0.f;
     // asynchronous copies (no registers) of a segment's inputs: its Z rows and, unless it ends the utterance, the beta
     // checkpoint row behind it — issued one segment ahead
     auto prefetch = [&](int c, int buf) {
       const int t0 = c * kSeg;
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int chunk = lane + 32 * h;  // 16-byte chunk of the [kSeg][32] tile
-        const int t = t0 + (chunk >> 3);
-        if (t < T) cp_async16(zt2 + (buf * kSeg * kW) * 4 + chunk * 16, Zb + (size_t)t * kW + (chunk & 7) * 4);
+      for (int h = 0; h < 2 * S; ++h) {
+        const int chunk = lane + 32 * h;  // 16-byte chunk of the [kSeg][NW] tile
+        const int t = t0 + (chunk >> (NW == 32 ? 3 : 4));  // (NW / 4 chunks per frame)
+        if (t < T) cp_async16(zt2 + (buf * kSeg * NW) * 4 + chunk * 16, Zb + (size_t)t * NW + (chunk & (NW / 4 - 1)) * 4);
       }
       if (t0 + kSeg < T) {
         const float* src = p.ckBa + ((size_t)b * p.nC + c) * Lp + lane * P;
@@ -827,8 +1081,8 @@ __global__ void __launch_bounds__(128, P <= 8 ? 4 : 2) asg_fac_grad_kernel(AsgPa
     if (c < p.nC) prefetch(c, 0);
     for (; c < p.nC; c += cstride, buf ^= 1) {
       const int t0 = c * kSeg, t1 = min(T, t0 + kSeg);
-      const uint32_t zt = zt2 + (buf * kSeg * kW) * 4;
-      const float* ztile = ztile2 + buf * kSeg * kW;
+      const uint32_t zt = zt2 + (buf * kSeg * NW) * 4;
+      const float* ztile = ztile2 + buf * kSeg * NW;
       cp_async_wait_all();
       __syncwarp();
       // ---- backwards: beta-tilde rows of frames t1-1 .. t0 into shared memory --------------------
@@ -838,7 +1092,7 @@ __global__ void __launch_bounds__(128, P <= 8 ? 4 : 2) asg_fac_grad_kernel(AsgPa
       int tstart;
       if (t1 >= T) {
 #pragma unroll
-        for (int k = 0; k < P; ++k) st.v[k] = (lane * P + k == L - 1) ? ztile[(T - 1 - t0) * kW + (st.y4[k] >> 2)] : kNeg;
+        for (int k = 0; k < P; ++k) st.v[k] = (lane * P + k == L - 1) ? ztile[(T - 1 - t0) * NW + (st.y4[k] >> 2)] : kNeg;
         fac_store_row<P>(st, brow + (size_t)(T - 1 - t0) * Lp, lane);
         tstart = T - 2;
       } else {
@@ -873,7 +1127,7 @@ __global__ void __launch_bounds__(128, P <= 8 ? 4 : 2) asg_fac_grad_kernel(AsgPa
         DA = lane > 0 ? (float)(ca[lane - 1] - CA) : 0.f;
       }
       for (int t = tstart; t >= t0; --t) {
-        fac_beta_step<P>(st, s2b, zt + (t - t0) * (4 * kW), lane, DB);
+        fac_beta_step<P>(st, s2b, zt + (t - t0) * (4 * NW), lane, DB);
         fac_store_row<P>(st, brow + (size_t)(t - t0) * Lp, lane);
       }
       // ---- forwards: alpha-tilde, occupancies, transition statistics -----------------------------
@@ -882,7 +1136,9 @@ __global__ void __launch_bounds__(128, P <= 8 ? 4 : 2) asg_fac_grad_kernel(AsgPa
 #pragma unroll
         for (int k = 0; k < P; ++k) st.v[k] = kNeg;
         if (lane == 0) st.v[0] = ztile[st.y4[0] >> 2];
-        Gb[lane] = (lane == y_s[0]) ? 1.0f : 0.0f;  // frame 0 sits at position 0 with probability one
+#pragma unroll
+        for (int q = 0; q < S; ++q)  // frame 0 sits at position 0 with probability one
+          Gb[lane + 32 * q] = (lane + 32 * q == y_s[0]) ? 1.0f : 0.0f;
         tfirst = 1;
       } else {
 #pragma unroll
@@ -894,7 +1150,7 @@ __global__ void __launch_bounds__(128, P <= 8 ? 4 : 2) asg_fac_grad_kernel(AsgPa
       const float2 K2 = make_float2(K, K);
       __syncwarp();
       for (int t = tfirst; t < t1; ++t) {
-        const uint32_t zrow = zt + (t - t0) * (4 * kW);
+        const uint32_t zrow = zt + (t - t0) * (4 * NW);
         const float* br = brow + (size_t)(t - t0) * Lp + lane * P;
         float up = __shfl_up_sync(0xffffffffu, st.v[P - 1], 1) + DA;
         if (lane == 0) up = kNeg;
@@ -919,9 +1175,15 @@ __global__ void __launch_bounds__(128, P <= 8 ? 4 : 2) asg_fac_grad_kernel(AsgPa
         __syncwarp();
         // occupancy per label = sum over its positions / frame total (true division): a frame's occupancies add up
         // to one exactly as the FCC posteriors do (N = 1: 1 - 1 = 0), and the same total normalises the statistics
-        const float gl = label_sum(grow_sa, grow, order_s, fx);
-        const float gt = warp_sum(gl);
-        Gb[(size_t)t * kW + lane] = gt > 0.f ? gl / gt : 0.f;
+        float gl[S];
+#pragma unroll
+        for (int q = 0; q < S; ++q) gl[q] = label_sum(grow_sa, grow, order_s, fx[q]);
+        float gs = gl[0];
+#pragma unroll
+        for (int q = 1; q < S; ++q) gs += gl[q];
+        const float gt = warp_sum(gs);
+#pragma unroll
+        for (int q = 0; q < S; ++q) Gb[(size_t)t * NW + lane + 32 * q] = gt > 0.f ? gl[q] / gt : 0.f;
         const float inv = gt > 0.f ? __fdividef(1.0f, gt) : 0.f;
         const float2 inv2 = make_float2(inv, inv);
 #pragma unroll
@@ -942,18 +1204,22 @@ __global__ void __launch_bounds__(128, P <= 8 ? 4 : 2) asg_fac_grad_kernel(AsgPa
     }
     __syncthreads();
   }
-  if (warp == 0) {  // lane n owns row n of the partial: positions with label n, in sorted order
-    float* row = dtr_s + lane * (kW + 1);
-    for (int i = start_s[lane]; i < start_s[lane + 1]; ++i) {
-      const int l = order_s[i];
-      row[lane] += dsum_s[l];
-      if (l > 0) row[y_s[l - 1]] += dsum_s[Lp + l];
+  if (warp == 0) {  // lane n owns rows n (+ 32) of the partial: positions with label n, in sorted order
+#pragma unroll
+    for (int q = 0; q < S; ++q) {
+      const int n = lane + 32 * q;
+      float* row = dtr_s + n * (NW + 1);
+      for (int i = start_s[n]; i < start_s[n + 1]; ++i) {
+        const int l = order_s[i];
+        row[n] += dsum_s[l];
+        if (l > 0) row[y_s[l - 1]] += dsum_s[Lp + l];
+      }
     }
   }
   __syncthreads();
   const float sgn = (p.terms & W2L_TERM_FCC) ? -1.0f : 1.0f;  // FAC enters ASG with a minus sign
   const float cf = sgn * p.coef[b];
-  for (int k = threadIdx.x; k < kW * kW; k += blockDim.x) part[k] = cf * dtr_s[(k / kW) * (kW + 1) + (k % kW)];
+  for (int k = threadIdx.x; k < NW * NW; k += blockDim.x) part[k] = cf * dtr_s[(k / NW) * (NW + 1) + (k % NW)];
 }
 
 // ---- long targets (Lp > 256): the halo path ---------------------------------------------------------------------
@@ -969,19 +1235,20 @@ constexpr int kHaloMaxW = 5;  // 1024 positions
 struct HaloLayout {
   int gsh, dtr, order, start, y, dsum, ztile, bnext, brow, grow, per_warp, total;
 };
+template <int NW>
 __host__ __device__ inline HaloLayout halo_layout(int warps) {
   HaloLayout f;
   int o = 0;
-  f.gsh = o;    o += 2 * kHaloMaxW * kW;  // [2 frame parities][W][32] per-label partial sums
-  f.dtr = o;    o += kW * (kW + 1);
+  f.gsh = o;    o += 2 * kHaloMaxW * NW;  // [2 frame parities][W][NW] per-label partial sums
+  f.dtr = o;    o += NW * (NW + 1);
   o = (o + 3) & ~3;
   const int w0 = o;
   f.order = 0;                        // offsets inside a warp's block
   f.start = kHaloRow;
-  f.y = f.start + 36;
+  f.y = f.start + NW + 4;
   f.dsum = f.y + kHaloRow + 16;
   f.ztile = (f.dsum + 2 * kHaloRow + 3) & ~3;
-  f.bnext = f.ztile + 2 * kSeg * kW;
+  f.bnext = f.ztile + 2 * kSeg * NW;
   f.brow = f.bnext + kHaloRow;
   f.grow = f.brow + kSeg * kHaloRow;
   f.per_warp = (f.grow + kHaloRow + 4 + 3) & ~3;
@@ -997,16 +1264,17 @@ __host__ __device__ inline HaloLayout halo_layout(int warps) {
   return f;
 }
 
+template <int NW>
 __global__ void __launch_bounds__(32 * kHaloMaxW) asg_fac_grad_halo_kernel(AsgParams p) {
-  constexpr int P = 8;
+  constexpr int P = 8, S = NW / 32;
   extern __shared__ __align__(16) float smem[];
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31, W = blockDim.x >> 5;  // warp = slice
   const int b = blockIdx.y;
   const int T = p.T;
-  const HaloLayout lay = halo_layout(W);
-  float* part = p.parts + ((size_t)p.n_fcc_parts + (size_t)b * gridDim.x + blockIdx.x) * (kW * kW);
+  const HaloLayout lay = halo_layout<NW>(W);
+  float* part = p.parts + ((size_t)p.n_fcc_parts + (size_t)b * gridDim.x + blockIdx.x) * (NW * NW);
   if (!p.valid[b]) {
-    for (int k = threadIdx.x; k < kW * kW; k += blockDim.x) part[k] = 0.f;
+    for (int k = threadIdx.x; k < NW * NW; k += blockDim.x) part[k] = 0.f;
     return;
   }
   const int L = p.tsz[b];
@@ -1020,13 +1288,15 @@ __global__ void __launch_bounds__(32 * kHaloMaxW) asg_fac_grad_halo_kernel(AsgPa
   int* y_s = reinterpret_cast<int*>(smem + lay.y + wo);          // label of position base + i
   float* dsum_s = smem + lay.dsum + wo;
   const int32_t* yg = p.target + (size_t)b * p.L;
-  for (int k = threadIdx.x; k < kW * (kW + 1); k += blockDim.x) dtr_s[k] = 0.f;
+  for (int k = threadIdx.x; k < NW * (NW + 1); k += blockDim.x) dtr_s[k] = 0.f;
   for (int i = lane; i < kHaloRow + 16; i += 32) {
     const int l = base + i;
     y_s[i] = (l >= 0 && l < L) ? __ldg(yg + l) : 0;
   }
   __syncwarp();
-  {  // label-sorted index of the slice's useful positions (stable)
+  // label-sorted index of the slice's useful positions (stable).  The 32-wide form is kept as written before the width
+  // became a parameter: the general form compiles the NW = 32 kernel to a different (equivalent) instruction order.
+  if constexpr (NW == 32) {
     int cnt = 0;
     for (int l = lo_use; l < hi_use; ++l) cnt += (y_s[l - base] == lane);
     int pre = cnt;
@@ -1037,9 +1307,41 @@ __global__ void __launch_bounds__(32 * kHaloMaxW) asg_fac_grad_halo_kernel(AsgPa
     }
     int w0 = pre - cnt;
     start_s[lane] = w0;
-    if (lane == 31) start_s[32] = pre;
+    if (lane == 31) start_s[NW] = pre;
     for (int l = lo_use; l < hi_use; ++l)
       if (y_s[l - base] == lane) order_s[w0++] = l - base;
+  } else {  // lane n lists labels n and n + 32
+    int cnt[S];
+#pragma unroll
+    for (int q = 0; q < S; ++q) cnt[q] = 0;
+    for (int l = lo_use; l < hi_use; ++l) {
+      const int v = y_s[l - base];
+#pragma unroll
+      for (int q = 0; q < S; ++q) cnt[q] += (v == lane + 32 * q);
+    }
+    int w0[S], below = 0;
+#pragma unroll
+    for (int q = 0; q < S; ++q) {
+      int pre = cnt[q];
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int v = __shfl_up_sync(0xffffffffu, pre, o);
+        if (lane >= o) pre += v;
+      }
+      w0[q] = below + pre - cnt[q];
+      start_s[lane + 32 * q] = w0[q];
+      if (q == S - 1) {
+        if (lane == 31) start_s[NW] = below + pre;
+      } else {
+        below += __shfl_sync(0xffffffffu, pre, 31);
+      }
+    }
+    for (int l = lo_use; l < hi_use; ++l) {
+      const int v = y_s[l - base];
+#pragma unroll
+      for (int q = 0; q < S; ++q)
+        if (v == lane + 32 * q) order_s[w0[q]++] = l - base;
+    }
   }
   __syncthreads();
 
@@ -1055,8 +1357,8 @@ __global__ void __launch_bounds__(32 * kHaloMaxW) asg_fac_grad_halo_kernel(AsgPa
     const uint32_t bnext_sa = (uint32_t)__cvta_generic_to_shared(bnext);
     const uint32_t grow_sa = (uint32_t)__cvta_generic_to_shared(grow);
     const float tmax = trans_max(p.trans, p.N, lane);
-    const float* Zb = p.Z + (size_t)b * T * kW;
-    float* Gb = p.G + (size_t)b * T * kW;
+    const float* Zb = p.Z + (size_t)b * T * NW;
+    float* Gb = p.G + (size_t)b * T * NW;
     const double logZ2 = p.facLogZ2[b];
     const bool useful = lane >= 1 && lane <= 30;
     FacState<P> st;
@@ -1065,8 +1367,9 @@ __global__ void __launch_bounds__(32 * kHaloMaxW) asg_fac_grad_halo_kernel(AsgPa
 #pragma unroll
     for (int k = 0; k < P; ++k) s2b[k] = st.s2[k];
     fac_load_target<P>(st, p, b, L, lane, false, tmax, base);
-    FlushIndex fx;
-    fx.load(order_s, start_s, lane, kHaloRow);
+    FlushIndex fx[S];  // labels lane + 32 s
+#pragma unroll
+    for (int q = 0; q < S; ++q) fx[q].load(order_s, start_s, lane + 32 * q, kHaloRow);
     if (lane == 0) grow[kHaloRow] = 0.f;
     const int l0 = base + lane * P;  // first position of this lane
     // the chain lane (p.P positions each) whose offset this lane's positions carry, and its neighbours' across the lane edges
@@ -1075,10 +1378,10 @@ __global__ void __launch_bounds__(32 * kHaloMaxW) asg_fac_grad_halo_kernel(AsgPa
     auto prefetch = [&](int c, int buf) {
       const int t0 = c * kSeg;
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
+      for (int h = 0; h < 2 * S; ++h) {
         const int chunk = lane + 32 * h;
-        const int t = t0 + (chunk >> 3);
-        if (t < T) cp_async16(zt2 + (buf * kSeg * kW) * 4 + chunk * 16, Zb + (size_t)t * kW + (chunk & 7) * 4);
+        const int t = t0 + (chunk >> (NW == 32 ? 3 : 4));  // (NW / 4 chunks per frame)
+        if (t < T) cp_async16(zt2 + (buf * kSeg * NW) * 4 + chunk * 16, Zb + (size_t)t * NW + (chunk & (NW / 4 - 1)) * 4);
       }
       if (t0 + kSeg < T) {
         const float* src = p.ckBa + ((size_t)b * p.nC + c) * p.Lp;
@@ -1098,8 +1401,8 @@ __global__ void __launch_bounds__(32 * kHaloMaxW) asg_fac_grad_halo_kernel(AsgPa
     if ((int)blockIdx.x < p.nC) prefetch(blockIdx.x, 0);
     for (int c = blockIdx.x; c < p.nC; c += gridDim.x, buf ^= 1) {
       const int t0 = c * kSeg, t1 = min(T, t0 + kSeg);
-      const uint32_t zt = zt2 + (buf * kSeg * kW) * 4;
-      const float* ztile = ztile2 + buf * kSeg * kW;
+      const uint32_t zt = zt2 + (buf * kSeg * NW) * 4;
+      const float* ztile = ztile2 + buf * kSeg * NW;
       cp_async_wait_all();
       __syncwarp();
       // ---- backwards: beta-tilde rows of frames t1-1 .. t0 (exact on the useful lanes: the right halo absorbs the edge) ----
@@ -1108,7 +1411,7 @@ __global__ void __launch_bounds__(32 * kHaloMaxW) asg_fac_grad_halo_kernel(AsgPa
       int tstart;
       if (t1 >= T) {
 #pragma unroll
-        for (int k = 0; k < P; ++k) st.v[k] = (l0 + k == L - 1) ? ztile[(T - 1 - t0) * kW + (st.y4[k] >> 2)] : kNeg;
+        for (int k = 0; k < P; ++k) st.v[k] = (l0 + k == L - 1) ? ztile[(T - 1 - t0) * NW + (st.y4[k] >> 2)] : kNeg;
         fac_store_row<P>(st, brow + (size_t)(T - 1 - t0) * kHaloRow, lane);
         tstart = T - 2;
       } else {
@@ -1139,7 +1442,7 @@ __global__ void __launch_bounds__(32 * kHaloMaxW) asg_fac_grad_halo_kernel(AsgPa
         DA = (float)(ca[cl_prev] - CA);
       }
       for (int t = tstart; t >= t0; --t) {
-        fac_beta_step<P>(st, s2b, zt + (t - t0) * (4 * kW), lane, DB);
+        fac_beta_step<P>(st, s2b, zt + (t - t0) * (4 * NW), lane, DB);
         fac_store_row<P>(st, brow + (size_t)(t - t0) * kHaloRow, lane);
       }
       // ---- forwards (exact on the useful lanes: the left halo absorbs the edge) --------------------------------------
@@ -1147,7 +1450,10 @@ __global__ void __launch_bounds__(32 * kHaloMaxW) asg_fac_grad_halo_kernel(AsgPa
       if (t0 == 0) {
 #pragma unroll
         for (int k = 0; k < P; ++k) st.v[k] = (l0 + k == 0) ? ztile[st.y4[k] >> 2] : kNeg;
-        if (w == 0) Gb[lane] = (lane == y_s[P]) ? 1.0f : 0.0f;  // frame 0 sits at position 0 (slice 0, local index P)
+        if (w == 0) {  // frame 0 sits at position 0 (slice 0, local index P)
+#pragma unroll
+          for (int q = 0; q < S; ++q) Gb[lane + 32 * q] = (lane + 32 * q == y_s[P]) ? 1.0f : 0.0f;
+        }
         tfirst = 1;
       } else {
 #pragma unroll
@@ -1158,7 +1464,7 @@ __global__ void __launch_bounds__(32 * kHaloMaxW) asg_fac_grad_halo_kernel(AsgPa
       const float2 K2 = make_float2(K, K);
       __syncwarp();
       for (int t = tfirst; t < t1; ++t) {
-        const uint32_t zrow = zt + (t - t0) * (4 * kW);
+        const uint32_t zrow = zt + (t - t0) * (4 * NW);
         const float* br = brow + (size_t)(t - t0) * kHaloRow + lane * P;
         float up = __shfl_up_sync(0xffffffffu, st.v[P - 1], 1) + DA;
         if (lane == 0) up = kNeg;
@@ -1174,13 +1480,24 @@ __global__ void __launch_bounds__(32 * kHaloMaxW) asg_fac_grad_halo_kernel(AsgPa
         }
         __syncwarp();
         // this slice's per-label sums meet the other slices' (one CTA barrier per frame, buffers alternate by parity)
-        float* gbuf = gsh + (t & 1) * (kHaloMaxW * kW);
-        gbuf[w * kW + lane] = label_sum(grow_sa, grow, order_s, fx);
+        float* gbuf = gsh + (t & 1) * (kHaloMaxW * NW);
+#pragma unroll
+        for (int q = 0; q < S; ++q) gbuf[w * NW + lane + 32 * q] = label_sum(grow_sa, grow, order_s, fx[q]);
         __syncthreads();
-        float gl = 0.f;
-        for (int ww = 0; ww < W; ++ww) gl += gbuf[ww * kW + lane];
-        const float gt = warp_sum(gl);
-        if (w == 0) Gb[(size_t)t * kW + lane] = gt > 0.f ? gl / gt : 0.f;
+        float gl[S];
+#pragma unroll
+        for (int q = 0; q < S; ++q) {
+          gl[q] = 0.f;
+          for (int ww = 0; ww < W; ++ww) gl[q] += gbuf[ww * NW + lane + 32 * q];
+        }
+        float gs = gl[0];
+#pragma unroll
+        for (int q = 1; q < S; ++q) gs += gl[q];
+        const float gt = warp_sum(gs);
+        if (w == 0) {
+#pragma unroll
+          for (int q = 0; q < S; ++q) Gb[(size_t)t * NW + lane + 32 * q] = gt > 0.f ? gl[q] / gt : 0.f;
+        }
         const float inv = gt > 0.f ? __fdividef(1.0f, gt) : 0.f;
         const float2 inv2 = make_float2(inv, inv);
 #pragma unroll
@@ -1197,35 +1514,44 @@ __global__ void __launch_bounds__(32 * kHaloMaxW) asg_fac_grad_halo_kernel(AsgPa
   }
   __syncwarp();
   for (int ww = 0; ww < W; ++ww) {
-    if (w == ww) {  // lane n adds this slice's useful positions with label n to row n
-      float* row = dtr_s + lane * (kW + 1);
-      for (int i = start_s[lane]; i < start_s[lane + 1]; ++i) {
-        const int li = order_s[i];
-        row[lane] += dsum_s[li];
-        if (base + li > 0) row[y_s[li - 1]] += dsum_s[kHaloRow + li];
+    if (w == ww) {  // lane n adds this slice's useful positions with label n (+ 32) to row n (+ 32)
+#pragma unroll
+      for (int q = 0; q < S; ++q) {
+        const int n = lane + 32 * q;
+        float* row = dtr_s + n * (NW + 1);
+        for (int i = start_s[n]; i < start_s[n + 1]; ++i) {
+          const int li = order_s[i];
+          row[n] += dsum_s[li];
+          if (base + li > 0) row[y_s[li - 1]] += dsum_s[kHaloRow + li];
+        }
       }
     }
     __syncthreads();
   }
   const float sgn = (p.terms & W2L_TERM_FCC) ? -1.0f : 1.0f;
   const float cf = sgn * p.coef[b];
-  for (int k = threadIdx.x; k < kW * kW; k += blockDim.x) part[k] = cf * dtr_s[(k / kW) * (kW + 1) + (k % kW)];
+  for (int k = threadIdx.x; k < NW * NW; k += blockDim.x) part[k] = cf * dtr_s[(k / NW) * (NW + 1) + (k % NW)];
 }
 
 // ------------------------------------------------------------------------------------------
 // 4. FCC gradient + emission gradient, from the stored a-hat / b-hat vectors: no dependence between frames
 // ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kFccGradWarps * 32, 2) asg_fcc_grad_kernel(AsgParams p) {
+// NW = 64: lane i accumulates rows i and i + 32 (128 registers), 4 warps of 8 frames, slabs in dynamic shared memory
+template <int NW>
+__global__ void __launch_bounds__(fcc_grad_warps<NW>() * 32, NW == 32 ? 2 : 1) asg_fcc_grad_kernel(AsgParams p) {
+  constexpr int S = NW / 32, kWarps = fcc_grad_warps<NW>(), kFrames = fcc_grad_frames<NW>();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int b = blockIdx.y;
-  const int chunk = blockIdx.x * kFccGradWarps + warp;
+  const int chunk = blockIdx.x * kWarps + warp;
   const int T = p.T, N = p.N;
   const bool has_fcc = p.terms & W2L_TERM_FCC, has_fac = p.terms & W2L_TERM_FAC;
   const int ok = p.valid[b];
-  // shared memory: first the warps' a-hat tiles ((kFccGradFrames + 1) x 32 each), later re-used as the warps'
-  // accumulator slabs (32 x 33 each) of the CTA reduction
-  __shared__ __align__(16) float sm[kFccGradWarps * kW * (kW + 1)];
-  static_assert((kFccGradFrames + 1) * kW <= kW * (kW + 1), "tile must fit in a slab");
+  // shared memory: first the warps' a-hat tiles ((kFrames + 1) x NW each), later re-used as the warps'
+  // accumulator slabs (NW x (NW + 1) each) of the CTA reduction
+  __shared__ __align__(16) float sm_static[NW == 32 ? kWarps * NW * (NW + 1) : 4];
+  extern __shared__ __align__(16) float smem[];
+  float* sm = NW == 32 ? sm_static : smem;
+  static_assert((kFrames + 1) * NW <= NW * (NW + 1), "tile must fit in a slab");
   if (chunk == 0 && lane == 0) {
     float l = NAN;
     if (ok) {
@@ -1236,63 +1562,91 @@ __global__ void __launch_bounds__(kFccGradWarps * 32, 2) asg_fcc_grad_kernel(Asg
     }
     p.loss[b] = l;
   }
-  const int t0 = chunk * kFccGradFrames, t1 = min(T, t0 + kFccGradFrames);
-  float2 acc[kW / 2];
+  const int t0 = chunk * kFrames, t1 = min(T, t0 + kFrames);
+  float2 acc[S][NW / 2];  // row lane + 32 s of the warp's transition statistics
 #pragma unroll
-  for (int j = 0; j < kW / 2; ++j) acc[j] = make_float2(0.f, 0.f);
+  for (int q = 0; q < S; ++q)
+#pragma unroll
+    for (int j = 0; j < NW / 2; ++j) acc[q][j] = make_float2(0.f, 0.f);
   if (t0 < T) {
     float* de = p.d_emis + (size_t)b * T * N;
-    const float* Gb = p.G + (size_t)b * T * kW;
+    const float* Gb = p.G + (size_t)b * T * NW;
     if (!ok) {
       for (int t = t0; t < t1; ++t)
-        if (lane < N) de[(size_t)t * N + lane] = 0.f;
+#pragma unroll
+        for (int q = 0; q < S; ++q)
+          if (lane + 32 * q < N) de[(size_t)t * N + lane + 32 * q] = 0.f;
     } else if (!has_fcc) {
       const float coef = p.coef[b];
       for (int t = t0; t < t1; ++t)
-        if (lane < N) de[(size_t)t * N + lane] = coef * Gb[(size_t)t * kW + lane];
+#pragma unroll
+        for (int q = 0; q < S; ++q)
+          if (lane + 32 * q < N) de[(size_t)t * N + lane + 32 * q] = coef * Gb[(size_t)t * NW + lane + 32 * q];
     } else {
       const float coef = p.coef[b];
-      const float* Ab = p.A + (size_t)b * T * kW + lane;
-      const float* Bb = p.Bh + (size_t)b * T * kW + lane;
-      const float* Zb = p.Z + (size_t)b * T * kW + lane;
+      const float* Ab = p.A + (size_t)b * T * NW + lane;
+      const float* Bb = p.Bh + (size_t)b * T * NW + lane;
+      const float* Zb = p.Z + (size_t)b * T * NW + lane;
       const float* Gl = Gb + lane;
-      float* tile = sm + warp * (kW * (kW + 1));
+      float* tile = sm + warp * (NW * (NW + 1));
       const uint32_t tile_sa = (uint32_t)__cvta_generic_to_shared(tile);
       // every global read of the chunk is issued before anything is consumed (the frames are independent)
-      float a[kFccGradFrames], bh[kFccGradFrames], z[kFccGradFrames], gf[kFccGradFrames];
+      float a[S][kFrames], bh[S][kFrames], z[S][kFrames], gf[S][kFrames];
 #pragma unroll
-      for (int k = 0; k < kFccGradFrames; ++k) {
+      for (int k = 0; k < kFrames; ++k) {
         const int t = t0 + k;
         const bool in = t < t1;
-        a[k] = in ? __ldg(Ab + (size_t)t * kW) : 0.f;
-        bh[k] = in ? __ldg(Bb + (size_t)t * kW) : 0.f;
-        z[k] = in ? __ldg(Zb + (size_t)t * kW) : 0.f;
-        gf[k] = (in && has_fac) ? __ldg(Gl + (size_t)t * kW) : 0.f;
-      }
-      const float aprev = t0 > 0 ? __ldg(Ab + (size_t)(t0 - 1) * kW) : 0.f;
-      const float sv = (lane < kFccGradFrames && t0 + lane < t1) ? __ldg(p.sA + (size_t)b * T + t0 + lane) : 0.f;  // lane k: s_{t0+k}
-      tile[lane] = aprev;
 #pragma unroll
-      for (int k = 0; k < kFccGradFrames; ++k) tile[(k + 1) * kW + lane] = a[k];
+        for (int q = 0; q < S; ++q) {
+          a[q][k] = in ? __ldg(Ab + (size_t)t * NW + 32 * q) : 0.f;
+          bh[q][k] = in ? __ldg(Bb + (size_t)t * NW + 32 * q) : 0.f;
+          z[q][k] = in ? __ldg(Zb + (size_t)t * NW + 32 * q) : 0.f;
+          gf[q][k] = (in && has_fac) ? __ldg(Gl + (size_t)t * NW + 32 * q) : 0.f;
+        }
+      }
+      float aprev[S];
+#pragma unroll
+      for (int q = 0; q < S; ++q) aprev[q] = t0 > 0 ? __ldg(Ab + (size_t)(t0 - 1) * NW + 32 * q) : 0.f;
+      const float sv = (lane < kFrames && t0 + lane < t1) ? __ldg(p.sA + (size_t)b * T + t0 + lane) : 0.f;  // lane k: s_{t0+k}
+#pragma unroll
+      for (int q = 0; q < S; ++q) tile[lane + 32 * q] = aprev[q];
+#pragma unroll
+      for (int k = 0; k < kFrames; ++k)
+#pragma unroll
+        for (int q = 0; q < S; ++q) tile[(k + 1) * NW + lane + 32 * q] = a[q][k];
       __syncwarp();
 #pragma unroll
-      for (int k = 0; k < kFccGradFrames; ++k) {
+      for (int k = 0; k < kFrames; ++k) {
         const int t = t0 + k;
         if (t >= t1) break;
-        const float g = a[k] * bh[k];
-        const float gsum = warp_sum(g);
-        if (lane < N) de[(size_t)t * N + lane] = coef * (g / gsum - gf[k]);  // (true division: N = 1 must give exactly 1 - 1)
+        float g[S];
+#pragma unroll
+        for (int q = 0; q < S; ++q) g[q] = a[q][k] * bh[q][k];
+        float gs = g[0];
+#pragma unroll
+        for (int q = 1; q < S; ++q) gs += g[q];
+        const float gsum = warp_sum(gs);
+#pragma unroll
+        for (int q = 0; q < S; ++q)  // (true division: N = 1 must give exactly 1 - 1)
+          if (lane + 32 * q < N) de[(size_t)t * N + lane + 32 * q] = coef * (g[q] / gsum - gf[q][k]);
         if (t >= 1) {
           // xi_t(i, j) = w_i * a_{t-1}[j] * M'[i][j],  w_i = X_t[i] * s_t * b_t[i] / sum_i a_t[i] b_t[i]
           const float st = __shfl_sync(0xffffffffu, sv, k);
-          const float w = ex2f(z[k]) * bh[k] * (st * __fdividef(1.0f, gsum));
-          const float2 w2 = make_float2(w, w);
+          float2 w2[S];
 #pragma unroll
-          for (int q = 0; q < kW / 4; ++q) {
+          for (int q = 0; q < S; ++q) {
+            const float w = ex2f(z[q][k]) * bh[q][k] * (st * __fdividef(1.0f, gsum));
+            w2[q] = make_float2(w, w);
+          }
+#pragma unroll
+          for (int u = 0; u < NW / 4; ++u) {
             float4 v;
-            asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(tile_sa + (k * kW + 4 * q) * 4));
-            acc[2 * q] = ffma2_rn(w2, make_float2(v.x, v.y), acc[2 * q]);
-            acc[2 * q + 1] = ffma2_rn(w2, make_float2(v.z, v.w), acc[2 * q + 1]);
+            asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(tile_sa + (k * NW + 4 * u) * 4));
+#pragma unroll
+            for (int q = 0; q < S; ++q) {
+              acc[q][2 * u] = ffma2_rn(w2[q], make_float2(v.x, v.y), acc[q][2 * u]);
+              acc[q][2 * u + 1] = ffma2_rn(w2[q], make_float2(v.z, v.w), acc[q][2 * u + 1]);
+            }
           }
         }
       }
@@ -1302,23 +1656,24 @@ __global__ void __launch_bounds__(kFccGradWarps * 32, 2) asg_fcc_grad_kernel(Asg
   // CTA partial of the FCC transition gradient: the warps' accumulators go to their slabs, one pass sums them in a
   // fixed order and applies coef * M'
   __syncthreads();
-  {
-    float* slab = sm + warp * (kW * (kW + 1)) + lane * (kW + 1);
 #pragma unroll
-    for (int j = 0; j < kW / 2; ++j) {
-      slab[2 * j] = acc[j].x;
-      slab[2 * j + 1] = acc[j].y;
+  for (int q = 0; q < S; ++q) {
+    float* slab = sm + warp * (NW * (NW + 1)) + (lane + 32 * q) * (NW + 1);
+#pragma unroll
+    for (int j = 0; j < NW / 2; ++j) {
+      slab[2 * j] = acc[q][j].x;
+      slab[2 * j + 1] = acc[q][j].y;
     }
   }
   __syncthreads();
   const float tmax = trans_max(p.trans, N, lane);
   const float coef = ok ? p.coef[b] : 0.f;
-  float* part = p.parts + ((size_t)b * gridDim.x + blockIdx.x) * (kW * kW);
-  for (int k = threadIdx.x; k < kW * kW; k += blockDim.x) {
-    const int i = k / kW, j = k % kW;
+  float* part = p.parts + ((size_t)b * gridDim.x + blockIdx.x) * (NW * NW);
+  for (int k = threadIdx.x; k < NW * NW; k += blockDim.x) {
+    const int i = k / NW, j = k % NW;
     float r = 0.f;
 #pragma unroll
-    for (int w = 0; w < kFccGradWarps; ++w) r += sm[w * (kW * (kW + 1)) + i * (kW + 1) + j];
+    for (int w = 0; w < kWarps; ++w) r += sm[w * (NW * (NW + 1)) + i * (NW + 1) + j];
     const float m = (i < N && j < N) ? __expf(__ldg(p.trans + i * N + j) - tmax) : 0.f;
     part[k] = coef * r * m;
   }
@@ -1326,9 +1681,10 @@ __global__ void __launch_bounds__(kFccGradWarps * 32, 2) asg_fcc_grad_kernel(Asg
 
 // 5. out[g][k] = sum of the partials q in [g*group, (g+1)*group) — fixed order, no atomics.  final_N > 0: the single
 // group is written as d_trans [N][N].
+template <int NW>
 __global__ void __launch_bounds__(256) asg_parts_reduce_kernel(const float* in, int n_in, int group, float* out, int final_N) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= kW * kW) return;
+  if (k >= NW * NW) return;
   const int q0 = blockIdx.y * group, q1 = min(n_in, q0 + group);
   float s[8];
 #pragma unroll
@@ -1336,15 +1692,15 @@ __global__ void __launch_bounds__(256) asg_parts_reduce_kernel(const float* in, 
   int q = q0;
   for (; q + 7 < q1; q += 8) {
 #pragma unroll
-    for (int u = 0; u < 8; ++u) s[u] += in[(size_t)(q + u) * (kW * kW) + k];
+    for (int u = 0; u < 8; ++u) s[u] += in[(size_t)(q + u) * (NW * NW) + k];
   }
-  for (; q < q1; ++q) s[0] += in[(size_t)q * (kW * kW) + k];
+  for (; q < q1; ++q) s[0] += in[(size_t)q * (NW * NW) + k];
   const float tot = ((s[0] + s[1]) + (s[2] + s[3])) + ((s[4] + s[5]) + (s[6] + s[7]));
   if (final_N > 0) {
-    const int i = k / kW, j = k % kW;
+    const int i = k / NW, j = k % NW;
     if (i < final_N && j < final_N) out[i * final_N + j] = tot;
   } else {
-    out[(size_t)blockIdx.y * (kW * kW) + k] = tot;
+    out[(size_t)blockIdx.y * (NW * NW) + k] = tot;
   }
 }
 
@@ -1361,34 +1717,46 @@ __global__ void asg_loss_only_kernel(AsgParams p) {
   p.loss[b] = l;
 }
 
+// P >= 16 means more than 256 positions, which always take the halo kernel: at NW = 64 the single-warp FAC grad kernel
+// is not instantiated for them (the NW = 32 instantiations are kept as they are).  asg_forward_backward refuses the
+// combination explicitly, so the P = 8 stand-in can never run with a wider row.
+#define W2L_FAC_GRAD_P(PP) ((NW == 32 || (PP) <= 8) ? (PP) : 8)
 int pick_P(int Le) {  // positions per lane: smallest power of two with 32*P >= Le
   int P = 1;
   while (32 * P < Le) P <<= 1;
   return P;
 }
+template <int NW>
 int fac_grad_warps(int Lp) {  // warps per FAC grad CTA: as many as ~96 KB of shared memory hold, at most 4
   for (int w = 4; w > 1; --w)
-    if ((size_t)fac_grad_layout(Lp, w).total * 4 <= 96 * 1024) return w;
+    if ((size_t)fac_grad_layout<NW>(Lp, w).total * 4 <= 96 * 1024) return w;
   return 1;
 }
 
-int fcc_grad_ctas(int T) { return (T + kFccGradWarps * kFccGradFrames - 1) / (kFccGradWarps * kFccGradFrames); }
+template <int NW>
+int fcc_grad_ctas(int T) {
+  constexpr int per_cta = fcc_grad_warps<NW>() * fcc_grad_frames<NW>();
+  return (T + per_cta - 1) / per_cta;
+}
+template <int NW>
+constexpr size_t fcc_grad_smem() { return NW == 32 ? 0 : (size_t)fcc_grad_warps<NW>() * NW * (NW + 1) * 4; }  // dynamic
 // CTAs per sample of the FAC grad kernel: one resident wave of the chip over the batch (the CTAs loop over their segments)
-template <int P>
+template <int P, int NW>
 int fac_grad_slots(int warps, size_t smem) {
   int per_sm = 0;
-  if (smem > 48 * 1024) cudaFuncSetAttribute(asg_fac_grad_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, asg_fac_grad_kernel<P>, warps * 32, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
+  if (smem > 48 * 1024) cudaFuncSetAttribute(asg_fac_grad_kernel<P, NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, asg_fac_grad_kernel<P, NW>, warps * 32, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
   int dev = 0, sms = 132;
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   return per_sm * sms;
 }
+template <int NW>
 int fac_grad_ctas(const AsgParams& p) {
   if (p.Wg > 1) {  // the halo kernel: one CTA of Wg warps per segment, CTAs loop over their sample's segments
-    const size_t smem = (size_t)halo_layout(p.Wg).total * 4;
+    const size_t smem = (size_t)halo_layout<NW>(p.Wg).total * 4;
     int per_sm = 0;
-    cudaFuncSetAttribute(asg_fac_grad_halo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, asg_fac_grad_halo_kernel, 32 * p.Wg, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
+    cudaFuncSetAttribute(asg_fac_grad_halo_kernel<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, asg_fac_grad_halo_kernel<NW>, 32 * p.Wg, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
     int dev = 0, sms = 132;
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     int want = per_sm * sms / p.B;
@@ -1399,14 +1767,14 @@ int fac_grad_ctas(const AsgParams& p) {
   static int slots_cache[6] = {0, 0, 0, 0, 0, 0};
   const int idx = p.P == 1 ? 0 : p.P == 2 ? 1 : p.P == 4 ? 2 : p.P == 8 ? 3 : p.P == 16 ? 4 : 5;
   if (slots_cache[idx] == 0) {
-    const size_t smem = (size_t)fac_grad_layout(p.Lp, p.fac_grad_warps).total * 4;
+    const size_t smem = (size_t)fac_grad_layout<NW>(p.Lp, p.fac_grad_warps).total * 4;
     switch (p.P) {
-      case 1: slots_cache[idx] = fac_grad_slots<1>(p.fac_grad_warps, smem); break;
-      case 2: slots_cache[idx] = fac_grad_slots<2>(p.fac_grad_warps, smem); break;
-      case 4: slots_cache[idx] = fac_grad_slots<4>(p.fac_grad_warps, smem); break;
-      case 8: slots_cache[idx] = fac_grad_slots<8>(p.fac_grad_warps, smem); break;
-      case 16: slots_cache[idx] = fac_grad_slots<16>(p.fac_grad_warps, smem); break;
-      default: slots_cache[idx] = fac_grad_slots<32>(p.fac_grad_warps, smem); break;
+      case 1: slots_cache[idx] = fac_grad_slots<1, NW>(p.fac_grad_warps, smem); break;
+      case 2: slots_cache[idx] = fac_grad_slots<2, NW>(p.fac_grad_warps, smem); break;
+      case 4: slots_cache[idx] = fac_grad_slots<4, NW>(p.fac_grad_warps, smem); break;
+      case 8: slots_cache[idx] = fac_grad_slots<8, NW>(p.fac_grad_warps, smem); break;
+      case 16: slots_cache[idx] = fac_grad_slots<W2L_FAC_GRAD_P(16), NW>(p.fac_grad_warps, smem); break;
+      default: slots_cache[idx] = fac_grad_slots<W2L_FAC_GRAD_P(32), NW>(p.fac_grad_warps, smem); break;
     }
   }
   int want = slots_cache[idx] / p.B;
@@ -1414,29 +1782,30 @@ int fac_grad_ctas(const AsgParams& p) {
   return want < most ? want : most;
 }
 
+template <int NW>
 void carve(AsgParams& p, void* ws, size_t& total) {
   Carver c(ws);
   const size_t BT = (size_t)p.B * p.T, BC = (size_t)p.B * p.nC;
-  p.Z = c.take<float>(BT * kW);
+  p.Z = c.take<float>(BT * NW);
   p.mrow = c.take<float>(BT);
-  p.A = c.take<float>(BT * kW);
-  p.Bh = c.take<float>(BT * kW);
+  p.A = c.take<float>(BT * NW);
+  p.Bh = c.take<float>(BT * NW);
   p.sA = c.take<float>(BT);
-  p.G = c.take<float>(BT * kW);
+  p.G = c.take<float>(BT * NW);
   p.ckAa = c.take<float>(BC * p.Lp);
   p.ckBa = c.take<float>(BC * p.Lp);
-  p.ckCA = c.take<double>(BC * kW);
+  p.ckCA = c.take<double>(BC * kW);  // (per FAC chain lane)
   p.ckCB = c.take<double>(BC * kW);
   p.fccLogZ = c.take<double>(p.B);
   p.facLogZ2 = c.take<double>(p.B);
   p.facLogZ = c.take<double>(p.B);
   p.msum = c.take<double>(p.B);
   // sized for the most CTAs the FAC grad kernel can use (the actual count depends on the device's occupancy)
-  const size_t nparts = (size_t)(fcc_grad_ctas(p.T) + (p.Wg > 1 ? p.nC : (p.nC + p.fac_grad_warps - 1) / p.fac_grad_warps)) * p.B;
-  p.parts = c.take<float>(nparts * kW * kW);
-  p.parts2 = c.take<float>((nparts + kRedGroup - 1) / kRedGroup * kW * kW);
+  const size_t nparts = (size_t)(fcc_grad_ctas<NW>(p.T) + (p.Wg > 1 ? p.nC : (p.nC + p.fac_grad_warps - 1) / p.fac_grad_warps)) * p.B;
+  p.parts = c.take<float>(nparts * NW * NW);
+  p.parts2 = c.take<float>((nparts + kRedGroup - 1) / kRedGroup * NW * NW);
   p.order = c.take<int>((size_t)p.B * p.Lp);
-  p.start = c.take<int>((size_t)p.B * 36);
+  p.start = c.take<int>((size_t)p.B * (NW + 4));
   p.tsz = c.take<int>(p.B);
   p.valid = c.take<int>(p.B);
   p.scale = c.take<float>(p.B);
@@ -1444,6 +1813,7 @@ void carve(AsgParams& p, void* ws, size_t& total) {
   total = c.off;
 }
 
+template <int NW>
 void shape(AsgParams& p, int B, int T, int N, int L) {
   p.B = B;
   p.T = T;
@@ -1457,45 +1827,47 @@ void shape(AsgParams& p, int B, int T, int N, int L) {
   p.nC = (T + kSeg - 1) / kSeg;
   // long targets: the FAC grad kernel cuts the row into slices of 240 useful positions (the halo path), 4 warps per CTA
   p.Wg = p.P >= 16 ? (Le + kHaloUse - 1) / kHaloUse : 1;
-  p.fac_grad_warps = p.Wg > 1 ? p.Wg : fac_grad_warps(p.Lp);
+  p.fac_grad_warps = p.Wg > 1 ? p.Wg : fac_grad_warps<NW>(p.Lp);
 }
 
-}  // namespace
-}  // namespace w2l
-
-using namespace w2l;
-
-extern "C" size_t w2l_asg_workspace_size(int B, int T, int N, int L) {
+template <int NW>
+size_t asg_workspace_size(int B, int T, int N, int L) {
   if (B <= 0 || T <= 0 || N <= 0) return 0;
   AsgParams p{};
-  shape(p, B, T, N, L);
+  shape<NW>(p, B, T, N, L);
   size_t total = 0;
-  carve(p, nullptr, total);
+  carve<NW>(p, nullptr, total);
   return total;
 }
 
-extern "C" int w2l_asg_forward_backward(void* stream_, int terms, int B, int T, int N, int L, int scale_mode,
-                                        const float* emis, const int32_t* target, const float* trans,
-                                        const float* dloss, float* loss, float* d_emis, float* d_trans,
-                                        void* workspace, size_t workspace_bytes) {
+// the body of w2l_asg_forward_backward (NW = 32) and w2l_asg64_forward_backward (NW = 64); `name` prefixes the errors
+template <int NW>
+int asg_forward_backward(const char* name, void* stream_, int terms, int B, int T, int N, int L, int scale_mode,
+                         const float* emis, const int32_t* target, const float* trans, const float* dloss, float* loss,
+                         float* d_emis, float* d_trans, void* workspace, size_t workspace_bytes) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (B <= 0 || T <= 0 || N <= 0) return fail(W2L_ERR_INVALID_ARGUMENT, "asg: B, T, N must be positive");
-  if (!(terms & W2L_TERM_ASG) || (terms & ~W2L_TERM_ASG)) return fail(W2L_ERR_INVALID_ARGUMENT, "asg: bad terms");
-  if (!emis || !trans || !loss) return fail(W2L_ERR_INVALID_ARGUMENT, "asg: null emissions/transitions/loss");
+  const std::string tag(name);
+  if (B <= 0 || T <= 0 || N <= 0) return fail(W2L_ERR_INVALID_ARGUMENT, tag + ": B, T, N must be positive");
+  if (!(terms & W2L_TERM_ASG) || (terms & ~W2L_TERM_ASG)) return fail(W2L_ERR_INVALID_ARGUMENT, tag + ": bad terms");
+  if (!emis || !trans || !loss) return fail(W2L_ERR_INVALID_ARGUMENT, tag + ": null emissions/transitions/loss");
   if ((terms & W2L_TERM_FAC) && (!target || L <= 0))
-    return fail(W2L_ERR_INVALID_ARGUMENT, "asg: ForceAlignment needs a target of width L > 0");
+    return fail(W2L_ERR_INVALID_ARGUMENT, tag + ": ForceAlignment needs a target of width L > 0");
   if ((d_emis == nullptr) != (d_trans == nullptr))
-    return fail(W2L_ERR_INVALID_ARGUMENT, "asg: d_emis and d_trans must be given together");
-  if (scale_mode < 0 || scale_mode > 4) return fail(W2L_ERR_INVALID_ARGUMENT, "asg: bad scale mode");
-  if (N > kW) return fail(W2L_ERR_UNSUPPORTED, "asg: N > 32 tokens is not covered by these kernels");
+    return fail(W2L_ERR_INVALID_ARGUMENT, tag + ": d_emis and d_trans must be given together");
+  if (scale_mode < 0 || scale_mode > 4) return fail(W2L_ERR_INVALID_ARGUMENT, tag + ": bad scale mode");
+  if (N > NW)
+    return fail(W2L_ERR_UNSUPPORTED, tag + ": N > " + std::to_string(NW) + " tokens is not covered by these kernels");
   AsgParams p{};
-  shape(p, B, T, N, L);  // the workspace is sized for the declared L whether or not a target is given
+  shape<NW>(p, B, T, N, L);  // the workspace is sized for the declared L whether or not a target is given
   if (!target) p.L = 0;
   size_t need = 0;
-  carve(p, workspace, need);
+  carve<NW>(p, workspace, need);
   if (!workspace || workspace_bytes < need)
-    return fail(W2L_ERR_WORKSPACE, "asg: workspace too small (need " + std::to_string(need) + " bytes)");
-  if ((terms & W2L_TERM_FAC) && p.P > 32) return fail(W2L_ERR_UNSUPPORTED, "asg: target longer than 1024 is not covered");
+    return fail(W2L_ERR_WORKSPACE, tag + ": workspace too small (need " + std::to_string(need) + " bytes)");
+  if ((terms & W2L_TERM_FAC) && p.P > 32) return fail(W2L_ERR_UNSUPPORTED, tag + ": target longer than 1024 is not covered");
+  // W2L_FAC_GRAD_P: at NW = 64 only P <= 8 has a single-warp FAC grad kernel; longer rows must take the halo kernel
+  if (NW != 32 && p.Wg == 1 && p.P > 8)
+    return fail(W2L_ERR_UNSUPPORTED, tag + ": no single-warp FAC gradient kernel for " + std::to_string(p.P) + " positions per lane");
   p.scale_mode = scale_mode;
   p.terms = terms;
   p.need_grad = d_emis != nullptr;
@@ -1514,14 +1886,14 @@ extern "C" int w2l_asg_forward_backward(void* stream_, int terms, int B, int T, 
   if (has_fcc) p.roles[p.n_roles++] = kRoleFccAlpha;
   if (has_fcc && p.need_grad) p.roles[p.n_roles++] = kRoleFccBeta;
   p.roles[p.n_roles++] = kRoleMsum;
-  const int gF = fcc_grad_ctas(T), gA = fac_grad_ctas(p);
+  const int gF = fcc_grad_ctas<NW>(T), gA = fac_grad_ctas<NW>(p);
   p.n_fcc_parts = (has_fcc && p.need_grad) ? gF * B : 0;
   p.n_fac_parts = (has_fac && p.need_grad) ? gA * B : 0;
 
   const long long nframes = (long long)B * T;
   const int frame_blocks = (int)std::min<long long>((nframes + 7) / 8, sm_count() * 8);
   const int meta_blocks = (B + 7) / 8;
-  asg_prep_kernel<<<frame_blocks + meta_blocks, 256, 0, stream>>>(p, frame_blocks);
+  asg_prep_kernel<NW><<<frame_blocks + meta_blocks, 256, 0, stream>>>(p, frame_blocks);
   W2L_LAUNCH_CHECK("asg_prep_kernel");
 
 #define W2L_FOR_P(MACRO)        \
@@ -1535,7 +1907,7 @@ extern "C" int w2l_asg_forward_backward(void* stream_, int terms, int B, int T, 
   }
   profile_kind(2);
   profile_start(stream);
-#define W2L_LAUNCH_CHAINS(PP) asg_chains_kernel<PP><<<p.n_roles * B, 32, 0, stream>>>(p)
+#define W2L_LAUNCH_CHAINS(PP) asg_chains_kernel<PP, NW><<<p.n_roles * B, 32, 0, stream>>>(p)
   W2L_FOR_P(W2L_LAUNCH_CHAINS)
   profile_stop(stream);
   W2L_LAUNCH_CHECK("asg_chains_kernel");
@@ -1546,33 +1918,61 @@ extern "C" int w2l_asg_forward_backward(void* stream_, int terms, int B, int T, 
     return W2L_OK;
   }
   if (has_fac && p.Wg > 1) {
-    const size_t smem = (size_t)halo_layout(p.Wg).total * 4;
-    W2L_CUDA_CHECK(cudaFuncSetAttribute(asg_fac_grad_halo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    asg_fac_grad_halo_kernel<<<dim3(gA, B), 32 * p.Wg, smem, stream>>>(p);
+    const size_t smem = (size_t)halo_layout<NW>(p.Wg).total * 4;
+    W2L_CUDA_CHECK(cudaFuncSetAttribute(asg_fac_grad_halo_kernel<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    asg_fac_grad_halo_kernel<NW><<<dim3(gA, B), 32 * p.Wg, smem, stream>>>(p);
     W2L_LAUNCH_CHECK("asg_fac_grad_halo_kernel");
   } else if (has_fac) {
-    const size_t smem = (size_t)fac_grad_layout(p.Lp, p.fac_grad_warps).total * 4;
+    const size_t smem = (size_t)fac_grad_layout<NW>(p.Lp, p.fac_grad_warps).total * 4;
     const dim3 grid(gA, B);
 #define W2L_LAUNCH_FAC_GRAD(PP)                                                                                          \
   do {                                                                                                                   \
     if (smem > 48 * 1024)                                                                                                \
-      W2L_CUDA_CHECK(cudaFuncSetAttribute(asg_fac_grad_kernel<PP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    asg_fac_grad_kernel<PP><<<grid, p.fac_grad_warps * 32, smem, stream>>>(p);                                           \
+      W2L_CUDA_CHECK(cudaFuncSetAttribute(asg_fac_grad_kernel<W2L_FAC_GRAD_P(PP), NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+    asg_fac_grad_kernel<W2L_FAC_GRAD_P(PP), NW><<<grid, p.fac_grad_warps * 32, smem, stream>>>(p);                     \
   } while (0)
     W2L_FOR_P(W2L_LAUNCH_FAC_GRAD)
     W2L_LAUNCH_CHECK("asg_fac_grad_kernel");
   }
   {
     const dim3 grid(gF, B);
-    asg_fcc_grad_kernel<<<grid, kFccGradWarps * 32, 0, stream>>>(p);
+    constexpr size_t smem = fcc_grad_smem<NW>();
+    if (smem > 48 * 1024)
+      W2L_CUDA_CHECK(cudaFuncSetAttribute(asg_fcc_grad_kernel<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    asg_fcc_grad_kernel<NW><<<grid, fcc_grad_warps<NW>() * 32, smem, stream>>>(p);
     W2L_LAUNCH_CHECK("asg_fcc_grad_kernel");
   }
   {
     const int n_parts = p.n_fcc_parts + p.n_fac_parts, n2 = (n_parts + kRedGroup - 1) / kRedGroup;
-    asg_parts_reduce_kernel<<<dim3((kW * kW + 255) / 256, n2), 256, 0, stream>>>(p.parts, n_parts, kRedGroup, p.parts2, 0);
+    asg_parts_reduce_kernel<NW><<<dim3((NW * NW + 255) / 256, n2), 256, 0, stream>>>(p.parts, n_parts, kRedGroup, p.parts2, 0);
     W2L_LAUNCH_CHECK("asg_parts_reduce_kernel");
-    asg_parts_reduce_kernel<<<dim3((kW * kW + 255) / 256, 1), 256, 0, stream>>>(p.parts2, n2, n2, p.d_trans, N);
+    asg_parts_reduce_kernel<NW><<<dim3((NW * NW + 255) / 256, 1), 256, 0, stream>>>(p.parts2, n2, n2, p.d_trans, N);
     W2L_LAUNCH_CHECK("asg_parts_reduce_kernel");
   }
   return W2L_OK;
+}
+
+}  // namespace
+}  // namespace w2l
+
+using namespace w2l;
+
+extern "C" size_t w2l_asg_workspace_size(int B, int T, int N, int L) { return asg_workspace_size<32>(B, T, N, L); }
+
+extern "C" int w2l_asg_forward_backward(void* stream, int terms, int B, int T, int N, int L, int scale_mode,
+                                        const float* emis, const int32_t* target, const float* trans,
+                                        const float* dloss, float* loss, float* d_emis, float* d_trans,
+                                        void* workspace, size_t workspace_bytes) {
+  return asg_forward_backward<32>("asg", stream, terms, B, T, N, L, scale_mode, emis, target, trans, dloss, loss, d_emis,
+                                  d_trans, workspace, workspace_bytes);
+}
+
+extern "C" size_t w2l_asg64_workspace_size(int B, int T, int N, int L) { return asg_workspace_size<64>(B, T, N, L); }
+
+extern "C" int w2l_asg64_forward_backward(void* stream, int terms, int B, int T, int N, int L, int scale_mode,
+                                          const float* emis, const int32_t* target, const float* trans,
+                                          const float* dloss, float* loss, float* d_emis, float* d_trans,
+                                          void* workspace, size_t workspace_bytes) {
+  return asg_forward_backward<64>("asg64", stream, terms, B, T, N, L, scale_mode, emis, target, trans, dloss, loss, d_emis,
+                                  d_trans, workspace, workspace_bytes);
 }

@@ -15,56 +15,81 @@
 namespace w2l {
 namespace {
 
-constexpr int kW = 32;
 __host__ __device__ inline size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
 
-// ---- FCC Viterbi: one warp per sample, lane i = state i ----------------------------------------
-// backpointers: uint8 [T][32] in shared memory when they fit, else in the global workspace.
+// ---- FCC Viterbi: one warp per sample, lane i = states i + 32 s (s < NW / 32) ------------------------------
+// backpointers: uint8 [T][NW] in shared memory when they fit, else in the global workspace.
+// NW = 32 serves w2l_fcc_viterbi (N <= 32), NW = 64 w2l_fcc_viterbi64 (N <= 64); every state takes its candidates j in
+// ascending order with the same add and strict compare, so both widths are bit-exact with the reference.
+template <int NW>
 __global__ void __launch_bounds__(32) fcc_viterbi_kernel(int T, int N, const float* __restrict__ emis,
                                                          const float* __restrict__ trans, int32_t* __restrict__ path,
                                                          uint8_t* bp_global, int bp_in_smem) {
+  constexpr int S = NW / 32;
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  float* vec = reinterpret_cast<float*>(smem_raw);             // [2][32]
-  int32_t* pstage = reinterpret_cast<int32_t*>(smem_raw + 256);  // [T] staged path (when bp in smem)
+  float* vec = reinterpret_cast<float*>(smem_raw);             // [2][NW]
+  int32_t* pstage = reinterpret_cast<int32_t*>(smem_raw + 8 * NW);  // [T] staged path (when bp in smem)
   const int b = blockIdx.x, lane = threadIdx.x;
-  uint8_t* bp = bp_in_smem ? reinterpret_cast<uint8_t*>(smem_raw + 256 + align16((size_t)T * 4))
-                           : bp_global + (size_t)b * T * kW;
+  uint8_t* bp = bp_in_smem ? reinterpret_cast<uint8_t*>(smem_raw + 8 * NW + align16((size_t)T * 4))
+                           : bp_global + (size_t)b * T * NW;
   const float* eb = emis + (size_t)b * T * N;
-  float tr[kW];
+  float tr[S][NW];
 #pragma unroll
-  for (int j = 0; j < kW; ++j) tr[j] = (lane < N && j < N) ? trans[lane * N + j] : kNegInf;
-  float alpha = lane < N ? eb[lane] : kNegInf;
+  for (int s = 0; s < S; ++s)
+#pragma unroll
+    for (int j = 0; j < NW; ++j) tr[s][j] = (lane + 32 * s < N && j < N) ? trans[(lane + 32 * s) * N + j] : kNegInf;
+  float alpha[S];
+#pragma unroll
+  for (int s = 0; s < S; ++s) alpha[s] = lane + 32 * s < N ? eb[lane + 32 * s] : kNegInf;
   int buf = 0;
   for (int t = 1; t < T; ++t) {
-    vec[buf * kW + lane] = alpha;
-    __syncwarp();
-    const float e = lane < N ? eb[(size_t)t * N + lane] : kNegInf;
-    float best = kNegInf;
-    int arg = 0;
-    const float4* v4 = reinterpret_cast<const float4*>(vec + buf * kW);
 #pragma unroll
-    for (int q = 0; q < kW / 4; ++q) {
+    for (int s = 0; s < S; ++s) vec[buf * NW + lane + 32 * s] = alpha[s];
+    __syncwarp();
+    float e[S], best[S];
+    int arg[S];
+#pragma unroll
+    for (int s = 0; s < S; ++s) {
+      e[s] = lane + 32 * s < N ? eb[(size_t)t * N + lane + 32 * s] : kNegInf;
+      best[s] = kNegInf;
+      arg[s] = 0;
+    }
+    const float4* v4 = reinterpret_cast<const float4*>(vec + buf * NW);
+#pragma unroll
+    for (int q = 0; q < NW / 4; ++q) {
       const float4 v = v4[q];
       const float vv[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
       for (int r = 0; r < 4; ++r) {
         const int j = 4 * q + r;
         if (j < N) {
-          const float val = __fadd_rn(vv[r], tr[j]);
-          if (val > best) {
-            best = val;
-            arg = j;
+#pragma unroll
+          for (int s = 0; s < S; ++s) {
+            const float val = __fadd_rn(vv[r], tr[s][j]);
+            if (val > best[s]) {
+              best[s] = val;
+              arg[s] = j;
+            }
           }
         }
       }
     }
-    alpha = __fadd_rn(best, e);
-    bp[(size_t)t * kW + lane] = (uint8_t)arg;
+#pragma unroll
+    for (int s = 0; s < S; ++s) {
+      alpha[s] = __fadd_rn(best[s], e[s]);
+      bp[(size_t)t * NW + lane + 32 * s] = (uint8_t)arg[s];
+    }
     buf ^= 1;
   }
-  // final state: first maximum over lanes
-  float bv = lane < N ? alpha : kNegInf;
+  // final state: first maximum over states (a lane's lower state first, then lanes)
+  float bv = lane < N ? alpha[0] : kNegInf;
   int bi = lane;
+#pragma unroll
+  for (int s = 1; s < S; ++s)
+    if (lane + 32 * s < N && alpha[s] > bv) {
+      bv = alpha[s];
+      bi = lane + 32 * s;
+    }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
@@ -81,7 +106,7 @@ __global__ void __launch_bounds__(32) fcc_viterbi_kernel(int T, int N, const flo
       int pos = bi;
       pstage[T - 1] = pos;
       for (int t = T - 1; t >= 1; --t) {
-        pos = bp[(size_t)t * kW + pos];
+        pos = bp[(size_t)t * NW + pos];
         pstage[t - 1] = pos;
       }
     }
@@ -93,7 +118,7 @@ __global__ void __launch_bounds__(32) fcc_viterbi_kernel(int T, int N, const flo
       int pos = bi;
       pb[T - 1] = pos;
       for (int t = T - 1; t >= 1; --t) {
-        pos = bp[(size_t)t * kW + pos];
+        pos = bp[(size_t)t * NW + pos];
         pb[t - 1] = pos;
       }
     }
@@ -237,27 +262,48 @@ __global__ void linseg_target_kernel(int B, int T, int L, const int32_t* __restr
 
 using namespace w2l;
 
-extern "C" size_t w2l_fcc_viterbi_workspace_size(int B, int T, int N) {
+namespace w2l {
+namespace {
+template <int NW>
+size_t fcc_viterbi_workspace_size(int B, int T, int N) {
   if (B <= 0 || T <= 0 || N <= 0) return 0;
-  return align_up((size_t)B * T * kW, 256);
+  return align_up((size_t)B * T * NW, 256);
 }
 
-extern "C" int w2l_fcc_viterbi(void* stream_, int B, int T, int N, const float* emis, const float* trans,
-                               int32_t* path, void* workspace, size_t workspace_bytes) {
+template <int NW>
+int fcc_viterbi(const char* name, void* stream_, int B, int T, int N, const float* emis, const float* trans, int32_t* path,
+                void* workspace, size_t workspace_bytes) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (B <= 0 || T <= 0 || N <= 0) return fail(W2L_ERR_INVALID_ARGUMENT, "fcc_viterbi: B, T, N must be positive");
-  if (!emis || !trans || !path) return fail(W2L_ERR_INVALID_ARGUMENT, "fcc_viterbi: null pointer");
-  if (N > kW) return fail(W2L_ERR_UNSUPPORTED, "fcc_viterbi: N > 32 tokens is not covered");
-  const size_t smem_fit = 256 + align16((size_t)T * 4) + (size_t)T * kW;
+  const std::string tag(name);
+  if (B <= 0 || T <= 0 || N <= 0) return fail(W2L_ERR_INVALID_ARGUMENT, tag + ": B, T, N must be positive");
+  if (!emis || !trans || !path) return fail(W2L_ERR_INVALID_ARGUMENT, tag + ": null pointer");
+  if (N > NW) return fail(W2L_ERR_UNSUPPORTED, tag + ": N > " + std::to_string(NW) + " tokens is not covered");
+  const size_t smem_fit = 8 * NW + align16((size_t)T * 4) + (size_t)T * NW;
   const int in_smem = smem_fit <= 200 * 1024;
-  size_t smem = in_smem ? smem_fit : 256 + 16;
-  if (!in_smem && (!workspace || workspace_bytes < w2l_fcc_viterbi_workspace_size(B, T, N)))
-    return fail(W2L_ERR_WORKSPACE, "fcc_viterbi: workspace too small");
+  size_t smem = in_smem ? smem_fit : 8 * NW + 16;
+  if (!in_smem && (!workspace || workspace_bytes < fcc_viterbi_workspace_size<NW>(B, T, N)))
+    return fail(W2L_ERR_WORKSPACE, tag + ": workspace too small");
   if (smem > 48 * 1024)
-    W2L_CUDA_CHECK(cudaFuncSetAttribute(fcc_viterbi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  fcc_viterbi_kernel<<<B, 32, smem, stream>>>(T, N, emis, trans, path, static_cast<uint8_t*>(workspace), in_smem);
+    W2L_CUDA_CHECK(cudaFuncSetAttribute(fcc_viterbi_kernel<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  fcc_viterbi_kernel<NW><<<B, 32, smem, stream>>>(T, N, emis, trans, path, static_cast<uint8_t*>(workspace), in_smem);
   W2L_LAUNCH_CHECK("fcc_viterbi_kernel");
   return W2L_OK;
+}
+}  // namespace
+}  // namespace w2l
+
+extern "C" size_t w2l_fcc_viterbi_workspace_size(int B, int T, int N) { return fcc_viterbi_workspace_size<32>(B, T, N); }
+
+extern "C" int w2l_fcc_viterbi(void* stream, int B, int T, int N, const float* emis, const float* trans, int32_t* path,
+                               void* workspace, size_t workspace_bytes) {
+  return fcc_viterbi<32>("fcc_viterbi", stream, B, T, N, emis, trans, path, workspace, workspace_bytes);
+}
+
+extern "C" size_t w2l_fcc_viterbi64_workspace_size(int B, int T, int N) { return fcc_viterbi_workspace_size<64>(B, T, N); }
+
+extern "C" int w2l_fcc_viterbi64(void* stream, int B, int T, int N, const float* emis, const float* trans, int32_t* path,
+                                 void* workspace, size_t workspace_bytes) {
+  return fcc_viterbi<64>("fcc_viterbi64", stream, B, T, N, emis, trans, path, workspace, workspace_bytes);
 }
 
 static size_t fac_vit_lp(int T, int L) {

@@ -328,6 +328,47 @@ __global__ void __launch_bounds__(256) glu_bwd_kernel(long long rows, int H, int
   }
 }
 
+// PReLU with one parameter (`PR`, fl::PReLU): y = (x >= 0 ? x : a x) * dropout(i), a read from device memory (no host
+// sync).  The Dropout that follows a PR is fused here and its mask regenerated in the backward pass: the standalone Dropout
+// backward reads "exactly zero = dropped" off its output, which is right after a ReLU but not after a PReLU (a kept x = 0,
+// or every x < 0 when a = 0, would be taken as dropped, and da would lose those terms).  The mask is dropout_scale's.
+__global__ void __launch_bounds__(256) prelu_fwd_kernel(long long n, const float* __restrict__ x, const float* __restrict__ a,
+                                                        float* __restrict__ y, float drop_p, unsigned long long seed) {
+  const float inv_keep = drop_p > 0.f ? 1.0f / (1.0f - drop_p) : 1.0f;
+  const float av = *a;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const float v = x[i];
+    float o = v >= 0.f ? v : av * v;
+    if (drop_p > 0.f) o *= dropout_scale(seed, (unsigned long long)i, drop_p, inv_keep);
+    y[i] = o;
+  }
+}
+// dx = m g (x >= 0 ? 1 : a);  da = sum_{x < 0} x m g: one partial per CTA (block_sum, fixed order), summed in CTA order by
+// prelu_da_finish_kernel — no atomics, the same bits every run
+constexpr int kPreluMaxCtas = 1024;
+__global__ void __launch_bounds__(256) prelu_bwd_kernel(long long n, const float* __restrict__ x, const float* __restrict__ dy,
+                                                        const float* __restrict__ a, float* __restrict__ dx, float* __restrict__ part,
+                                                        float drop_p, unsigned long long seed) {
+  __shared__ float red[33];
+  const float inv_keep = drop_p > 0.f ? 1.0f / (1.0f - drop_p) : 1.0f;
+  const float av = *a;
+  float s = 0.f;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const float v = x[i];
+    float d = dy[i];
+    if (drop_p > 0.f) d *= dropout_scale(seed, (unsigned long long)i, drop_p, inv_keep);
+    dx[i] = v >= 0.f ? d : av * d;
+    if (v < 0.f) s += v * d;
+  }
+  const float tot = block_sum(s, red);
+  if (threadIdx.x == 0) part[blockIdx.x] = tot;
+}
+__global__ void prelu_da_finish_kernel(int parts, const float* __restrict__ part, float* __restrict__ da) {
+  float t = 0.f;
+  for (int k = 0; k < parts; ++k) t += part[k];
+  *da = t;
+}
+
 int blocks_for_n(long long n) { return (int)std::min<long long>((n + 2047) / 2048, sm_count() * 8); }
 
 }  // namespace
@@ -424,5 +465,34 @@ extern "C" int w2l_glu_bwd(void* stream_, long long rows, int half, const float*
   const int vec = (half % 4 == 0) && !((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dx)) & 15);
   glu_bwd_kernel<<<blocks_for_n(rows * half / (vec ? 4 : 1)), 256, 0, stream>>>(rows, half, vec, x, dy, dx, dropout_p, seed);
   W2L_LAUNCH_CHECK("glu_bwd_kernel");
+  return W2L_OK;
+}
+extern "C" int w2l_prelu_fwd(void* stream_, long long n, const float* x, const float* a, float* y, float dropout_p,
+                             unsigned long long seed) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (n <= 0 || !x || !a || !y || dropout_p < 0.f || dropout_p >= 1.f) return fail(W2L_ERR_INVALID_ARGUMENT, "prelu_fwd: bad arguments");
+  prelu_fwd_kernel<<<blocks_for_n(n), 256, 0, stream>>>(n, x, a, y, dropout_p, seed);
+  W2L_LAUNCH_CHECK("prelu_fwd_kernel");
+  return W2L_OK;
+}
+extern "C" int w2l_prelu_bwd(void* stream_, long long n, const float* x, const float* dy, const float* a, float* dx, float* da,
+                             float dropout_p, unsigned long long seed) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (n <= 0 || !x || !dy || !a || !dx || !da || dropout_p < 0.f || dropout_p >= 1.f)
+    return fail(W2L_ERR_INVALID_ARGUMENT, "prelu_bwd: bad arguments");
+  // the CTA count depends on n only (not on the device), so the partials and their sum are the same on every H100
+  const int ctas = (int)std::min<long long>((n + 2047) / 2048, kPreluMaxCtas);
+  float* part = nullptr;
+  W2L_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&part), sizeof(float) * (size_t)ctas, stream));
+  prelu_bwd_kernel<<<ctas, 256, 0, stream>>>(n, x, dy, a, dx, part, dropout_p, seed);
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) {
+    count_launch();
+    trace_launch("prelu_bwd_kernel");
+    prelu_da_finish_kernel<<<1, 1, 0, stream>>>(ctas, part, da);
+  }
+  cudaFreeAsync(part, stream);
+  if (e != cudaSuccess) return fail(W2L_ERR_CUDA, std::string("launch prelu_bwd_kernel: ") + cudaGetErrorString(e));
+  W2L_LAUNCH_CHECK("prelu_da_finish_kernel");
   return W2L_OK;
 }

@@ -794,6 +794,31 @@ Variable GatedLinearUnit::forward(const Variable& in) {
   return out;
 }
 
+PReLU::PReLU(int numParams, double init) {
+  if (numParams != 1) throw std::invalid_argument("PReLU: only one parameter is covered (numParams = " + std::to_string(numParams) + ")");
+  af::array a = af::array::empty(af::dim4(1));
+  a.fill((float)init);
+  params_.push_back(Variable(a, true));
+}
+std::string PReLU::prettyString() const { return std::string("PReLU (1)") + (dropP_ > 0 ? " +Dropout" : ""); }
+Variable PReLU::forward(const Variable& in) {
+  const long long n = in.elements();
+  af::array y = af::array::empty(in.dims());
+  const float dp = (train_ && dropP_ > 0) ? dropP_ : 0.f;
+  const unsigned long long seed = nextSeed();
+  check(w2l_prelu_fwd(currentStream(), n, in.array().f32(), params_[0].array().f32(), y.f32(), dp, seed));
+  Variable out(y, {in, params_[0]}, [=](std::vector<Variable>& ins, const Variable& g) {
+    af::array dx = af::array::empty(ins[0].dims());
+    af::array da = af::array::empty(af::dim4(1));
+    check(w2l_prelu_bwd(currentStream(), n, ins[0].array().f32(), g.array().f32(), ins[1].array().f32(), dx.f32(), da.f32(), dp, seed));
+    ins[0].addGrad(Variable(dx, false), true);
+    ins[1].addGrad(Variable(da, false));
+  });
+  // element-wise: the next convolution must still know which frames are data (a W = 1 convolution leaves slack rows)
+  out.setValidFrames(in.validFrames());
+  return out;
+}
+
 WeightNorm::WeightNorm(std::shared_ptr<Module> module, int dim) : module_(std::move(module)), dim_(dim) {
   Variable v, b;
   bool hasBias = false;
@@ -1526,6 +1551,7 @@ std::shared_ptr<Sequential> buildSequentialModule(const std::string& archText, i
   std::shared_ptr<Conv2D> lastConv;           // `C2` conv: a following R / DO is fused into its epilogue
   std::shared_ptr<Conv2D> lastBigConv;        // `C` conv that a following GLU splits
   std::shared_ptr<GatedLinearUnit> lastGlu;   // GLU: a following DO is fused
+  std::shared_ptr<PReLU> lastPrelu;           // PR: a following DO is fused
   int pendingPadL = -1, pendingPadR = -1;     // `PD`: must be consumed by the very next line (a C2)
   int lineNo = 0;
   while (std::getline(in, line)) {
@@ -1546,9 +1572,11 @@ std::shared_ptr<Sequential> buildSequentialModule(const std::string& archText, i
     // candidates taken over by this line; everything else is dropped
     std::shared_ptr<Conv2D> conv0 = std::move(lastConv), big0 = std::move(lastBigConv);
     std::shared_ptr<GatedLinearUnit> glu0 = std::move(lastGlu);
+    std::shared_ptr<PReLU> prelu0 = std::move(lastPrelu);
     lastConv.reset();
     lastBigConv.reset();
     lastGlu.reset();
+    lastPrelu.reset();
     if (op == "V") {
       if (p.size() != 5) throw bad("V expects 4 dims");
       net->add(std::make_shared<View>(af::dim4(num(1), num(2), num(3), num(4))));
@@ -1620,10 +1648,20 @@ std::shared_ptr<Sequential> buildSequentialModule(const std::string& archText, i
       if (p.size() != 2) throw bad("DO expects a probability");
       if (glu0)
         glu0->fuseDropout((float)std::stod(p[1]));
+      else if (prelu0)
+        prelu0->fuseDropout((float)std::stod(p[1]));
       else if (conv0)
         conv0->fuseDropout(std::stof(p[1]));
       else
         net->add(std::make_shared<Dropout>(std::stod(p[1])));
+    } else if (op == "PR") {
+      // `PR [numParams] [init]` (cpc/SequentialBuilder.cpp:437-444)
+      if (p.size() > 3) throw bad("PR expects [numParams] [init]");
+      const int np = p.size() > 1 ? num(1) : 1;
+      if (np != 1) throw bad("PR with " + std::to_string(np) + " parameters is not covered (only numParams = 1)");
+      auto pr = std::make_shared<PReLU>(np, p.size() > 2 ? std::stod(p[2]) : 0.25);
+      net->add(pr);
+      lastPrelu = pr;
     } else if (op == "LN") {
       std::vector<int> axes;
       for (size_t i = 1; i < p.size(); ++i) axes.push_back(num(i));
@@ -1641,7 +1679,7 @@ std::shared_ptr<Sequential> buildSequentialModule(const std::string& archText, i
       if (p.size() != 7) throw bad("SAUG expects tWarpW fMaskF nFMask tMaskT tMaskP nTMask");
       net->add(std::make_shared<SpecAugment>(num(1), num(2), num(3), num(4), std::stod(p[5]), num(6)));
     } else {
-      throw bad("opcode '" + op + "' is outside the hot-path subset (V RO PD C C2 WN GLU R DO LN TDS L SAUG)");
+      throw bad("opcode '" + op + "' is outside the hot-path subset (V RO PD C C2 WN GLU R DO LN TDS L SAUG PR)");
     }
   }
   if (pendingPadL >= 0) throw std::invalid_argument("arch: trailing PD without a convolution");
@@ -1699,25 +1737,45 @@ AutoSegmentationCriterion::AutoSegmentationCriterion(int N, CriterionScaleMode s
 std::string AutoSegmentationCriterion::prettyString() const { return "AutoSegmentationCriterion"; }
 
 namespace {
+// ASG / LinSeg and their Viterbi take the 32-wide entry points for N <= 32 (so such models compute exactly what they
+// always did) and the 64-wide ones for 33 <= N <= 64 (the TIMIT phone set); both refuse N > 64.
+size_t asgWorkspaceSize(int B, int T, int N, int L) {
+  return N <= 32 ? w2l_asg_workspace_size(B, T, N, L) : w2l_asg64_workspace_size(B, T, N, L);
+}
+int asgCall(int terms, int B, int T, int N, int L, CriterionScaleMode mode, const float* emis, const int32_t* target,
+            const float* trans, const float* dloss, float* loss, float* dEmis, float* dTrans, af::array& ws) {
+  auto call = N <= 32 ? w2l_asg_forward_backward : w2l_asg64_forward_backward;
+  return call(currentStream(), terms, B, T, N, L, (int)mode, emis, target, trans, dloss, loss, dEmis, dTrans, ws.ptr(), ws.bytes());
+}
+af::array fccViterbiPath(const af::array& input, const Variable& trans) {
+  const int N = (int)input.dims(0), T = (int)input.dims(1), B = (int)input.dims(2);
+  af::array path = af::array::empty(af::dim4(T, B), DType::i32);
+  const size_t wsb = N <= 32 ? w2l_fcc_viterbi_workspace_size(B, T, N) : w2l_fcc_viterbi64_workspace_size(B, T, N);
+  af::array ws = af::array::empty(af::dim4((long long)std::max<size_t>(wsb, 256)), DType::u8);
+  auto call = N <= 32 ? w2l_fcc_viterbi : w2l_fcc_viterbi64;
+  check(call(currentStream(), B, T, N, input.f32(), trans.array().f32(), path.i32(), ws.ptr(), ws.bytes()));
+  return path;
+}
+
 // shared by ASG and LinSeg (ASG on the linearly stretched target)
 std::vector<Variable> asgForward(int terms, int N, CriterionScaleMode mode, bool train, Variable trans, af::array& wsCache,
                                  const Variable& emis, const af::array& target) {
   const int T = (int)emis.dims(1), B = (int)emis.dims(2), L = (int)target.dims(0);
   if (emis.dims(0) != N) throw std::invalid_argument("ASG: emissions have " + std::to_string(emis.dims(0)) + " classes, expected " + std::to_string(N));
-  const size_t wsb = w2l_asg_workspace_size(B, T, N, L);
+  const size_t wsb = asgWorkspaceSize(B, T, N, L);
   af::array ws = workspaceFor(wsCache, wsb);
   af::array loss = af::array::empty(af::dim4(B));
   const bool needGrad = train && (emis.isCalcGrad() || trans.isCalcGrad());
   if (!needGrad) {
-    check(w2l_asg_forward_backward(currentStream(), terms, B, T, N, L, (int)mode, emis.array().f32(), target.i32(), trans.array().f32(), nullptr,
-                                   loss.f32(), nullptr, nullptr, ws.ptr(), ws.bytes()));
+    check(asgCall(terms, B, T, N, L, mode, emis.array().f32(), target.i32(), trans.array().f32(), nullptr, loss.f32(), nullptr,
+                  nullptr, ws));
     return {Variable(loss, false)};
   }
   // fused forward+backward with dloss = 1 (what loss.backward() seeds, Train.cpp:1720)
   af::array dEmis = af::array::empty(emis.dims());
   af::array dTrans = af::array::empty(trans.dims());
-  check(w2l_asg_forward_backward(currentStream(), terms, B, T, N, L, (int)mode, emis.array().f32(), target.i32(), trans.array().f32(), nullptr,
-                                 loss.f32(), dEmis.f32(), dTrans.f32(), ws.ptr(), ws.bytes()));
+  check(asgCall(terms, B, T, N, L, mode, emis.array().f32(), target.i32(), trans.array().f32(), nullptr, loss.f32(), dEmis.f32(),
+                dTrans.f32(), ws));
   return {Variable(loss, {emis, trans}, [=](std::vector<Variable>& ins, const Variable& g) mutable {
     af::array de = dEmis, dt = dTrans;
     if (!g.isOnesSeed()) {  // arbitrary upstream gradient: re-run the fused call with it (rare path)
@@ -1725,8 +1783,8 @@ std::vector<Variable> asgForward(int terms, int N, CriterionScaleMode mode, bool
       af::array l2 = af::array::empty(af::dim4(B));
       de = af::array::empty(ins[0].dims());
       dt = af::array::empty(ins[1].dims());
-      check(w2l_asg_forward_backward(currentStream(), terms, B, T, N, L, (int)mode, ins[0].array().f32(), target.i32(), ins[1].array().f32(),
-                                     g.array().f32(), l2.f32(), de.f32(), dt.f32(), ws2.ptr(), ws2.bytes()));
+      check(asgCall(terms, B, T, N, L, mode, ins[0].array().f32(), target.i32(), ins[1].array().f32(), g.array().f32(), l2.f32(),
+                    de.f32(), dt.f32(), ws2));
     }
     ins[0].addGrad(Variable(de, false));
     ins[1].addGrad(Variable(dt, false));
@@ -1741,10 +1799,7 @@ std::vector<Variable> AutoSegmentationCriterion::forward(const std::vector<Varia
 af::array AutoSegmentationCriterion::viterbiPath(const af::array& input, const af::array&) {
   const int N = (int)input.dims(0), T = (int)input.dims(1), B = (int)input.dims(2);
   if (N != N_) throw std::invalid_argument("ASG viterbiPath: class count mismatch");
-  af::array path = af::array::empty(af::dim4(T, B), DType::i32);
-  af::array ws = af::array::empty(af::dim4((long long)std::max<size_t>(w2l_fcc_viterbi_workspace_size(B, T, N), 256)), DType::u8);
-  check(w2l_fcc_viterbi(currentStream(), B, T, N, input.f32(), params_[0].array().f32(), path.i32(), ws.ptr(), ws.bytes()));
-  return path;
+  return fccViterbiPath(input, params_[0]);
 }
 
 af::array SequenceCriterion::viterbiPathWithTarget(const af::array&, const af::array&, af::array*) {
@@ -1836,11 +1891,7 @@ std::vector<Variable> LinearSegmentationCriterion::forward(const std::vector<Var
   return asgForward(W2L_TERM_ASG, N_, scaleMode_, train_, params_[0], ws_, inputs[0], stretched);
 }
 af::array LinearSegmentationCriterion::viterbiPath(const af::array& input, const af::array&) {
-  const int N = (int)input.dims(0), T = (int)input.dims(1), B = (int)input.dims(2);
-  af::array path = af::array::empty(af::dim4(T, B), DType::i32);
-  af::array ws = af::array::empty(af::dim4((long long)std::max<size_t>(w2l_fcc_viterbi_workspace_size(B, T, N), 256)), DType::u8);
-  check(w2l_fcc_viterbi(currentStream(), B, T, N, input.f32(), params_[0].array().f32(), path.i32(), ws.ptr(), ws.bytes()));
-  return path;
+  return fccViterbiPath(input, params_[0]);
 }
 
 af::array LinearSegmentationCriterion::viterbiPathWithTarget(const af::array& input, const af::array& target, af::array* index) {
