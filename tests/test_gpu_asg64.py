@@ -1,62 +1,17 @@
 """The 64-wide ASG and FCC-Viterbi entry points (w2l_asg64_forward_backward, w2l_fcc_viterbi64) for
 1 <= N <= 64 against the CPU oracle, with the tolerances of test_gpu_criterion.py: loss and gradients
 <= 1e-4 relative, Viterbi paths bit-exact."""
+import functools
+
 import numpy as np
 import pytest
-import torch
 
 import oracle
+from test_gpu_criterion import TOL, check_asg, dev, make_asg, rel
 
 pytestmark = pytest.mark.gpu
 
-TOL = 1e-4
-
-
-def dev(a):
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
-def rel(a, b, floor=2e-3):
-    """max abs error over max abs reference; `floor` = scale of the cancelling components when the reference is ~0."""
-    a = np.asarray(a, np.float64)
-    b = np.asarray(b, np.float64)
-    return float(np.abs(a - b).max() / max(floor, np.abs(b).max()))
-
-
-def make_asg(B, T, N, L, seed, escale=3.0, ragged=True):
-    rng = np.random.default_rng(seed)
-    e = (rng.normal(0, 1, (B, T, N)) * escale).astype(np.float32)
-    tr = (4 * np.eye(N) + rng.normal(0, 0.1, (N, N))).astype(np.float32)
-    y = rng.integers(0, N, (B, L)).astype(np.int32)
-    if ragged and L > 1:
-        for b in range(B):
-            n = int(rng.integers(max(1, L // 2), L + 1))
-            y[b, n:] = -1
-    return e, tr, y
-
-
-def check_asg64(e, tr, y, mode="none", dloss=None, terms=None, tol=TOL):
-    import wav2letter_b200 as w
-
-    terms = w.TERM_ASG if terms is None else terms
-    if terms == w.TERM_FCC:
-        ol, ode, odt = oracle.fcc(e, tr, mode, target=y, dloss=dloss)
-    else:
-        fn = {w.TERM_ASG: oracle.asg, w.TERM_FAC: oracle.fac}[terms]
-        ol, ode, odt = fn(e, y, tr, mode, dloss=dloss)
-    gl, gde, gdt = w.asg64_forward_backward(dev(e), dev(y), dev(tr), mode, None if dloss is None else dev(dloss), terms)
-    torch.cuda.synchronize()
-    gl, gde, gdt = gl.cpu().numpy(), gde.cpu().numpy(), gdt.cpu().numpy()
-    lerr = np.abs(gl - ol) / np.maximum(1.0, np.abs(ol))
-    assert np.nanmax(lerr) <= tol, f"loss rel err {np.nanmax(lerr)}"
-    assert np.array_equal(np.isnan(gl), np.isnan(ol))
-    assert rel(gde, ode) <= tol, f"d_emis rel err {rel(gde, ode)}"
-    if e.shape[1] > 1:
-        floor = 1e-2 * e.shape[0] * e.shape[1]  # each of FCC / FAC contributes ~B*(T-1) mass
-        assert rel(gdt, odt, floor if e.shape[2] == 1 else 2e-3) <= tol, f"d_trans rel err {rel(gdt, odt)}"
-    fl, _, _ = w.asg64_forward_backward(dev(e), dev(y), dev(tr), mode, None, terms, need_grad=False)
-    np.testing.assert_allclose(fl.cpu().numpy(), ol, rtol=tol, atol=tol)
-    return gl, gde, gdt
+check_asg64 = functools.partial(check_asg, entry="asg64_forward_backward")
 
 
 @pytest.mark.parametrize("B,T,N,L,mode", [

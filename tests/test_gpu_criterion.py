@@ -40,16 +40,18 @@ def make_asg(B, T, N, L, seed, escale=3.0, ragged=True):
     return e, tr, y
 
 
-def check_asg(e, tr, y, mode="none", dloss=None, terms=None, tol=TOL):
+def check_asg(e, tr, y, mode="none", dloss=None, terms=None, tol=TOL, entry="asg_forward_backward"):
+    """`entry`: the wav2letter_b200 call under test (asg_forward_backward or asg64_forward_backward)."""
     import wav2letter_b200 as w
 
+    fb = getattr(w, entry)
     terms = w.TERM_ASG if terms is None else terms
     fn = {w.TERM_ASG: oracle.asg, w.TERM_FAC: oracle.fac}.get(terms)
     if terms == w.TERM_FCC:
         ol, ode, odt = oracle.fcc(e, tr, mode, target=y, dloss=dloss)
     else:
         ol, ode, odt = fn(e, y, tr, mode, dloss=dloss)
-    gl, gde, gdt = w.asg_forward_backward(dev(e), dev(y), dev(tr), mode, None if dloss is None else dev(dloss), terms)
+    gl, gde, gdt = fb(dev(e), dev(y), dev(tr), mode, None if dloss is None else dev(dloss), terms)
     torch.cuda.synchronize()
     gl, gde, gdt = gl.cpu().numpy(), gde.cpu().numpy(), gdt.cpu().numpy()
     lerr = np.abs(gl - ol) / np.maximum(1.0, np.abs(ol))
@@ -60,7 +62,7 @@ def check_asg(e, tr, y, mode="none", dloss=None, terms=None, tol=TOL):
         floor = 1e-2 * e.shape[0] * e.shape[1]  # each of FCC / FAC contributes ~B*(T-1) mass
         assert rel(gdt, odt, floor if e.shape[2] == 1 else 2e-3) <= tol, f"d_trans rel err {rel(gdt, odt)}"
     # forward-only entry gives the same loss
-    fl, _, _ = w.asg_forward_backward(dev(e), dev(y), dev(tr), mode, None, terms, need_grad=False)
+    fl, _, _ = fb(dev(e), dev(y), dev(tr), mode, None, terms, need_grad=False)
     np.testing.assert_allclose(fl.cpu().numpy(), ol, rtol=tol, atol=tol)
     return gl, gde, gdt
 

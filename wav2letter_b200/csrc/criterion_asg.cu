@@ -32,19 +32,20 @@
 //                          of the segment backwards from the checkpoint into shared memory, then
 //                          the alpha rows forwards, emitting per-frame normalised occupancies per
 //                          label (through the label-sorted index) and transition statistics.
-//                          Targets longer than 256: asg_fac_grad_halo_kernel, the row cut into
-//                          slices of 240 positions + halo lanes, one warp per slice.
+//                          Targets longer than 256 (P >= 16): asg_fac_grad_halo_kernel, the row cut
+//                          into slices of 240 positions + halo lanes, one warp per slice.  Both
+//                          kernels run the same segment walk (fac_grad_walk).
 //   4. asg_fcc_grad_kernel parallel over frames, from the stored FCC vectors:
 //                          d_emis = coef*(gamma_fcc - gamma_fac), d_trans partials.
 //   5. asg_parts_reduce_kernel (x2)  deterministic tree sum of the d_trans partials (no atomics).
 //
-// Two widths.  Every kernel is a template over the padded FCC state width NW (S = NW/32 states per lane, lane i owning
-// states i and i+32 when NW = 64).  w2l_asg_forward_backward instantiates NW = 32 (N <= 32, the published contract);
-// w2l_asg64_forward_backward instantiates NW = 64 (N <= 64: the 39 folded phones of TIMIT).  At NW = 64 the FCC chains
-// keep both M' rows of a lane in registers (128 floats) with a half-depth Z prefetch, and the FCC grad kernel runs 4 warps
-// of 8 frames with a 64 x 65 slab per warp in opt-in dynamic shared memory.  The FAC chains are unchanged but for the
-// width of the Z tile; the FAC grad kernels sum occupancies for two labels per lane.  The FAC chain lanes (and with them
-// the per-lane re-centring offsets ckCA / ckCB) stay 32 wide at both widths.
+// Two widths.  Every kernel is one template over the padded FCC state width NW (S = NW/32 states per lane, lane i owning
+// states i and i+32 when NW = 64), with no separate 32-wide copy.  w2l_asg_forward_backward instantiates NW = 32
+// (N <= 32, the published contract); w2l_asg64_forward_backward instantiates NW = 64 (N <= 64: the 39 folded phones of
+// TIMIT).  At NW = 64 the FCC chains keep both M' rows of a lane in registers (128 floats) with a half-depth Z prefetch,
+// and the FCC grad kernel runs 4 warps of 8 frames with a 64 x 65 slab per warp in opt-in dynamic shared memory.  The FAC
+// chains are unchanged but for the width of the Z tile; the FAC grad kernels sum occupancies for two labels per lane.
+// The FAC chain lanes (and with them the per-lane re-centring offsets ckCA / ckCB) stay 32 wide at both widths.
 #include <cuda_runtime.h>
 
 #include "common.cuh"
@@ -137,6 +138,45 @@ __device__ __forceinline__ float lse2_log2(float a, float b) {
 // ------------------------------------------------------------------------------------------
 // 1. prep
 // ------------------------------------------------------------------------------------------
+// Stable label-sorted index of the positions [lo, hi) (one warp): lane n lists the positions l with label(l) == n (and
+// n + 32) in ascending order, as l - shift, from order[start[n]] on; start[NW] = the number of positions listed.
+template <int NW, typename Label>
+__device__ __forceinline__ void label_index(Label label, int lo, int hi, int shift, int* start, int* order) {
+  constexpr int S = NW / 32;
+  const int lane = threadIdx.x & 31;
+  int cnt[S];
+#pragma unroll
+  for (int s = 0; s < S; ++s) cnt[s] = 0;
+  for (int l = lo; l < hi; ++l) {
+    const int v = label(l);
+#pragma unroll
+    for (int s = 0; s < S; ++s) cnt[s] += (v == lane + 32 * s);
+  }
+  int w0[S], below = 0;
+#pragma unroll
+  for (int s = 0; s < S; ++s) {
+    int pre = cnt[s];
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int v = __shfl_up_sync(0xffffffffu, pre, o);
+      if (lane >= o) pre += v;
+    }
+    w0[s] = below + pre - cnt[s];
+    start[lane + 32 * s] = w0[s];
+    if (s == S - 1) {
+      if (lane == 31) start[NW] = below + pre;
+    } else {
+      below += __shfl_sync(0xffffffffu, pre, 31);
+    }
+  }
+  for (int l = lo; l < hi; ++l) {
+    const int v = label(l);
+#pragma unroll
+    for (int s = 0; s < S; ++s)
+      if (v == lane + 32 * s) order[w0[s]++] = l - shift;
+  }
+}
+
 template <int NW>
 __global__ void __launch_bounds__(256) asg_prep_kernel(AsgParams p, int frame_blocks) {
   constexpr int S = NW / 32;
@@ -199,42 +239,8 @@ __global__ void __launch_bounds__(256) asg_prep_kernel(AsgParams p, int frame_bl
     p.scale[b] = sc;
     p.coef[b] = ok ? sc * (p.dloss ? p.dloss[b] : 1.0f) : 0.0f;
   }
-  // label-sorted index of the target positions (stable): lane n lists the positions with y_l == n (and n + 32)
-  if ((p.terms & W2L_TERM_FAC) && p.need_grad && ok) {
-    int cnt[S];
-#pragma unroll
-    for (int s = 0; s < S; ++s) cnt[s] = 0;
-    for (int l = 0; l < tsz; ++l) {
-      const int v = __ldg(y + l);
-#pragma unroll
-      for (int s = 0; s < S; ++s) cnt[s] += (v == lane + 32 * s);
-    }
-    int* st = p.start + (size_t)b * (NW + 4);
-    int* od = p.order + (size_t)b * p.Lp;
-    int w0[S], below = 0;
-#pragma unroll
-    for (int s = 0; s < S; ++s) {
-      int pre = cnt[s];
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const int v = __shfl_up_sync(0xffffffffu, pre, o);
-        if (lane >= o) pre += v;
-      }
-      w0[s] = below + pre - cnt[s];
-      st[lane + 32 * s] = w0[s];
-      if (s == S - 1) {
-        if (lane == 31) st[NW] = below + pre;
-      } else {
-        below += __shfl_sync(0xffffffffu, pre, 31);
-      }
-    }
-    for (int l = 0; l < tsz; ++l) {
-      const int v = __ldg(y + l);
-#pragma unroll
-      for (int s = 0; s < S; ++s)
-        if (v == lane + 32 * s) od[w0[s]++] = l;
-    }
-  }
+  if ((p.terms & W2L_TERM_FAC) && p.need_grad && ok)
+    label_index<NW>([&](int l) { return __ldg(y + l); }, 0, tsz, 0, p.start + (size_t)b * (NW + 4), p.order + (size_t)b * p.Lp);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -334,121 +340,6 @@ __device__ __forceinline__ float trans_max(const float* trans, int N, int lane) 
   float tmax = kNegInf;
   for (int k = lane; k < N * N; k += 32) tmax = fmaxf(tmax, __ldg(trans + k));
   return warp_max(tmax);
-}
-
-// The 32-wide FCC chains, one state per lane.  They are kept apart from the width template below (which computes the
-// same recursion at any NW) because the template, instantiated at NW = 32, orders a few register moves differently:
-// the NW = 32 kernels compile to exactly the instructions they always had.
-// alpha chain: a_t = (X_t * s_t) .* (M' a_{t-1})
-__device__ void fcc_alpha_chain32(const AsgParams& p, int b, float* vec /* [2][32] shared */) {
-  const int lane = threadIdx.x & 31;
-  const int T = p.T, N = p.N;
-  const float tmax = trans_max(p.trans, N, lane);
-  float M[kW];
-#pragma unroll
-  for (int j = 0; j < kW; ++j) M[j] = (lane < N && j < N) ? __expf(__ldg(p.trans + lane * N + j) - tmax) : 0.f;
-  const float* Zl = p.Z + (size_t)b * T * kW + lane;
-  float* Al = p.A + (size_t)b * T * kW + lane;
-  float* sAb = p.sA + (size_t)b * T;
-  const bool store = p.need_grad != 0;
-  const int nblk = (T + kBlk - 1) / kBlk;
-  float zn[kBlk];
-#pragma unroll
-  for (int k = 0; k < kBlk; ++k) zn[k] = k < T ? __ldg(Zl + (size_t)k * kW) : 0.f;
-  float a = 0.f, s = 1.0f;
-  int ksum = 0, kcur = 0;
-  float* Ap = Al;
-  float* sp = sAb;
-  for (int c = 0; c < nblk; ++c) {
-    float zc[kBlk];
-    const int tb = c * kBlk;
-#pragma unroll
-    for (int k = 0; k < kBlk; ++k) {
-      zc[k] = zn[k];
-      const int tn = tb + kBlk + k;
-      zn[k] = tn < T ? __ldg(Zl + (size_t)tn * kW) : 0.f;
-    }
-#pragma unroll
-    for (int k = 0; k < kBlk; ++k) {
-      const int t = tb + k;
-      if (t >= T) break;
-      const float x = ex2f(zc[k]);
-      if (t == 0) {
-        a = x;
-        if (store) {
-          Al[0] = a;
-          if (lane == 0) sAb[0] = 1.0f;
-        }
-        continue;
-      }
-      const float xs = x * s;
-      float* vb = vec + (k & 1) * kW;
-      vb[lane] = a;
-      const float mx = warp_max(a);  // max_j a_{t-1}[j]: five shuffles, off the dependent chain
-      __syncwarp();
-      a = xs * matvec32(M, vb);
-      ksum += kcur;
-      if (store) {
-        Ap += kW;  // (running pointers: frame t)
-        sp += 1;
-        *Ap = a;
-        if (lane == 0) *sp = s;
-      }
-      s = pow2_rescale<1>(mx, kcur);  // applied at t+1 from |a_{t-1}| (lag two): damped
-    }
-  }
-  const float tot = warp_sum(a);
-  if (lane == 0) p.fccLogZ[b] = (double)(T - 1) * (double)tmax + kLn2 * (double)ksum + log((double)tot);
-}
-
-// beta chain: b_t = M'^T (X_{t+1} .* b_{t+1} * s)
-__device__ void fcc_beta_chain32(const AsgParams& p, int b, float* vec) {
-  const int lane = threadIdx.x & 31;
-  const int T = p.T, N = p.N;
-  const float tmax = trans_max(p.trans, N, lane);
-  float M[kW];
-#pragma unroll
-  for (int i = 0; i < kW; ++i) M[i] = (lane < N && i < N) ? __expf(__ldg(p.trans + i * N + lane) - tmax) : 0.f;
-  const float* Zl = p.Z + (size_t)b * T * kW + lane;
-  float* Bl = p.Bh + (size_t)b * T * kW + lane;
-  float bh = lane < N ? 1.0f : 0.0f;  // b_{T-1}
-  Bl[(size_t)(T - 1) * kW] = bh;
-  if (T < 2) return;
-  // step t (T-2 .. 0) consumes X_{t+1}; block c covers t in [c*kBlk, c*kBlk + kBlk) and reads frames t+1
-  const int ctop = (T - 2) / kBlk;
-  float zn[kBlk];
-#pragma unroll
-  for (int k = 0; k < kBlk; ++k) {
-    const int f = ctop * kBlk + k + 1;
-    zn[k] = f < T ? __ldg(Zl + (size_t)f * kW) : 0.f;
-  }
-  float s = 1.0f;
-  int kdummy;
-  float* Bp = Bl + (size_t)(T - 1) * kW;
-  for (int c = ctop; c >= 0; --c) {
-    float zc[kBlk];
-    const int tb = c * kBlk;
-#pragma unroll
-    for (int k = 0; k < kBlk; ++k) {
-      zc[k] = zn[k];
-      const int f = tb - kBlk + k + 1;
-      zn[k] = f >= 1 ? __ldg(Zl + (size_t)f * kW) : 0.f;
-    }
-#pragma unroll
-    for (int k = kBlk - 1; k >= 0; --k) {
-      const int t = tb + k;
-      if (t > T - 2) continue;
-      const float u = bh * (ex2f(zc[k]) * s);
-      float* vb = vec + (k & 1) * kW;
-      vb[lane] = u;
-      const float mx = warp_max(u);
-      __syncwarp();
-      bh = matvec32(M, vb);
-      Bp -= kW;  // (running pointer: frame t)
-      *Bp = bh;
-      s = pow2_rescale<0>(mx, kdummy);
-    }
-  }
 }
 
 // alpha chain: a_t = (X_t * s_t) .* (M' a_{t-1}); lane i holds the states i + 32 s (rows i + 32 s of M')
@@ -922,9 +813,9 @@ __global__ void __launch_bounds__(32) asg_chains_kernel(AsgParams p) {
   else if (role == kRoleFacBeta)
     fac_chain<P, true, NW>(p, b, sm);
   else if (role == kRoleFccAlpha)
-    if constexpr (NW == 32) fcc_alpha_chain32(p, b, sm); else fcc_alpha_chain<NW>(p, b, sm);
+    fcc_alpha_chain<NW>(p, b, sm);
   else
-    if constexpr (NW == 32) fcc_beta_chain32(p, b, sm); else fcc_beta_chain<NW>(p, b, sm);
+    fcc_beta_chain<NW>(p, b, sm);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -959,9 +850,14 @@ __device__ __forceinline__ float label_sum(uint32_t row_sa, const float* row, co
   return s0 + s1;
 }
 
-// dynamic shared memory of the FAC grad kernel (4-byte words)
+// Shared memory of a warp in the FAC grad kernels (4-byte words): two Z tiles [2][kSeg][NW] (this segment's / the next
+// one's), the next segment's beta checkpoint row, the segment's beta rows [kSeg][stride] and the gamma row (+ a zero slot)
+template <int NW>
+__host__ __device__ constexpr int fac_seg_words(int stride) { return 2 * kSeg * NW + stride + kSeg * stride + stride + 4; }
+
+// dynamic shared memory of the single-warp FAC grad kernel (4-byte words)
 struct FacGradLayout {
-  int start, ztile, bnext, brow, grow, dsum, dtr, per_warp, total;
+  int start, ztile, dsum, dtr, per_warp, total;
 };
 template <int NW>
 __host__ __device__ inline FacGradLayout fac_grad_layout(int Lp, int warps) {
@@ -971,12 +867,45 @@ __host__ __device__ inline FacGradLayout fac_grad_layout(int Lp, int warps) {
   f.dsum = o;   o += 2 * Lp;
   f.dtr = o;    o += NW * (NW + 1);
   o = (o + 3) & ~3;
-  f.per_warp = 2 * kSeg * NW + Lp + kSeg * Lp + Lp + 4;  // two Z tiles, next beta row, beta rows, gamma row (+ a zero slot)
+  f.per_warp = fac_seg_words<NW>(Lp);
   f.ztile = o;
-  f.bnext = o + 2 * kSeg * NW;
-  f.brow = f.bnext + Lp;
-  f.grow = f.brow + kSeg * Lp;
   f.total = o + warps * f.per_warp;
+  return f;
+}
+
+// ---- long targets (Lp > 256): the halo path ---------------------------------------------------------------------
+// A warp cannot hold more than 8 positions per lane without spilling (and a 16- or 32-position lane serialises 200-400
+// instructions per step).  Within an 8-frame segment the recursion reaches only 8 positions sideways, so a row is cut into
+// W slices of 240 useful positions (lanes 1..30) plus one halo lane on either side: the W warps of a CTA take the W
+// slices of one segment with the 8-per-lane walk below and exchange nothing about the recursion — the 6 % of redundant
+// halo arithmetic buys it.  They meet once per frame (one CTA barrier) to add their per-label occupancy sums, so the
+// frame is normalised by its true total exactly as on the single-warp path.
+constexpr int kHaloUse = 240;
+constexpr int kHaloRow = 256;
+constexpr int kHaloMaxW = 5;  // 1024 positions
+struct HaloLayout {
+  int gsh, dtr, order, start, y, dsum, ztile, per_warp, total;
+};
+template <int NW>
+__host__ __device__ inline HaloLayout halo_layout(int warps) {
+  HaloLayout f;
+  int o = 0;
+  f.gsh = o;    o += 2 * kHaloMaxW * NW;  // [2 frame parities][W][NW] per-label partial sums
+  f.dtr = o;    o += NW * (NW + 1);
+  o = (o + 3) & ~3;
+  const int w0 = o;
+  f.order = 0;                        // offsets inside a warp's block
+  f.start = kHaloRow;
+  f.y = f.start + NW + 4;
+  f.dsum = f.y + kHaloRow + 16;
+  f.ztile = (f.dsum + 2 * kHaloRow + 3) & ~3;
+  f.per_warp = (f.ztile + fac_seg_words<NW>(kHaloRow) + 3) & ~3;
+  f.total = w0 + warps * f.per_warp;
+  f.order += w0;  // absolute offsets of warp 0's block
+  f.start += w0;
+  f.y += w0;
+  f.dsum += w0;
+  f.ztile += w0;
   return f;
 }
 
@@ -998,6 +927,214 @@ __device__ __forceinline__ float2 fac_grad_pair(float va, float na, float s1a, f
   return fadd2_rn(base, make_float2(lg2f(q.x), lg2f(q.y)));
 }
 
+// One warp's FAC gradient walk over the segments c0, c0 + cstride, ... of sample b.  Per segment it recomputes the beta
+// rows backwards from the checkpoint into shared memory, then walks alpha forwards, emitting per-frame normalised
+// occupancies per label (through the label-sorted index order / start) and adding the transition statistics of the
+// lane's positions to ds.
+//   ws               the warp's segment buffers (fac_seg_words), rows `stride` floats apart
+//   l0               the lane's first position (a row slice: positions outside [0, L) are dead)
+//   cl, cl_prev/next the FAC chain lane whose checkpoint offset this lane's positions carry, and the chain lanes of the
+//                    neighbouring lanes' positions (the value that crosses a lane edge is re-based by the difference;
+//                    lane 0 reads no cl_prev and lane 31 no cl_next: nothing crosses the warp's edges)
+//   useful           false switches the lane's posteriors off through the exponent (halo lanes)
+//   writes_g         this warp stores G
+// kSliced: the CTA's warps hold slices of one row and add a frame's per-label sums through gsh behind one CTA barrier per
+// frame; otherwise the warp holds the whole row and totals the frame within itself.
+template <int P, int NW, bool kSliced>
+__device__ __forceinline__ void fac_grad_walk(const AsgParams& p, int b, int c0, int cstride, float* ws, int stride, const int* order,
+                                              const int* start, int l0, int cl, int cl_prev, int cl_next, bool useful, bool writes_g,
+                                              float* gsh, float2 (&ds)[P]) {
+  constexpr int S = NW / 32;
+  const int lane = threadIdx.x & 31;
+  const int T = p.T, L = p.tsz[b];
+  float* ztile2 = ws;
+  float* bnext = ztile2 + 2 * kSeg * NW;
+  float* brow = bnext + stride;
+  float* grow = brow + kSeg * stride;
+  const uint32_t zt2 = (uint32_t)__cvta_generic_to_shared(ztile2);
+  const uint32_t bnext_sa = (uint32_t)__cvta_generic_to_shared(bnext);
+  const uint32_t grow_sa = (uint32_t)__cvta_generic_to_shared(grow);
+  const float tmax = trans_max(p.trans, p.N, lane);
+  const float* Zb = p.Z + (size_t)b * T * NW;
+  float* Gb = p.G + (size_t)b * T * NW;
+  const double logZ2 = p.facLogZ2[b];
+  FacState<P> st;  // s2 = the alpha walk's advance scores; the beta walk's live in s2b
+  float s2b[P];
+  fac_load_target<P>(st, p, b, L, lane, true, tmax, l0 - lane * P);
+#pragma unroll
+  for (int k = 0; k < P; ++k) s2b[k] = st.s2[k];
+  fac_load_target<P>(st, p, b, L, lane, false, tmax, l0 - lane * P);
+  FlushIndex fx[S];  // labels lane + 32 s
+#pragma unroll
+  for (int q = 0; q < S; ++q) fx[q].load(order, start, lane + 32 * q, stride);
+  if (lane == 0) grow[stride] = 0.f;
+  // asynchronous copies (no registers) of a segment's inputs: its Z rows and, unless it ends the utterance, the beta
+  // checkpoint row behind it — issued one segment ahead
+  auto prefetch = [&](int c, int buf) {
+    const int t0 = c * kSeg;
+#pragma unroll
+    for (int h = 0; h < 2 * S; ++h) {
+      const int chunk = lane + 32 * h;  // 16-byte chunk of the [kSeg][NW] tile
+      const int t = t0 + (chunk >> (NW == 32 ? 3 : 4));  // (NW / 4 chunks per frame)
+      if (t < T) cp_async16(zt2 + (buf * kSeg * NW) * 4 + chunk * 16, Zb + (size_t)t * NW + (chunk & (NW / 4 - 1)) * 4);
+    }
+    if (t0 + kSeg < T) {
+      const float* src = p.ckBa + ((size_t)b * p.nC + c) * p.Lp;
+      if constexpr (P >= 4) {
+#pragma unroll
+        for (int k = 0; k < P; k += 4) {
+          const int l = l0 + k;
+          if (l >= 0 && l < p.Lp)
+            cp_async16(bnext_sa + (lane * P + k) * 4, src + l);
+          else
+            *reinterpret_cast<float4*>(bnext + lane * P + k) = make_float4(kNeg, kNeg, kNeg, kNeg);
+        }
+      } else {  // (P < 4: the whole row in one warp, every position inside it)
+#pragma unroll
+        for (int k = 0; k < P; ++k) cp_async4(bnext_sa + (lane * P + k) * 4, src + l0 + k);
+      }
+    }
+    cp_async_commit();
+  };
+  int buf = 0;
+  if (c0 < p.nC) prefetch(c0, 0);
+  for (int c = c0; c < p.nC; c += cstride, buf ^= 1) {
+    const int t0 = c * kSeg, t1 = min(T, t0 + kSeg);
+    const uint32_t zt = zt2 + (buf * kSeg * NW) * 4;
+    const float* ztile = ztile2 + buf * kSeg * NW;
+    cp_async_wait_all();
+    __syncwarp();
+    // ---- backwards: beta-tilde rows of frames t1-1 .. t0 into shared memory --------------------
+    // (checkpoint rows come with one offset per chain lane; DA / DB re-base the value that crosses a lane boundary.  A
+    // row slice is exact on its useful lanes: the right halo absorbs the edge)
+    double CB = 0.0;
+    float DB = 0.f, DA = 0.f;
+    int tstart;
+    if (t1 >= T) {
+#pragma unroll
+      for (int k = 0; k < P; ++k) st.v[k] = (l0 + k == L - 1) ? ztile[(T - 1 - t0) * NW + (st.y4[k] >> 2)] : kNeg;
+      fac_store_row<P>(st, brow + (size_t)(T - 1 - t0) * stride, lane);
+      tstart = T - 2;
+    } else {
+      fac_load_row<P>(st, bnext, lane);
+      const double* cb = p.ckCB + ((size_t)b * p.nC + c) * kW;
+      CB = cb[cl];
+      DB = lane < 31 ? (float)(cb[cl_next] - CB) : 0.f;
+      tstart = t1 - 1;
+    }
+    __syncwarp();
+    if (c + cstride < p.nC) prefetch(c + cstride, buf ^ 1);
+    // this segment's alpha checkpoint: requested now, used after the backward pass
+    float arow[P];
+    double CA = 0.0;
+    if (t0 > 0) {
+      const float* src = p.ckAa + ((size_t)b * p.nC + c) * p.Lp;
+      if constexpr (P >= 4) {
+#pragma unroll
+        for (int k = 0; k < P; k += 4) {
+          const int l = l0 + k;
+          float4 q = make_float4(kNeg, kNeg, kNeg, kNeg);
+          if (l >= 0 && l < p.Lp) q = __ldg(reinterpret_cast<const float4*>(src + l));
+          arow[k] = q.x;
+          arow[k + 1] = q.y;
+          arow[k + 2] = q.z;
+          arow[k + 3] = q.w;
+        }
+      } else {
+#pragma unroll
+        for (int k = 0; k < P; ++k) arow[k] = __ldg(src + l0 + k);
+      }
+      const double* ca = p.ckCA + ((size_t)b * p.nC + c) * kW;
+      CA = ca[cl];
+      DA = lane > 0 ? (float)(ca[cl_prev] - CA) : 0.f;
+    }
+    for (int t = tstart; t >= t0; --t) {
+      fac_beta_step<P>(st, s2b, zt + (t - t0) * (4 * NW), lane, DB);
+      fac_store_row<P>(st, brow + (size_t)(t - t0) * stride, lane);
+    }
+    // ---- forwards: alpha-tilde, occupancies, transition statistics (a row slice: the left halo absorbs the edge) ----
+    int tfirst = t0;
+    if (t0 == 0) {
+#pragma unroll
+      for (int k = 0; k < P; ++k) st.v[k] = (l0 + k == 0) ? ztile[st.y4[k] >> 2] : kNeg;
+      if (writes_g) {  // frame 0 sits at position 0 with probability one
+        const int y0 = p.target[(size_t)b * p.L];
+#pragma unroll
+        for (int q = 0; q < S; ++q) Gb[lane + 32 * q] = (lane + 32 * q == y0) ? 1.0f : 0.0f;
+      }
+      tfirst = 1;
+    } else {
+#pragma unroll
+      for (int k = 0; k < P; ++k) st.v[k] = arow[k];
+    }
+    // alpha_{t-1}[l] + s + beta_t[l] - log2 Z  =  tilde values + (CA + CB - facLogZ2): the t * tmax terms cancel
+    // (+ kLgShift: the transition scores in s1 / s2 carry the folded -log2(1.25))
+    const float K = useful ? (float)(CA + CB - logZ2) + kLgShift : kNeg;
+    const float2 K2 = make_float2(K, K);
+    __syncwarp();
+    for (int t = tfirst; t < t1; ++t) {
+      const uint32_t zrow = zt + (t - t0) * (4 * NW);
+      const float* br = brow + (size_t)(t - t0) * stride + lane * P;
+      float up = __shfl_up_sync(0xffffffffu, st.v[P - 1], 1) + DA;
+      if (lane == 0) up = kNeg;
+      float2 xv[P];  // (stay, advance) posteriors of the owned positions, unnormalised
+      if constexpr (P == 1) {
+        const float a0 = st.v[0] + st.s1[0], a1 = up + st.s2[0];
+        const float o = br[0] + K;
+        xv[0] = make_float2(ex2f(a0 + o), ex2f(a1 + o));
+        grow[lane] = xv[0].x + xv[0].y;
+        st.v[0] = lds_f(zrow + st.y4[0]) + lse2_log2(a0, a1);
+      } else {
+#pragma unroll
+        for (int k = P - 2; k >= 0; k -= 2) {  // pairs, descending: v[k-1], v[k] are still alpha_{t-1}
+          const float2 brk = fadd2_rn(*reinterpret_cast<const float2*>(br + k), K2);
+          const float2 nv = fac_grad_pair(st.v[k], k ? st.v[k - 1] : up, st.s1[k], st.s2[k], lds_f(zrow + st.y4[k]), brk.x,  //
+                                          st.v[k + 1], st.v[k], st.s1[k + 1], st.s2[k + 1], lds_f(zrow + st.y4[k + 1]), brk.y, xv[k], xv[k + 1]);
+          *reinterpret_cast<float2*>(grow + lane * P + k) = make_float2(xv[k].x + xv[k].y, xv[k + 1].x + xv[k + 1].y);
+          st.v[k] = nv.x;
+          st.v[k + 1] = nv.y;
+        }
+      }
+      __syncwarp();
+      // occupancy per label = sum over its positions / frame total (true division): a frame's occupancies add up
+      // to one exactly as the FCC posteriors do (N = 1: 1 - 1 = 0), and the same total normalises the statistics
+      float gl[S];
+      if constexpr (kSliced) {
+        // this slice's per-label sums meet the other slices' (one CTA barrier per frame, buffers alternate by parity)
+        const int w = threadIdx.x >> 5, W = blockDim.x >> 5;
+        float* gbuf = gsh + (t & 1) * (kHaloMaxW * NW);
+#pragma unroll
+        for (int q = 0; q < S; ++q) gbuf[w * NW + lane + 32 * q] = label_sum(grow_sa, grow, order, fx[q]);
+        __syncthreads();
+#pragma unroll
+        for (int q = 0; q < S; ++q) {
+          gl[q] = 0.f;
+          for (int ww = 0; ww < W; ++ww) gl[q] += gbuf[ww * NW + lane + 32 * q];
+        }
+      } else {
+#pragma unroll
+        for (int q = 0; q < S; ++q) gl[q] = label_sum(grow_sa, grow, order, fx[q]);
+      }
+      float gs = gl[0];
+#pragma unroll
+      for (int q = 1; q < S; ++q) gs += gl[q];
+      const float gt = warp_sum(gs);
+      if (writes_g) {
+#pragma unroll
+        for (int q = 0; q < S; ++q) Gb[(size_t)t * NW + lane + 32 * q] = gt > 0.f ? gl[q] / gt : 0.f;
+      }
+      const float inv = gt > 0.f ? __fdividef(1.0f, gt) : 0.f;
+      const float2 inv2 = make_float2(inv, inv);
+#pragma unroll
+      for (int k = 0; k < P; ++k) ds[k] = ffma2_rn(xv[k], inv2, ds[k]);
+      __syncwarp();
+    }
+  }
+  cp_async_wait_all();
+}
+
+// Rows that fit one warp (P <= 8): one warp per kSeg-frame segment, the segments dealt round-robin to the warps of the
+// sample's CTAs.
 // (NW = 64: the second label's flush index costs 16 registers, so P = 8 runs at 2 CTAs per SM instead of spilling)
 template <int P, int NW>
 __global__ void __launch_bounds__(128, P <= 8 * 32 / NW ? 4 : 2) asg_fac_grad_kernel(AsgParams p) {
@@ -1005,14 +1142,13 @@ __global__ void __launch_bounds__(128, P <= 8 * 32 / NW ? 4 : 2) asg_fac_grad_ke
   extern __shared__ __align__(16) float smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
   const int b = blockIdx.y;
-  const int T = p.T, Lp = p.Lp;
+  const int Lp = p.Lp;
   const FacGradLayout lay = fac_grad_layout<NW>(Lp, nw);
   float* part = p.parts + ((size_t)p.n_fcc_parts + (size_t)b * gridDim.x + blockIdx.x) * (NW * NW);
   if (!p.valid[b]) {
     for (int k = threadIdx.x; k < NW * NW; k += blockDim.x) part[k] = 0.f;
     return;  // the FCC grad kernel writes the zero gradient rows
   }
-  const int L = p.tsz[b];
   // the label-sorted index and the target stay in global memory (read once per CTA into registers / by the epilogue):
   // at 55.6 KB per CTA four CTAs fit an SM
   const int* order_s = p.order + (size_t)b * Lp;
@@ -1031,168 +1167,8 @@ __global__ void __launch_bounds__(128, P <= 8 * 32 / NW ? 4 : 2) asg_fac_grad_ke
   float2 ds[P];  // (stay, advance) transition statistics of the owned positions
 #pragma unroll
   for (int k = 0; k < P; ++k) ds[k] = make_float2(0.f, 0.f);
-  {
-    float* ztile2 = smem + lay.ztile + warp * lay.per_warp;  // [2][kSeg][32]: this segment's Z rows / the next one's
-    float* bnext = smem + lay.bnext + warp * lay.per_warp;   // the next segment's beta checkpoint row
-    float* brow = smem + lay.brow + warp * lay.per_warp;
-    float* grow = smem + lay.grow + warp * lay.per_warp;
-    const uint32_t zt2 = (uint32_t)__cvta_generic_to_shared(ztile2);
-    const uint32_t bnext_sa = (uint32_t)__cvta_generic_to_shared(bnext);
-    const uint32_t grow_sa = (uint32_t)__cvta_generic_to_shared(grow);
-    const float tmax = trans_max(p.trans, p.N, lane);
-    const float* Zb = p.Z + (size_t)b * T * NW;
-    float* Gb = p.G + (size_t)b * T * NW;
-    const double logZ2 = p.facLogZ2[b];
-    FacState<P> st;  // s2 = the alpha walk's advance scores; the beta walk's live in s2b
-    float s2b[P];
-    fac_load_target<P>(st, p, b, L, lane, true, tmax);
-#pragma unroll
-    for (int k = 0; k < P; ++k) s2b[k] = st.s2[k];
-    fac_load_target<P>(st, p, b, L, lane, false, tmax);
-    FlushIndex fx[S];  // labels lane + 32 s
-#pragma unroll
-    for (int q = 0; q < S; ++q) fx[q].load(order_s, start_s, lane + 32 * q, Lp);
-    if (lane == 0) grow[Lp] = 0.f;
-    // asynchronous copies (no registers) of a segment's inputs: its Z rows and, unless it ends the utterance, the beta
-    // checkpoint row behind it — issued one segment ahead
-    auto prefetch = [&](int c, int buf) {
-      const int t0 = c * kSeg;
-#pragma unroll
-      for (int h = 0; h < 2 * S; ++h) {
-        const int chunk = lane + 32 * h;  // 16-byte chunk of the [kSeg][NW] tile
-        const int t = t0 + (chunk >> (NW == 32 ? 3 : 4));  // (NW / 4 chunks per frame)
-        if (t < T) cp_async16(zt2 + (buf * kSeg * NW) * 4 + chunk * 16, Zb + (size_t)t * NW + (chunk & (NW / 4 - 1)) * 4);
-      }
-      if (t0 + kSeg < T) {
-        const float* src = p.ckBa + ((size_t)b * p.nC + c) * Lp + lane * P;
-        if constexpr (P >= 4) {
-#pragma unroll
-          for (int k = 0; k < P; k += 4) cp_async16(bnext_sa + (lane * P + k) * 4, src + k);
-        } else {
-#pragma unroll
-          for (int k = 0; k < P; ++k) cp_async4(bnext_sa + (lane * P + k) * 4, src + k);
-        }
-      }
-      cp_async_commit();
-    };
-    // segments are dealt round-robin to the warps of the sample's CTAs
-    const int cstride = gridDim.x * nw;
-    int c = blockIdx.x * nw + warp, buf = 0;
-    if (c < p.nC) prefetch(c, 0);
-    for (; c < p.nC; c += cstride, buf ^= 1) {
-      const int t0 = c * kSeg, t1 = min(T, t0 + kSeg);
-      const uint32_t zt = zt2 + (buf * kSeg * NW) * 4;
-      const float* ztile = ztile2 + buf * kSeg * NW;
-      cp_async_wait_all();
-      __syncwarp();
-      // ---- backwards: beta-tilde rows of frames t1-1 .. t0 into shared memory --------------------
-      // (checkpoint rows come with one offset per lane; DA / DB re-base the value that crosses a lane boundary)
-      double CB = 0.0;
-      float DB = 0.f, DA = 0.f;
-      int tstart;
-      if (t1 >= T) {
-#pragma unroll
-        for (int k = 0; k < P; ++k) st.v[k] = (lane * P + k == L - 1) ? ztile[(T - 1 - t0) * NW + (st.y4[k] >> 2)] : kNeg;
-        fac_store_row<P>(st, brow + (size_t)(T - 1 - t0) * Lp, lane);
-        tstart = T - 2;
-      } else {
-        fac_load_row<P>(st, bnext, lane);
-        const double* cb = p.ckCB + ((size_t)b * p.nC + c) * kW;
-        CB = cb[lane];
-        DB = lane < 31 ? (float)(cb[lane + 1] - CB) : 0.f;
-        tstart = t1 - 1;
-      }
-      __syncwarp();
-      if (c + cstride < p.nC) prefetch(c + cstride, buf ^ 1);
-      // this segment's alpha checkpoint: requested now, used after the backward pass
-      float arow[P];
-      double CA = 0.0;
-      if (t0 > 0) {
-        const float* src = p.ckAa + ((size_t)b * p.nC + c) * Lp + lane * P;
-        if constexpr (P >= 4) {
-#pragma unroll
-          for (int k = 0; k < P; k += 4) {
-            const float4 q = __ldg(reinterpret_cast<const float4*>(src + k));
-            arow[k] = q.x;
-            arow[k + 1] = q.y;
-            arow[k + 2] = q.z;
-            arow[k + 3] = q.w;
-          }
-        } else {
-#pragma unroll
-          for (int k = 0; k < P; ++k) arow[k] = __ldg(src + k);
-        }
-        const double* ca = p.ckCA + ((size_t)b * p.nC + c) * kW;
-        CA = ca[lane];
-        DA = lane > 0 ? (float)(ca[lane - 1] - CA) : 0.f;
-      }
-      for (int t = tstart; t >= t0; --t) {
-        fac_beta_step<P>(st, s2b, zt + (t - t0) * (4 * NW), lane, DB);
-        fac_store_row<P>(st, brow + (size_t)(t - t0) * Lp, lane);
-      }
-      // ---- forwards: alpha-tilde, occupancies, transition statistics -----------------------------
-      int tfirst = t0;
-      if (t0 == 0) {
-#pragma unroll
-        for (int k = 0; k < P; ++k) st.v[k] = kNeg;
-        if (lane == 0) st.v[0] = ztile[st.y4[0] >> 2];
-#pragma unroll
-        for (int q = 0; q < S; ++q)  // frame 0 sits at position 0 with probability one
-          Gb[lane + 32 * q] = (lane + 32 * q == y_s[0]) ? 1.0f : 0.0f;
-        tfirst = 1;
-      } else {
-#pragma unroll
-        for (int k = 0; k < P; ++k) st.v[k] = arow[k];
-      }
-      // alpha_{t-1}[l] + s + beta_t[l] - log2 Z  =  tilde values + (CA + CB - facLogZ2): the t * tmax terms cancel
-      // (+ kLgShift: the transition scores in s1 / s2 carry the folded -log2(1.25))
-      const float K = (float)(CA + CB - logZ2) + kLgShift;
-      const float2 K2 = make_float2(K, K);
-      __syncwarp();
-      for (int t = tfirst; t < t1; ++t) {
-        const uint32_t zrow = zt + (t - t0) * (4 * NW);
-        const float* br = brow + (size_t)(t - t0) * Lp + lane * P;
-        float up = __shfl_up_sync(0xffffffffu, st.v[P - 1], 1) + DA;
-        if (lane == 0) up = kNeg;
-        float2 xv[P];  // (stay, advance) posteriors of the owned positions, unnormalised
-        if constexpr (P == 1) {
-          const float a0 = st.v[0] + st.s1[0], a1 = up + st.s2[0];
-          const float o = br[0] + K;
-          xv[0] = make_float2(ex2f(a0 + o), ex2f(a1 + o));
-          grow[lane] = xv[0].x + xv[0].y;
-          st.v[0] = lds_f(zrow + st.y4[0]) + lse2_log2(a0, a1);
-        } else {
-#pragma unroll
-          for (int k = P - 2; k >= 0; k -= 2) {  // pairs, descending: v[k-1], v[k] are still alpha_{t-1}
-            const float2 brk = fadd2_rn(*reinterpret_cast<const float2*>(br + k), K2);
-            const float2 nv = fac_grad_pair(st.v[k], k ? st.v[k - 1] : up, st.s1[k], st.s2[k], lds_f(zrow + st.y4[k]), brk.x,  //
-                                            st.v[k + 1], st.v[k], st.s1[k + 1], st.s2[k + 1], lds_f(zrow + st.y4[k + 1]), brk.y, xv[k], xv[k + 1]);
-            *reinterpret_cast<float2*>(grow + lane * P + k) = make_float2(xv[k].x + xv[k].y, xv[k + 1].x + xv[k + 1].y);
-            st.v[k] = nv.x;
-            st.v[k + 1] = nv.y;
-          }
-        }
-        __syncwarp();
-        // occupancy per label = sum over its positions / frame total (true division): a frame's occupancies add up
-        // to one exactly as the FCC posteriors do (N = 1: 1 - 1 = 0), and the same total normalises the statistics
-        float gl[S];
-#pragma unroll
-        for (int q = 0; q < S; ++q) gl[q] = label_sum(grow_sa, grow, order_s, fx[q]);
-        float gs = gl[0];
-#pragma unroll
-        for (int q = 1; q < S; ++q) gs += gl[q];
-        const float gt = warp_sum(gs);
-#pragma unroll
-        for (int q = 0; q < S; ++q) Gb[(size_t)t * NW + lane + 32 * q] = gt > 0.f ? gl[q] / gt : 0.f;
-        const float inv = gt > 0.f ? __fdividef(1.0f, gt) : 0.f;
-        const float2 inv2 = make_float2(inv, inv);
-#pragma unroll
-        for (int k = 0; k < P; ++k) ds[k] = ffma2_rn(xv[k], inv2, ds[k]);
-        __syncwarp();
-      }
-    }
-    cp_async_wait_all();
-  }
+  fac_grad_walk<P, NW, false>(p, b, blockIdx.x * nw + warp, gridDim.x * nw, smem + lay.ztile + warp * lay.per_warp, Lp, order_s,
+                              start_s, lane * P, lane, lane - 1, lane + 1, true, true, nullptr, ds);
   // ---- CTA partial of the transition gradient (fixed order: deterministic) ----------------------
   for (int w = 0; w < nw; ++w) {
     if (warp == w) {
@@ -1222,55 +1198,13 @@ __global__ void __launch_bounds__(128, P <= 8 * 32 / NW ? 4 : 2) asg_fac_grad_ke
   for (int k = threadIdx.x; k < NW * NW; k += blockDim.x) part[k] = cf * dtr_s[(k / NW) * (NW + 1) + (k % NW)];
 }
 
-// ---- long targets (Lp > 256): the halo path ---------------------------------------------------------------------
-// A warp cannot hold more than 8 positions per lane without spilling (and a 16- or 32-position lane serialises 200-400
-// instructions per step).  Within an 8-frame segment the recursion reaches only 8 positions sideways, so a row is cut into
-// W slices of 240 useful positions (lanes 1..30) plus one halo lane on either side: the W warps of a CTA take the W
-// slices of one segment with the 8-per-lane code above and exchange nothing about the recursion — the 6 % of redundant
-// halo arithmetic buys it.  They meet once per frame (one CTA barrier) to add their per-label occupancy sums, so the
-// frame is normalised by its true total exactly as on the single-warp path.
-constexpr int kHaloUse = 240;
-constexpr int kHaloRow = 256;
-constexpr int kHaloMaxW = 5;  // 1024 positions
-struct HaloLayout {
-  int gsh, dtr, order, start, y, dsum, ztile, bnext, brow, grow, per_warp, total;
-};
-template <int NW>
-__host__ __device__ inline HaloLayout halo_layout(int warps) {
-  HaloLayout f;
-  int o = 0;
-  f.gsh = o;    o += 2 * kHaloMaxW * NW;  // [2 frame parities][W][NW] per-label partial sums
-  f.dtr = o;    o += NW * (NW + 1);
-  o = (o + 3) & ~3;
-  const int w0 = o;
-  f.order = 0;                        // offsets inside a warp's block
-  f.start = kHaloRow;
-  f.y = f.start + NW + 4;
-  f.dsum = f.y + kHaloRow + 16;
-  f.ztile = (f.dsum + 2 * kHaloRow + 3) & ~3;
-  f.bnext = f.ztile + 2 * kSeg * NW;
-  f.brow = f.bnext + kHaloRow;
-  f.grow = f.brow + kSeg * kHaloRow;
-  f.per_warp = (f.grow + kHaloRow + 4 + 3) & ~3;
-  f.total = w0 + warps * f.per_warp;
-  f.order += w0;  // absolute offsets of warp 0's block
-  f.start += w0;
-  f.y += w0;
-  f.dsum += w0;
-  f.ztile += w0;
-  f.bnext += w0;
-  f.brow += w0;
-  f.grow += w0;
-  return f;
-}
-
+// Longer rows: one warp per slice, every warp of the CTA on the same segment (the barrier per frame pairs them up).
 template <int NW>
 __global__ void __launch_bounds__(32 * kHaloMaxW) asg_fac_grad_halo_kernel(AsgParams p) {
   constexpr int P = 8, S = NW / 32;
   extern __shared__ __align__(16) float smem[];
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31, W = blockDim.x >> 5;  // warp = slice
   const int b = blockIdx.y;
-  const int T = p.T;
   const HaloLayout lay = halo_layout<NW>(W);
   float* part = p.parts + ((size_t)p.n_fcc_parts + (size_t)b * gridDim.x + blockIdx.x) * (NW * NW);
   if (!p.valid[b]) {
@@ -1280,7 +1214,6 @@ __global__ void __launch_bounds__(32 * kHaloMaxW) asg_fac_grad_halo_kernel(AsgPa
   const int L = p.tsz[b];
   const int base = kHaloUse * w - P;                              // position of lane 0, k = 0 (the left halo lane)
   const int lo_use = kHaloUse * w, hi_use = min(L, lo_use + kHaloUse);  // the useful positions of this slice
-  float* gsh = smem + lay.gsh;
   float* dtr_s = smem + lay.dtr;
   const int wo = w * lay.per_warp;
   int* order_s = reinterpret_cast<int*>(smem + lay.order + wo);  // useful positions (slice-local index l - base), sorted by label
@@ -1294,218 +1227,17 @@ __global__ void __launch_bounds__(32 * kHaloMaxW) asg_fac_grad_halo_kernel(AsgPa
     y_s[i] = (l >= 0 && l < L) ? __ldg(yg + l) : 0;
   }
   __syncwarp();
-  // label-sorted index of the slice's useful positions (stable).  The 32-wide form is kept as written before the width
-  // became a parameter: the general form compiles the NW = 32 kernel to a different (equivalent) instruction order.
-  if constexpr (NW == 32) {
-    int cnt = 0;
-    for (int l = lo_use; l < hi_use; ++l) cnt += (y_s[l - base] == lane);
-    int pre = cnt;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int v = __shfl_up_sync(0xffffffffu, pre, o);
-      if (lane >= o) pre += v;
-    }
-    int w0 = pre - cnt;
-    start_s[lane] = w0;
-    if (lane == 31) start_s[NW] = pre;
-    for (int l = lo_use; l < hi_use; ++l)
-      if (y_s[l - base] == lane) order_s[w0++] = l - base;
-  } else {  // lane n lists labels n and n + 32
-    int cnt[S];
-#pragma unroll
-    for (int q = 0; q < S; ++q) cnt[q] = 0;
-    for (int l = lo_use; l < hi_use; ++l) {
-      const int v = y_s[l - base];
-#pragma unroll
-      for (int q = 0; q < S; ++q) cnt[q] += (v == lane + 32 * q);
-    }
-    int w0[S], below = 0;
-#pragma unroll
-    for (int q = 0; q < S; ++q) {
-      int pre = cnt[q];
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const int v = __shfl_up_sync(0xffffffffu, pre, o);
-        if (lane >= o) pre += v;
-      }
-      w0[q] = below + pre - cnt[q];
-      start_s[lane + 32 * q] = w0[q];
-      if (q == S - 1) {
-        if (lane == 31) start_s[NW] = below + pre;
-      } else {
-        below += __shfl_sync(0xffffffffu, pre, 31);
-      }
-    }
-    for (int l = lo_use; l < hi_use; ++l) {
-      const int v = y_s[l - base];
-#pragma unroll
-      for (int q = 0; q < S; ++q)
-        if (v == lane + 32 * q) order_s[w0[q]++] = l - base;
-    }
-  }
+  label_index<NW>([&](int l) { return y_s[l - base]; }, lo_use, hi_use, base, start_s, order_s);
   __syncthreads();
 
   float2 ds[P];
 #pragma unroll
   for (int k = 0; k < P; ++k) ds[k] = make_float2(0.f, 0.f);
-  {
-    float* ztile2 = smem + lay.ztile + wo;
-    float* bnext = smem + lay.bnext + wo;
-    float* brow = smem + lay.brow + wo;
-    float* grow = smem + lay.grow + wo;
-    const uint32_t zt2 = (uint32_t)__cvta_generic_to_shared(ztile2);
-    const uint32_t bnext_sa = (uint32_t)__cvta_generic_to_shared(bnext);
-    const uint32_t grow_sa = (uint32_t)__cvta_generic_to_shared(grow);
-    const float tmax = trans_max(p.trans, p.N, lane);
-    const float* Zb = p.Z + (size_t)b * T * NW;
-    float* Gb = p.G + (size_t)b * T * NW;
-    const double logZ2 = p.facLogZ2[b];
-    const bool useful = lane >= 1 && lane <= 30;
-    FacState<P> st;
-    float s2b[P];
-    fac_load_target<P>(st, p, b, L, lane, true, tmax, base);
-#pragma unroll
-    for (int k = 0; k < P; ++k) s2b[k] = st.s2[k];
-    fac_load_target<P>(st, p, b, L, lane, false, tmax, base);
-    FlushIndex fx[S];  // labels lane + 32 s
-#pragma unroll
-    for (int q = 0; q < S; ++q) fx[q].load(order_s, start_s, lane + 32 * q, kHaloRow);
-    if (lane == 0) grow[kHaloRow] = 0.f;
-    const int l0 = base + lane * P;  // first position of this lane
-    // the chain lane (p.P positions each) whose offset this lane's positions carry, and its neighbours' across the lane edges
-    auto chain_lane = [&](int l) { return min(max(l, 0), p.Lp - 1) / p.P; };
-    const int cl = chain_lane(l0), cl_prev = chain_lane(l0 - P), cl_next = chain_lane(l0 + P);
-    auto prefetch = [&](int c, int buf) {
-      const int t0 = c * kSeg;
-#pragma unroll
-      for (int h = 0; h < 2 * S; ++h) {
-        const int chunk = lane + 32 * h;
-        const int t = t0 + (chunk >> (NW == 32 ? 3 : 4));  // (NW / 4 chunks per frame)
-        if (t < T) cp_async16(zt2 + (buf * kSeg * NW) * 4 + chunk * 16, Zb + (size_t)t * NW + (chunk & (NW / 4 - 1)) * 4);
-      }
-      if (t0 + kSeg < T) {
-        const float* src = p.ckBa + ((size_t)b * p.nC + c) * p.Lp;
-#pragma unroll
-        for (int k = 0; k < P; k += 4) {
-          const int l = l0 + k;
-          if (l >= 0 && l < p.Lp)
-            cp_async16(bnext_sa + (lane * P + k) * 4, src + l);
-          else
-            *reinterpret_cast<float4*>(bnext + lane * P + k) = make_float4(kNeg, kNeg, kNeg, kNeg);
-        }
-      }
-      cp_async_commit();
-    };
-    // every warp of the CTA walks the same segments (one barrier per frame pairs them up)
-    int buf = 0;
-    if ((int)blockIdx.x < p.nC) prefetch(blockIdx.x, 0);
-    for (int c = blockIdx.x; c < p.nC; c += gridDim.x, buf ^= 1) {
-      const int t0 = c * kSeg, t1 = min(T, t0 + kSeg);
-      const uint32_t zt = zt2 + (buf * kSeg * NW) * 4;
-      const float* ztile = ztile2 + buf * kSeg * NW;
-      cp_async_wait_all();
-      __syncwarp();
-      // ---- backwards: beta-tilde rows of frames t1-1 .. t0 (exact on the useful lanes: the right halo absorbs the edge) ----
-      double CB = 0.0;
-      float DB = 0.f, DA = 0.f;
-      int tstart;
-      if (t1 >= T) {
-#pragma unroll
-        for (int k = 0; k < P; ++k) st.v[k] = (l0 + k == L - 1) ? ztile[(T - 1 - t0) * NW + (st.y4[k] >> 2)] : kNeg;
-        fac_store_row<P>(st, brow + (size_t)(T - 1 - t0) * kHaloRow, lane);
-        tstart = T - 2;
-      } else {
-        fac_load_row<P>(st, bnext, lane);
-        const double* cb = p.ckCB + ((size_t)b * p.nC + c) * kW;
-        CB = cb[cl];
-        DB = (float)(cb[cl_next] - CB);
-        tstart = t1 - 1;
-      }
-      __syncwarp();
-      if (c + (int)gridDim.x < p.nC) prefetch(c + gridDim.x, buf ^ 1);
-      float arow[P];
-      double CA = 0.0;
-      if (t0 > 0) {
-        const float* src = p.ckAa + ((size_t)b * p.nC + c) * p.Lp;
-#pragma unroll
-        for (int k = 0; k < P; k += 4) {
-          const int l = l0 + k;
-          float4 q = make_float4(kNeg, kNeg, kNeg, kNeg);
-          if (l >= 0 && l < p.Lp) q = __ldg(reinterpret_cast<const float4*>(src + l));
-          arow[k] = q.x;
-          arow[k + 1] = q.y;
-          arow[k + 2] = q.z;
-          arow[k + 3] = q.w;
-        }
-        const double* ca = p.ckCA + ((size_t)b * p.nC + c) * kW;
-        CA = ca[cl];
-        DA = (float)(ca[cl_prev] - CA);
-      }
-      for (int t = tstart; t >= t0; --t) {
-        fac_beta_step<P>(st, s2b, zt + (t - t0) * (4 * NW), lane, DB);
-        fac_store_row<P>(st, brow + (size_t)(t - t0) * kHaloRow, lane);
-      }
-      // ---- forwards (exact on the useful lanes: the left halo absorbs the edge) --------------------------------------
-      int tfirst = t0;
-      if (t0 == 0) {
-#pragma unroll
-        for (int k = 0; k < P; ++k) st.v[k] = (l0 + k == 0) ? ztile[st.y4[k] >> 2] : kNeg;
-        if (w == 0) {  // frame 0 sits at position 0 (slice 0, local index P)
-#pragma unroll
-          for (int q = 0; q < S; ++q) Gb[lane + 32 * q] = (lane + 32 * q == y_s[P]) ? 1.0f : 0.0f;
-        }
-        tfirst = 1;
-      } else {
-#pragma unroll
-        for (int k = 0; k < P; ++k) st.v[k] = arow[k];
-      }
-      // halo lanes contribute nothing: their posteriors are switched off through the exponent
-      const float K = useful ? (float)(CA + CB - logZ2) + kLgShift : kNeg;
-      const float2 K2 = make_float2(K, K);
-      __syncwarp();
-      for (int t = tfirst; t < t1; ++t) {
-        const uint32_t zrow = zt + (t - t0) * (4 * NW);
-        const float* br = brow + (size_t)(t - t0) * kHaloRow + lane * P;
-        float up = __shfl_up_sync(0xffffffffu, st.v[P - 1], 1) + DA;
-        if (lane == 0) up = kNeg;
-        float2 xv[P];
-#pragma unroll
-        for (int k = P - 2; k >= 0; k -= 2) {
-          const float2 brk = fadd2_rn(*reinterpret_cast<const float2*>(br + k), K2);
-          const float2 nv = fac_grad_pair(st.v[k], k ? st.v[k - 1] : up, st.s1[k], st.s2[k], lds_f(zrow + st.y4[k]), brk.x,  //
-                                          st.v[k + 1], st.v[k], st.s1[k + 1], st.s2[k + 1], lds_f(zrow + st.y4[k + 1]), brk.y, xv[k], xv[k + 1]);
-          *reinterpret_cast<float2*>(grow + lane * P + k) = make_float2(xv[k].x + xv[k].y, xv[k + 1].x + xv[k + 1].y);
-          st.v[k] = nv.x;
-          st.v[k + 1] = nv.y;
-        }
-        __syncwarp();
-        // this slice's per-label sums meet the other slices' (one CTA barrier per frame, buffers alternate by parity)
-        float* gbuf = gsh + (t & 1) * (kHaloMaxW * NW);
-#pragma unroll
-        for (int q = 0; q < S; ++q) gbuf[w * NW + lane + 32 * q] = label_sum(grow_sa, grow, order_s, fx[q]);
-        __syncthreads();
-        float gl[S];
-#pragma unroll
-        for (int q = 0; q < S; ++q) {
-          gl[q] = 0.f;
-          for (int ww = 0; ww < W; ++ww) gl[q] += gbuf[ww * NW + lane + 32 * q];
-        }
-        float gs = gl[0];
-#pragma unroll
-        for (int q = 1; q < S; ++q) gs += gl[q];
-        const float gt = warp_sum(gs);
-        if (w == 0) {
-#pragma unroll
-          for (int q = 0; q < S; ++q) Gb[(size_t)t * NW + lane + 32 * q] = gt > 0.f ? gl[q] / gt : 0.f;
-        }
-        const float inv = gt > 0.f ? __fdividef(1.0f, gt) : 0.f;
-        const float2 inv2 = make_float2(inv, inv);
-#pragma unroll
-        for (int k = 0; k < P; ++k) ds[k] = ffma2_rn(xv[k], inv2, ds[k]);
-      }
-    }
-    cp_async_wait_all();
-  }
+  // the chain lane (p.P positions each) whose offset a position carries
+  auto chain_lane = [&](int l) { return min(max(l, 0), p.Lp - 1) / p.P; };
+  const int l0 = base + lane * P;
+  fac_grad_walk<P, NW, true>(p, b, blockIdx.x, gridDim.x, smem + lay.ztile + wo, kHaloRow, order_s, start_s, l0, chain_lane(l0),
+                             chain_lane(l0 - P), chain_lane(l0 + P), lane >= 1 && lane <= 30, w == 0, smem + lay.gsh, ds);
   // ---- CTA partial of the transition gradient: slice by slice (fixed order: deterministic) ------------------------
 #pragma unroll
   for (int k = 0; k < P; ++k) {
@@ -1536,6 +1268,17 @@ __global__ void __launch_bounds__(32 * kHaloMaxW) asg_fac_grad_halo_kernel(AsgPa
 // ------------------------------------------------------------------------------------------
 // 4. FCC gradient + emission gradient, from the stored a-hat / b-hat vectors: no dependence between frames
 // ------------------------------------------------------------------------------------------
+// loss[b] = scale * (FCC - FAC) (or the one term asked for), NaN for an invalid sample
+__device__ __forceinline__ void write_loss(const AsgParams& p, int b, bool valid, bool has_fcc, bool has_fac) {
+  float l = NAN;
+  if (valid) {
+    double v = 0.0;
+    if (has_fcc) v += p.fccLogZ[b] + p.msum[b];
+    if (has_fac) v += (has_fcc ? -1.0 : 1.0) * (p.facLogZ[b] + p.msum[b]);
+    l = (float)((double)p.scale[b] * v);
+  }
+  p.loss[b] = l;
+}
 // NW = 64: lane i accumulates rows i and i + 32 (128 registers), 4 warps of 8 frames, slabs in dynamic shared memory
 template <int NW>
 __global__ void __launch_bounds__(fcc_grad_warps<NW>() * 32, NW == 32 ? 2 : 1) asg_fcc_grad_kernel(AsgParams p) {
@@ -1552,16 +1295,7 @@ __global__ void __launch_bounds__(fcc_grad_warps<NW>() * 32, NW == 32 ? 2 : 1) a
   extern __shared__ __align__(16) float smem[];
   float* sm = NW == 32 ? sm_static : smem;
   static_assert((kFrames + 1) * NW <= NW * (NW + 1), "tile must fit in a slab");
-  if (chunk == 0 && lane == 0) {
-    float l = NAN;
-    if (ok) {
-      double v = 0.0;
-      if (has_fcc) v += p.fccLogZ[b] + p.msum[b];
-      if (has_fac) v += (has_fcc ? -1.0 : 1.0) * (p.facLogZ[b] + p.msum[b]);
-      l = (float)((double)p.scale[b] * v);
-    }
-    p.loss[b] = l;
-  }
+  if (chunk == 0 && lane == 0) write_loss(p, b, ok, has_fcc, has_fac);
   const int t0 = chunk * kFrames, t1 = min(T, t0 + kFrames);
   float2 acc[S][NW / 2];  // row lane + 32 s of the warp's transition statistics
 #pragma unroll
@@ -1705,22 +1439,10 @@ __global__ void __launch_bounds__(256) asg_parts_reduce_kernel(const float* in, 
 }
 
 __global__ void asg_loss_only_kernel(AsgParams p) {
-  int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= p.B) return;
-  float l = NAN;
-  if (p.valid[b]) {
-    double v = 0.0;
-    if (p.terms & W2L_TERM_FCC) v += p.fccLogZ[b] + p.msum[b];
-    if (p.terms & W2L_TERM_FAC) v += ((p.terms & W2L_TERM_FCC) ? -1.0 : 1.0) * (p.facLogZ[b] + p.msum[b]);
-    l = (float)((double)p.scale[b] * v);
-  }
-  p.loss[b] = l;
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b < p.B) write_loss(p, b, p.valid[b], p.terms & W2L_TERM_FCC, p.terms & W2L_TERM_FAC);
 }
 
-// P >= 16 means more than 256 positions, which always take the halo kernel: at NW = 64 the single-warp FAC grad kernel
-// is not instantiated for them (the NW = 32 instantiations are kept as they are).  asg_forward_backward refuses the
-// combination explicitly, so the P = 8 stand-in can never run with a wider row.
-#define W2L_FAC_GRAD_P(PP) ((NW == 32 || (PP) <= 8) ? (PP) : 8)
 int pick_P(int Le) {  // positions per lane: smallest power of two with 32*P >= Le
   int P = 1;
   while (32 * P < Le) P <<= 1;
@@ -1740,43 +1462,38 @@ int fcc_grad_ctas(int T) {
 }
 template <int NW>
 constexpr size_t fcc_grad_smem() { return NW == 32 ? 0 : (size_t)fcc_grad_warps<NW>() * NW * (NW + 1) * 4; }  // dynamic
-// CTAs per sample of the FAC grad kernel: one resident wave of the chip over the batch (the CTAs loop over their segments)
-template <int P, int NW>
-int fac_grad_slots(int warps, size_t smem) {
+// CTAs of `kernel` resident in one wave of the device at this block size and dynamic shared memory
+template <typename Kernel>
+int wave_ctas(Kernel kernel, int threads, size_t smem) {
   int per_sm = 0;
-  if (smem > 48 * 1024) cudaFuncSetAttribute(asg_fac_grad_kernel<P, NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, asg_fac_grad_kernel<P, NW>, warps * 32, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
-  int dev = 0, sms = 132;
-  if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  return per_sm * sms;
+  if (smem > 48 * 1024) cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
+  return per_sm * sm_count();
 }
+// the single-warp FAC grad kernel for P positions per lane (P <= 8: longer rows take the halo kernel, see shape())
+template <int NW>
+void (*fac_grad_kernel(int P))(AsgParams) {
+  switch (P) {
+    case 1: return asg_fac_grad_kernel<1, NW>;
+    case 2: return asg_fac_grad_kernel<2, NW>;
+    case 4: return asg_fac_grad_kernel<4, NW>;
+    case 8: return asg_fac_grad_kernel<8, NW>;
+  }
+  return nullptr;
+}
+// CTAs per sample of the FAC grad kernel: one resident wave of the chip over the batch (the CTAs loop over their segments)
 template <int NW>
 int fac_grad_ctas(const AsgParams& p) {
   if (p.Wg > 1) {  // the halo kernel: one CTA of Wg warps per segment, CTAs loop over their sample's segments
-    const size_t smem = (size_t)halo_layout<NW>(p.Wg).total * 4;
-    int per_sm = 0;
-    cudaFuncSetAttribute(asg_fac_grad_halo_kernel<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, asg_fac_grad_halo_kernel<NW>, 32 * p.Wg, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
-    int dev = 0, sms = 132;
-    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    int want = per_sm * sms / p.B;
+    int want = wave_ctas(asg_fac_grad_halo_kernel<NW>, 32 * p.Wg, (size_t)halo_layout<NW>(p.Wg).total * 4) / p.B;
     if (want < 1) want = 1;
     return want < p.nC ? want : p.nC;
   }
   const int most = (p.nC + p.fac_grad_warps - 1) / p.fac_grad_warps;
-  static int slots_cache[6] = {0, 0, 0, 0, 0, 0};
-  const int idx = p.P == 1 ? 0 : p.P == 2 ? 1 : p.P == 4 ? 2 : p.P == 8 ? 3 : p.P == 16 ? 4 : 5;
-  if (slots_cache[idx] == 0) {
-    const size_t smem = (size_t)fac_grad_layout<NW>(p.Lp, p.fac_grad_warps).total * 4;
-    switch (p.P) {
-      case 1: slots_cache[idx] = fac_grad_slots<1, NW>(p.fac_grad_warps, smem); break;
-      case 2: slots_cache[idx] = fac_grad_slots<2, NW>(p.fac_grad_warps, smem); break;
-      case 4: slots_cache[idx] = fac_grad_slots<4, NW>(p.fac_grad_warps, smem); break;
-      case 8: slots_cache[idx] = fac_grad_slots<8, NW>(p.fac_grad_warps, smem); break;
-      case 16: slots_cache[idx] = fac_grad_slots<W2L_FAC_GRAD_P(16), NW>(p.fac_grad_warps, smem); break;
-      default: slots_cache[idx] = fac_grad_slots<W2L_FAC_GRAD_P(32), NW>(p.fac_grad_warps, smem); break;
-    }
-  }
+  static int slots_cache[4] = {0, 0, 0, 0};  // by log2 P
+  const int idx = p.P == 1 ? 0 : p.P == 2 ? 1 : p.P == 4 ? 2 : 3;
+  if (slots_cache[idx] == 0)
+    slots_cache[idx] = wave_ctas(fac_grad_kernel<NW>(p.P), p.fac_grad_warps * 32, (size_t)fac_grad_layout<NW>(p.Lp, p.fac_grad_warps).total * 4);
   int want = slots_cache[idx] / p.B;
   if (want < 1) want = 1;
   return want < most ? want : most;
@@ -1825,7 +1542,8 @@ void shape(AsgParams& p, int B, int T, int N, int L) {
   p.Lp = 32 * p.P;
 
   p.nC = (T + kSeg - 1) / kSeg;
-  // long targets: the FAC grad kernel cuts the row into slices of 240 useful positions (the halo path), 4 warps per CTA
+  // long targets: the FAC grad kernel cuts the row into slices of 240 useful positions (the halo path), one warp per
+  // slice.  P >= 16 means Le > 256, so Wg >= 2: the single-warp FAC grad kernel only ever sees P <= 8.
   p.Wg = p.P >= 16 ? (Le + kHaloUse - 1) / kHaloUse : 1;
   p.fac_grad_warps = p.Wg > 1 ? p.Wg : fac_grad_warps<NW>(p.Lp);
 }
@@ -1865,9 +1583,6 @@ int asg_forward_backward(const char* name, void* stream_, int terms, int B, int 
   if (!workspace || workspace_bytes < need)
     return fail(W2L_ERR_WORKSPACE, tag + ": workspace too small (need " + std::to_string(need) + " bytes)");
   if ((terms & W2L_TERM_FAC) && p.P > 32) return fail(W2L_ERR_UNSUPPORTED, tag + ": target longer than 1024 is not covered");
-  // W2L_FAC_GRAD_P: at NW = 64 only P <= 8 has a single-warp FAC grad kernel; longer rows must take the halo kernel
-  if (NW != 32 && p.Wg == 1 && p.P > 8)
-    return fail(W2L_ERR_UNSUPPORTED, tag + ": no single-warp FAC gradient kernel for " + std::to_string(p.P) + " positions per lane");
   p.scale_mode = scale_mode;
   p.terms = terms;
   p.need_grad = d_emis != nullptr;
@@ -1896,19 +1611,16 @@ int asg_forward_backward(const char* name, void* stream_, int terms, int B, int 
   asg_prep_kernel<NW><<<frame_blocks + meta_blocks, 256, 0, stream>>>(p, frame_blocks);
   W2L_LAUNCH_CHECK("asg_prep_kernel");
 
-#define W2L_FOR_P(MACRO)        \
-  switch (p.P) {                \
-    case 1: MACRO(1); break;    \
-    case 2: MACRO(2); break;    \
-    case 4: MACRO(4); break;    \
-    case 8: MACRO(8); break;    \
-    case 16: MACRO(16); break;  \
-    default: MACRO(32); break;  \
-  }
   profile_kind(2);
   profile_start(stream);
-#define W2L_LAUNCH_CHAINS(PP) asg_chains_kernel<PP, NW><<<p.n_roles * B, 32, 0, stream>>>(p)
-  W2L_FOR_P(W2L_LAUNCH_CHAINS)
+  switch (p.P) {
+    case 1: asg_chains_kernel<1, NW><<<p.n_roles * B, 32, 0, stream>>>(p); break;
+    case 2: asg_chains_kernel<2, NW><<<p.n_roles * B, 32, 0, stream>>>(p); break;
+    case 4: asg_chains_kernel<4, NW><<<p.n_roles * B, 32, 0, stream>>>(p); break;
+    case 8: asg_chains_kernel<8, NW><<<p.n_roles * B, 32, 0, stream>>>(p); break;
+    case 16: asg_chains_kernel<16, NW><<<p.n_roles * B, 32, 0, stream>>>(p); break;
+    default: asg_chains_kernel<32, NW><<<p.n_roles * B, 32, 0, stream>>>(p); break;
+  }
   profile_stop(stream);
   W2L_LAUNCH_CHECK("asg_chains_kernel");
 
@@ -1923,15 +1635,10 @@ int asg_forward_backward(const char* name, void* stream_, int terms, int B, int 
     asg_fac_grad_halo_kernel<NW><<<dim3(gA, B), 32 * p.Wg, smem, stream>>>(p);
     W2L_LAUNCH_CHECK("asg_fac_grad_halo_kernel");
   } else if (has_fac) {
+    const auto kernel = fac_grad_kernel<NW>(p.P);
     const size_t smem = (size_t)fac_grad_layout<NW>(p.Lp, p.fac_grad_warps).total * 4;
-    const dim3 grid(gA, B);
-#define W2L_LAUNCH_FAC_GRAD(PP)                                                                                          \
-  do {                                                                                                                   \
-    if (smem > 48 * 1024)                                                                                                \
-      W2L_CUDA_CHECK(cudaFuncSetAttribute(asg_fac_grad_kernel<W2L_FAC_GRAD_P(PP), NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    asg_fac_grad_kernel<W2L_FAC_GRAD_P(PP), NW><<<grid, p.fac_grad_warps * 32, smem, stream>>>(p);                     \
-  } while (0)
-    W2L_FOR_P(W2L_LAUNCH_FAC_GRAD)
+    if (smem > 48 * 1024) W2L_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<dim3(gA, B), p.fac_grad_warps * 32, smem, stream>>>(p);
     W2L_LAUNCH_CHECK("asg_fac_grad_kernel");
   }
   {
