@@ -485,6 +485,45 @@ W2L_API int w2l_stream_run(void* s, void* stream, int n, const int* slots, const
                            float* emissions, long long capacity, int* frames_out);
 W2L_API int w2l_stream_plan(const char* arch_text, int n_feat, int n_label, int n_calls, const int* frames_host, int finish_last,
                             int max_convs, int* n_convs, int* conv_spec_host, int* frames_out_host, int* tails_host);
+/* ----------------------------------------------------------------------------------------
+ * Streaming MFSC front end: raw audio chunk by chunk over many concurrent streams, with the semantics of the in-tree
+ * inference library's feature module (inference/module/feature/LogMelFeature.cpp, then LocalNorm(F, left_ctx, 0) of
+ * inference/module/nn/LocalNorm.cpp).  Its output is the features argument of w2l_stream_run.  Per stream, the features
+ * of all run calls put end to end are the same bits whatever the split into chunks and whatever other streams share
+ * the calls, and match w2l_mfsc(..., left_ctx) of the whole stream up to the order of the window sums (DESIGN.md §4).
+ *   Settings: the frame and stride rounding, the mel filters, the log floor, the sample scale and the W2L_ERR_UNSUPPORTED
+ *   limits of w2l_mfsc (stride a multiple of 4 samples, frames up to 2048 samples, at most 256 filters).  left_ctx >= 1:
+ *   per-utterance normalisation (w2l_mfsc's left_ctx = 0) cannot be computed causally.
+ *   start  holds nothing;
+ *   run    appends samples_in[i] samples; with avail samples held, frames = avail < frame ? 0 : 1 + (avail - frame) /
+ *          stride come out and frames * stride samples are consumed (fewer than frame stay);
+ *   finish runs, then drops the remainder (no right padding); the slot refuses run until the next start.
+ *   A stream's frame g (counted from start) is normalised over its frames max(0, g - left_ctx) .. g: mean and population
+ *   standard deviation, a std <= 1e-5 counting as 1.
+ * Frame counts are integer arithmetic on the host: a run call neither reads from the device nor synchronises.  The DFT
+ * is an fp32-accurate (3xTF32) GEMM whatever w2l_set_precision says.  Calls on one handle must be ordered.
+ *
+ *   w2l_mfsc_stream_create   allocates state and per-call buffers for max_streams slots (at most 1024) and chunks of at
+ *                            most max_chunk_samples samples (at most 65535) and builds the DFT basis and the filters.
+ *                            Checks every argument before its first CUDA call.  NULL on failure (w2l_last_error).
+ *   w2l_mfsc_stream_state_bytes     device bytes of carried state per slot (two planes of the held samples and of the
+ *                                   held per-frame sums)
+ *   w2l_mfsc_stream_max_frames_out  the most frames one call can give a stream (sizes the feature buffer)
+ *   w2l_mfsc_stream_start    resets the n slots (host int slots[n]); a running slot forgets its past
+ *   w2l_mfsc_stream_run      slots[n], samples_in[n] (host ints, each <= Sc <= max_chunk_samples), audio device [n][Sc];
+ *                            features device [n][1][F][Tf] (ArrayFire [Tf,F,1,n], the trainer's layout) with Tf = max
+ *                            frames_out, frames t >= frames_out[i] of stream i are 0; capacity in floats; frames_out[n]
+ *                            host.  Errors (W2L_ERR_INVALID_ARGUMENT): a slot out of range or listed twice, a slot not
+ *                            started or already finished, samples_in[i] > Sc, Sc > max_chunk_samples, too small a capacity.
+ * ---------------------------------------------------------------------------------------- */
+W2L_API void* w2l_mfsc_stream_create(void* stream, int max_streams, int max_chunk_samples, int sample_rate, int frame_ms, int stride_ms,
+                                     int n_filters, int left_ctx);
+W2L_API void w2l_mfsc_stream_destroy(void* h);
+W2L_API long long w2l_mfsc_stream_state_bytes(void* h);
+W2L_API int w2l_mfsc_stream_max_frames_out(void* h);
+W2L_API int w2l_mfsc_stream_start(void* h, void* stream, int n, const int* slots);
+W2L_API int w2l_mfsc_stream_run(void* h, void* stream, int n, const int* slots, const int* samples_in, const float* audio, int Sc, int finish,
+                                float* features, long long capacity, int* frames_out);
 /* data-parallel rendezvous: rank 0 creates the 128-byte NCCL id, the launcher ships it to every rank */
 W2L_API int w2l_nccl_unique_id(void* out128);
 W2L_API int w2l_init_distributed(int rank, int world, const void* id128);

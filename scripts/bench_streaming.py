@@ -12,6 +12,12 @@ For each precision and each count of concurrent streams, every stream is fed 500
 and the card's name and power limit, read in the same process.  Needs a CUDA device; there is no CPU path.
 
   python scripts/bench_streaming.py [--labels 10000] [--streams 1 64 512] [--precisions bf16 f32] [--calls 40]
+
+--audio feeds raw audio instead: every stream gets 500 ms chunks (8000 samples at 16 kHz) through the MFSC front end
+(StreamingFeatures, 80 filters, left_ctx 300) and its features go to the acoustic model in the same iteration.  Per
+case it prints the device ms per call (median of event pairs) of the front end alone, of front end + AM, and of the AM
+fed precomputed features, measured in alternating rounds in the same process, and the audio seconds per wall second of
+front end + AM.
 """
 import argparse
 import json
@@ -60,6 +66,8 @@ def main():
     ap.add_argument("--chunk", type=int, default=50)
     ap.add_argument("--calls", type=int, default=40)
     ap.add_argument("--warmup", type=int, default=8)
+    ap.add_argument("--audio", action="store_true", help="raw 16 kHz audio through the streaming MFSC front end")
+    ap.add_argument("--rounds", type=int, default=3, help="--audio: alternating rounds of the three variants")
     args = ap.parse_args()
 
     from wav2letter_b200 import archs, capi, streaming
@@ -80,6 +88,8 @@ def main():
     from wav2letter_b200.trainer import Trainer
 
     dev = card()
+    if args.audio:
+        return audio_bench(args, arch, dev)
     for precision in args.precisions:
         tr = Trainer(arch, 80, args.labels, "ctc", "none", precision=precision)
         for S in args.streams:
@@ -118,6 +128,67 @@ def main():
                 "gemm_launches_timed": used, "gemm_ms_per_call": round(gemm_ms / args.calls, 4),
                 "state_bytes_per_stream": am.state_bytes, "card": dev}), flush=True)
             am.close()
+        tr.close()
+
+
+def audio_bench(args, arch, dev):
+    import torch
+
+    from wav2letter_b200 import streaming
+    from wav2letter_b200.trainer import Trainer
+
+    samples = args.chunk * 160  # 10 ms stride at 16 kHz
+    for precision in args.precisions:
+        tr = Trainer(arch, 80, args.labels, "ctc", "none", precision=precision)
+        for S in args.streams:
+            fe = streaming.StreamingFeatures(S, samples)
+            am = streaming.StreamingAM(tr, S, max_chunk=fe.max_frames_out, precision=precision)
+            slots = list(range(S))
+            fe.start(slots)
+            am.start(slots)
+            g = torch.Generator(device="cuda").manual_seed(S)
+            audio = (torch.randn((S, samples), device="cuda", generator=g) * 1000).contiguous()
+            x = torch.randn((S, 1, 80, args.chunk), device="cuda", generator=g)
+
+            def front():
+                fe.run(slots, audio)
+
+            def both():
+                f, frames = fe.run(slots, audio)
+                am.run(slots, f, frames)
+
+            def model():
+                am.run(slots, x)
+
+            variants = {"frontend": front, "frontend_am": both, "am_features": model}
+            for fn in variants.values():  # warm every shape
+                for _ in range(args.warmup):
+                    fn()
+            torch.cuda.synchronize()
+            times = {k: [] for k in variants}
+            walls = []
+            for _ in range(args.rounds):
+                for name, fn in variants.items():
+                    ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.calls)]
+                    t0 = time.perf_counter()
+                    for a, b in ev:
+                        a.record()
+                        fn()
+                        b.record()
+                    torch.cuda.synchronize()
+                    if name == "frontend_am":
+                        walls.append(time.perf_counter() - t0)
+                    times[name] += [a.elapsed_time(b) for a, b in ev]
+            med = {k: sorted(v)[len(v) // 2] for k, v in times.items()}
+            print(json.dumps({
+                "precision": precision, "streams": S, "chunk_samples": samples, "labels": args.labels, "calls": args.calls, "rounds": args.rounds,
+                "frontend_ms_device": round(med["frontend"], 4), "frontend_am_ms_device": round(med["frontend_am"], 4),
+                "am_features_ms_device": round(med["am_features"], 4),
+                "frontend_share_of_am": round(med["frontend"] / med["am_features"], 4),
+                "audio_s_per_s": round(S * args.calls * samples / 16000 / min(walls), 1),
+                "frontend_state_bytes_per_stream": fe.state_bytes, "card": dev}), flush=True)
+            am.close()
+            fe.close()
         tr.close()
 
 

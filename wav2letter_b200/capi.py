@@ -41,6 +41,8 @@ EXPORTS = [
     "w2l_mfsc_num_frames", "w2l_mfsc_workspace_size", "w2l_mfsc",
     "w2l_stream_create", "w2l_stream_destroy", "w2l_stream_state_bytes", "w2l_stream_max_frames_out", "w2l_stream_start",
     "w2l_stream_run", "w2l_stream_plan",
+    "w2l_mfsc_stream_create", "w2l_mfsc_stream_destroy", "w2l_mfsc_stream_state_bytes", "w2l_mfsc_stream_max_frames_out",
+    "w2l_mfsc_stream_start", "w2l_mfsc_stream_run",
 ]
 
 
@@ -179,6 +181,15 @@ def _load() -> ctypes.CDLL:
     lib.w2l_stream_start.argtypes = [vp, vp, i, vp]
     lib.w2l_stream_run.argtypes = [vp, vp, i, vp, vp, vp, i, i, vp, ctypes.c_longlong, vp]
     lib.w2l_stream_plan.argtypes = [ctypes.c_char_p, i, i, i, vp, i, i, vp, vp, vp, vp]
+    lib.w2l_mfsc_stream_create.restype = vp
+    lib.w2l_mfsc_stream_create.argtypes = [vp, i, i, i, i, i, i, i]
+    lib.w2l_mfsc_stream_destroy.argtypes = [vp]
+    lib.w2l_mfsc_stream_destroy.restype = None
+    lib.w2l_mfsc_stream_state_bytes.restype = ctypes.c_longlong
+    lib.w2l_mfsc_stream_state_bytes.argtypes = [vp]
+    lib.w2l_mfsc_stream_max_frames_out.argtypes = [vp]
+    lib.w2l_mfsc_stream_start.argtypes = [vp, vp, i, vp]
+    lib.w2l_mfsc_stream_run.argtypes = [vp, vp, i, vp, vp, vp, i, i, vp, ctypes.c_longlong, vp]
     return lib
 
 

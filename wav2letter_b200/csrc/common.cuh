@@ -17,6 +17,8 @@ int fail(int code, const std::string& msg);
 void count_launch(int n = 1);
 int current_precision();  // W2L_PRECISION_* of the calling thread (w2l_set_precision)
 int sm_count();           // multiprocessors of the current device (132 on an H100 SXM), for grid sizing
+int gemm_view_unsplit(cudaStream_t stream, int kind, int M, int N, int K, const float* A, int lda, const float* B, int ldb, float* C,
+                      int ldc);  // gemm_wgmma.cu: w2l_gemm of a K-major view with split-K off
 void trace_launch(const char* name);  // trace mode (w2l_trace_begin): one event after every launch, on the trace stream
 // bench hook: events recorded around a call's dominant kernel (nullptr when unset)
 void profile_kind(int kind);  // 1 = GEMM, 2 = criterion chains (set right before profile_start)

@@ -6,10 +6,13 @@
 //      frames are an overlapping-row view of the packed samples (row = frame, row stride = the frame stride);
 //   2. magnitude -> triangular mel filters -> log(max(., 1)) per frame, with each frame's sum and sum of squares;
 //   3. per-utterance prefix sums of those (double, fixed order) and the normalisation into [B][F][T_out].
+// The streaming front end (host/mfsc_stream_capi.cpp) runs 1 and 2 per call on the frames the AM's window kernel cut, and
+// its own LocalNorm kernel (mfsc_stream_norm_kernel) over the per-frame sums it carries between calls.
 #include <algorithm>
 #include <vector>
 
 #include "common.cuh"
+#include "../host/stream_internal.h"
 
 namespace w2l {
 namespace {
@@ -23,9 +26,7 @@ constexpr int kMelFrames = 32;  // frames per CTA of the mel kernel
 constexpr int kMaxFft = 2048;   // the mel kernel keeps 32 frames' magnitudes (32 x (nfft/2+1) floats) in shared memory
 constexpr int kMaxFilters = 256;
 
-struct Geom {
-  int frame, stride, nfft, bins, ncols, ldb, nfilt;
-};
+using Geom = streaming::MfscGeom;
 
 int frame_samples(int sample_rate, int ms) { return (int)(((long long)sample_rate * ms + 500) / 1000); }  // round half up
 int frames_of(long long n, const Geom& g) { return n < g.frame ? 0 : (int)(1 + (n - g.frame) / g.stride); }
@@ -228,9 +229,102 @@ __global__ void __launch_bounds__(256) mfsc_norm_kernel(int nfilt, int t_out, in
   }
 }
 
+// CTA = (kNormFrames frames, stream blockIdx.y).  One thread per frame sums the (sum, sum of squares) pairs of its window
+// [held pairs | this call's pairs] oldest first, so a frame's sums depend on its position in the stream only (not on
+// the chunking or the other streams); the block then normalises its frames and zeroes the slack ones.  CTA 0 of a stream
+// writes the last min(held + fresh, left) pairs to the other plane.
+constexpr int kNormFrames = 64;
+__global__ void __launch_bounds__(256) mfsc_stream_norm_kernel(const __grid_constant__ streaming::MfscNormArgs a) {
+  __shared__ double2 stat[kNormFrames];  // (mean, std) per frame
+  const int i = blockIdx.y, t0 = blockIdx.x * kNormFrames;
+  const int code = a.code[i], h = a.held[i], nt = a.fresh[i];
+  const long long slot = (long long)(code >> 1) * 2 * a.left;
+  const double2* held = reinterpret_cast<const double2*>(a.state) + slot + (long long)(code & 1) * a.left;
+  double2* next = reinterpret_cast<double2*>(a.state) + slot + (long long)((code & 1) ^ 1) * a.left;
+  const double2* fresh = reinterpret_cast<const double2*>(a.sums) + (long long)i * a.tWs;
+  auto pair = [&](int c) { return c < h ? held[c] : fresh[c - h]; };
+  const int t = t0 + (int)threadIdx.x;
+  if (threadIdx.x < kNormFrames && t < nt) {
+    const int hi = h + t, lo = max(0, hi - a.left);
+    double s1 = 0.0, s2 = 0.0;
+    for (int c = lo; c <= hi; ++c) {
+      const double2 p = pair(c);
+      s1 += p.x;
+      s2 += p.y;
+    }
+    const double cnt = (double)(hi - lo + 1) * a.nfilt, mean = s1 / cnt;
+    double sd = sqrt(fmax(s2 / cnt - mean * mean, 0.0));
+    if (sd <= kStdFloor) sd = 1.0;
+    stat[threadIdx.x] = make_double2(mean, sd);
+  }
+  __syncthreads();
+  const int nf = min(kNormFrames, a.tOut - t0);
+  float* out = a.feat + (long long)i * a.nfilt * a.tOut + t0;
+  for (int e = threadIdx.x; e < a.nfilt * nf; e += blockDim.x) {
+    const int f = e / nf, j = e - f * nf;
+    float* o = out + (long long)f * a.tOut + j;
+    *o = t0 + j < nt ? (float)(((double)*o - stat[j].x) / stat[j].y) : 0.f;
+  }
+  if (blockIdx.x == 0) {
+    const int total = h + nt, keep = min(total, a.left);
+    for (int k = threadIdx.x; k < keep; k += blockDim.x) next[k] = pair(total - keep + k);
+  }
+}
+
 unsigned grid_for(long long n, int per_block = 256, long long cap = 4096) { return (unsigned)std::max(1LL, std::min((n + per_block - 1) / per_block, cap)); }
 
+int launch_tables(cudaStream_t stream, const Geom& g, int sample_rate, float* basis, float* wts, int2* range) {
+  mfsc_basis_kernel<<<grid_for((long long)g.ncols * g.ldb), 256, 0, stream>>>(g.frame, g.nfft, g.bins, g.ncols, g.ldb, basis);
+  W2L_LAUNCH_CHECK("mfsc_basis_kernel");
+  mfsc_filter_kernel<<<grid_for((long long)g.nfilt * g.bins), 256, 0, stream>>>(g.nfilt, g.bins, sample_rate, wts, range);
+  W2L_LAUNCH_CHECK("mfsc_filter_kernel");
+  return W2L_OK;
+}
+
+int launch_mel(cudaStream_t stream, const Geom& g, int B, int t_max, int t_out, int t_ws, const int4* tab, const float* spec, const float* wts,
+               const int2* range, float* feat, double2* sums) {
+  const size_t smem = sizeof(float) * ((size_t)kMelFrames * g.bins + (size_t)g.nfilt * (kMelFrames + 1));
+  static bool configured = false;
+  if (!configured) {
+    W2L_CUDA_CHECK(cudaFuncSetAttribute(mfsc_mel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)(sizeof(float) * ((size_t)kMelFrames * (kMaxFft / 2 + 1) + (size_t)kMaxFilters * (kMelFrames + 1)))));
+    configured = true;
+  }
+  mfsc_mel_kernel<<<dim3((t_max + kMelFrames - 1) / kMelFrames, B), 256, smem, stream>>>(g.bins, g.ncols, g.nfilt, t_out, t_ws, tab, spec, wts,
+                                                                                        range, feat, sums);
+  W2L_LAUNCH_CHECK("mfsc_mel_kernel");
+  return W2L_OK;
+}
+
 }  // namespace
+
+namespace streaming {
+
+int mfscGeom(int sample_rate, int frame_ms, int stride_ms, int n_filters, MfscGeom* g) {
+  const int rc = make_geom(sample_rate, frame_ms, stride_ms, n_filters, g);
+  return rc ? rc : check_supported(*g);
+}
+
+int launchMfscTables(void* stream, const MfscGeom& g, int sample_rate, float* basis, float* wts, int* range) {
+  return launch_tables(static_cast<cudaStream_t>(stream), g, sample_rate, basis, wts, reinterpret_cast<int2*>(range));
+}
+
+int launchMfscStreamFrames(void* stream_, const MfscGeom& g, long long rows, int tMax, const float* x, const float* basis, const float* wts,
+                           const int* range, const int* tab, float* spec, const MfscNormArgs& a) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (rows <= 0 || rows > 0x3fffffffLL || tMax <= 0 || a.n <= 0 || a.n > kMaxCallStreams || a.left <= 0 || a.tOut < tMax || a.tWs < tMax)
+    return fail(W2L_ERR_INVALID_ARGUMENT, "mfsc stream: bad sizes");
+  int rc = gemm_view_unsplit(stream, W2L_GEMM_F32X3, (int)rows, g.ncols, g.frame, x, g.stride, basis, g.ldb, spec, g.ncols);
+  if (rc) return rc;
+  rc = launch_mel(stream, g, a.n, tMax, a.tOut, a.tWs, reinterpret_cast<const int4*>(tab), spec, wts, reinterpret_cast<const int2*>(range), a.feat,
+                  reinterpret_cast<double2*>(a.sums));
+  if (rc) return rc;
+  mfsc_stream_norm_kernel<<<dim3((a.tOut + kNormFrames - 1) / kNormFrames, a.n), 256, 0, stream>>>(a);
+  W2L_LAUNCH_CHECK("mfsc_stream_norm_kernel");
+  return W2L_OK;
+}
+
+}  // namespace streaming
 }  // namespace w2l
 
 using namespace w2l;
@@ -284,10 +378,8 @@ extern "C" int w2l_mfsc(void* stream_, int B, int max_samples, const float* audi
   const int t_ws = std::max(1, frames_of(max_samples, g));
   W2L_CUDA_CHECK(cudaMemcpyAsync(l.tab, tab.data(), sizeof(int4) * B, cudaMemcpyHostToDevice, stream));
   if (t_max > 0) {
-    mfsc_basis_kernel<<<grid_for((long long)g.ncols * g.ldb), 256, 0, stream>>>(g.frame, g.nfft, g.bins, g.ncols, g.ldb, l.basis);
-    W2L_LAUNCH_CHECK("mfsc_basis_kernel");
-    mfsc_filter_kernel<<<grid_for((long long)g.nfilt * g.bins), 256, 0, stream>>>(g.nfilt, g.bins, sample_rate, l.wts, l.range);
-    W2L_LAUNCH_CHECK("mfsc_filter_kernel");
+    rc = launch_tables(stream, g, sample_rate, l.basis, l.wts, l.range);
+    if (rc) return rc;
     const int max_slot = (max_samples + g.stride - 1) / g.stride;
     mfsc_pack_kernel<<<dim3(grid_for((long long)max_slot * g.stride, 256, 1024), B), 256, 0, stream>>>(max_samples, g.stride, audio, l.tab, l.x);
     W2L_LAUNCH_CHECK("mfsc_pack_kernel");
@@ -297,16 +389,8 @@ extern "C" int w2l_mfsc(void* stream_, int B, int max_samples, const float* audi
     rc = w2l_gemm(stream, W2L_GEMM_F32X3, 0, 0, (int)rows, g.ncols, g.frame, l.x, g.stride, l.basis, g.ldb, l.spec, g.ncols, 0, nullptr, 0,
                   0, nullptr, 0, 0, 0, 1.f, 0.f, 0ull, 1);
     if (rc) return rc;
-    const size_t smem = sizeof(float) * ((size_t)kMelFrames * g.bins + (size_t)g.nfilt * (kMelFrames + 1));
-    static bool configured = false;
-    if (!configured) {
-      W2L_CUDA_CHECK(cudaFuncSetAttribute(mfsc_mel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          (int)(sizeof(float) * ((size_t)kMelFrames * (kMaxFft / 2 + 1) + (size_t)kMaxFilters * (kMelFrames + 1)))));
-      configured = true;
-    }
-    mfsc_mel_kernel<<<dim3((t_max + kMelFrames - 1) / kMelFrames, B), 256, smem, stream>>>(g.bins, g.ncols, g.nfilt, T_out, t_ws, l.tab,
-                                                                                          l.spec, l.wts, l.range, features, l.sums);
-    W2L_LAUNCH_CHECK("mfsc_mel_kernel");
+    rc = launch_mel(stream, g, B, t_max, T_out, t_ws, l.tab, l.spec, l.wts, l.range, features, l.sums);
+    if (rc) return rc;
     mfsc_scan_kernel<<<B, kScanThreads, 0, stream>>>(t_ws, l.tab, l.sums);
     W2L_LAUNCH_CHECK("mfsc_scan_kernel");
   }

@@ -698,7 +698,7 @@ int choose_bn(int mode, bool a_mn, bool b_mn, int M, int N, int total_kb, bool p
 
 int gemm_impl(void* stream_, int mode, int a_mn_major, int b_mn_major, int M, int N, int K, const void* A, int lda, const void* B, int ldb,
               void* C, int ldc, int c_bf16, const float* bias, int act, int accumulate, const void* aux, int ld_aux, int aux_bf16,
-              int aux_mode, float aux_scale, float dropout_p, unsigned long long seed, bool allow_overlap) {
+              int aux_mode, float aux_scale, float dropout_p, unsigned long long seed, bool allow_overlap, bool allow_split_k = true) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (mode != kTf32 && mode != kF32x3 && mode != kBf16 && mode != kF32x3SplitB) return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: unknown operand kind");
   if (mode == kF32x3SplitB && b_mn_major) return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: F32X3_SPLIT_B takes K-major B planes");
@@ -720,7 +720,7 @@ int gemm_impl(void* stream_, int mode, int a_mn_major, int b_mn_major, int M, in
   const int total_kb = (K + bke - 1) / bke;
   const bool plain = act == 0 && aux_mode == 0 && dropout_p == 0.f && bias == nullptr && !c_bf16;
   int splits = 1;
-  const int BN = choose_bn(mode, a_mn_major != 0, b_mn_major != 0, M, N, total_kb, plain, &splits);
+  const int BN = choose_bn(mode, a_mn_major != 0, b_mn_major != 0, M, N, total_kb, plain && allow_split_k, &splits);
   const bool raw = a_in_regs(mode, a_mn_major != 0, b_mn_major != 0);
   const bool bf16 = mode == kBf16;
   CUtensorMap ma, mb;
@@ -810,6 +810,13 @@ extern "C" int w2l_gemm(void* stream, int kind, int a_mn_major, int b_mn_major, 
                         int aux_bf16, int aux_mode, float aux_scale, float dropout_p, unsigned long long seed, int allow_overlap) {
   return gemm_impl(stream, kind, a_mn_major, b_mn_major, M, N, K, A, lda, B, ldb, C, ldc, c_bf16, bias, act, accumulate, aux, ld_aux, aux_bf16,
                    aux_mode, aux_scale, dropout_p, seed, allow_overlap != 0);
+}
+
+// C = A B^T with both operands K-major and overlapping A rows allowed, never split along K: every row of C is then the
+// same sum in the same order whatever M is (the streaming front end's DFT, whose M depends on the other streams)
+int w2l::gemm_view_unsplit(cudaStream_t stream, int kind, int M, int N, int K, const float* A, int lda, const float* B, int ldb, float* C,
+                           int ldc) {
+  return gemm_impl(stream, kind, 0, 0, M, N, K, A, lda, B, ldb, C, ldc, 0, nullptr, 0, 0, nullptr, 0, 0, 0, 1.f, 0.f, 0ull, true, false);
 }
 
 extern "C" int w2l_gemm_tf32_ex(void* stream_, int a_mn_major, int b_mn_major, int M, int N, int K, const float* A, int lda,

@@ -26,7 +26,6 @@
 #include "w2l_b200.h"
 
 namespace w2l {
-int fail(int code, const std::string& msg);
 void check(int rc);
 
 namespace streaming {
@@ -113,20 +112,6 @@ Arch parseArch(const std::string& archText, int nFeat, int nLabel) {
 using namespace w2l::streaming;
 
 namespace {
-template <typename F>
-int guarded(F&& f) {
-  try {
-    f();
-    return W2L_OK;
-  } catch (const std::invalid_argument& e) {
-    return w2l::fail(W2L_ERR_INVALID_ARGUMENT, e.what());
-  } catch (const std::exception& e) {
-    return w2l::fail(W2L_ERR_CUDA, e.what());
-  }
-}
-void cuda(cudaError_t e, const char* what) {
-  if (e != cudaSuccess) throw std::runtime_error(std::string(what) + ": " + cudaGetErrorString(e));
-}
 long long up4(long long n) { return (n + 3) / 4 * 4; }
 long long up8(long long n) { return (n + 7) / 8 * 8; }
 

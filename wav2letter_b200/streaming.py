@@ -1,4 +1,5 @@
-"""Python handle on the streaming acoustic model (w2l_stream_* in include/w2l_b200.h).
+"""Python handles on the streaming acoustic model (w2l_stream_* in include/w2l_b200.h) and on its MFSC front end
+(StreamingFeatures, w2l_mfsc_stream_*), whose features StreamingAM.run takes as they come.
 
 A trained streaming TDS network run chunk by chunk over many concurrent streams, as the in-tree inference library
 runs it.  Per stream, the emissions of every `run` and of `finish`, put end to end, do not change by a bit with the
@@ -78,6 +79,62 @@ class StreamingAM:
     def close(self):
         if getattr(self, "h", None):
             lib.w2l_stream_destroy(self.h)
+            self.h = None
+
+    __del__ = close
+
+
+class StreamingFeatures:
+    def __init__(self, max_streams: int, max_chunk_samples: int, n_filters: int = 80, left_ctx: int = 300, sample_rate: int = 16000,
+                 frame_ms: int = 25, stride_ms: int = 10):
+        """MFSC front end (w2l_mfsc_stream_*) for `max_streams` slots and chunks of at most `max_chunk_samples` samples
+        (at most 65535), normalised over the last `left_ctx` frames and the current one (`--localnrmlleftctx`, >= 1).
+        Its features are what StreamingAM(trainer, n, max_chunk=self.max_frames_out).run takes."""
+        h = lib.w2l_mfsc_stream_create(_stream(), int(max_streams), int(max_chunk_samples), int(sample_rate), int(frame_ms), int(stride_ms),
+                                       int(n_filters), int(left_ctx))
+        if not h:
+            raise capi.W2LError(1, lib.w2l_last_error().decode())
+        self.h = ctypes.c_void_p(h)
+        self.max_streams, self.max_chunk_samples, self.n_filters = int(max_streams), int(max_chunk_samples), int(n_filters)
+        self.sample_rate, self.frame_ms, self.stride_ms, self.left_ctx = int(sample_rate), int(frame_ms), int(stride_ms), int(left_ctx)
+        self.max_frames_out = int(lib.w2l_mfsc_stream_max_frames_out(self.h))
+
+    @property
+    def state_bytes(self) -> int:
+        """device bytes of carried state per slot"""
+        return int(lib.w2l_mfsc_stream_state_bytes(self.h))
+
+    def start(self, slots):
+        """reset the slots; a running slot forgets its past"""
+        _check(lib.w2l_mfsc_stream_start(self.h, _stream(), len(slots), _ints(slots)))
+
+    def run(self, slots, audio: torch.Tensor | None, samples=None, finish: bool = False):
+        """audio: CUDA float [n,Sc] contiguous (w2l_mfsc's sample scale), samples: new samples per stream (default Sc).
+        Returns (features [n,1,F,Tf], frames list) with Tf = max(frames); frames t >= frames[i] of stream i are 0."""
+        n = len(slots)
+        if audio is None:
+            Sc, aptr = 0, None
+            samples = [0] * n if samples is None else samples
+        else:
+            if not audio.is_cuda or audio.dtype != torch.float32 or not audio.is_contiguous() or audio.dim() != 2 or audio.shape[0] != n:
+                raise TypeError("audio must be a contiguous CUDA float32 tensor [n,Sc]")
+            Sc, aptr = int(audio.shape[1]), _ptr(audio)
+            samples = [Sc] * n if samples is None else samples
+        cap = n * self.n_filters * self.max_frames_out
+        out = torch.empty(max(cap, 1), dtype=torch.float32, device="cuda")
+        fo = (ctypes.c_int * n)()
+        _check(lib.w2l_mfsc_stream_run(self.h, _stream(), n, _ints(slots), _ints(samples), aptr, Sc, int(finish), _ptr(out), cap, fo))
+        frames = list(fo)
+        tf = max(frames) if frames else 0
+        return out[: n * self.n_filters * tf].view(n, 1, self.n_filters, tf), frames
+
+    def finish(self, slots, audio: torch.Tensor | None = None, samples=None):
+        """run the last chunk (may be None) and drop the remainder; the slots stay finished until the next start"""
+        return self.run(slots, audio, samples, finish=True)
+
+    def close(self):
+        if getattr(self, "h", None):
+            lib.w2l_mfsc_stream_destroy(self.h)
             self.h = None
 
     __del__ = close
