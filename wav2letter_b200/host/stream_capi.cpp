@@ -115,12 +115,6 @@ namespace {
 long long up4(long long n) { return (n + 3) / 4 * 4; }
 long long up8(long long n) { return (n + 7) / 8 * 8; }
 
-struct PrecisionScope {  // the runtime's precision for the duration of one call; the thread's own setting is restored
-  int saved;
-  explicit PrecisionScope(int p) : saved(w2l_get_precision()) { w2l_set_precision(p); }
-  ~PrecisionScope() { w2l_set_precision(saved); }
-};
-
 // a Linear layer's weight as the B operand of the forward GEMM in the runtime's precision, made once at create exactly
 // as fl::Linear makes it per call: TF32 the fp32 rows ([nout][K], K = nin padded to 4 floats), F32 the pre-split
 // tf32 hi / lo planes of those rows, BF16 the rows cast to bf16 ([nout][nin padded to 8])
@@ -130,26 +124,24 @@ struct DenseWeight {
   const float* bias = nullptr;
 };
 
-struct Slot {
-  int status = 0;  // 0 never started, 1 running, 2 finished
-  int plane = 0;   // the state plane holding the current tails
-  std::vector<int> tails;  // per convolution
-};
+// the state buffers of an arch: one per convolution (the C2 layers and the convolution of each TDS block), in order
+std::vector<ConvBuffer> convBuffers(const Arch& arch) {
+  std::vector<ConvBuffer> b;
+  for (const Layer& l : arch.layers)
+    if (l.op == Op::Conv || l.op == Op::Tds) b.push_back({l.cin * arch.W, l.kw, l.stride, l.padL, l.padR});
+  return b;
+}
 
 struct Stream {
   Arch arch;
-  int nFeat = 0, nLabel = 0, precision = 0, maxStreams = 0, maxChunk = 0;
-  std::vector<int> convOf;         // layer -> index among the convolutions (-1 for other layers)
+  int nFeat = 0, nLabel = 0, precision = 0, maxChunk = 0;
   std::vector<size_t> paramBase;   // layer -> index of its first parameter
-  std::vector<int> padL;           // per convolution: the zero frames start puts in front
-  std::vector<long long> stateOff;  // per convolution: offset of its region inside a plane
-  long long planeFloats = 0;
-  std::vector<char*> blocks;  // cudaMalloc'd
+  DeviceBlocks mem{"stream"};
+  SlotTable slots;            // one buffer per convolution
   float* snapshot = nullptr;  // parameter copy
   std::vector<const float*> params;  // per parameter, into snapshot
   std::vector<DenseWeight> dense;    // per Linear (TDS blocks: two)
   std::vector<int> denseOf;          // layer -> first index into dense (-1)
-  float* state = nullptr;
   float* xT = nullptr;  // [n][Tc][nFeat]
   float* win = nullptr;
   float* act[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -159,74 +151,7 @@ struct Stream {
   void* convWs = nullptr;
   size_t convWsBytes = 0;
   int maxOut = 0;  // bound on the output frames of one call
-  std::vector<Slot> slots;
-
-  ~Stream() {
-    for (char* b : blocks) cudaFree(b);
-  }
-  template <typename T>
-  T* alloc(size_t n) {
-    char* p = nullptr;
-    cuda(cudaMalloc(&p, std::max<size_t>(n * sizeof(T), 256)), "stream: cudaMalloc");
-    blocks.push_back(p);
-    return reinterpret_cast<T*>(p);
-  }
-  long long slotFloats() const { return 2 * planeFloats; }
 };
-
-// frames of every layer of one call: per convolution and stream the buffer rule, per layer the padded batch
-struct Plan {
-  std::vector<std::vector<int>> fresh, out, tails;  // [conv][stream]
-  std::vector<int> winFrames, outFrames;            // [conv]: longest window, longest output (the padded batch)
-  std::vector<int> framesOut;                       // [stream]
-  int tOutMax = 0;
-};
-Plan plan(const Arch& arch, int n, const std::vector<std::vector<int>>& tails, const int* framesIn, bool finish) {
-  Plan p;
-  std::vector<int> cur(framesIn, framesIn + n);
-  int ci = 0;
-  for (const Layer& l : arch.layers) {
-    if (l.op != Op::Conv && l.op != Op::Tds) continue;
-    p.fresh.push_back(cur);
-    std::vector<int> o(n), t(n);
-    int wmax = 0, omax = 0;
-    for (int i = 0; i < n; ++i) {
-      const ConvStep s = convStep(tails[ci][i], cur[i], finish ? l.padR : 0, l.kw, l.stride);
-      o[i] = s.nOut;
-      t[i] = s.tail;
-      wmax = std::max(wmax, s.avail);
-      omax = std::max(omax, s.nOut);
-    }
-    p.out.push_back(o);
-    p.tails.push_back(t);
-    p.winFrames.push_back(wmax);
-    p.outFrames.push_back(omax);
-    cur = o;
-    ++ci;
-  }
-  p.framesOut = cur;
-  p.tOutMax = n ? *std::max_element(cur.begin(), cur.end()) : 0;
-  return p;
-}
-
-Stream* asStream(void* h) {
-  if (!h) throw std::invalid_argument("stream: null handle");
-  return static_cast<Stream*>(h);
-}
-
-void checkSlots(const Stream* s, int n, const int* slots, bool forRun) {
-  if (n <= 0 || n > s->maxStreams) throw std::invalid_argument("stream: n must be in [1, max_streams]");
-  if (!slots) throw std::invalid_argument("stream: null slot list");
-  std::vector<char> seen(s->maxStreams, 0);
-  for (int i = 0; i < n; ++i) {
-    const int k = slots[i];
-    if (k < 0 || k >= s->maxStreams) throw std::invalid_argument("stream: slot " + std::to_string(k) + " out of range [0, max_streams)");
-    if (seen[k]) throw std::invalid_argument("stream: slot " + std::to_string(k) + " listed twice in one call");
-    seen[k] = 1;
-    if (forRun && s->slots[k].status == 0) throw std::invalid_argument("stream: run on slot " + std::to_string(k) + ", which is not started");
-    if (forRun && s->slots[k].status == 2) throw std::invalid_argument("stream: run on slot " + std::to_string(k) + ", which is finished (start it again)");
-  }
-}
 
 // C[M][nout] = act(A[M][nin] W^T + bias) on the GEMM, A prepared as fl::Linear prepares it
 void dense(Stream* s, cudaStream_t st, const DenseWeight& w, long long M, const float* A, float* C, int act) {
@@ -260,28 +185,28 @@ W2L_API int w2l_stream_plan(const char* arch_text, int n_feat, int n_label, int 
   return guarded([&] {
     if (!arch_text || n_feat <= 0 || n_label <= 0 || n_calls < 0 || (n_calls && !frames_host) || !n_convs)
       throw std::invalid_argument("stream_plan: bad arguments");
-    const Arch arch = parseArch(arch_text, n_feat, n_label);
-    std::vector<const Layer*> convs;
-    for (const Layer& l : arch.layers)
-      if (l.op == Op::Conv || l.op == Op::Tds) convs.push_back(&l);
+    const std::vector<ConvBuffer> convs = convBuffers(parseArch(arch_text, n_feat, n_label));
     *n_convs = (int)convs.size();
     if ((int)convs.size() > max_convs) throw std::invalid_argument("stream_plan: more convolutions than max_convs");
     for (size_t c = 0; c < convs.size() && conv_spec_host; ++c) {
-      conv_spec_host[4 * c] = convs[c]->kw;
-      conv_spec_host[4 * c + 1] = convs[c]->stride;
-      conv_spec_host[4 * c + 2] = convs[c]->padL;
-      conv_spec_host[4 * c + 3] = convs[c]->padR;
+      conv_spec_host[4 * c] = convs[c].kw;
+      conv_spec_host[4 * c + 1] = convs[c].stride;
+      conv_spec_host[4 * c + 2] = convs[c].padL;
+      conv_spec_host[4 * c + 3] = convs[c].padR;
     }
-    std::vector<std::vector<int>> tails(convs.size(), std::vector<int>(1));
-    for (size_t c = 0; c < convs.size(); ++c) tails[c][0] = convs[c]->padL;
+    // one slot of the runtime's own table, without a device
+    SlotTable table("stream_plan", 1, convs);
+    const int slot = 0;
+    table.start(1, &slot);
     for (int k = 0; k < n_calls; ++k) {
       if (frames_host[k] < 0) throw std::invalid_argument("stream_plan: negative frame count");
-      const Plan p = plan(arch, 1, tails, frames_host + k, finish_last && k == n_calls - 1);
+      const Plan p = table.plan(1, &slot, frames_host + k, finish_last && k == n_calls - 1);
       for (size_t c = 0; c < convs.size(); ++c) {
         if (frames_out_host) frames_out_host[(size_t)k * max_convs + c] = p.out[c][0];
         if (tails_host) tails_host[(size_t)k * max_convs + c] = p.tails[c][0];
-        tails[c][0] = p.tails[c][0];
       }
+      int framesOut;
+      table.commit(p, &framesOut);
     }
   });
 }
@@ -290,23 +215,22 @@ W2L_API void* w2l_stream_create(void* trainer, void* stream, int max_streams, in
   Stream* out = nullptr;
   guarded([&] {
     if (!trainer) throw std::invalid_argument("stream_create: null trainer");
-    if (max_streams <= 0 || max_streams > kMaxCallStreams)
-      throw std::invalid_argument("stream_create: max_streams must be in [1, " + std::to_string(kMaxCallStreams) + "]");
+    checkMaxStreams("stream", max_streams);
     if (max_chunk <= 0 || max_chunk > 32767) throw std::invalid_argument("stream_create: max_chunk must be in [1, 32767] frames");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const TrainerSnapshotSource src = trainerSnapshotSource(trainer);
     auto s = std::make_unique<Stream>();
     s->arch = parseArch(src.arch, src.nFeat, src.nLabel);
+    s->slots = SlotTable("stream", max_streams, convBuffers(s->arch));
     s->nFeat = src.nFeat;
     s->nLabel = src.nLabel;
     s->precision = w2l_get_precision();  // the creating thread's setting, as for the trainer
-    s->maxStreams = max_streams;
     s->maxChunk = max_chunk;
     const int W = src.nFeat;
     // parameters: one copy, so training can go on while streams run
     long long total = 0;
     for (const auto& p : src.params) total += up4(p.second);
-    s->snapshot = s->alloc<float>((size_t)total);
+    s->snapshot = s->mem.alloc<float>((size_t)total);
     {
       long long off = 0;
       for (const auto& p : src.params) {
@@ -331,7 +255,7 @@ W2L_API void* w2l_stream_create(void* trainer, void* stream, int max_streams, in
       d.bias = b;
       if (kind == W2L_GEMM_BF16) {
         d.K = (int)up8(nin);
-        void* wb = s->alloc<uint16_t>((size_t)nout * d.K);
+        void* wb = s->mem.alloc<uint16_t>((size_t)nout * d.K);
         if (d.K == nin)
           w2l::check(w2l_cast_bf16(st, (long long)nout * nin, w, wb));
         else
@@ -341,14 +265,14 @@ W2L_API void* w2l_stream_create(void* trainer, void* stream, int max_streams, in
         d.K = (int)up4(nin);
         const float* rows = w;
         if (d.K != nin) {
-          float* p = s->alloc<float>((size_t)nout * d.K);
+          float* p = s->mem.alloc<float>((size_t)nout * d.K);
           cuda(cudaMemsetAsync(p, 0, sizeof(float) * (size_t)nout * d.K, st), "stream: pad weight");
           cuda(cudaMemcpy2DAsync(p, sizeof(float) * d.K, w, sizeof(float) * nin, sizeof(float) * nin, (size_t)nout, cudaMemcpyDeviceToDevice, st),
                "stream: pad weight");
           rows = p;
         }
         if (kind == W2L_GEMM_F32X3_SPLIT_B) {
-          float* planes = s->alloc<float>((size_t)2 * nout * d.K);
+          float* planes = s->mem.alloc<float>((size_t)2 * nout * d.K);
           w2l::check(w2l_split_tf32(st, 0, nout, d.K, d.K, d.K, rows, planes));
           d.B = planes;
         } else {
@@ -359,25 +283,20 @@ W2L_API void* w2l_stream_create(void* trainer, void* stream, int max_streams, in
     };
     int fresh = max_chunk, feat = W;  // most new frames a layer can receive; floats per frame
     long long maxAct = 1, maxWin = 1, maxHidden = 1, maxOpA = 1, maxFrames = 1;  // per stream
-    size_t ws = 0;
+    size_t ws = 0, ci = 0;
     for (size_t li = 0; li < s->arch.layers.size(); ++li) {
       const Layer& l = s->arch.layers[li];
-      s->convOf.push_back(-1);
       s->denseOf.push_back(-1);
       s->paramBase.push_back(pi);
       if (l.op == Op::Conv || l.op == Op::Tds) {
         if (feat != l.cin * W) throw std::invalid_argument("stream_create: a convolution does not take the frames the layer before it makes");
-        s->convOf.back() = (int)s->stateOff.size();
-        s->stateOff.push_back(s->planeFloats);
-        s->padL.push_back(l.padL);
-        s->planeFloats += up4((long long)maxTail(l) * feat);
-        const int win = maxTail(l) + fresh + l.padR;
-        const int outF = win >= l.kw ? (win - l.kw) / l.stride + 1 : 0;
-        maxWin = std::max(maxWin, (long long)win * feat);
-        ws = std::max(ws, w2l_conv_time_workspace_size(max_streams, std::max(outF, 1), l.cin, l.cout, l.kw));
+        const ConvBuffer& b = s->slots.buffers()[ci++];
+        const ConvStep most = convStep(maxTail(b), fresh, b.padR, b.kw, b.stride);  // the longest window
+        maxWin = std::max(maxWin, (long long)most.avail * feat);
+        ws = std::max(ws, w2l_conv_time_workspace_size(max_streams, std::max(most.nOut, 1), l.cin, l.cout, l.kw));
         next((long long)l.cout * l.cin * l.kw);
         next(l.cout);
-        fresh = outF;
+        fresh = most.nOut;
         feat = l.cout * W;
         maxFrames = std::max(maxFrames, (long long)fresh);
         if (l.op == Op::Tds) {
@@ -410,23 +329,21 @@ W2L_API void* w2l_stream_create(void* trainer, void* stream, int max_streams, in
       maxAct = std::max(maxAct, (long long)fresh * feat);
     }
     if (pi != src.params.size()) throw std::runtime_error("export: parameters left over after walking the arch");
-    if (s->stateOff.empty()) throw std::invalid_argument("stream_create: the arch has no convolution, nothing to stream");
+    if (ci == 0) throw std::invalid_argument("stream_create: the arch has no convolution, nothing to stream");
     if (feat != src.nLabel) throw std::invalid_argument("stream_create: the last layer does not produce NLABEL values per frame");
     s->maxOut = fresh;
     // state and per-call buffers, all up front
-    s->state = s->alloc<float>((size_t)max_streams * (size_t)s->slotFloats());
-    s->xT = s->alloc<float>((size_t)max_streams * max_chunk * W);
-    s->win = s->alloc<float>((size_t)max_streams * maxWin);
-    for (auto& a : s->act) a = s->alloc<float>((size_t)max_streams * maxAct);
-    s->hidden = s->alloc<float>((size_t)max_streams * maxHidden);
-    s->opA = s->alloc<float>((size_t)max_streams * maxOpA);
+    s->slots.state = s->mem.alloc<float>((size_t)max_streams * (size_t)s->slots.slotFloats());
+    s->xT = s->mem.alloc<float>((size_t)max_streams * max_chunk * W);
+    s->win = s->mem.alloc<float>((size_t)max_streams * maxWin);
+    for (auto& a : s->act) a = s->mem.alloc<float>((size_t)max_streams * maxAct);
+    s->hidden = s->mem.alloc<float>((size_t)max_streams * maxHidden);
+    s->opA = s->mem.alloc<float>((size_t)max_streams * maxOpA);
     const long long rows = (long long)max_streams * maxFrames;
-    s->meanRstd = s->alloc<float>((size_t)(2 * rows));
+    s->meanRstd = s->mem.alloc<float>((size_t)(2 * rows));
     s->convWsBytes = std::max<size_t>(ws, 256);
-    s->convWs = s->alloc<char>(s->convWsBytes);
-    s->slots.resize(max_streams);
-    for (auto& sl : s->slots) sl.tails.assign(s->stateOff.size(), 0);
-    cuda(cudaMemsetAsync(s->state, 0, sizeof(float) * (size_t)max_streams * (size_t)s->slotFloats(), st), "stream: state");
+    s->convWs = s->mem.alloc<char>(s->convWsBytes);
+    cuda(cudaMemsetAsync(s->slots.state, 0, sizeof(float) * (size_t)max_streams * (size_t)s->slots.slotFloats(), st), "stream: state");
     cuda(cudaStreamSynchronize(st), "stream_create");
     out = s.release();
   });
@@ -437,7 +354,7 @@ W2L_API void w2l_stream_destroy(void* h) { delete static_cast<Stream*>(h); }
 
 W2L_API long long w2l_stream_state_bytes(void* h) {
   if (!h) return -1;
-  return (long long)sizeof(float) * static_cast<Stream*>(h)->slotFloats();
+  return (long long)sizeof(float) * static_cast<Stream*>(h)->slots.slotFloats();
 }
 
 W2L_API int w2l_stream_max_frames_out(void* h) {
@@ -447,24 +364,19 @@ W2L_API int w2l_stream_max_frames_out(void* h) {
 
 W2L_API int w2l_stream_start(void* h, void* stream, int n, const int* slots) {
   return guarded([&] {
-    Stream* s = asStream(h);
-    checkSlots(s, n, slots, false);
-    w2l::check(launchZeroSlots(stream, s->state, s->slotFloats(), n, slots));
-    for (int i = 0; i < n; ++i) {
-      Slot& sl = s->slots[slots[i]];
-      sl.status = 1;
-      sl.plane = 0;
-      sl.tails = s->padL;  // left padding: zero frames held before the first input frame
-    }
+    Stream* s = handleOf<Stream>(h, "stream");
+    s->slots.check(n, slots, false);
+    w2l::check(launchZeroSlots(stream, s->slots.state, s->slots.slotFloats(), n, slots));
+    s->slots.start(n, slots);
   });
 }
 
 W2L_API int w2l_stream_run(void* h, void* stream, int n, const int* slots, const int* frames_in, const float* features, int Tc, int finish,
                            float* emissions, long long capacity, int* frames_out) {
   return guarded([&] {
-    Stream* s = asStream(h);
+    Stream* s = handleOf<Stream>(h, "stream");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    checkSlots(s, n, slots, true);
+    s->slots.check(n, slots, true);
     if (!frames_in || !frames_out) throw std::invalid_argument("stream_run: null frame-count array");
     if (Tc < 0 || Tc > s->maxChunk) throw std::invalid_argument("stream_run: Tc must be in [0, max_chunk]");
     int most = 0;
@@ -475,11 +387,7 @@ W2L_API int w2l_stream_run(void* h, void* stream, int n, const int* slots, const
     }
     if (most > 0 && !features) throw std::invalid_argument("stream_run: null features");
     const int W = s->nFeat;
-    const size_t nc = s->stateOff.size();
-    std::vector<std::vector<int>> tails(nc, std::vector<int>(n));
-    for (size_t c = 0; c < nc; ++c)
-      for (int i = 0; i < n; ++i) tails[c][i] = s->slots[slots[i]].tails[c];
-    const Plan p = plan(s->arch, n, tails, frames_in, finish != 0);
+    const Plan p = s->slots.plan(n, slots, frames_in, finish != 0);
     if ((long long)n * p.tOutMax * s->nLabel > capacity) throw std::invalid_argument("stream_run: emission buffer too small (capacity)");
     if (p.tOutMax > 0 && !emissions) throw std::invalid_argument("stream_run: null emissions");
     PrecisionScope scope(s->precision);
@@ -494,32 +402,14 @@ W2L_API int w2l_stream_run(void* h, void* stream, int n, const int* slots, const
       throw std::logic_error("stream: no free activation buffer");
     };
     const auto& layers = s->arch.layers;
+    size_t ci = 0;  // the convolution's index among the state buffers
     for (size_t li = 0; li < layers.size(); ++li) {
       const Layer& l = layers[li];
       const int feat = l.curC * W;
       if (l.op == Op::Conv || l.op == Op::Tds) {
-        const int c = s->convOf[li];
-        const int win = p.winFrames[c], tout = p.outFrames[c];
-        if (win > 0) {
-          WindowArgs a;
-          a.in = cur;
-          a.win = s->win;
-          a.state = s->state + s->stateOff[c];
-          a.slotFloats = s->slotFloats();
-          a.planeFloats = s->planeFloats;
-          a.inFrames = curFrames;
-          a.winFrames = win;
-          a.F = feat;
-          a.kw = l.kw;
-          a.stride = l.stride;
-          a.padR = finish ? l.padR : 0;
-          a.n = n;
-          for (int i = 0; i < n; ++i) {
-            a.code[i] = slots[i] << 1 | s->slots[slots[i]].plane;
-            a.cnt[i] = tails[c][i] << 16 | p.fresh[c][i];
-          }
-          w2l::check(launchWindow(st, a));
-        }
+        const int win = p.winFrames[ci], tout = p.outFrames[ci];
+        if (win > 0) w2l::check(launchWindow(st, s->slots.window(p, ci, cur, curFrames, s->win, win)));
+        ++ci;
         live = tout > 0;
         curFrames = tout;
         if (!live) continue;
@@ -575,13 +465,7 @@ W2L_API int w2l_stream_run(void* h, void* stream, int n, const int* slots, const
     }
     if (live && cur != emissions)
       cuda(cudaMemcpyAsync(emissions, cur, sizeof(float) * (size_t)n * p.tOutMax * s->nLabel, cudaMemcpyDeviceToDevice, st), "stream: emissions");
-    for (int i = 0; i < n; ++i) {
-      Slot& sl = s->slots[slots[i]];
-      for (size_t c = 0; c < nc; ++c) sl.tails[c] = p.tails[c][i];
-      sl.plane ^= 1;
-      if (finish) sl.status = 2;
-      frames_out[i] = p.framesOut[i];
-    }
+    s->slots.commit(p, frames_out);
   });
 }
 

@@ -1,9 +1,12 @@
 // stream_internal.h — pieces shared by the streaming acoustic-model runtime (stream_capi.cpp), its state kernel
 // (csrc/stream_kernels.cu), the export of trainer_capi.cpp and the streaming MFSC front end (mfsc_stream_capi.cpp,
-// csrc/features.cu).  Not part of the C ABI.
+// csrc/features.cu).  Both streaming runtimes keep their slots in one SlotTable (stream_slots.cpp): the call checks,
+// start, the buffer rule of every call and the commit after it are written once, and each runtime declares its state
+// buffers (the acoustic model one per convolution, the front end one for its samples).  Not part of the C ABI.
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <stdexcept>
 #include <string>
 #include <utility>
@@ -32,6 +35,33 @@ int guarded(F&& f) {
 inline void cuda(cudaError_t e, const char* what) {
   if (e != cudaSuccess) throw std::runtime_error(std::string(what) + ": " + cudaGetErrorString(e));
 }
+struct PrecisionScope {  // a handle's precision for the duration of one call; the thread's own setting is restored
+  int saved;
+  explicit PrecisionScope(int p) : saved(w2l_get_precision()) { w2l_set_precision(p); }
+  ~PrecisionScope() { w2l_set_precision(saved); }
+};
+
+// The device blocks a handle owns: cudaMalloc'd as it is created, freed with it.  `who` prefixes the error text.
+class DeviceBlocks {
+ public:
+  explicit DeviceBlocks(const char* who) : who_(who) {}
+  DeviceBlocks(const DeviceBlocks&) = delete;
+  DeviceBlocks& operator=(const DeviceBlocks&) = delete;
+  ~DeviceBlocks() {
+    for (char* b : blocks_) cudaFree(b);
+  }
+  template <typename T>
+  T* alloc(size_t n) {
+    char* p = nullptr;
+    cuda(cudaMalloc(&p, std::max<size_t>(n * sizeof(T), 256)), (std::string(who_) + ": cudaMalloc").c_str());
+    blocks_.push_back(p);
+    return reinterpret_cast<T*>(p);
+  }
+
+ private:
+  const char* who_;
+  std::vector<char*> blocks_;
+};
 
 // One layer of a streaming TDS arch as the in-tree inference library runs it (the order and the parameter use of
 // w2l_trainer_export_streaming).  V / RO / DO / SAUG are dropped: in eval mode they are relabellings or identities.
@@ -51,19 +81,6 @@ struct Arch {
 };
 // Walks the arch text with the export's checks and error text (std::invalid_argument / std::logic_error).
 Arch parseArch(const std::string& archText, int nFeat, int nLabel);
-
-// The buffer rule of one convolution (inference/module/nn/backend/fbgemm/Conv1dFbGemm.cpp): `tail` frames are held,
-// `fresh` arrive, `padR` zero frames follow on finish.  nOut frames come out, nOut * stride are consumed.
-struct ConvStep {
-  int avail, nOut, tail;
-};
-inline ConvStep convStep(int tail, int fresh, int padR, int kw, int stride) {
-  const int avail = tail + fresh + padR;
-  const int nOut = avail >= kw ? (avail - kw) / stride + 1 : 0;
-  return {avail, nOut, avail - nOut * stride};
-}
-// frames a convolution may hold between calls: the left padding after start, at most kw - 1 afterwards
-inline int maxTail(const Layer& l) { return l.padL > l.kw - 1 ? l.padL : l.kw - 1; }
 
 // what the stream runtime needs of a trainer: the arch, the sizes, the precision and the parameters in module order
 struct TrainerSnapshotSource {
@@ -87,6 +104,84 @@ struct WindowArgs {
 int launchWindow(void* stream, const WindowArgs& a);
 // zero both planes of the n slots' state (slotFloats each): start
 int launchZeroSlots(void* stream, float* state, long long slotFloats, int n, const int* slots);
+
+// ---- the slot model of both streaming runtimes (host/stream_slots.cpp) -----------------------------------------
+// One state buffer: a convolution's input frames of F floats, held under the buffer rule of
+// inference/module/nn/backend/fbgemm/Conv1dFbGemm.cpp.  The acoustic model declares one per convolution; the MFSC
+// front end declares one for its samples (F = 1, kw = frame, stride = the frame stride, no padding), which is
+// LogMelFeature::run's rule.
+struct ConvBuffer {
+  int F = 1, kw = 1, stride = 1, padL = 0, padR = 0;
+};
+// `tail` frames are held, `fresh` arrive, `padR` zero frames follow on finish.  nOut frames come out, nOut * stride are
+// consumed.
+struct ConvStep {
+  int avail, nOut, tail;
+};
+inline ConvStep convStep(int tail, int fresh, int padR, int kw, int stride) {
+  const int avail = tail + fresh + padR;
+  const int nOut = avail >= kw ? (avail - kw) / stride + 1 : 0;
+  return {avail, nOut, avail - nOut * stride};
+}
+// frames a buffer may hold between calls: the left padding after start, at most kw - 1 afterwards
+inline int maxTail(const ConvBuffer& b) { return std::max(b.padL, b.kw - 1); }
+
+// The frames of one call through a runtime's buffers, in order: the frames one buffer's convolution puts out are the
+// next buffer's new frames.
+struct Plan {
+  int n = 0;
+  const int* slots = nullptr;
+  bool finish = false;
+  std::vector<std::vector<int>> fresh, out, tails;  // [buffer][stream]: new frames, output, tail after the call
+  std::vector<int> winFrames, outFrames;            // [buffer]: longest window, longest output (the padded batch)
+  std::vector<int> framesOut;                       // [stream]: the last buffer's output
+  int tOutMax = 0;
+};
+
+// The slots of one runtime: each slot's status, its plane bit and the host mirror of every buffer's held tail, so that
+// all frame counts are host arithmetic and a call neither reads from the device nor synchronises.  A slot's state is
+// two planes, one region of up4(maxTail * F) floats per buffer in each: a call reads the tails from one plane and writes
+// the new tails to the other.  The device work (zeroing on start, the window kernel) stays with the runtime.  `who`
+// prefixes the error text.
+class SlotTable {
+ public:
+  SlotTable() = default;
+  SlotTable(const char* who, int maxStreams, std::vector<ConvBuffer> buffers);
+  float* state = nullptr;  // [slot][2][planeFloats] on the device; the runtime allocates it
+
+  const std::vector<ConvBuffer>& buffers() const { return bufs_; }
+  long long slotFloats() const { return 2 * planeFloats_; }
+  // n in [1, max_streams], every slot in range and listed once; for run also started and not finished
+  void check(int n, const int* slots, bool forRun) const;
+  // running, plane 0, every buffer holding its left padding (zero frames before the first input frame)
+  void start(int n, const int* slots);
+  // framesIn[i] new frames for slots[i]; finish appends every buffer's right padding
+  Plan plan(int n, const int* slots, const int* framesIn, bool finish) const;
+  // buffer b's window kernel for the call: in = [n][inFrames][F] new frames, win = [n][winFrames][F]
+  WindowArgs window(const Plan& p, size_t b, const float* in, int inFrames, float* win, int winFrames) const;
+  // after the call: the new tails, the other plane, finished after finish; the output frames into framesOut[n]
+  void commit(const Plan& p, int* framesOut);
+
+ private:
+  struct Slot {
+    int status = 0;  // 0 never started, 1 running, 2 finished
+    int plane = 0;   // the plane holding the current tails
+    std::vector<int> tails;  // per buffer
+  };
+  std::string who_;
+  std::vector<ConvBuffer> bufs_;
+  std::vector<long long> off_;  // per buffer: its region inside a plane
+  long long planeFloats_ = 0;
+  std::vector<Slot> slots_;
+};
+// create's check of max_streams, with the text "<who>_create: max_streams must be in [1, kMaxCallStreams]"
+void checkMaxStreams(const char* who, int maxStreams);
+// a runtime's handle as its type; null is "<who>: null handle"
+template <typename H>
+H* handleOf(void* h, const char* who) {
+  if (!h) throw std::invalid_argument(std::string(who) + ": null handle");
+  return static_cast<H*>(h);
+}
 
 // ---- streaming MFSC front end (csrc/features.cu, host/mfsc_stream_capi.cpp) --------------------------------------
 struct MfscGeom {

@@ -78,23 +78,8 @@ struct GradStreamScope {
   }
 };
 
-struct PrecisionScope {  // the trainer's precision for the duration of one call; the thread's own setting is restored
-  int saved;
-  explicit PrecisionScope(int p) : saved(w2l_get_precision()) { w2l_set_precision(p); }
-  ~PrecisionScope() { w2l_set_precision(saved); }
-};
-
-template <typename F>
-int guarded(F&& f) {
-  try {
-    f();
-    return W2L_OK;
-  } catch (const std::invalid_argument& e) {
-    return w2l::fail(W2L_ERR_INVALID_ARGUMENT, e.what());
-  } catch (const std::exception& e) {
-    return w2l::fail(W2L_ERR_CUDA, e.what());
-  }
-}
+using w2l::streaming::guarded;
+using w2l::streaming::PrecisionScope;  // the trainer's precision for the duration of one call
 }  // namespace
 
 namespace {
