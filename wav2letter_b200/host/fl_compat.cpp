@@ -20,6 +20,7 @@
 #include <stdexcept>
 #include <unordered_set>
 
+#include "dense_operands.h"
 #include "w2l_b200.h"
 
 namespace w2l {
@@ -426,70 +427,18 @@ af::array workspaceFor(af::array& cache, size_t bytes) {
 thread_local af::array g_conv_ws;
 thread_local af::array g_conv_grad_ws;  // time-convolution weight gradients on the gradient stream
 
-// ---- precision of the dense contractions (w2l_set_precision; DESIGN.md §4) ----------------------------------
-bool bf16Mode() { return w2l_get_precision() == W2L_PRECISION_BF16; }
-int gemmKind() { return bf16Mode() ? W2L_GEMM_BF16 : (w2l_get_precision() == W2L_PRECISION_F32 ? W2L_GEMM_F32X3 : W2L_GEMM_TF32); }
-// operand rows are TMA rows: 16-byte multiples = 4 floats or 8 bf16; channel counts are carried padded to that
-int chanPad() { return bf16Mode() ? 8 : 4; }
-long long padUp(long long n, long long a) { return (n + a - 1) / a * a; }
-// rows of `cols` floats (row stride ld) -> [rows][colsP], zero-padded columns: fp32 copy, or bf16 in BF16 mode
-af::array padRowsF32(const float* x, long long rows, int cols, int ld, int colsP) {
-  af::array out = af::array::zeros(af::dim4(colsP, rows));
-  w2l::copyRows(out.f32(), sizeof(float) * (size_t)colsP, x, sizeof(float) * (size_t)ld, sizeof(float) * (size_t)cols, (size_t)rows);
-  return out;
-}
-af::array castRowsBf16(const float* x, long long rows, int cols, int ld, int colsP) {
-  af::array out = af::array::empty(af::dim4(colsP, rows), DType::bf16);
-  if (cols == colsP && ld == cols)
-    check(w2l_cast_bf16(currentStream(), rows * cols, x, out.ptr()));
-  else
-    check(w2l_cast_bf16_rows(currentStream(), rows, cols, ld, colsP, x, out.ptr()));
-  return out;
-}
-// GEMM operand in the thread's precision: the fp32 rows themselves when they are already TMA rows (TF32 / F32X3), a
-// zero-padded fp32 copy when not, a (padded) bf16 copy in BF16 mode.  `ld` out = row stride in elements.
-struct GemmOperand {
-  af::array a;
-  int ld = 0;
+// ---- dense-layer GEMM operands in the thread's precision (w2l_set_precision; host/dense_operands.h) -----------
+namespace dense = w2l::dense;
+int rowKind() { return dense::rowKind(w2l_get_precision()); }
+// the memory an operand is read from: its copy, or the source array when that serves as it is
+af::array operandMemory(size_t bytes, const af::array& src) { return bytes ? af::array::empty(af::dim4((long long)bytes), DType::u8) : src; }
+struct HeldOperand {
+  af::array mem;
+  dense::Operand op;
 };
-GemmOperand gemmOperand(const af::array& x, long long rows, int cols, int ld) {
-  GemmOperand op;
-  if (bf16Mode()) {
-    op.ld = (int)padUp(cols, 8);
-    op.a = castRowsBf16(x.f32(), rows, cols, ld, op.ld);
-  } else if (ld % 4 == 0 && (reinterpret_cast<uintptr_t>(x.ptr()) & 15) == 0) {
-    op.a = x;
-    op.ld = ld;
-  } else {
-    op.ld = (int)padUp(cols, 4);
-    op.a = padRowsF32(x.f32(), rows, cols, ld, op.ld);
-  }
-  return op;
-}
-int gemmP(int a_mn, int b_mn, int M, int N, int K, const GemmOperand& A, const GemmOperand& B, float* C, int ldc, const float* bias, int act,
-          int accumulate, const float* aux = nullptr, int ld_aux = 0, int aux_mode = 0, float aux_scale = 1.f, float dropP = 0.f,
-          unsigned long long seed = 0, int allowOverlap = 0) {
-  return w2l_gemm(currentStream(), gemmKind(), a_mn, b_mn, M, N, K, A.a.ptr(), A.ld, B.a.ptr(), B.ld, C, ldc, 0, bias, act, accumulate, aux, ld_aux, 0,
-                  aux_mode, aux_scale, dropP, seed, allowOverlap);
-}
-// A weight W as the B operand of gemmWeight: b_mn = 0, B = W [N][K] (forward); b_mn = 1, B = W^T with W [K][N] (data
-// gradient).  In F32 mode the weight is split once per call into tf32 hi / lo planes ([2][N][K padded to 4]), which the
-// kernel reads instead of converting W in every row of output tiles; in the other modes nothing is made (empty).
-GemmOperand weightPlanes(int b_mn, int N, int K, const GemmOperand& W) {
-  GemmOperand planes;
-  if (gemmKind() != W2L_GEMM_F32X3) return planes;
-  planes.ld = (int)padUp(K, 4);
-  planes.a = af::array::empty(af::dim4(planes.ld, N, 2));
-  check(w2l_split_tf32(currentStream(), b_mn, b_mn ? K : N, b_mn ? N : K, W.ld, planes.ld, W.a.f32(), planes.a.f32()));
-  return planes;
-}
-// gemmP with a weight as B (K-major A), from its planes when there are any: results are bit-identical either way
-int gemmWeight(int b_mn, int M, int N, int K, const GemmOperand& A, const GemmOperand& W, const GemmOperand& planes, float* C, int ldc,
-               const float* bias, int act, int accumulate, const float* aux = nullptr, int ld_aux = 0, int aux_mode = 0, float aux_scale = 1.f,
-               float dropP = 0.f, unsigned long long seed = 0) {
-  if (planes.a.isEmpty()) return gemmP(0, b_mn, M, N, K, A, W, C, ldc, bias, act, accumulate, aux, ld_aux, aux_mode, aux_scale, dropP, seed);
-  return w2l_gemm(currentStream(), W2L_GEMM_F32X3_SPLIT_B, 0, 0, M, N, K, A.a.ptr(), A.ld, planes.a.ptr(), planes.ld, C, ldc, 0, bias, act, accumulate,
-                  aux, ld_aux, 0, aux_mode, aux_scale, dropP, seed, 0);
+HeldOperand rowOperand(const af::array& x, long long rows, int cols, int zeroRows = 0) {
+  const af::array mem = operandMemory(dense::rowBytes(rowKind(), rows, cols, x.f32(), zeroRows), x);
+  return {mem, dense::rows(currentStream(), rowKind(), rows, cols, x.f32(), mem.ptr(), zeroRows)};
 }
 }  // namespace
 
@@ -507,7 +456,7 @@ Variable View::forward(const Variable& in) {
   // head of a conv_glu arch: `V -1 1 NFEAT 0` -> [T,1,F,B]: the features are CHANNELS (W = 1); same transposition
   if (dims_[1] == 1 && dims_[0] == -1 && dims_[2] > 1 && in.dims(2) == 1 && in.dims(1) == dims_[2]) {
     const long long T = in.dims(0), F = in.dims(1), B = in.dims(3);
-    if (F % chanPad()) throw std::invalid_argument("View: the channel-major head needs a feature count that is a multiple of 4 (8 in bf16 mode)");
+    if (F != dense::padRow(rowKind(), F)) throw std::invalid_argument("View: the channel-major head needs a feature count that is a multiple of 4 (8 in bf16 mode)");
     af::array out = af::array::empty(af::dim4(1, F, T, B));
     check(w2l_transpose_input(currentStream(), (int)B, (int)F, (int)T, in.array().f32(), out.f32()));
     return Variable(out, in.isCalcGrad());
@@ -556,7 +505,7 @@ Variable Conv2D::forwardWith(const Variable& in, const Variable& weight, const V
   requireInternal(in, "Conv2D");
   const int W = (int)in.dims(0), Cin = (int)in.dims(1), T = (int)in.dims(2), B = (int)in.dims(3);
   // W = 1 (`V -1 1 NFEAT 0` archs: features are channels): the large-channel GEMM path
-  if (W == 1 && (Cin == padUp(nIn, 4) || Cin == padUp(nIn, 8))) return forwardGemm(in, weight, biasVar);
+  if (W == 1 && (Cin == dense::padRow(W2L_GEMM_TF32, nIn) || Cin == dense::padRow(W2L_GEMM_BF16, nIn))) return forwardGemm(in, weight, biasVar);
   if (Cin != nIn) throw std::invalid_argument("Conv2D: input has " + std::to_string(Cin) + " channels, expected " + std::to_string(nIn));
   int pl, pr;
   if (explicitPad_) {
@@ -650,8 +599,8 @@ Variable Conv2D::forwardGemm(const Variable& in, const Variable& weight, const V
   // shrinks by kw-1 per layer and travels with the variable (validFrames); fl::Reorder drops the slack at the end.
   if (stride != 1) throw std::invalid_argument("Conv2D: the large-channel path covers stride 1 only");
   const int Cp = (int)in.dims(1), TsIn = (int)in.dims(2), B = (int)in.dims(3);
-  const int align = chanPad();
-  if (Cp % align) throw std::invalid_argument("Conv2D: the activation's channel padding does not match the precision mode (bf16 rows are multiples of 8 channels)");
+  const int kind = rowKind();
+  if (Cp != dense::padRow(kind, Cp)) throw std::invalid_argument("Conv2D: the activation's channel padding does not match the precision mode (bf16 rows are multiples of 8 channels)");
   const int TvIn = in.validFrames() >= 0 ? (int)in.validFrames() : TsIn;
   int pl, pr;
   if (explicitPad_) {
@@ -669,19 +618,17 @@ Variable Conv2D::forwardGemm(const Variable& in, const Variable& weight, const V
   if (Tout <= 0) throw std::invalid_argument("Conv2D: input shorter than the kernel");
   const bool glu = gluSplit_;
   if (glu && (nOut % 2)) throw std::invalid_argument("Conv2D: a GLU needs an even channel count");
-  const int CoutP = glu ? 2 * (int)padUp(nOut / 2, align) : (int)padUp(nOut, align);
+  const int CoutP = glu ? 2 * (int)dense::padRow(kind, nOut / 2) : (int)dense::padRow(kind, nOut);
   const int cin = nIn, cout = nOut, k = kw;
   const bool hasBias = hasBias_, relu = relu_;
   // GEMM operands of the weights, arranged once per step in the thread's precision (bf16 operands are written directly)
-  const DType wtype = bf16Mode() ? DType::bf16 : DType::f32;
-  GemmOperand fwdOp, flipOp;
-  fwdOp.a = af::array::empty(af::dim4((long long)k * Cp, CoutP), wtype);
-  fwdOp.ld = k * Cp;
-  flipOp.a = af::array::empty(af::dim4((long long)k * CoutP, Cp), wtype);
-  flipOp.ld = k * CoutP;
+  const bool bf16 = kind == W2L_GEMM_BF16;
+  const DType wtype = bf16 ? DType::bf16 : DType::f32;
+  af::array fwd = af::array::empty(af::dim4((long long)k * Cp, CoutP), wtype);
+  af::array flip = af::array::empty(af::dim4((long long)k * CoutP, Cp), wtype);
   af::array biasP = af::array::empty(af::dim4(CoutP));
   check(w2l_conv1d_arrange_ex(currentStream(), cin, cout, k, Cp, CoutP, glu ? 1 : 0, weight.array().f32(),
-                              hasBias ? biasVar.array().f32() : nullptr, fwdOp.a.ptr(), flipOp.a.ptr(), biasP.f32(), bf16Mode() ? 1 : 0));
+                              hasBias ? biasVar.array().f32() : nullptr, fwd.ptr(), flip.ptr(), biasP.f32(), bf16 ? 1 : 0));
   af::array xp = in.array();
   if (padded) {
     xp = af::array::zeros(af::dim4(1, Cp, Ts, B));
@@ -690,10 +637,11 @@ Variable Conv2D::forwardGemm(const Variable& in, const Variable& weight, const V
   const long long rowsAll = (long long)B * Ts, M = rowsAll - k + 1;  // output rows that have a full window in the buffer
   if (rowsAll > 0x7fffffffLL / 2) throw std::invalid_argument("Conv2D: batch too long for one GEMM");
   // operands in the thread's precision (bf16 copies in BF16 mode; the fp32 buffers themselves otherwise)
-  const GemmOperand xop = gemmOperand(xp, rowsAll, Cp, Cp);
+  const HeldOperand xop = rowOperand(xp, rowsAll, Cp);
   af::array y = af::array::empty(af::dim4(1, CoutP, Ts, B));
   cudaMemsetAsync(y.f32() + (size_t)M * CoutP, 0, sizeof(float) * (size_t)(k - 1) * CoutP, static_cast<cudaStream_t>(currentStream()));
-  check(gemmP(0, 0, (int)M, CoutP, k * Cp, xop, fwdOp, y.f32(), CoutP, biasP.f32(), relu ? 1 : 0, 0, nullptr, 0, 0, 1.f, 0.f, 0ull, 1));
+  check(dense::gemm(currentStream(), (int)M, CoutP, k * Cp, xop.op, {kind, fwd.ptr(), k * Cp}, y.f32(), CoutP, biasP.f32(), relu ? 1 : 0, 0, nullptr, 0,
+                    0, 1.f, 0.f, 0ull, 1));
   std::vector<Variable> inputs{in, weight};
   if (hasBias) inputs.push_back(biasVar);
   Variable out(y, inputs, [=](std::vector<Variable>& ins, const Variable& gout) {
@@ -706,8 +654,9 @@ Variable Conv2D::forwardGemm(const Variable& in, const Variable& weight, const V
     }
     if (ins[1].isCalcGrad()) {
       af::array dWarr = af::array::empty(af::dim4((long long)k * Cp, CoutP));
-      const GemmOperand dyop = gemmOperand(dy, rowsAll, CoutP, CoutP);
-      check(gemmP(1, 1, CoutP, k * Cp, (int)M, dyop, xop, dWarr.f32(), k * Cp, nullptr, 0, 0, nullptr, 0, 0, 1.f, 0.f, 0ull, 1));
+      const HeldOperand dyop = rowOperand(dy, rowsAll, CoutP);
+      check(w2l_gemm(currentStream(), kind, 1, 1, CoutP, k * Cp, (int)M, dyop.op.ptr, dyop.op.ld, xop.op.ptr, xop.op.ld, dWarr.f32(), k * Cp, 0, nullptr,
+                     0, 0, nullptr, 0, 0, 0, 1.f, 0.f, 0ull, 1));
       af::array dw = ins[1].gradStorage();
       if (dw.isEmpty()) dw = af::array::zeros(ins[1].dims());
       af::array db;
@@ -723,20 +672,10 @@ Variable Conv2D::forwardGemm(const Variable& in, const Variable& weight, const V
     if (ins[0].isCalcGrad()) {
       // dXp[m][ci] = sum_j dY[m - (kw-1) + j][..] Wflip: a copy of dY with kw-1 zero rows in front gives the view its
       // left context; a sample's first frames see the previous sample's slack rows, which are zero
-      GemmOperand dypOp;
-      dypOp.ld = CoutP;
-      if (bf16Mode()) {
-        dypOp.a = af::array::empty(af::dim4(CoutP, rowsAll + k - 1), DType::bf16);
-        cudaMemsetAsync(dypOp.a.ptr(), 0, 2 * (size_t)(k - 1) * CoutP, static_cast<cudaStream_t>(currentStream()));
-        check(w2l_cast_bf16(currentStream(), rowsAll * CoutP, dy.f32(), static_cast<char*>(dypOp.a.ptr()) + 2 * (size_t)(k - 1) * CoutP));
-      } else {
-        dypOp.a = af::array::empty(af::dim4(CoutP, rowsAll + k - 1));
-        cudaMemsetAsync(dypOp.a.ptr(), 0, sizeof(float) * (size_t)(k - 1) * CoutP, static_cast<cudaStream_t>(currentStream()));
-        w2l::copyRows(dypOp.a.f32() + (size_t)(k - 1) * CoutP, sizeof(float) * (size_t)rowsAll * CoutP, dy.f32(), sizeof(float) * (size_t)rowsAll * CoutP,
-                      sizeof(float) * (size_t)rowsAll * CoutP, 1);
-      }
+      const HeldOperand dypOp = rowOperand(dy, rowsAll, CoutP, k - 1);
       af::array dxp = af::array::empty(af::dim4(1, Cp, Ts, B));
-      check(gemmP(0, 0, (int)rowsAll, Cp, k * CoutP, dypOp, flipOp, dxp.f32(), Cp, nullptr, 0, 0, nullptr, 0, 0, 1.f, 0.f, 0ull, 1));
+      check(dense::gemm(currentStream(), (int)rowsAll, Cp, k * CoutP, dypOp.op, {kind, flip.ptr(), k * CoutP}, dxp.f32(), Cp, nullptr, 0, 0, nullptr, 0, 0,
+                        1.f, 0.f, 0ull, 1));
       if (Tv < Ts)  // gradients of slack input frames must not reach the previous layer
         cudaMemset2DAsync(dxp.f32() + (size_t)Tv * Cp, sizeof(float) * (size_t)Ts * Cp, 0, sizeof(float) * (size_t)(Ts - Tv) * Cp, (size_t)B,
                           static_cast<cudaStream_t>(currentStream()));
@@ -1041,7 +980,7 @@ Variable Linear::forwardWith(const Variable& in, const Variable& weight, const V
     throw std::invalid_argument("Linear: the input carries slack frames (large-channel convolutions); a Reorder must come first");
   // input rows: nIn features, or nIn features followed by the zero channels the large-channel convolutions carry
   // (channel counts padded to 4 floats / 8 bf16)
-  auto isPadded = [&](long long c) { return c == nIn || (c > nIn && (c == padUp(nIn, 4) || c == padUp(nIn, 8))); };
+  auto isPadded = [&](long long c) { return c == nIn || c == dense::padRow(W2L_GEMM_TF32, nIn) || c == dense::padRow(W2L_GEMM_BF16, nIn); };
   long long T, B;
   int inCols;
   if (in.dims(0) == 1 && isPadded(in.dims(1))) {  // [1, C(+pad), T, B]: the large-channel convolutions' activations
@@ -1065,21 +1004,15 @@ Variable Linear::forwardWith(const Variable& in, const Variable& weight, const V
   Variable bv = hasBias_ ? bias : Variable();
   const float dp = (train_ && dropP > 0) ? dropP : 0.f;
   // operands in the thread's precision; K = the operand row length Kp >= inCols >= nIn (extra columns are zero)
-  const GemmOperand xop = gemmOperand(in.array(), M, inCols, inCols);
-  const int Kp = xop.ld;
-  GemmOperand wop;
-  if (bf16Mode()) {
-    wop.ld = Kp;
-    wop.a = castRowsBf16(wv.array().f32(), nOut, nIn, nIn, Kp);
-  } else if (Kp == nIn) {
-    wop.a = wv.array();  // NOTE: the weight is stored [nOut][nIn] row-major (K-major B operand)
-    wop.ld = nIn;
-  } else {
-    wop.ld = Kp;
-    wop.a = padRowsF32(wv.array().f32(), nOut, nIn, nIn, Kp);
-  }
-  check(gemmWeight(0, M, nOut, Kp, xop, wop, weightPlanes(0, nOut, Kp, wop), y.f32(), nOut, hasBias_ ? bv.array().f32() : nullptr, relu ? 1 : 0, 0,
-                   nullptr, 0, 0, 1.f, dp, nextSeed()));
+  const HeldOperand xop = rowOperand(in.array(), M, inCols);
+  const int Kp = xop.op.ld;
+  HeldOperand wop;  // NOTE: the weight is stored [nOut][nIn] row-major (K-major B operand)
+  wop.mem = operandMemory(dense::weightBytes(w2l_get_precision(), nOut, nIn, Kp, wv.array().f32()), wv.array());
+  wop.op = dense::weight(currentStream(), w2l_get_precision(), nOut, nIn, Kp, wv.array().f32(), wop.mem.ptr());
+  check(dense::gemm(currentStream(), M, nOut, Kp, xop.op, wop.op, y.f32(), nOut, hasBias_ ? bv.array().f32() : nullptr, relu ? 1 : 0, 0, nullptr, 0, 0,
+                    1.f, dp, nextSeed()));
+  // the data gradient reads the forward's weight operand again, except F32's planes: those are split anew from W^T
+  if (wop.op.kind == W2L_GEMM_F32X3_SPLIT_B) wop.mem = af::array();
   const int nin = nIn, nout = nOut;
   const bool hasBias = hasBias_;
   std::vector<Variable> inputs{in, wv};
@@ -1087,39 +1020,37 @@ Variable Linear::forwardWith(const Variable& in, const Variable& weight, const V
   return Variable(y, inputs, [=](std::vector<Variable>& ins, const Variable& gout) {
     // the data gradient's weight planes come first: split after the weight gradient is forked to the gradient stream, they
     // would wait for the SMs that GEMM holds, and the data-gradient chain behind them with them
-    const GemmOperand wtPlanes = ins[0].isCalcGrad() ? weightPlanes(1, Kp, nout, wop) : GemmOperand();
+    HeldOperand wt;
+    if (ins[0].isCalcGrad()) {
+      wt.mem = operandMemory(dense::weightTBytes(wop.op, nout, nin, inCols), wop.mem);
+      wt.op = dense::weightT(currentStream(), wop.op, nout, nin, inCols, ins[1].array().f32(), wt.mem.ptr());
+    }
     af::array dy = gout.array();
     if (!maskByConsumer && (relu || dp > 0.f)) {
       af::array m = af::array::empty(y.dims());
       check(w2l_mask_mul(currentStream(), y.elements(), dy.f32(), y.f32(), relu ? 1 : 2, dp > 0.f ? 1.0f / (1.0f - dp) : 1.0f, m.f32()));
       dy = m;
     }
-    const GemmOperand dyop = gemmOperand(dy, M, nout, nout);  // zero-padded columns when nout is not a TMA row length
-    if (ins[1].isCalcGrad()) {  // dW[nout][Kp] = dy^T x  (both operands MN-major, no transposition pass)
+    const HeldOperand dyop = rowOperand(dy, M, nout);  // zero-padded columns when nout is not a TMA row length
+    if (ins[1].isCalcGrad()) {  // dW[nout][nin] = dy^T x  (both operands MN-major, no transposition pass; x's pad columns are not read)
+      // an arena slot (zeroed by zeroGrad) takes the GEMM's sum in its epilogue (C +=).  Padded input rows keep a fresh
+      // buffer that addGrad adds: a split-K GEMM would sum a nonzero C in another order.
+      af::array dw = ins[1].gradStorage();
+      const int accumulate = Kp == nin && !dw.isEmpty() ? 1 : 0;
+      if (!accumulate) dw = af::array::empty(ins[1].dims());
       // gradients that go straight into arena slots, read by nothing before the optimizer, are computed on the gradient
       // stream (when the trainer has one), overlapping the data-gradient chain that follows
       void* wstream = currentStream();
-      if (gradStream() && Kp == nin && !ins[1].gradStorage().isEmpty() && (!hasBias || !ins[2].gradStorage().isEmpty())) {
+      if (gradStream() && accumulate && (!hasBias || !ins[2].gradStorage().isEmpty())) {
         wstream = gradStream();
         forkGradStream();
         readOnGradStream(dy);
-        readOnGradStream(dyop.a);
-        readOnGradStream(xop.a);
+        readOnGradStream(dyop.mem);
+        readOnGradStream(xop.mem);
       }
-      if (Kp == nin) {
-        af::array dw = ins[1].gradStorage();
-        const int accumulate = dw.isEmpty() ? 0 : 1;  // arena slot (zeroed by zeroGrad): C += in the GEMM epilogue
-        if (!accumulate) dw = af::array::empty(ins[1].dims());
-        check(w2l_gemm(wstream, gemmKind(), 1, 1, nout, nin, M, dyop.a.ptr(), dyop.ld, xop.a.ptr(), xop.ld, dw.f32(), nin, 0, nullptr, 0, accumulate,
-                       nullptr, 0, 0, 0, 1.f, 0.f, 0ull, 0));
-        ins[1].addGrad(Variable(dw, false));
-      } else {  // padded K: the gradient of the zero columns is dropped
-        af::array dwp = af::array::empty(af::dim4(Kp, nout));
-        check(gemmP(1, 1, nout, Kp, M, dyop, xop, dwp.f32(), Kp, nullptr, 0, 0));
-        af::array dw = af::array::empty(ins[1].dims());
-        w2l::copyRows(dw.f32(), sizeof(float) * (size_t)nin, dwp.f32(), sizeof(float) * (size_t)Kp, sizeof(float) * (size_t)nin, (size_t)nout);
-        ins[1].addGrad(Variable(dw, false));
-      }
+      check(w2l_gemm(wstream, xop.op.kind, 1, 1, nout, nin, M, dyop.op.ptr, dyop.op.ld, xop.op.ptr, xop.op.ld, dw.f32(), nin, 0, nullptr, 0, accumulate,
+                     nullptr, 0, 0, 0, 1.f, 0.f, 0ull, 0));
+      ins[1].addGrad(Variable(dw, false));
       if (hasBias) {
         af::array db = ins[2].gradStorage();
         if (db.isEmpty()) db = af::array::zeros(ins[2].dims());
@@ -1127,25 +1058,14 @@ Variable Linear::forwardWith(const Variable& in, const Variable& weight, const V
         ins[2].addGrad(Variable(db, false));
       }
     }
-    if (ins[0].isCalcGrad()) {  // dx[M][Kp] = dy W  (B = W MN-major)
-      if (Kp == inCols) {
-        af::array acc = ins[0].accumulableGrad();  // e.g. LN2's residual gradient: C += in the GEMM epilogue
-        af::array dx = acc.isEmpty() ? af::array::empty(ins[0].dims()) : acc;
-        check(gemmWeight(1, M, Kp, nout, dyop, wop, wtPlanes, dx.f32(), Kp, nullptr, 0, acc.isEmpty() ? 0 : 1, inMaskMode ? ins[0].array().f32() : nullptr,
-                         Kp, inMaskMode, inMaskScale));
-        if (acc.isEmpty()) ins[0].addGrad(Variable(dx, false), true);
-      } else {  // the input rows were padded for the GEMM: drop the pad columns again
-        af::array dxp = af::array::empty(af::dim4(Kp, M));
-        check(gemmWeight(1, M, Kp, nout, dyop, wop, wtPlanes, dxp.f32(), Kp, nullptr, 0, 0));
-        af::array dx = af::array::empty(ins[0].dims());
-        w2l::copyRows(dx.f32(), sizeof(float) * (size_t)inCols, dxp.f32(), sizeof(float) * (size_t)Kp, sizeof(float) * (size_t)inCols, (size_t)M);
-        if (inMaskMode) {
-          af::array m = af::array::empty(dx.dims());
-          check(w2l_mask_mul(currentStream(), dx.elements(), dx.f32(), ins[0].array().f32(), inMaskMode, inMaskScale, m.f32()));
-          dx = m;
-        }
-        ins[0].addGrad(Variable(dx, false), true);
-      }
+    if (ins[0].isCalcGrad()) {  // dx[M][inCols] = dy W, the input's mask in the epilogue
+      // a gradient already on the input (e.g. LN2's residual gradient) takes the sum in the epilogue (C +=), unless the
+      // input rows were padded (as for the weight gradient)
+      af::array acc = Kp == inCols ? ins[0].accumulableGrad() : af::array();
+      af::array dx = acc.isEmpty() ? af::array::empty(ins[0].dims()) : acc;
+      check(dense::gemm(currentStream(), M, inCols, nout, dyop.op, wt.op, dx.f32(), inCols, nullptr, 0, acc.isEmpty() ? 0 : 1,
+                        inMaskMode ? ins[0].array().f32() : nullptr, inCols, inMaskMode, inMaskScale));
+      if (acc.isEmpty()) ins[0].addGrad(Variable(dx, false), true);
     }
   });
 }

@@ -5,7 +5,8 @@
 // Only the convolutions keep state.  For every call and every convolution the state kernel (csrc/stream_kernels.cu)
 // builds each stream's window [held tail | new frames | right padding on finish] in a batch padded to the longest
 // window, and keeps the unconsumed frames as the stream's next tail; the convolution, the GEMMs and the per-frame
-// LayerNorms then run once over that batch, with the kernels and operands of the training network's eval forward, except
+// LayerNorms then run once over that batch, with the kernels and operands of the training network's eval forward (the
+// Linear layers' GEMM operands come from host/dense_operands.h, as fl::Linear's do), except
 // that the LayerNorm is always its one-warp-per-frame kernel (the forward chooses by row count; here the row count
 // depends on the other streams in the call, and a stream's emissions must not).  Rows past a
 // stream's valid frames are slack: computed, finite, never read as data (every layer after a convolution is per
@@ -22,6 +23,7 @@
 #include <string>
 #include <vector>
 
+#include "dense_operands.h"
 #include "stream_internal.h"
 #include "w2l_b200.h"
 
@@ -112,15 +114,13 @@ Arch parseArch(const std::string& archText, int nFeat, int nLabel) {
 using namespace w2l::streaming;
 
 namespace {
+namespace dense = w2l::dense;
 long long up4(long long n) { return (n + 3) / 4 * 4; }
-long long up8(long long n) { return (n + 7) / 8 * 8; }
 
-// a Linear layer's weight as the B operand of the forward GEMM in the runtime's precision, made once at create exactly
-// as fl::Linear makes it per call: TF32 the fp32 rows ([nout][K], K = nin padded to 4 floats), F32 the pre-split
-// tf32 hi / lo planes of those rows, BF16 the rows cast to bf16 ([nout][nin padded to 8])
-struct DenseWeight {
-  int nin = 0, nout = 0, K = 0, kind = W2L_GEMM_TF32;
-  const void* B = nullptr;
+// a Linear layer: its weight as the forward GEMM's B operand, made once at create
+struct DenseLayer {
+  int nin = 0, nout = 0;
+  dense::Operand w;
   const float* bias = nullptr;
 };
 
@@ -140,7 +140,7 @@ struct Stream {
   SlotTable slots;            // one buffer per convolution
   float* snapshot = nullptr;  // parameter copy
   std::vector<const float*> params;  // per parameter, into snapshot
-  std::vector<DenseWeight> dense;    // per Linear (TDS blocks: two)
+  std::vector<DenseLayer> dense;     // per Linear (TDS blocks: two)
   std::vector<int> denseOf;          // layer -> first index into dense (-1)
   float* xT = nullptr;  // [n][Tc][nFeat]
   float* win = nullptr;
@@ -153,22 +153,10 @@ struct Stream {
   int maxOut = 0;  // bound on the output frames of one call
 };
 
-// C[M][nout] = act(A[M][nin] W^T + bias) on the GEMM, A prepared as fl::Linear prepares it
-void dense(Stream* s, cudaStream_t st, const DenseWeight& w, long long M, const float* A, float* C, int act) {
-  const void* a = A;
-  if (w.kind == W2L_GEMM_BF16) {
-    if (w.K == w.nin)
-      w2l::check(w2l_cast_bf16(st, M * w.nin, A, s->opA));
-    else
-      w2l::check(w2l_cast_bf16_rows(st, M, w.nin, w.nin, w.K, A, s->opA));
-    a = s->opA;
-  } else if (w.K != w.nin) {
-    cuda(cudaMemsetAsync(s->opA, 0, sizeof(float) * (size_t)(M * w.K), st), "stream: pad");
-    cuda(cudaMemcpy2DAsync(s->opA, sizeof(float) * w.K, A, sizeof(float) * w.nin, sizeof(float) * w.nin, (size_t)M, cudaMemcpyDeviceToDevice, st),
-         "stream: pad");
-    a = s->opA;
-  }
-  w2l::check(w2l_gemm(st, w.kind, 0, 0, (int)M, w.nout, w.K, a, w.K, w.B, w.K, C, w.nout, 0, w.bias, act, 0, nullptr, 0, 0, 0, 1.f, 0.f, 0ull, 0));
+// C[M][nout] = act(A[M][nin] W^T + bias)
+void linear(Stream* s, cudaStream_t st, const DenseLayer& d, long long M, const float* A, float* C, int act) {
+  const dense::Operand a = dense::rows(st, dense::rowKind(s->precision), M, d.nin, A, s->opA);
+  w2l::check(dense::gemm(st, (int)M, d.nout, a.ld, a, d.w, C, d.nout, d.bias, act));
 }
 
 // the per-frame LayerNorm always on its one-warp-per-frame kernel: w2l_layernorm_fwd would choose its kernel by the row
@@ -246,43 +234,15 @@ W2L_API void* w2l_stream_create(void* trainer, void* stream, int max_streams, in
       if (expect >= 0 && src.params[pi].second != expect) throw std::invalid_argument("stream_create: a parameter does not have the arch's shape");
       return s->params[pi++];
     };
-    const int kind = s->precision == W2L_PRECISION_BF16 ? W2L_GEMM_BF16 : s->precision == W2L_PRECISION_F32 ? W2L_GEMM_F32X3_SPLIT_B : W2L_GEMM_TF32;
+    const int kind = dense::rowKind(s->precision);
     auto makeDense = [&](int nin, int nout, const float* w, const float* b) {
-      DenseWeight d;
-      d.nin = nin;
-      d.nout = nout;
-      d.kind = kind;
-      d.bias = b;
-      if (kind == W2L_GEMM_BF16) {
-        d.K = (int)up8(nin);
-        void* wb = s->mem.alloc<uint16_t>((size_t)nout * d.K);
-        if (d.K == nin)
-          w2l::check(w2l_cast_bf16(st, (long long)nout * nin, w, wb));
-        else
-          w2l::check(w2l_cast_bf16_rows(st, nout, nin, nin, d.K, w, wb));
-        d.B = wb;
-      } else {
-        d.K = (int)up4(nin);
-        const float* rows = w;
-        if (d.K != nin) {
-          float* p = s->mem.alloc<float>((size_t)nout * d.K);
-          cuda(cudaMemsetAsync(p, 0, sizeof(float) * (size_t)nout * d.K, st), "stream: pad weight");
-          cuda(cudaMemcpy2DAsync(p, sizeof(float) * d.K, w, sizeof(float) * nin, sizeof(float) * nin, (size_t)nout, cudaMemcpyDeviceToDevice, st),
-               "stream: pad weight");
-          rows = p;
-        }
-        if (kind == W2L_GEMM_F32X3_SPLIT_B) {
-          float* planes = s->mem.alloc<float>((size_t)2 * nout * d.K);
-          w2l::check(w2l_split_tf32(st, 0, nout, d.K, d.K, d.K, rows, planes));
-          d.B = planes;
-        } else {
-          d.B = rows;
-        }
-      }
-      s->dense.push_back(d);
+      const int len = (int)dense::padRow(kind, nin);
+      const size_t bytes = dense::weightBytes(s->precision, nout, nin, len, w);
+      s->dense.push_back({nin, nout, dense::weight(st, s->precision, nout, nin, len, w, bytes ? s->mem.alloc<char>(bytes) : nullptr), b});
     };
     int fresh = max_chunk, feat = W;  // most new frames a layer can receive; floats per frame
-    long long maxAct = 1, maxWin = 1, maxHidden = 1, maxOpA = 1, maxFrames = 1;  // per stream
+    long long maxAct = 1, maxWin = 1, maxHidden = 1, maxFrames = 1;  // per stream
+    size_t maxOpA = 1;                                                // bytes per stream
     size_t ws = 0, ci = 0;
     for (size_t li = 0; li < s->arch.layers.size(); ++li) {
       const Layer& l = s->arch.layers[li];
@@ -312,7 +272,7 @@ W2L_API void* w2l_stream_create(void* trainer, void* stream, int max_streams, in
           makeDense(feat, l.inner, w1, b1);
           makeDense(l.inner, feat, w2, b2);
           maxHidden = std::max(maxHidden, (long long)fresh * l.inner);
-          maxOpA = std::max(maxOpA, (long long)fresh * up8(std::max(feat, l.inner)));
+          maxOpA = std::max({maxOpA, dense::rowBytes(kind, fresh, feat, nullptr), dense::rowBytes(kind, fresh, l.inner, nullptr)});
         }
       } else if (l.op == Op::LayerNorm) {
         next(1);
@@ -323,7 +283,7 @@ W2L_API void* w2l_stream_create(void* trainer, void* stream, int max_streams, in
         const float* b = next(l.nout);
         s->denseOf.back() = (int)s->dense.size();
         makeDense(l.nin, l.nout, w, b);
-        maxOpA = std::max(maxOpA, (long long)fresh * up8(l.nin));
+        maxOpA = std::max(maxOpA, dense::rowBytes(kind, fresh, l.nin, nullptr));
         feat = l.nout;
       }
       maxAct = std::max(maxAct, (long long)fresh * feat);
@@ -338,7 +298,7 @@ W2L_API void* w2l_stream_create(void* trainer, void* stream, int max_streams, in
     s->win = s->mem.alloc<float>((size_t)max_streams * maxWin);
     for (auto& a : s->act) a = s->mem.alloc<float>((size_t)max_streams * maxAct);
     s->hidden = s->mem.alloc<float>((size_t)max_streams * maxHidden);
-    s->opA = s->mem.alloc<float>((size_t)max_streams * maxOpA);
+    s->opA = s->mem.alloc<char>((size_t)max_streams * maxOpA);
     const long long rows = (long long)max_streams * maxFrames;
     s->meanRstd = s->mem.alloc<float>((size_t)(2 * rows));
     s->convWsBytes = std::max<size_t>(ws, 256);
@@ -438,10 +398,8 @@ W2L_API int w2l_stream_run(void* h, void* stream, int n, const int* slots, const
              "stream: residual");
         float* z = pick({cur, y1, res});
         layerNorm(s, st, rows, fout, y1, res, s->params[pidx + 2], s->params[pidx + 3], z);
-        const DenseWeight& d1 = s->dense[s->denseOf[li]];
-        const DenseWeight& d2 = s->dense[s->denseOf[li] + 1];
-        dense(s, st, d1, rows, z, s->hidden, 1);
-        dense(s, st, d2, rows, s->hidden, y1, 0);
+        linear(s, st, s->dense[s->denseOf[li]], rows, z, s->hidden, 1);
+        linear(s, st, s->dense[s->denseOf[li] + 1], rows, s->hidden, y1, 0);
         layerNorm(s, st, rows, fout, y1, z, s->params[pidx + 8], s->params[pidx + 9], res);
         cur = res;
         continue;
@@ -459,7 +417,7 @@ W2L_API int w2l_stream_run(void* h, void* stream, int n, const int* slots, const
         cur = y;
       } else if (l.op == Op::Linear) {
         float* y = li + 1 == layers.size() ? emissions : pick({cur});
-        dense(s, st, s->dense[s->denseOf[li]], rows, cur, y, 0);
+        linear(s, st, s->dense[s->denseOf[li]], rows, cur, y, 0);
         cur = y;
       }
     }
