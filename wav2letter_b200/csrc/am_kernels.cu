@@ -306,34 +306,46 @@ __global__ void conv_wgrad_reduce_kernel(int n_parts, int n_w, int n_b, const fl
 // LayerNorm over a whole sample (R = T*C*W elements) with scalar gain/bias, fused residual:
 //   s = a + r ; y = (s - mean) * rstd * gain + bias
 // ------------------------------------------------------------------------------------------
-// All four passes stream float4 (R % 4 == 0 and 16-byte aligned bases: `vec`), two loads in flight per operand;
-// the per-sample sums are accumulated in double from 4-element fp32 partials.
-__device__ __forceinline__ float4 ld4(const float* p, long long i) { return *reinterpret_cast<const float4*>(p + i); }
-__device__ __forceinline__ float4 add4(float4 a, float4 b) { return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w); }
+// Every pass streams V-wide chunks: V = 4 (float4) when R % 4 == 0 and the bases are 16-byte aligned, else V = 1; two loads
+// in flight per operand.  The per-sample sums are accumulated in double from each chunk's fp32 fold (fsum, fsq, fdot).
 
+// a chunk's sum of squares in the forward passes: V = 4 fuses the second square of each pair, fma(y, y, x * x)
+template <class Acc> __device__ __forceinline__ Acc fsq(float v) { return fdot<Acc>(v, v); }
+template <class Acc> __device__ __forceinline__ Acc fsq(float4 v) { return (Acc)(fmaf(v.y, v.y, v.x * v.x) + fmaf(v.w, v.w, v.z * v.z)); }
+// a + the residual r (nullable) at i, as each width has always added it (V = 1 adds 0.f when there is no residual)
+__device__ __forceinline__ float add_res(float a, const float* r, long long i) { return a + (r ? r[i] : 0.f); }
+__device__ __forceinline__ float4 add_res(float4 a, const float* r, long long i) { return r ? vadd(a, ldv<4>(r, i)) : a; }
+
+// CTA totals of the per-thread values v[0..K): warp sums, then thread 0 adds the NW warps' sums in warp order (no atomics,
+// the same bits every run).  The totals are left in thread 0's v.
+template <int NW, class T, int K>
+__device__ __forceinline__ void cta_sum(T (&v)[K]) {
+  __shared__ T red[K][NW];
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    v[k] = warp_sum(v[k]);
+    if ((threadIdx.x & 31) == 0) red[k][threadIdx.x >> 5] = v[k];
+  }
+  __syncthreads();
+  if (threadIdx.x == 0)
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+      v[k] = 0;
+      for (int w = 0; w < NW; ++w) v[k] += red[k][w];
+    }
+}
 // CTA partial (sum, sum of squares / products) -> out[0..1]; the consumer kernel adds the CTAs' partials in a fixed order
 // (no zero-fill of the scratch, no atomics, deterministic)
 __device__ __forceinline__ void block_sum2_store(double s, double q, double* out) {
-  s = warp_sum(s);
-  q = warp_sum(q);
-  __shared__ double ss[8], qq[8];
-  if ((threadIdx.x & 31) == 0) {
-    ss[threadIdx.x >> 5] = s;
-    qq[threadIdx.x >> 5] = q;
-  }
-  __syncthreads();
+  double v[2] = {s, q};
+  cta_sum<8>(v);
   if (threadIdx.x == 0) {
-    double S = 0, Q = 0;
-    for (int w = 0; w < 8; ++w) {
-      S += ss[w];
-      Q += qq[w];
-    }
-    out[0] = S;
-    out[1] = Q;
+    out[0] = v[0];
+    out[1] = v[1];
   }
 }
-// sum of the gridDim.x CTA partials of sample b (every thread gets the totals)
-__device__ __forceinline__ void sum_partials(const double* __restrict__ parts, int nparts, double& S, double& Q) {
+// sum of the nparts partial pairs of one sample, on warp 0 (every thread gets the totals)
+__device__ __forceinline__ void sum_partials(const double* parts, int nparts, double& S, double& Q) {
   __shared__ double tot[2];
   if (threadIdx.x < 32) {
     double s = 0.0, q = 0.0;
@@ -353,35 +365,28 @@ __device__ __forceinline__ void sum_partials(const double* __restrict__ parts, i
   Q = tot[1];
 }
 
-__global__ void __launch_bounds__(256) ln_stats_kernel(long long R, int vec, const float* __restrict__ a, const float* __restrict__ r,
+template <int V>
+__global__ void __launch_bounds__(256) ln_stats_kernel(long long R, const float* __restrict__ a, const float* __restrict__ r,
                                                        double* __restrict__ stats /*[B][2] sum, sumsq*/) {
   const int b = blockIdx.y;
   const float* ab = a + (size_t)b * R;
   const float* rb = r ? r + (size_t)b * R : nullptr;
   double s = 0.0, q = 0.0;
-  const long long start = (long long)blockIdx.x * blockDim.x + threadIdx.x, step = (long long)gridDim.x * blockDim.x;
-  if (vec) {
+  const long long start = V * ((long long)blockIdx.x * blockDim.x + threadIdx.x), step = V * (long long)gridDim.x * blockDim.x;
 #pragma unroll 4
-    for (long long i = 4 * start; i < R; i += 4 * step) {
-      float4 v = ld4(ab, i);
-      if (rb) v = add4(v, ld4(rb, i));
-      s += (double)((v.x + v.y) + (v.z + v.w));
-      q += (double)((v.x * v.x + v.y * v.y) + (v.z * v.z + v.w * v.w));
-    }
-  } else {
-    for (long long i = start; i < R; i += step) {
-      const float v = ab[i] + (rb ? rb[i] : 0.f);
-      s += v;
-      q += (double)v * v;
-    }
+  for (long long i = start; i < R; i += step) {
+    const vec_t<V> v = add_res(ldv<V>(ab, i), rb, i);
+    s += fsum<double>(v);
+    q += fsq<double>(v);
   }
   block_sum2_store(s, q, stats + 2 * ((size_t)b * gridDim.x + blockIdx.x));
 }
 
-__global__ void __launch_bounds__(256) ln_apply_kernel(long long R, int vec, float eps, const float* __restrict__ a,
-                                                       const float* __restrict__ r, const float* __restrict__ gain,
-                                                       const float* __restrict__ bias, const double* __restrict__ stats,
-                                                       float* __restrict__ y, float* __restrict__ mean_rstd /*[B][2]*/) {
+template <int V>
+__global__ void __launch_bounds__(256) ln_apply_kernel(long long R, float eps, const float* __restrict__ a, const float* __restrict__ r,
+                                                       const float* __restrict__ gain, const float* __restrict__ bias,
+                                                       const double* __restrict__ stats, float* __restrict__ y,
+                                                       float* __restrict__ mean_rstd /*[B][2]*/) {
   const int b = blockIdx.y;
   double S, Q;
   sum_partials(stats + 2 * (size_t)b * gridDim.x, gridDim.x, S, Q);
@@ -397,21 +402,10 @@ __global__ void __launch_bounds__(256) ln_apply_kernel(long long R, int vec, flo
   const float* rb = r ? r + (size_t)b * R : nullptr;
   float* yb = y + (size_t)b * R;
   const float sc = rstd * g;
-  const long long start = (long long)blockIdx.x * blockDim.x + threadIdx.x, step = (long long)gridDim.x * blockDim.x;
-  if (vec) {
+  const long long start = V * ((long long)blockIdx.x * blockDim.x + threadIdx.x), step = V * (long long)gridDim.x * blockDim.x;
 #pragma unroll 2
-    for (long long i = 4 * start; i < R; i += 4 * step) {
-      float4 v = ld4(ab, i);
-      if (rb) v = add4(v, ld4(rb, i));
-      *reinterpret_cast<float4*>(yb + i) =
-          make_float4((v.x - mu) * sc + bi, (v.y - mu) * sc + bi, (v.z - mu) * sc + bi, (v.w - mu) * sc + bi);
-    }
-  } else {
-    for (long long i = start; i < R; i += step) {
-      const float v = ab[i] + (rb ? rb[i] : 0.f);
-      yb[i] = (v - mu) * sc + bi;
-    }
-  }
+  for (long long i = start; i < R; i += step)
+    stv<V>(yb, i, vmap([&](float v) { return (v - mu) * sc + bi; }, add_res(ldv<V>(ab, i), rb, i)));
 }
 
 // ---- single-launch forward (cooperative): every CTA owns one contiguous chunk of one sample and KEEPS what it reads in
@@ -428,58 +422,31 @@ __global__ void __launch_bounds__(kLnFusedThreads, 2) ln_fused_fwd_kernel(long l
                                                                            float* __restrict__ y, float* __restrict__ mean_rstd,
                                                                            double* __restrict__ scratch) {
   extern __shared__ __align__(16) float ln_sv[];
-  __shared__ double red[2][kLnFusedThreads / 32];
-  __shared__ double tot[2];
   const int b = blockIdx.y, parts = gridDim.x;
   const long long lo = (long long)blockIdx.x * chunk, hi = min(R, lo + chunk);
   const float* ab = a + (size_t)b * R;
   const float* rb = r ? r + (size_t)b * R : nullptr;
   float* yb = y + (size_t)b * R;
-  double s = 0.0, q = 0.0;
+  double sq[2] = {0.0, 0.0};
 #pragma unroll 4
   for (long long i = lo + 4 * threadIdx.x; i < hi; i += 4 * kLnFusedThreads) {
-    float4 v = ld4(ab, i);
-    if (rb) v = add4(v, ld4(rb, i));
+    const float4 v = add_res(ldv<4>(ab, i), rb, i);
     const long long k = i - lo;
-    if (k < keep) *reinterpret_cast<float4*>(ln_sv + k) = v;
-    s += (double)((v.x + v.y) + (v.z + v.w));
-    q += (double)((v.x * v.x + v.y * v.y) + (v.z * v.z + v.w * v.w));
+    if (k < keep) stv<4>(ln_sv, k, v);
+    sq[0] += fsum<double>(v);
+    sq[1] += fsq<double>(v);
   }
-  s = warp_sum(s);
-  q = warp_sum(q);
-  if ((threadIdx.x & 31) == 0) {
-    red[0][threadIdx.x >> 5] = s;
-    red[1][threadIdx.x >> 5] = q;
-  }
-  __syncthreads();
+  cta_sum<kLnFusedThreads / 32>(sq);
   if (threadIdx.x == 0) {
-    double S = 0, Q = 0;
-    for (int w = 0; w < kLnFusedThreads / 32; ++w) {
-      S += red[0][w];
-      Q += red[1][w];
-    }
-    scratch[2 * ((size_t)b * parts + blockIdx.x)] = S;
-    scratch[2 * ((size_t)b * parts + blockIdx.x) + 1] = Q;
+    scratch[2 * ((size_t)b * parts + blockIdx.x)] = sq[0];
+    scratch[2 * ((size_t)b * parts + blockIdx.x) + 1] = sq[1];
   }
   __threadfence();
   cooperative_groups::this_grid().sync();
-  if (threadIdx.x < 32) {  // fixed-order sum of the sample's partials: deterministic
-    double S = 0.0, Q = 0.0;
-    const double* pp = scratch + 2 * (size_t)b * parts;
-    for (int i = threadIdx.x; i < parts; i += 32) {
-      S += pp[2 * i];
-      Q += pp[2 * i + 1];
-    }
-    S = warp_sum(S);
-    Q = warp_sum(Q);
-    if (threadIdx.x == 0) {
-      tot[0] = S;
-      tot[1] = Q;
-    }
-  }
-  __syncthreads();
-  const double mean = tot[0] / (double)R;
-  const double var = fmax(tot[1] / (double)R - mean * mean, 0.0);
+  double S, Q;
+  sum_partials(scratch + 2 * (size_t)b * parts, parts, S, Q);
+  const double mean = S / (double)R;
+  const double var = fmax(Q / (double)R - mean * mean, 0.0);
   const float rstd = (float)(1.0 / sqrt(var + (double)eps));
   const float mu = (float)mean, g = gain ? *gain : 1.f, bi = bias ? *bias : 0.f;
   if (blockIdx.x == 0 && threadIdx.x == 0) {
@@ -490,21 +457,16 @@ __global__ void __launch_bounds__(kLnFusedThreads, 2) ln_fused_fwd_kernel(long l
 #pragma unroll 2
   for (long long i = lo + 4 * threadIdx.x; i < hi; i += 4 * kLnFusedThreads) {
     const long long k = i - lo;
-    float4 v;
-    if (k < keep) {
-      v = *reinterpret_cast<const float4*>(ln_sv + k);
-    } else {  // the tail that did not fit in shared memory: L2
-      v = ld4(ab, i);
-      if (rb) v = add4(v, ld4(rb, i));
-    }
-    *reinterpret_cast<float4*>(yb + i) = make_float4((v.x - mu) * sc + bi, (v.y - mu) * sc + bi, (v.z - mu) * sc + bi, (v.w - mu) * sc + bi);
+    // the tail that did not fit in shared memory comes from L2
+    const float4 v = k < keep ? ldv<4>(ln_sv, k) : add_res(ldv<4>(ab, i), rb, i);
+    stv<4>(yb, i, vmap([&](float x) { return (x - mu) * sc + bi; }, v));
   }
 }
 
 // backward pass 1: per-sample sums of dy and dy * xhat
-__global__ void __launch_bounds__(256) ln_bwd_stats_kernel(long long R, int vec, const float* __restrict__ a,
-                                                           const float* __restrict__ r, const float* __restrict__ dy,
-                                                           const float* __restrict__ mean_rstd,
+template <int V>
+__global__ void __launch_bounds__(256) ln_bwd_stats_kernel(long long R, const float* __restrict__ a, const float* __restrict__ r,
+                                                           const float* __restrict__ dy, const float* __restrict__ mean_rstd,
                                                            double* __restrict__ sums /*[B][2]*/) {
   const int b = blockIdx.y;
   const float mu = mean_rstd[2 * b], rstd = mean_rstd[2 * b + 1];
@@ -512,23 +474,12 @@ __global__ void __launch_bounds__(256) ln_bwd_stats_kernel(long long R, int vec,
   const float* rb = r ? r + (size_t)b * R : nullptr;
   const float* db = dy + (size_t)b * R;
   double s = 0.0, q = 0.0;
-  const long long start = (long long)blockIdx.x * blockDim.x + threadIdx.x, step = (long long)gridDim.x * blockDim.x;
-  if (vec) {
+  const long long start = V * ((long long)blockIdx.x * blockDim.x + threadIdx.x), step = V * (long long)gridDim.x * blockDim.x;
 #pragma unroll 4
-    for (long long i = 4 * start; i < R; i += 4 * step) {
-      float4 v = ld4(ab, i);
-      const float4 d = ld4(db, i);
-      if (rb) v = add4(v, ld4(rb, i));
-      s += (double)((d.x + d.y) + (d.z + d.w));
-      q += (double)((d.x * ((v.x - mu) * rstd) + d.y * ((v.y - mu) * rstd)) + (d.z * ((v.z - mu) * rstd) + d.w * ((v.w - mu) * rstd)));
-    }
-  } else {
-    for (long long i = start; i < R; i += step) {
-      const float xh = (ab[i] + (rb ? rb[i] : 0.f) - mu) * rstd;
-      const float d = db[i];
-      s += d;
-      q += (double)d * xh;
-    }
+  for (long long i = start; i < R; i += step) {
+    const vec_t<V> xh = vmap([&](float v) { return (v - mu) * rstd; }, add_res(ldv<V>(ab, i), rb, i)), d = ldv<V>(db, i);
+    s += fsum<double>(d);
+    q += fdot<double>(d, xh);
   }
   block_sum2_store(s, q, sums + 2 * ((size_t)b * gridDim.x + blockIdx.x));
 }
@@ -539,11 +490,12 @@ __global__ void __launch_bounds__(256) ln_bwd_stats_kernel(long long R, int vec,
 __device__ __forceinline__ float ln_mask(int mode, float av, float scale) {
   return mode == 0 ? 1.f : ((mode == 1 ? av > 0.f : av != 0.f) ? scale : 0.f);
 }
-__global__ void __launch_bounds__(256) ln_bwd_apply_kernel(long long R, int vec, const float* __restrict__ a,
-                                                           const float* __restrict__ r, const float* __restrict__ dy,
-                                                           const float* __restrict__ gain, const float* __restrict__ mean_rstd,
-                                                           const double* __restrict__ sums, float* __restrict__ d_branch,
-                                                           float* __restrict__ d_res, int branch_mode, float branch_scale) {
+template <int V>
+__global__ void __launch_bounds__(256) ln_bwd_apply_kernel(long long R, const float* __restrict__ a, const float* __restrict__ r,
+                                                           const float* __restrict__ dy, const float* __restrict__ gain,
+                                                           const float* __restrict__ mean_rstd, const double* __restrict__ sums,
+                                                           float* __restrict__ d_branch, float* __restrict__ d_res, int branch_mode,
+                                                           float branch_scale) {
   const int b = blockIdx.y;
   const float mu = mean_rstd[2 * b], rstd = mean_rstd[2 * b + 1], g = gain ? *gain : 1.f;
   double S, Q;
@@ -555,38 +507,21 @@ __global__ void __launch_bounds__(256) ln_bwd_apply_kernel(long long R, int vec,
   float* ob = d_branch + (size_t)b * R;
   float* orr = d_res ? d_res + (size_t)b * R : nullptr;
   const float rg = rstd * g;
-  const long long start = (long long)blockIdx.x * blockDim.x + threadIdx.x, step = (long long)gridDim.x * blockDim.x;
-  if (vec) {
+  const long long start = V * ((long long)blockIdx.x * blockDim.x + threadIdx.x), step = V * (long long)gridDim.x * blockDim.x;
 #pragma unroll 2
-    for (long long i = 4 * start; i < R; i += 4 * step) {
-      const float4 av = ld4(ab, i);
-      const float4 d = ld4(db, i);
-      float4 v = av;
-      if (rb) v = add4(v, ld4(rb, i));
-      float4 ds;
-      ds.x = rg * (d.x - m1 - (v.x - mu) * rstd * m2);
-      ds.y = rg * (d.y - m1 - (v.y - mu) * rstd * m2);
-      ds.z = rg * (d.z - m1 - (v.z - mu) * rstd * m2);
-      ds.w = rg * (d.w - m1 - (v.w - mu) * rstd * m2);
-      if (orr) *reinterpret_cast<float4*>(orr + i) = ds;
-      *reinterpret_cast<float4*>(ob + i) =
-          make_float4(ds.x * ln_mask(branch_mode, av.x, branch_scale), ds.y * ln_mask(branch_mode, av.y, branch_scale),
-                      ds.z * ln_mask(branch_mode, av.z, branch_scale), ds.w * ln_mask(branch_mode, av.w, branch_scale));
-    }
-  } else {
-    for (long long i = start; i < R; i += step) {
-      const float av = ab[i];
-      const float xh = (av + (rb ? rb[i] : 0.f) - mu) * rstd;
-      const float ds = rg * (db[i] - m1 - xh * m2);
-      if (orr) orr[i] = ds;
-      ob[i] = ds * ln_mask(branch_mode, av, branch_scale);
-    }
+  for (long long i = start; i < R; i += step) {
+    const vec_t<V> av = ldv<V>(ab, i);
+    const vec_t<V> ds = vmap([&](float d, float v) { return rg * (d - m1 - (v - mu) * rstd * m2); }, ldv<V>(db, i), add_res(av, rb, i));
+    if (orr) stv<V>(orr, i, ds);
+    stv<V>(ob, i, vmap([&](float d, float x) { return d * ln_mask(branch_mode, x, branch_scale); }, ds, av));
   }
 }
 
 // ---- per-row variant: many short groups (per-frame LayerNorm of the streaming TDS family: R = C*W <= a few
 // thousand, groups = T*B).  One warp per group, two sweeps inside one kernel (the second hits L1), no scratch.
-__global__ void __launch_bounds__(256) ln_row_fwd_kernel(long long G, int R, int vec, float eps, const float* __restrict__ a,
+// The sums are accumulated in float.
+template <int V>
+__global__ void __launch_bounds__(256) ln_row_fwd_kernel(long long G, int R, float eps, const float* __restrict__ a,
                                                          const float* __restrict__ r, const float* __restrict__ gain,
                                                          const float* __restrict__ bias, float* __restrict__ y,
                                                          float* __restrict__ mean_rstd) {
@@ -597,19 +532,10 @@ __global__ void __launch_bounds__(256) ln_row_fwd_kernel(long long G, int R, int
   const float* rb = r ? r + grp * R : nullptr;
   float* yb = y + grp * R;
   float s = 0.f, q = 0.f;
-  if (vec) {
-    for (int i = 4 * lane; i < R; i += 128) {
-      float4 v = ld4(ab, i);
-      if (rb) v = add4(v, ld4(rb, i));
-      s += (v.x + v.y) + (v.z + v.w);
-      q += (v.x * v.x + v.y * v.y) + (v.z * v.z + v.w * v.w);
-    }
-  } else {
-    for (int i = lane; i < R; i += 32) {
-      const float v = ab[i] + (rb ? rb[i] : 0.f);
-      s += v;
-      q += v * v;
-    }
+  for (int i = V * lane; i < R; i += 32 * V) {
+    const vec_t<V> v = add_res(ldv<V>(ab, i), rb, i);
+    s += fsum<float>(v);
+    q += fsq<float>(v);
   }
   const double S = warp_sum((double)s), Q = warp_sum((double)q);
   const double mean = S / R, var = fmax(Q / R - mean * mean, 0.0);
@@ -619,17 +545,10 @@ __global__ void __launch_bounds__(256) ln_row_fwd_kernel(long long G, int R, int
     mean_rstd[2 * grp] = mu;
     mean_rstd[2 * grp + 1] = rstd;
   }
-  if (vec) {
-    for (int i = 4 * lane; i < R; i += 128) {
-      float4 v = ld4(ab, i);
-      if (rb) v = add4(v, ld4(rb, i));
-      *reinterpret_cast<float4*>(yb + i) = make_float4((v.x - mu) * sc + bi, (v.y - mu) * sc + bi, (v.z - mu) * sc + bi, (v.w - mu) * sc + bi);
-    }
-  } else {
-    for (int i = lane; i < R; i += 32) yb[i] = (ab[i] + (rb ? rb[i] : 0.f) - mu) * sc + bi;
-  }
+  for (int i = V * lane; i < R; i += 32 * V) stv<V>(yb, i, vmap([&](float v) { return (v - mu) * sc + bi; }, add_res(ldv<V>(ab, i), rb, i)));
 }
 
+// (kept with its runtime `vec` flag: as a width template it ran about 5% slower)
 __global__ void __launch_bounds__(256) ln_row_bwd_kernel(long long G, int R, int vec, const float* __restrict__ a,
                                                          const float* __restrict__ r, const float* __restrict__ dy,
                                                          const float* __restrict__ gain, const float* __restrict__ mean_rstd,
@@ -649,9 +568,9 @@ __global__ void __launch_bounds__(256) ln_row_bwd_kernel(long long G, int R, int
     float s = 0.f, q = 0.f;
     if (vec) {
       for (int i = 4 * lane; i < R; i += 128) {
-        float4 v = ld4(ab, i);
-        const float4 d = ld4(db, i);
-        if (rb) v = add4(v, ld4(rb, i));
+        float4 v = ldv<4>(ab, i);
+        const float4 d = ldv<4>(db, i);
+        if (rb) v = vadd(v, ldv<4>(rb, i));
         s += (d.x + d.y) + (d.z + d.w);
         q += (d.x * ((v.x - mu) * rstd) + d.y * ((v.y - mu) * rstd)) + (d.z * ((v.z - mu) * rstd) + d.w * ((v.w - mu) * rstd));
       }
@@ -667,10 +586,10 @@ __global__ void __launch_bounds__(256) ln_row_bwd_kernel(long long G, int R, int
     const float m1 = S / R, m2 = Q / R, rg = rstd * g;
     if (vec) {
       for (int i = 4 * lane; i < R; i += 128) {
-        const float4 av = ld4(ab, i);
-        const float4 d = ld4(db, i);
+        const float4 av = ldv<4>(ab, i);
+        const float4 d = ldv<4>(db, i);
         float4 v = av;
-        if (rb) v = add4(v, ld4(rb, i));
+        if (rb) v = vadd(v, ldv<4>(rb, i));
         float4 ds;
         ds.x = rg * (d.x - m1 - (v.x - mu) * rstd * m2);
         ds.y = rg * (d.y - m1 - (v.y - mu) * rstd * m2);
@@ -711,79 +630,39 @@ __global__ void __launch_bounds__(256) ln_row_bwd_kernel(long long G, int R, int
 // one block, fixed summation order (run to run identical)
 __global__ void __launch_bounds__(256) ln_scalar_grads_kernel(int n, const double* __restrict__ part, float* __restrict__ dgain,
                                                               float* __restrict__ dbias) {
-  double s = 0.0, q = 0.0;
+  double sq[2] = {0.0, 0.0};
   for (int i = threadIdx.x; i < n; i += 256) {
-    s += part[2 * i];
-    q += part[2 * i + 1];
+    sq[0] += part[2 * i];
+    sq[1] += part[2 * i + 1];
   }
-  s = warp_sum(s);
-  q = warp_sum(q);
-  __shared__ double ss[8], sq[8];
-  if ((threadIdx.x & 31) == 0) {
-    ss[threadIdx.x >> 5] = s;
-    sq[threadIdx.x >> 5] = q;
-  }
-  __syncthreads();
+  cta_sum<8>(sq);
   if (threadIdx.x == 0) {
-    double S = 0.0, Q = 0.0;
-    for (int w = 0; w < 8; ++w) {
-      S += ss[w];
-      Q += sq[w];
-    }
-    if (dbias) *dbias += (float)S;
-    if (dgain) *dgain += (float)Q;
+    if (dbias) *dbias += (float)sq[0];
+    if (dgain) *dgain += (float)sq[1];
   }
 }
 
-// part[blockIdx.y][n] = sum of X[m][n] over this CTA's rows   (bias gradients of Linear; colsum_finish_kernel adds the parts)
+// part[blockIdx.y][n] = sum of X[m][n] over this CTA's rows   (bias gradients of Linear; colsum_finish_kernel adds the parts).
+// A CTA covers 32 V-wide column chunks (V = 4: N, ld multiples of 4 and a 16-byte aligned base) x rows_per_cta rows.
+template <int V>
 __global__ void __launch_bounds__(256) colsum_kernel(int M, int N, const float* __restrict__ X, int ld, int rows_per_cta,
                                                      float* __restrict__ part) {
-  const int n = blockIdx.x * 32 + (threadIdx.x & 31);
-  const int m0 = blockIdx.y * rows_per_cta, m1 = min(M, m0 + rows_per_cta);
-  float s = 0.f;
-  if (n < N)
-    for (int m = m0 + (threadIdx.x >> 5); m < m1; m += 8) s += X[(size_t)m * ld + n];
-  __shared__ float red[8][33];
-  red[threadIdx.x >> 5][threadIdx.x & 31] = s;
-  __syncthreads();
-  if (threadIdx.x < 32 && n < N) {
-    float t = 0.f;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) t += red[w][threadIdx.x];
-    part[(size_t)blockIdx.y * N + n] = t;  // this row block's partial column sums
-  }
-}
-
-// float4 variant (N, ld multiples of 4, 16-byte aligned base): a block covers 128 columns x rows_per_cta rows
-__global__ void __launch_bounds__(256) colsum4_kernel(int M, int N, const float* __restrict__ X, int ld, int rows_per_cta,
-                                                      float* __restrict__ part) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int n = blockIdx.x * 128 + 4 * lane;
+  const int n = blockIdx.x * 32 * V + V * lane;
   const int m0 = blockIdx.y * rows_per_cta, m1 = min(M, m0 + rows_per_cta);
-  float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+  vec_t<V> s{};
   if (n < N) {
 #pragma unroll 4
-    for (int m = m0 + warp; m < m1; m += 8) {
-      const float4 v = *reinterpret_cast<const float4*>(X + (size_t)m * ld + n);
-      s.x += v.x;
-      s.y += v.y;
-      s.z += v.z;
-      s.w += v.w;
-    }
+    for (int m = m0 + warp; m < m1; m += 8) s = vadd(s, ldv<V>(X, (size_t)m * ld + n));
   }
-  __shared__ float4 red[8][32];
+  __shared__ vec_t<V> red[8][V == 4 ? 32 : 33];
   red[warp][lane] = s;
   __syncthreads();
   if (warp == 0 && n < N) {
-    float4 t = red[0][lane];
+    vec_t<V> t = red[0][lane];
 #pragma unroll
-    for (int w = 1; w < 8; ++w) {
-      t.x += red[w][lane].x;
-      t.y += red[w][lane].y;
-      t.z += red[w][lane].z;
-      t.w += red[w][lane].w;
-    }
-    *reinterpret_cast<float4*>(part + (size_t)blockIdx.y * N + n) = t;  // this row block's partial column sums
+    for (int w = 1; w < 8; ++w) t = vadd(t, red[w][lane]);
+    stv<V>(part, (size_t)blockIdx.y * N + n, t);  // this row block's partial column sums
   }
 }
 
@@ -798,35 +677,21 @@ __global__ void __launch_bounds__(256) colsum_finish_kernel(int N, int row_block
 
 // ---- optimizer on a flat parameter arena -------------------------------------------------------
 __global__ void __launch_bounds__(256) sq_norm_kernel(long long n, const float* __restrict__ g, double* __restrict__ part) {
-  double s = 0.0;
+  double s[1] = {0.0};
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const float v = g[i];
-    s += (double)v * v;
+    s[0] += (double)v * v;
   }
-  s = warp_sum(s);
-  __shared__ double ss[8];
-  if ((threadIdx.x & 31) == 0) ss[threadIdx.x >> 5] = s;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double S = 0;
-    for (int w = 0; w < 8; ++w) S += ss[w];
-    part[blockIdx.x] = S;
-  }
+  cta_sum<8>(s);
+  if (threadIdx.x == 0) part[blockIdx.x] = s[0];
 }
 
 // *out += sum of the n block partials, fixed order (run to run identical)
 __global__ void __launch_bounds__(256) sq_norm_finish_kernel(int n, const double* __restrict__ part, double* __restrict__ out) {
-  double s = 0.0;
-  for (int i = threadIdx.x; i < n; i += 256) s += part[i];
-  s = warp_sum(s);
-  __shared__ double ss[8];
-  if ((threadIdx.x & 31) == 0) ss[threadIdx.x >> 5] = s;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double S = 0.0;
-    for (int w = 0; w < 8; ++w) S += ss[w];
-    *out += S;
-  }
+  double s[1] = {0.0};
+  for (int i = threadIdx.x; i < n; i += 256) s[0] += part[i];
+  cta_sum<8>(s);
+  if (threadIdx.x == 0) *out += s[0];
 }
 
 // fl::SGDOptimizer::step with the loop's gradient scaling and fl::clipGradNorm folded in:
@@ -906,22 +771,11 @@ __global__ void transpose_bft_kernel(int F, int T, const float* __restrict__ in,
     if (t < T && f < F) ob[(size_t)t * F + f] = tile[threadIdx.x][j];
   }
 }
-__global__ void axpy_kernel(long long n, int vec, float a, const float* __restrict__ x, float* __restrict__ y) {
-  const long long start = (long long)blockIdx.x * blockDim.x + threadIdx.x, step = (long long)gridDim.x * blockDim.x;
-  if (vec) {
+template <int V>
+__global__ void axpy_kernel(long long n, float a, const float* __restrict__ x, float* __restrict__ y) {
+  const long long start = V * ((long long)blockIdx.x * blockDim.x + threadIdx.x), step = V * (long long)gridDim.x * blockDim.x;
 #pragma unroll 2
-    for (long long i = 4 * start; i < n; i += 4 * step) {
-      const float4 xv = *reinterpret_cast<const float4*>(x + i);
-      float4 yv = *reinterpret_cast<float4*>(y + i);
-      yv.x = fmaf(a, xv.x, yv.x);
-      yv.y = fmaf(a, xv.y, yv.y);
-      yv.z = fmaf(a, xv.z, yv.z);
-      yv.w = fmaf(a, xv.w, yv.w);
-      *reinterpret_cast<float4*>(y + i) = yv;
-    }
-  } else {
-    for (long long i = start; i < n; i += step) y[i] = fmaf(a, x[i], y[i]);
-  }
+  for (long long i = start; i < n; i += step) stv<V>(y, i, vmap([&](float xv, float yv) { return fmaf(a, xv, yv); }, ldv<V>(x, i), ldv<V>(y, i)));
 }
 __global__ void fill_kernel(long long n, float v, float* __restrict__ y) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) y[i] = v;
@@ -1112,7 +966,7 @@ extern "C" int w2l_layernorm_fwd(void* stream_, int B, long long R, float eps, c
   if (B <= 0 || R <= 0 || !a || !y || !mean_rstd || !scratch) return fail(W2L_ERR_INVALID_ARGUMENT, "layernorm_fwd: bad arguments");
   const int vec = (R % 4 == 0) && !((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(r) | reinterpret_cast<uintptr_t>(y)) & 15);
   if (ln_use_rows(B, R)) {  // many short groups (per-frame LayerNorm): one warp per group
-    ln_row_fwd_kernel<<<(B + 7) / 8, 256, 0, stream>>>(B, (int)R, vec, eps, a, r, gain, bias, y, mean_rstd);
+    (vec ? ln_row_fwd_kernel<4> : ln_row_fwd_kernel<1>)<<<(B + 7) / 8, 256, 0, stream>>>(B, (int)R, eps, a, r, gain, bias, y, mean_rstd);
     W2L_LAUNCH_CHECK("ln_row_fwd_kernel");
     return W2L_OK;
   }
@@ -1149,9 +1003,9 @@ extern "C" int w2l_layernorm_fwd(void* stream_, int B, long long R, float eps, c
   // whole multiples of the SMs at full occupancy (8 CTAs of 256 threads per SM) when the samples are long enough;
   // at most W2L_LN_MAX_PARTS CTAs per sample (the scratch holds one partial pair per CTA)
   dim3 grid(std::max(1, std::min(std::min(blocks_for(R, 256 * 4 * 4), W2L_LN_MAX_PARTS), sm_count() * 8 / std::max(1, std::min(B, sm_count() * 8)))), B);
-  ln_stats_kernel<<<grid, 256, 0, stream>>>(R, vec, a, r, scratch);
+  (vec ? ln_stats_kernel<4> : ln_stats_kernel<1>)<<<grid, 256, 0, stream>>>(R, a, r, scratch);
   W2L_LAUNCH_CHECK("ln_stats_kernel");
-  ln_apply_kernel<<<grid, 256, 0, stream>>>(R, vec, eps, a, r, gain, bias, scratch, y, mean_rstd);
+  (vec ? ln_apply_kernel<4> : ln_apply_kernel<1>)<<<grid, 256, 0, stream>>>(R, eps, a, r, gain, bias, scratch, y, mean_rstd);
   W2L_LAUNCH_CHECK("ln_apply_kernel");
   return W2L_OK;
 }
@@ -1162,7 +1016,7 @@ extern "C" int w2l_layernorm_rows_fwd(void* stream_, long long G, int R, float e
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (G <= 0 || R <= 0 || !a || !y || !mean_rstd) return fail(W2L_ERR_INVALID_ARGUMENT, "layernorm_rows_fwd: bad arguments");
   const int vec = (R % 4 == 0) && !((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(r) | reinterpret_cast<uintptr_t>(y)) & 15);
-  ln_row_fwd_kernel<<<(unsigned)((G + 7) / 8), 256, 0, stream>>>(G, R, vec, eps, a, r, gain, bias, y, mean_rstd);
+  (vec ? ln_row_fwd_kernel<4> : ln_row_fwd_kernel<1>)<<<(unsigned)((G + 7) / 8), 256, 0, stream>>>(G, R, eps, a, r, gain, bias, y, mean_rstd);
   W2L_LAUNCH_CHECK("ln_row_fwd_kernel");
   return W2L_OK;
 }
@@ -1190,9 +1044,10 @@ extern "C" int w2l_layernorm_bwd(void* stream_, int B, long long R, const float*
   // whole multiples of the SMs at full occupancy (8 CTAs of 256 threads per SM) when the samples are long enough;
   // at most W2L_LN_MAX_PARTS CTAs per sample (the scratch holds one partial pair per CTA)
   dim3 grid(std::max(1, std::min(std::min(blocks_for(R, 256 * 4 * 4), W2L_LN_MAX_PARTS), sm_count() * 8 / std::max(1, std::min(B, sm_count() * 8)))), B);
-  ln_bwd_stats_kernel<<<grid, 256, 0, stream>>>(R, vec, a, r, dy, mean_rstd, scratch);
+  (vec ? ln_bwd_stats_kernel<4> : ln_bwd_stats_kernel<1>)<<<grid, 256, 0, stream>>>(R, a, r, dy, mean_rstd, scratch);
   W2L_LAUNCH_CHECK("ln_bwd_stats_kernel");
-  ln_bwd_apply_kernel<<<grid, 256, 0, stream>>>(R, vec, a, r, dy, gain, mean_rstd, scratch, d_branch, d_res, branch_mode, branch_scale);
+  (vec ? ln_bwd_apply_kernel<4> : ln_bwd_apply_kernel<1>)<<<grid, 256, 0, stream>>>(R, a, r, dy, gain, mean_rstd, scratch, d_branch, d_res,
+                                                                                   branch_mode, branch_scale);
   W2L_LAUNCH_CHECK("ln_bwd_apply_kernel");
   if (dgain || dbias) {
     ln_scalar_grads_kernel<<<1, 256, 0, stream>>>(B * (int)grid.x, scratch, dgain, dbias);
@@ -1204,30 +1059,14 @@ extern "C" int w2l_layernorm_bwd(void* stream_, int B, long long R, const float*
 extern "C" int w2l_colsum_accumulate(void* stream_, int M, int N, const float* X, int ld, float* out) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (M <= 0 || N <= 0 || !X || !out) return fail(W2L_ERR_INVALID_ARGUMENT, "colsum: bad arguments");
-  if (N % 4 == 0 && ld % 4 == 0 && !(reinterpret_cast<uintptr_t>(X) & 15)) {
-    const int col_blocks = (N + 127) / 128;
-    // ~4 CTAs per SM: rows per CTA so that col_blocks * row_blocks ~ 600, at least 64 rows each
-    const int rows_per_cta = std::max(64, (int)(((long long)M * col_blocks + 599) / 600));
-    dim3 grid(col_blocks, (M + rows_per_cta - 1) / rows_per_cta);
-    float* part = nullptr;
-    W2L_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&part), sizeof(float) * (size_t)grid.y * N, stream));
-    colsum4_kernel<<<grid, 256, 0, stream>>>(M, N, X, ld, rows_per_cta, part);
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) {
-      count_launch();
-      trace_launch("colsum_kernel");
-      colsum_finish_kernel<<<(N + 255) / 256, 256, 0, stream>>>(N, (int)grid.y, part, out);
-    }
-    cudaFreeAsync(part, stream);
-    if (e != cudaSuccess) return fail(W2L_ERR_CUDA, std::string("launch colsum_kernel: ") + cudaGetErrorString(e));
-    W2L_LAUNCH_CHECK("colsum_finish_kernel");
-    return W2L_OK;
-  }
-  const int rows_per_cta = 256;
-  dim3 grid((N + 31) / 32, (M + rows_per_cta - 1) / rows_per_cta);
+  const bool vec = N % 4 == 0 && ld % 4 == 0 && !(reinterpret_cast<uintptr_t>(X) & 15);
+  const int cols = vec ? 128 : 32, col_blocks = (N + cols - 1) / cols;
+  // float4: ~4 CTAs per SM, rows per CTA so that col_blocks * row_blocks ~ 600, at least 64 rows each; scalar: 256 rows each
+  const int rows_per_cta = vec ? std::max(64, (int)(((long long)M * col_blocks + 599) / 600)) : 256;
+  dim3 grid(col_blocks, (M + rows_per_cta - 1) / rows_per_cta);
   float* part = nullptr;
   W2L_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&part), sizeof(float) * (size_t)grid.y * N, stream));
-  colsum_kernel<<<grid, 256, 0, stream>>>(M, N, X, ld, rows_per_cta, part);
+  (vec ? colsum_kernel<4> : colsum_kernel<1>)<<<grid, 256, 0, stream>>>(M, N, X, ld, rows_per_cta, part);
   cudaError_t e = cudaGetLastError();
   if (e == cudaSuccess) {
     count_launch();
@@ -1315,7 +1154,7 @@ extern "C" int w2l_axpy(void* stream_, long long n, float a, const float* x, flo
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (n <= 0 || !x || !y) return fail(W2L_ERR_INVALID_ARGUMENT, "axpy: bad arguments");
   const int vec = (n % 4 == 0) && !((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15);
-  axpy_kernel<<<blocks_for(n), 256, 0, stream>>>(n, vec, a, x, y);
+  (vec ? axpy_kernel<4> : axpy_kernel<1>)<<<blocks_for(n), 256, 0, stream>>>(n, a, x, y);
   W2L_LAUNCH_CHECK("axpy_kernel");
   return W2L_OK;
 }

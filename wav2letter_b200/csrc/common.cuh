@@ -102,6 +102,29 @@ __device__ __forceinline__ double warp_sum(double v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
+
+// ---- one V-wide chunk of a memory-bound pass: V = 4 (float4: 16-byte aligned, lengths multiples of 4) or V = 1 ----------
+template <int V> struct VecOf { using type = float; };
+template <> struct VecOf<4> { using type = float4; };
+template <int V> using vec_t = typename VecOf<V>::type;
+template <int V> __device__ __forceinline__ vec_t<V> ldv(const float* p, long long i) { return *reinterpret_cast<const vec_t<V>*>(p + i); }
+template <int V> __device__ __forceinline__ void stv(float* p, long long i, vec_t<V> v) { *reinterpret_cast<vec_t<V>*>(p + i) = v; }
+// f applied element by element across chunks of the same width
+template <class F, class... T> __device__ __forceinline__ float vmap(F f, float a, T... b) { return f(a, b...); }
+template <class F, class... T> __device__ __forceinline__ float4 vmap(F f, float4 a, T... b) {
+  return make_float4(f(a.x, b.x...), f(a.y, b.y...), f(a.z, b.z...), f(a.w, b.w...));
+}
+__device__ __forceinline__ float vadd(float a, float b) { return a + b; }
+__device__ __forceinline__ float4 vadd(float4 a, float4 b) { return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w); }
+// A chunk's sum / dot product as a term of an Acc accumulator, in the order each width has always added it: V = 4 adds the
+// chunk in float as (x + y) + (z + w), each product pair as fma(x, x', y * y'), and widens the result; V = 1 widens the
+// element first.  The fmas are explicit: left to contraction, a pair can fuse either product.
+template <class Acc> __device__ __forceinline__ Acc fsum(float v) { return (Acc)v; }
+template <class Acc> __device__ __forceinline__ Acc fsum(float4 v) { return (Acc)((v.x + v.y) + (v.z + v.w)); }
+template <class Acc> __device__ __forceinline__ Acc fdot(float a, float b) { return (Acc)a * b; }
+template <class Acc> __device__ __forceinline__ Acc fdot(float4 a, float4 b) {
+  return (Acc)(fmaf(a.x, b.x, a.y * b.y) + fmaf(a.z, b.z, a.w * b.w));
+}
 // log(exp(a)+exp(b)) in fp32, safe for -inf operands.
 __device__ __forceinline__ float lse2f(float a, float b) {
   float m = fmaxf(a, b);

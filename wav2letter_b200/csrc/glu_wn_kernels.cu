@@ -33,77 +33,40 @@ __device__ __forceinline__ float block_sum(float v, float* red /*[33]*/) {
   return red[32];
 }
 
-// one CTA per output unit (row of `len` floats); float4 streams when the rows are 16-byte aligned; the second sweep of a row
-// (scale / gradient) re-reads what the first sweep just brought into L1/L2
-__global__ void __launch_bounds__(256) wn_fwd_kernel(int len, int vec, const float* __restrict__ v, const float* __restrict__ g,
+// one CTA per output unit (row of `len` floats), V-wide chunks (V = 4 when the rows are 16-byte aligned); the second sweep of a
+// row (scale / gradient) re-reads what the first sweep just brought into L1/L2
+template <int V>
+__global__ void __launch_bounds__(256) wn_fwd_kernel(int len, const float* __restrict__ v, const float* __restrict__ g,
                                                      float* __restrict__ w, float* __restrict__ inv_norm) {
   __shared__ float red[33];
   const size_t r = blockIdx.x;
   const float* vr = v + r * len;
   float s = 0.f;
-  if (vec) {
-    const float4* v4 = reinterpret_cast<const float4*>(vr);
-    for (int i = threadIdx.x; i < len / 4; i += blockDim.x) {
-      const float4 x = v4[i];
-      s += (x.x * x.x + x.y * x.y) + (x.z * x.z + x.w * x.w);
-    }
-  } else {
-    for (int i = threadIdx.x; i < len; i += blockDim.x) s += vr[i] * vr[i];
-  }
+  for (int i = V * threadIdx.x; i < len; i += V * blockDim.x) s += fdot<float>(ldv<V>(vr, i), ldv<V>(vr, i));
   const float tot = block_sum(s, red);
   const float inv = rsqrtf(fmaxf(tot, 1e-30f));
   if (threadIdx.x == 0) inv_norm[r] = inv;
   const float sc = g[r] * inv;
-  if (vec) {
-    const float4* v4 = reinterpret_cast<const float4*>(vr);
-    float4* w4 = reinterpret_cast<float4*>(w + r * len);
-    for (int i = threadIdx.x; i < len / 4; i += blockDim.x) {
-      const float4 x = v4[i];
-      w4[i] = make_float4(x.x * sc, x.y * sc, x.z * sc, x.w * sc);
-    }
-  } else {
-    for (int i = threadIdx.x; i < len; i += blockDim.x) w[r * len + i] = vr[i] * sc;
-  }
+  for (int i = V * threadIdx.x; i < len; i += V * blockDim.x) stv<V>(w + r * len, i, vmap([&](float x) { return x * sc; }, ldv<V>(vr, i)));
 }
 
 // dg[r] += <dw, v> / ||v||;  dv += g/||v|| * (dw - v <dw, v> / ||v||^2)
-__global__ void __launch_bounds__(256) wn_bwd_kernel(int len, int vec, const float* __restrict__ v, const float* __restrict__ g,
+template <int V>
+__global__ void __launch_bounds__(256) wn_bwd_kernel(int len, const float* __restrict__ v, const float* __restrict__ g,
                                                      const float* __restrict__ inv_norm, const float* __restrict__ dw,
                                                      float* __restrict__ dv, float* __restrict__ dg) {
   __shared__ float red[33];
   const size_t r = blockIdx.x;
   const float* vr = v + r * len;
   const float* dr = dw + r * len;
+  float* ovr = dv + r * len;
   float s = 0.f;
-  if (vec) {
-    const float4* v4 = reinterpret_cast<const float4*>(vr);
-    const float4* d4 = reinterpret_cast<const float4*>(dr);
-    for (int i = threadIdx.x; i < len / 4; i += blockDim.x) {
-      const float4 x = v4[i], d = d4[i];
-      s += (x.x * d.x + x.y * d.y) + (x.z * d.z + x.w * d.w);
-    }
-  } else {
-    for (int i = threadIdx.x; i < len; i += blockDim.x) s += vr[i] * dr[i];
-  }
+  for (int i = V * threadIdx.x; i < len; i += V * blockDim.x) s += fdot<float>(ldv<V>(vr, i), ldv<V>(dr, i));
   const float dot = block_sum(s, red);
   const float inv = inv_norm[r], gi = g[r] * inv, c = dot * inv * inv;
   if (threadIdx.x == 0) dg[r] += dot * inv;
-  if (vec) {
-    const float4* v4 = reinterpret_cast<const float4*>(vr);
-    const float4* d4 = reinterpret_cast<const float4*>(dr);
-    float4* o4 = reinterpret_cast<float4*>(dv + r * len);
-    for (int i = threadIdx.x; i < len / 4; i += blockDim.x) {
-      const float4 x = v4[i], d = d4[i];
-      float4 o = o4[i];
-      o.x += gi * (d.x - x.x * c);
-      o.y += gi * (d.y - x.y * c);
-      o.z += gi * (d.z - x.z * c);
-      o.w += gi * (d.w - x.w * c);
-      o4[i] = o;
-    }
-  } else {
-    for (int i = threadIdx.x; i < len; i += blockDim.x) dv[r * len + i] += gi * (dr[i] - vr[i] * c);
-  }
+  for (int i = V * threadIdx.x; i < len; i += V * blockDim.x)
+    stv<V>(ovr, i, vmap([&](float o, float d, float x) { return o + gi * (d - x * c); }, ldv<V>(ovr, i), ldv<V>(dr, i), ldv<V>(vr, i)));
 }
 
 // row of the padded operand that holds output channel co (GLU split: the two halves are padded separately)
@@ -254,77 +217,50 @@ __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + __ex
 // y[r][c] = x[r][c] * sigmoid(x[r][H + c]) * dropout(r*H + c).  Four consecutive channels per thread when H % 4 == 0 (the
 // padded channel counts always are): 128-bit loads / stores and ONE Philox block for the four masks (element index i is a
 // multiple of 4, so the block idx >> 2 with words 0..3 is exactly dropout_scale's mask of the four elements).
-__device__ __forceinline__ float4 keep4(unsigned long long seed, unsigned long long i, float p, float inv_keep) {
-  const uint4 r = philox4x32((uint32_t)(i >> 2), (uint32_t)(i >> 34), (uint32_t)seed, (uint32_t)(seed >> 32));
-  auto k = [&](uint32_t v) { return ((float)(v >> 8) * (1.0f / 16777216.0f)) >= p ? inv_keep : 0.f; };
-  return make_float4(k(r.x), k(r.y), k(r.z), k(r.w));
+template <int V>
+__device__ __forceinline__ vec_t<V> keep(unsigned long long seed, unsigned long long i, float p, float inv_keep) {
+  if constexpr (V == 1) {
+    return dropout_scale(seed, i, p, inv_keep);
+  } else {
+    const uint4 r = philox4x32((uint32_t)(i >> 2), (uint32_t)(i >> 34), (uint32_t)seed, (uint32_t)(seed >> 32));
+    auto k = [&](uint32_t v) { return ((float)(v >> 8) * (1.0f / 16777216.0f)) >= p ? inv_keep : 0.f; };
+    return make_float4(k(r.x), k(r.y), k(r.z), k(r.w));
+  }
 }
-__global__ void __launch_bounds__(256) glu_fwd_kernel(long long rows, int H, int vec, const float* __restrict__ x, float* __restrict__ y,
+struct Mul {
+  __device__ float operator()(float a, float b) const { return a * b; }
+};
+template <int V>
+__global__ void __launch_bounds__(256) glu_fwd_kernel(long long rows, int H, const float* __restrict__ x, float* __restrict__ y,
                                                       float drop_p, unsigned long long seed) {
   const float inv_keep = drop_p > 0.f ? 1.0f / (1.0f - drop_p) : 1.0f;
-  const long long n = rows * H;
-  if (vec) {
-    const int H4 = H / 4;
-    for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n / 4; q += (long long)gridDim.x * blockDim.x) {
-      const long long r = q / H4;
-      const int c = (int)(q - r * H4) * 4;
-      const float4 a = *reinterpret_cast<const float4*>(x + r * 2 * H + c), b = *reinterpret_cast<const float4*>(x + r * 2 * H + H + c);
-      float4 v = make_float4(a.x * sigmoidf_(b.x), a.y * sigmoidf_(b.y), a.z * sigmoidf_(b.z), a.w * sigmoidf_(b.w));
-      if (drop_p > 0.f) {
-        const float4 m = keep4(seed, (unsigned long long)(4 * q), drop_p, inv_keep);
-        v.x *= m.x;
-        v.y *= m.y;
-        v.z *= m.z;
-        v.w *= m.w;
-      }
-      *reinterpret_cast<float4*>(y + 4 * q) = v;
-    }
-    return;
-  }
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const long long r = i / H;
-    const int c = (int)(i - r * H);
-    const float a = x[r * 2 * H + c], b = x[r * 2 * H + H + c];
-    float v = a * sigmoidf_(b);
-    if (drop_p > 0.f) v *= dropout_scale(seed, (unsigned long long)i, drop_p, inv_keep);
-    y[i] = v;
+  const long long n = rows * H / V;  // chunks
+  const int HV = H / V;
+#pragma unroll 1  // unrolled, the V = 1 loop spills around its division calls
+  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
+    const long long r = q / HV, i = V * q;
+    const int c = (int)(q - r * HV) * V;
+    vec_t<V> v = vmap([](float a, float b) { return a * sigmoidf_(b); }, ldv<V>(x, r * 2 * H + c), ldv<V>(x, r * 2 * H + H + c));
+    if (drop_p > 0.f) v = vmap(Mul(), v, keep<V>(seed, i, drop_p, inv_keep));
+    stv<V>(y, i, v);
   }
 }
 // dx[r][c] = dy * m * sig(b) ; dx[r][H+c] = dy * m * a * sig(b) (1 - sig(b))
-__global__ void __launch_bounds__(256) glu_bwd_kernel(long long rows, int H, int vec, const float* __restrict__ x, const float* __restrict__ dy,
+template <int V>
+__global__ void __launch_bounds__(256) glu_bwd_kernel(long long rows, int H, const float* __restrict__ x, const float* __restrict__ dy,
                                                       float* __restrict__ dx, float drop_p, unsigned long long seed) {
   const float inv_keep = drop_p > 0.f ? 1.0f / (1.0f - drop_p) : 1.0f;
-  const long long n = rows * H;
-  if (vec) {
-    const int H4 = H / 4;
-    for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n / 4; q += (long long)gridDim.x * blockDim.x) {
-      const long long r = q / H4;
-      const int c = (int)(q - r * H4) * 4;
-      const float4 a = *reinterpret_cast<const float4*>(x + r * 2 * H + c), b = *reinterpret_cast<const float4*>(x + r * 2 * H + H + c);
-      float4 d = *reinterpret_cast<const float4*>(dy + 4 * q);
-      if (drop_p > 0.f) {
-        const float4 m = keep4(seed, (unsigned long long)(4 * q), drop_p, inv_keep);
-        d.x *= m.x;
-        d.y *= m.y;
-        d.z *= m.z;
-        d.w *= m.w;
-      }
-      const float4 s = make_float4(sigmoidf_(b.x), sigmoidf_(b.y), sigmoidf_(b.z), sigmoidf_(b.w));
-      *reinterpret_cast<float4*>(dx + r * 2 * H + c) = make_float4(d.x * s.x, d.y * s.y, d.z * s.z, d.w * s.w);
-      *reinterpret_cast<float4*>(dx + r * 2 * H + H + c) =
-          make_float4(d.x * a.x * s.x * (1.0f - s.x), d.y * a.y * s.y * (1.0f - s.y), d.z * a.z * s.z * (1.0f - s.z), d.w * a.w * s.w * (1.0f - s.w));
-    }
-    return;
-  }
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const long long r = i / H;
-    const int c = (int)(i - r * H);
-    const float a = x[r * 2 * H + c], b = x[r * 2 * H + H + c];
-    const float s = sigmoidf_(b);
-    float d = dy[i];
-    if (drop_p > 0.f) d *= dropout_scale(seed, (unsigned long long)i, drop_p, inv_keep);
-    dx[r * 2 * H + c] = d * s;
-    dx[r * 2 * H + H + c] = d * a * s * (1.0f - s);
+  const long long n = rows * H / V;  // chunks
+  const int HV = H / V;
+#pragma unroll 1
+  for (long long q = (long long)blockIdx.x * blockDim.x + threadIdx.x; q < n; q += (long long)gridDim.x * blockDim.x) {
+    const long long r = q / HV, i = V * q;
+    const int c = (int)(q - r * HV) * V;
+    vec_t<V> d = ldv<V>(dy, i);
+    if (drop_p > 0.f) d = vmap(Mul(), d, keep<V>(seed, i, drop_p, inv_keep));
+    const vec_t<V> a = ldv<V>(x, r * 2 * H + c), s = vmap([](float b) { return sigmoidf_(b); }, ldv<V>(x, r * 2 * H + H + c));
+    stv<V>(dx, r * 2 * H + c, vmap(Mul(), d, s));
+    stv<V>(dx, r * 2 * H + H + c, vmap([](float d, float a, float s) { return d * a * s * (1.0f - s); }, d, a, s));
   }
 }
 
@@ -380,7 +316,7 @@ extern "C" int w2l_weightnorm_fwd(void* stream_, int rows, int len, const float*
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (rows <= 0 || len <= 0 || !v || !g || !w || !inv_norm) return fail(W2L_ERR_INVALID_ARGUMENT, "weightnorm_fwd: bad arguments");
   const int vec = (len % 4 == 0) && !((reinterpret_cast<uintptr_t>(v) | reinterpret_cast<uintptr_t>(w)) & 15);
-  wn_fwd_kernel<<<rows, 256, 0, stream>>>(len, vec, v, g, w, inv_norm);
+  (vec ? wn_fwd_kernel<4> : wn_fwd_kernel<1>)<<<rows, 256, 0, stream>>>(len, v, g, w, inv_norm);
   W2L_LAUNCH_CHECK("wn_fwd_kernel");
   return W2L_OK;
 }
@@ -389,7 +325,7 @@ extern "C" int w2l_weightnorm_bwd(void* stream_, int rows, int len, const float*
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (rows <= 0 || len <= 0 || !v || !g || !inv_norm || !dw || !dv || !dg) return fail(W2L_ERR_INVALID_ARGUMENT, "weightnorm_bwd: bad arguments");
   const int vec = (len % 4 == 0) && !((reinterpret_cast<uintptr_t>(v) | reinterpret_cast<uintptr_t>(dw) | reinterpret_cast<uintptr_t>(dv)) & 15);
-  wn_bwd_kernel<<<rows, 256, 0, stream>>>(len, vec, v, g, inv_norm, dw, dv, dg);
+  (vec ? wn_bwd_kernel<4> : wn_bwd_kernel<1>)<<<rows, 256, 0, stream>>>(len, v, g, inv_norm, dw, dv, dg);
   W2L_LAUNCH_CHECK("wn_bwd_kernel");
   return W2L_OK;
 }
@@ -454,7 +390,7 @@ extern "C" int w2l_glu_fwd(void* stream_, long long rows, int half, const float*
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (rows <= 0 || half <= 0 || !x || !y || dropout_p < 0.f || dropout_p >= 1.f) return fail(W2L_ERR_INVALID_ARGUMENT, "glu_fwd: bad arguments");
   const int vec = (half % 4 == 0) && !((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15);
-  glu_fwd_kernel<<<blocks_for_n(rows * half / (vec ? 4 : 1)), 256, 0, stream>>>(rows, half, vec, x, y, dropout_p, seed);
+  (vec ? glu_fwd_kernel<4> : glu_fwd_kernel<1>)<<<blocks_for_n(rows * half / (vec ? 4 : 1)), 256, 0, stream>>>(rows, half, x, y, dropout_p, seed);
   W2L_LAUNCH_CHECK("glu_fwd_kernel");
   return W2L_OK;
 }
@@ -463,7 +399,7 @@ extern "C" int w2l_glu_bwd(void* stream_, long long rows, int half, const float*
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (rows <= 0 || half <= 0 || !x || !dy || !dx || dropout_p < 0.f || dropout_p >= 1.f) return fail(W2L_ERR_INVALID_ARGUMENT, "glu_bwd: bad arguments");
   const int vec = (half % 4 == 0) && !((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dx)) & 15);
-  glu_bwd_kernel<<<blocks_for_n(rows * half / (vec ? 4 : 1)), 256, 0, stream>>>(rows, half, vec, x, dy, dx, dropout_p, seed);
+  (vec ? glu_bwd_kernel<4> : glu_bwd_kernel<1>)<<<blocks_for_n(rows * half / (vec ? 4 : 1)), 256, 0, stream>>>(rows, half, x, dy, dx, dropout_p, seed);
   W2L_LAUNCH_CHECK("glu_bwd_kernel");
   return W2L_OK;
 }
