@@ -322,7 +322,9 @@ W2L_API int w2l_prelu_bwd(void* stream, long long n, const float* x, const float
 /* fl::LayerNorm over a whole sample (R = T*C*W elements; `LN 0 1 2` / TDSBlock with lnIncludeTime)
  * with scalar gain/bias (device scalars, nullable = 1/0) and a fused residual: y = LN(a + r).
  * mean_rstd [B][2] is saved for the backward pass; scratch = W2L_LN_SCRATCH_DOUBLES(B) doubles (one partial
- * pair per CTA: no zero-fill, no atomics, deterministic).
+ * pair per CTA: no zero-fill, no atomics, deterministic).  Where a group's mean is far above its spread, the statistics
+ * are summed about a pivot taken from the group (the mean of its first 32 values), so that costs no accuracy, and a
+ * constant group comes out exactly `bias`; other groups keep plain sums.
  * Backward: d_res = ds, d_branch = ds * mask(a) where the mask undoes the fused ReLU/dropout of the
  * branch that produced `a` (branch_mode 0 none, 1 (a>0)*scale, 2 (a!=0)*scale); dgain/dbias accumulate. */
 #define W2L_LN_MAX_PARTS 80

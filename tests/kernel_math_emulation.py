@@ -409,3 +409,45 @@ def ctc_chain_emulate(e, y, P=4, kRc=2):
         occ[:, zlab[s_]] += post[:, s_]
     soft = np.exp(e64 - lz[:, None])
     return -ll2 / LOG2E, soft - occ
+
+
+def layernorm_rows_emulate(x, V, pivot="sample", eps=1e-5):
+    """float32 arithmetic of the statistics of ln_row_fwd_kernel<V> (am_kernels.cu): one warp per group, lane l sums the
+    V-wide chunks at V*l, V*l + 32V, ... in fp32 (V = 4 folds a chunk as (x + y) + (z + w) and its squares as
+    fma(y, y, x*x) + fma(w, w, z*z)), the lanes' sums are combined in double.  The sums are taken about a pivot K:
+    "sample" (the kernel's: plain sums, and where they cancel (mean^2 > 64 var) sums again about the mean of the values at
+    l * R / 32, l = 0..31, added by a warp's xor butterfly), "first" (the first value) or "none" (K = 0, the one-pass
+    Q/R - mean^2).  x [G][R] float32 -> xhat = (x - mu) * rstd [G][R], mu [G], rstd [G], float32."""
+    G, R = x.shape
+    x = x.astype(F)
+
+    def fma(a, b, c):
+        return (a.astype(np.float64) * b + c).astype(F)
+
+    def sums(K):
+        s, q = np.zeros((G, 32), F), np.zeros((G, 32), F)
+        for i0 in range(0, R, V):
+            lane = (i0 // V) % 32
+            d = (x[:, i0:i0 + V] - K[:, None]).astype(F)
+            if V == 4:
+                cs = (d[:, 0] + d[:, 1]) + (d[:, 2] + d[:, 3])
+                cq = fma(d[:, 1], d[:, 1], d[:, 0] * d[:, 0]) + fma(d[:, 3], d[:, 3], d[:, 2] * d[:, 2])
+            else:
+                cs, cq = d[:, 0], d[:, 0] * d[:, 0]
+            s[:, lane] += cs
+            q[:, lane] += cq
+        return s.astype(np.float64).sum(1) / R, q.astype(np.float64).sum(1) / R
+
+    K = x[:, 0].copy() if pivot == "first" else np.zeros(G, F)
+    S, Q = sums(K)
+    if pivot == "sample":
+        v = x[:, np.arange(32) * R // 32]
+        for o in (16, 8, 4, 2, 1):  # the xor butterfly of warp_sum
+            v = v + v[:, np.arange(32) ^ o]
+        cancels = S * S > 64 * (Q - S * S)
+        K = np.where(cancels, v[:, 0] * F(1 / 32), F(0)).astype(F)
+        S2, Q2 = sums(K)
+        S, Q = np.where(cancels, S2, S), np.where(cancels, Q2, Q)
+    mu = (K.astype(np.float64) + S).astype(F)
+    rstd = (1.0 / np.sqrt(np.maximum(Q - S * S, 0.0) + float(F(eps)))).astype(F)
+    return ((x - mu[:, None]) * rstd[:, None]).astype(F), mu, rstd

@@ -1,10 +1,11 @@
-"""CPU check of the arithmetic formulation used by the CUDA ASG kernels (see
+"""CPU check of the arithmetic formulation used by the CUDA ASG, CTC and per-row LayerNorm kernels (see
 tests/kernel_math_emulation.py) against the oracle, incl. adversarial emission ranges."""
 import numpy as np
 import pytest
 
 import oracle
-from kernel_math_emulation import ctc_chain_emulate, fac_chain_emulate, fac_emulate, fac_posteriors_float64, fcc_emulate
+from kernel_math_emulation import (ctc_chain_emulate, fac_chain_emulate, fac_emulate, fac_posteriors_float64, fcc_emulate,
+                                   layernorm_rows_emulate)
 
 
 def rel(a, b):
@@ -147,3 +148,39 @@ def test_halo_slices_reproduce_the_full_row():
         use = ok & (np.arange(256) >= 8) & (np.arange(256) < 248)
         np.testing.assert_array_equal(sl_a[use], full_a[idx[use]])
         np.testing.assert_array_equal(sl_b[use], full_b[idx[use]])
+
+
+def _xhat_err(x, xhat, eps=1e-5):
+    x64 = x.astype(np.float64)
+    m = x64.mean(1, keepdims=True)
+    ref = (x64 - m) / np.sqrt(((x64 - m) ** 2).mean(1, keepdims=True) + eps)
+    return rel(xhat, ref)
+
+
+@pytest.mark.parametrize("V", [4, 1])
+def test_layernorm_row_sums_about_a_pivot(V):
+    """Why the per-row LayerNorm sums about a pivot: its fp32 lane sums lose about 2 log10(mean / sigma) digits in
+    Q/R - mean^2 (1e-2 of the output at mean / sigma = 1e3, the variance clamped to 0 at 1e4), and about the mean of
+    32 values spread over the group (used where the plain sums cancel: mean above 8 sigma) they lose none: what remains is
+    the fp32 rounding of the stored mean (half an ulp of 1e4 is 5e-4 sigma).  The pivot is a mean because a first value
+    50 sigma off the mean would cost 2 log10(50) digits; well-conditioned rows (post-ReLU: half of them zeros) keep the
+    plain sums."""
+    rng = np.random.default_rng(40 + V)
+    G, R = 64, 640
+    bound = {0.5: 3e-7, 30: 1e-6, 1e3: 3e-5, 1e4: 5e-4}
+    for ratio, tol in bound.items():
+        x = rng.normal(ratio, 1.0, (G, R)).astype(np.float32)
+        assert _xhat_err(x, layernorm_rows_emulate(x, V)[0]) < tol, ratio
+        if ratio >= 1e3:
+            assert _xhat_err(x, layernorm_rows_emulate(x, V, "none")[0]) > 100 * tol, ratio  # the unshifted sums
+    x = rng.normal(0.0, 1.0, (G, R)).astype(np.float32)
+    x[:, 0] = 50.0
+    assert _xhat_err(x, layernorm_rows_emulate(x, V)[0]) < 3e-7
+    assert _xhat_err(x, layernorm_rows_emulate(x, V, "first")[0]) > 3e-6  # the first value as the pivot
+    x = (np.maximum(rng.normal(0.0, 1.0, (256, 2160)), 0) * 1.3).astype(np.float32)
+    assert _xhat_err(x, layernorm_rows_emulate(x, V)[0]) < 5e-7
+    for c in (17.7, 3.3, -250.1, 0.0):  # a constant group, also shorter than the 32 samples: exact mean, variance 0, xhat 0
+        for n in (4, 12, 1200):
+            xhat, mu, rstd = layernorm_rows_emulate(np.full((2, n), c, np.float32), V)
+            assert (xhat == 0).all() and (mu == np.float32(c)).all()
+            assert (rstd == np.float32(1 / np.sqrt(float(np.float32(1e-5))))).all()

@@ -308,6 +308,20 @@ __global__ void conv_wgrad_reduce_kernel(int n_parts, int n_w, int n_b, const fl
 // ------------------------------------------------------------------------------------------
 // Every pass streams V-wide chunks: V = 4 (float4) when R % 4 == 0 and the bases are 16-byte aligned, else V = 1; two loads
 // in flight per operand.  The per-sample sums are accumulated in double from each chunk's fp32 fold (fsum, fsq, fdot).
+//
+// The variance is formed in one pass from sums about a pivot K taken from the group itself: S' = sum(x - K) and
+// Q' = sum((x - K)^2), then mean = K + S'/R and var = Q'/R - (S'/R)^2.  Unshifted, Q/R - mean^2 loses about
+// 2 log10(|mean| / sigma) digits to cancellation (all of them at mean / sigma = 1e4 in fp32); about a pivot within a few
+// sigma of the mean it loses none.  A pivot is used only where the plain sums lose more than about 2 digits (mean above 8
+// sigma); every other group keeps K = 0, the plain sums and exactly their results.  The pivot is the mean of 32 values
+// spread evenly over the group (ln_sample): within the spread of the group, also for skewed (post-ReLU) rows and rows with
+// an outlier, where a single value or the median of a few can sit several sigma off the mean.  A constant group (value
+// c != 0) gets K = c (32 equal values add exactly), so S' = Q' = 0, the mean is exact, the variance exactly 0 and the
+// output exactly `bias`.
+//   - the per-row kernel sums plainly first and, in a group whose plain sums cancel, sums again about the pivot;
+//   - the two-pass and single-launch kernels, whose CTAs must agree on K before they sum, decide from the sample alone:
+//     K = its mean where that exceeds 8 of its standard deviations, else 0 (ln_pivot).  Every warp of every CTA computes
+//     it from the same values in the same order: one K per group.
 
 // a chunk's sum of squares in the forward passes: V = 4 fuses the second square of each pair, fma(y, y, x * x)
 template <class Acc> __device__ __forceinline__ Acc fsq(float v) { return fdot<Acc>(v, v); }
@@ -315,6 +329,32 @@ template <class Acc> __device__ __forceinline__ Acc fsq(float4 v) { return (Acc)
 // a + the residual r (nullable) at i, as each width has always added it (V = 1 adds 0.f when there is no residual)
 __device__ __forceinline__ float add_res(float a, const float* r, long long i) { return a + (r ? r[i] : 0.f); }
 __device__ __forceinline__ float4 add_res(float4 a, const float* r, long long i) { return r ? vadd(a, ldv<4>(r, i)) : a; }
+// mean and variance (fp32) of 32 values of the group at a (+ r), at l * R / 32 for l = 0..31 (repeats when R < 32), summed
+// by the calling warp (all 32 lanes; the xor butterfly leaves the same bits in every lane)
+__device__ __forceinline__ float2 ln_sample(const float* a, const float* r, long long R) {
+  const long long i = (threadIdx.x & 31) * R / 32;
+  const float x = add_res(a[i], r, i);
+  const float p = warp_sum(x) * (1.f / 32);
+  return make_float2(p, warp_sum((x - p) * (x - p)) * (1.f / 32));
+}
+// the pivot of the two-pass and single-launch kernels: the sample's mean where it exceeds 8 of its standard deviations, else 0
+__device__ __forceinline__ float ln_pivot(const float* a, const float* r, long long R) {
+  const float2 m = ln_sample(a, r, R);
+  return m.x * m.x > 64.f * m.y ? m.x : 0.f;
+}
+// whether plain sums S = sum(x), Q = sum(x^2) of R values lose more than about 2 digits: mean^2 > 64 var, times R^2
+__device__ __forceinline__ bool ln_cancels(double S, double Q, long long R) { return S * S > 64.0 * (Q * (double)R - S * S); }
+// the V-wide chunk x - K
+template <int V> __device__ __forceinline__ vec_t<V> sub_pivot(vec_t<V> x, float K) {
+  return vmap([K](float v) { return v - K; }, x);
+}
+// mean and 1 / sqrt(var + eps) of R values from their sums about the pivot K
+__device__ __forceinline__ void ln_moments(float K, double S, double Q, long long R, float eps, float& mu, float& rstd) {
+  const double d = S / (double)R;
+  const double var = fmax(Q / (double)R - d * d, 0.0);
+  mu = (float)(K != 0.f ? (double)K + d : d);  // K = 0: the plain sums' mean, bit for bit (also its sign of zero)
+  rstd = (float)(1.0 / sqrt(var + (double)eps));
+}
 
 // CTA totals of the per-thread values v[0..K): warp sums, then thread 0 adds the NW warps' sums in warp order (no atomics,
 // the same bits every run).  The totals are left in thread 0's v.
@@ -367,18 +407,23 @@ __device__ __forceinline__ void sum_partials(const double* parts, int nparts, do
 
 template <int V>
 __global__ void __launch_bounds__(256) ln_stats_kernel(long long R, const float* __restrict__ a, const float* __restrict__ r,
-                                                       double* __restrict__ stats /*[B][2] sum, sumsq*/) {
+                                                       double* __restrict__ stats /*[B][2] sums about the pivot*/) {
   const int b = blockIdx.y;
   const float* ab = a + (size_t)b * R;
   const float* rb = r ? r + (size_t)b * R : nullptr;
-  double s = 0.0, q = 0.0;
   const long long start = V * ((long long)blockIdx.x * blockDim.x + threadIdx.x), step = V * (long long)gridDim.x * blockDim.x;
+  const long long c0 = min(start, R - V);  // the first chunk (clamped: always a valid load) is read together with the pivot
+  const vec_t<V> v0 = add_res(ldv<V>(ab, c0), rb, c0);
+  const float K = ln_pivot(ab, rb, R);
+  double s = 0.0, q = 0.0;
+  auto add = [&](vec_t<V> v) {
+    const vec_t<V> d = sub_pivot<V>(v, K);
+    s += fsum<double>(d);
+    q += fsq<double>(d);
+  };
+  if (start < R) add(v0);
 #pragma unroll 4
-  for (long long i = start; i < R; i += step) {
-    const vec_t<V> v = add_res(ldv<V>(ab, i), rb, i);
-    s += fsum<double>(v);
-    q += fsq<double>(v);
-  }
+  for (long long i = start + step; i < R; i += step) add(add_res(ldv<V>(ab, i), rb, i));
   block_sum2_store(s, q, stats + 2 * ((size_t)b * gridDim.x + blockIdx.x));
 }
 
@@ -388,18 +433,18 @@ __global__ void __launch_bounds__(256) ln_apply_kernel(long long R, float eps, c
                                                        const double* __restrict__ stats, float* __restrict__ y,
                                                        float* __restrict__ mean_rstd /*[B][2]*/) {
   const int b = blockIdx.y;
+  const float* ab = a + (size_t)b * R;
+  const float* rb = r ? r + (size_t)b * R : nullptr;
+  const float K = ln_pivot(ab, rb, R);  // loaded alongside the partials
   double S, Q;
   sum_partials(stats + 2 * (size_t)b * gridDim.x, gridDim.x, S, Q);
-  const double mean = S / (double)R;
-  const double var = fmax(Q / (double)R - mean * mean, 0.0);
-  const float rstd = (float)(1.0 / sqrt(var + (double)eps));
-  const float mu = (float)mean, g = gain ? *gain : 1.f, bi = bias ? *bias : 0.f;
+  float mu, rstd;
+  ln_moments(K, S, Q, R, eps, mu, rstd);
+  const float g = gain ? *gain : 1.f, bi = bias ? *bias : 0.f;
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     mean_rstd[2 * b] = mu;
     mean_rstd[2 * b + 1] = rstd;
   }
-  const float* ab = a + (size_t)b * R;
-  const float* rb = r ? r + (size_t)b * R : nullptr;
   float* yb = y + (size_t)b * R;
   const float sc = rstd * g;
   const long long start = V * ((long long)blockIdx.x * blockDim.x + threadIdx.x), step = V * (long long)gridDim.x * blockDim.x;
@@ -427,14 +472,16 @@ __global__ void __launch_bounds__(kLnFusedThreads, 2) ln_fused_fwd_kernel(long l
   const float* ab = a + (size_t)b * R;
   const float* rb = r ? r + (size_t)b * R : nullptr;
   float* yb = y + (size_t)b * R;
+  const float K = ln_pivot(ab, rb, R);
   double sq[2] = {0.0, 0.0};
 #pragma unroll 4
   for (long long i = lo + 4 * threadIdx.x; i < hi; i += 4 * kLnFusedThreads) {
     const float4 v = add_res(ldv<4>(ab, i), rb, i);
     const long long k = i - lo;
     if (k < keep) stv<4>(ln_sv, k, v);
-    sq[0] += fsum<double>(v);
-    sq[1] += fsq<double>(v);
+    const float4 d = sub_pivot<4>(v, K);
+    sq[0] += fsum<double>(d);
+    sq[1] += fsq<double>(d);
   }
   cta_sum<kLnFusedThreads / 32>(sq);
   if (threadIdx.x == 0) {
@@ -445,10 +492,9 @@ __global__ void __launch_bounds__(kLnFusedThreads, 2) ln_fused_fwd_kernel(long l
   cooperative_groups::this_grid().sync();
   double S, Q;
   sum_partials(scratch + 2 * (size_t)b * parts, parts, S, Q);
-  const double mean = S / (double)R;
-  const double var = fmax(Q / (double)R - mean * mean, 0.0);
-  const float rstd = (float)(1.0 / sqrt(var + (double)eps));
-  const float mu = (float)mean, g = gain ? *gain : 1.f, bi = bias ? *bias : 0.f;
+  float mu, rstd;
+  ln_moments(K, S, Q, R, eps, mu, rstd);
+  const float g = gain ? *gain : 1.f, bi = bias ? *bias : 0.f;
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     mean_rstd[2 * b] = mu;
     mean_rstd[2 * b + 1] = rstd;
@@ -519,7 +565,7 @@ __global__ void __launch_bounds__(256) ln_bwd_apply_kernel(long long R, const fl
 
 // ---- per-row variant: many short groups (per-frame LayerNorm of the streaming TDS family: R = C*W <= a few
 // thousand, groups = T*B).  One warp per group, two sweeps inside one kernel (the second hits L1), no scratch.
-// The sums are accumulated in float.
+// The sums about the pivot are accumulated in float per lane and combined in double.
 template <int V>
 __global__ void __launch_bounds__(256) ln_row_fwd_kernel(long long G, int R, float eps, const float* __restrict__ a,
                                                          const float* __restrict__ r, const float* __restrict__ gain,
@@ -531,15 +577,24 @@ __global__ void __launch_bounds__(256) ln_row_fwd_kernel(long long G, int R, flo
   const float* ab = a + grp * R;
   const float* rb = r ? r + grp * R : nullptr;
   float* yb = y + grp * R;
-  float s = 0.f, q = 0.f;
-  for (int i = V * lane; i < R; i += 32 * V) {
-    const vec_t<V> v = add_res(ldv<V>(ab, i), rb, i);
-    s += fsum<float>(v);
-    q += fsq<float>(v);
+  auto sums = [&](float K) {  // the group's (sum, sum of squares) about K
+    float s = 0.f, q = 0.f;
+    for (int i = V * lane; i < R; i += 32 * V) {
+      const vec_t<V> d = sub_pivot<V>(add_res(ldv<V>(ab, i), rb, i), K);
+      s += fsum<float>(d);
+      q += fsq<float>(d);
+    }
+    return make_double2(warp_sum((double)s), warp_sum((double)q));
+  };
+  // plain sums first; only a group where they cancel (a warp-uniform test) is summed again, from L1, about a pivot
+  float K = 0.f;
+  double2 SQ = sums(K);
+  if (ln_cancels(SQ.x, SQ.y, R)) {
+    K = ln_sample(ab, rb, R).x;
+    SQ = sums(K);
   }
-  const double S = warp_sum((double)s), Q = warp_sum((double)q);
-  const double mean = S / R, var = fmax(Q / R - mean * mean, 0.0);
-  const float mu = (float)mean, rstd = (float)(1.0 / sqrt(var + (double)eps));
+  float mu, rstd;
+  ln_moments(K, SQ.x, SQ.y, R, eps, mu, rstd);
   const float sc = rstd * (gain ? *gain : 1.f), bi = bias ? *bias : 0.f;
   if (lane == 0) {
     mean_rstd[2 * grp] = mu;
