@@ -396,15 +396,18 @@ W2L_API int w2l_mfsc(void* stream, int B, int max_samples, const float* audio, c
 /* ----------------------------------------------------------------------------------------
  * Training-step driver:the body of the reference loop (recipes/slimIPL/src/Train.cpp:1454-1803) written
  * in C++ against include/fl_compat/fl_compat.h — network forward, criterion, loss.backward(), NCCL
- * all-reduce of every gradient, division by the global batch size, clipGradNorm over net U criterion,
+ * all-reduce of every gradient, division by the global batch size, clipGradNorm over net U criterion (over the
+ * network alone for "linseg", whose transitions step unclipped, as Train.cpp's --linseg warm start does),
  * criterion + network SGD steps.  `arch_text` is a wav2letter arch file (opcodes V RO PD C2 R DO LN TDS L
- * SAUG), `criterion` "ctc" or "asg".  All pointers below are DEVICE pointers:
+ * SAUG), `criterion` "ctc", "asg" or "linseg".  All pointers below are DEVICE pointers:
  * features [T,F,1,B] (ArrayFire layout, T fastest), target [L,B] int32 (-1 padded), loss_out [B].
  * Returns NULL / a status code; w2l_last_error() has the text.
  * ---------------------------------------------------------------------------------------- */
 W2L_API void* w2l_trainer_create(void* stream, const char* arch_text, int n_feat, int n_label, const char* criterion,
                                  int scale_mode, float transdiag, float lr, float lrcrit, float momentum, float maxgradnorm);
 W2L_API void w2l_trainer_destroy(void* trainer);
+/* train != 0: backward, clip and update; total_batch (the batch summed over ranks, which divides every gradient) must
+ * then be finite and > 0, else W2L_ERR_INVALID_ARGUMENT and nothing runs.  train == 0: loss only, total_batch unused. */
 W2L_API int w2l_trainer_step(void* trainer, void* stream, int B, int T, const float* features, int L, const int32_t* target,
                              float* loss_out, int train, float total_batch);
 W2L_API int w2l_trainer_forward(void* trainer, void* stream, int B, int T, const float* features, float* emissions_out,

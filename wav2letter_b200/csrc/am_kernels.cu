@@ -777,10 +777,14 @@ __global__ void __launch_bounds__(256) sgd_step_kernel(long long n, float* __res
 }
 // the loop's numerical guards without a host round trip: Train.cpp:1686-1698 (NaN / Inf in the loss) and
 // :1753-1771 (non-finite gradients under mixed precision: skip the update).  guard[0] = this step is bad,
-// guard[1] += 1 per bad step (read by the host whenever it wants).
-__global__ void finite_guard_kernel(int n_loss, const float* __restrict__ loss, const double* __restrict__ sq_norm, int* __restrict__ guard) {
+// guard[1] += 1 per bad step (read by the host whenever it wants).  sq_norm[0 .. n_norm): the step's squared gradient norms.
+__global__ void finite_guard_kernel(int n_loss, const float* __restrict__ loss, int n_norm, const double* __restrict__ sq_norm,
+                                    int* __restrict__ guard) {
   __shared__ int bad;
-  if (threadIdx.x == 0) bad = (sq_norm != nullptr && !isfinite(*sq_norm)) ? 1 : 0;
+  if (threadIdx.x == 0) {
+    bad = 0;
+    for (int i = 0; i < n_norm; ++i) bad |= !isfinite(sq_norm[i]);
+  }
   __syncthreads();
   int b = 0;
   for (int i = threadIdx.x; i < n_loss; i += blockDim.x) b |= !isfinite(loss[i]);
@@ -1168,12 +1172,19 @@ extern "C" int w2l_sgd_step(void* stream_, long long n, float* params, const flo
                             float momentum, float weight_decay, float grad_scale, float max_grad_norm, const double* sq_norm) {
   return w2l_sgd_step_ex(stream_, n, params, grads, velocity, lr, momentum, weight_decay, grad_scale, max_grad_norm, sq_norm, 0, nullptr);
 }
-extern "C" int w2l_finite_guard(void* stream_, int n_loss, const float* loss, const double* sq_norm, int* guard) {
+// w2l_finite_guard over n_norm squared norms (the trainer keeps the norms of its clipped and unclipped gradients apart)
+namespace w2l {
+int finiteGuard(void* stream_, int n_loss, const float* loss, int n_norm, const double* sq_norm, int* guard) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (n_loss < 0 || (n_loss > 0 && !loss) || !guard) return fail(W2L_ERR_INVALID_ARGUMENT, "finite_guard: bad arguments");
-  finite_guard_kernel<<<1, 256, 0, stream>>>(n_loss, loss, sq_norm, guard);
+  if (n_loss < 0 || (n_loss > 0 && !loss) || n_norm < 0 || (n_norm > 0 && !sq_norm) || !guard)
+    return fail(W2L_ERR_INVALID_ARGUMENT, "finite_guard: bad arguments");
+  finite_guard_kernel<<<1, 256, 0, stream>>>(n_loss, loss, n_norm, sq_norm, guard);
   W2L_LAUNCH_CHECK("finite_guard_kernel");
   return W2L_OK;
+}
+}  // namespace w2l
+extern "C" int w2l_finite_guard(void* stream_, int n_loss, const float* loss, const double* sq_norm, int* guard) {
+  return w2l::finiteGuard(stream_, n_loss, loss, sq_norm ? 1 : 0, sq_norm, guard);
 }
 extern "C" int w2l_mask_bands(void* stream_, int B, int T, int C, int W, const float* x, float* y, int n_f, const int* f0_host,
                               const int* f1_host, int n_t, const int* t0_host, const int* t1_host, float value) {

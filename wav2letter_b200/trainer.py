@@ -101,7 +101,9 @@ class Trainer:
 
     def step(self, features: torch.Tensor, target: torch.Tensor, train: bool = True, total_batch: float | None = None,
              loss_out: torch.Tensor | None = None) -> torch.Tensor:
-        """features: CUDA float [B,1,F,T] contiguous (== ArrayFire [T,F,1,B]); target CUDA int32 [B,L]."""
+        """features: CUDA float [B,1,F,T] contiguous (== ArrayFire [T,F,1,B]); target CUDA int32 [B,L].
+        total_batch: the batch summed over ranks (default B); every gradient is divided by it.  A training step raises
+        W2LError (code 1) before running anything unless it is finite and > 0; an eval step does not use it."""
         B, _, F, T = features.shape
         L = target.shape[1]
         if loss_out is None:
