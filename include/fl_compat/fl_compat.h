@@ -280,7 +280,27 @@ class SpecAugment : public UnaryModule {
   int tWarpW_, fMaskF_, nFMask_, tMaskT_, nTMask_;
   double tMaskP_;
   std::mt19937_64 rng_;
+  friend class RandomReplay;
 };
+
+// The random draws of a network's forward passes on this thread (dropout seeds, SpecAugment bands), captured so that a
+// step can be run again on the same draws: from construction every seed drawn on this thread is recorded, together
+// with the state of every SpecAugment generator in `net` (through Sequential and WeightNorm); rewind() restores those
+// generators and hands out the recorded seeds again, in order, before drawing new ones.  One per thread at a time.
+class RandomReplay {
+ public:
+  explicit RandomReplay(const std::shared_ptr<Module>& net);
+  ~RandomReplay();
+  void rewind();
+
+ private:
+  std::vector<std::pair<SpecAugment*, std::mt19937_64>> gens_;
+};
+
+// Mixed-precision loss scaling (Train.cpp:1681-1684, loss * scaleFactor before backward): the criteria's fused backward
+// computes the gradient of scale * loss, so every backward tensor carries the scale; the loss values themselves are not
+// scaled.  Thread-local; 1 (the default) is off.
+void setLossGradScale(float scale);
 
 // fl::LayerNorm over axes {0,1,2} (whole sample) with the scalar affine the TDS archs use.
 class LayerNorm : public UnaryModule {

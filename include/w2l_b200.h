@@ -213,6 +213,9 @@ W2L_API int w2l_gemm_tf32_view(void* stream, int a_mn_major, int b_mn_major, int
  *           3xTF32 the same way.
  *   BF16  : bf16 operands in HBM (activations / weights cast by their producers), fp32 accumulation — the AMP mode of
  *           the reference (recipes/slimIPL/src/Train.cpp:211-219) with bf16 instead of fp16, configs[2]/[3].
+ *   FP16  : fp16 operands in HBM, fp32 accumulation — the reference's own AMP operand type
+ *           (--fl_amp_use_mixed_precision casts conv and matmul inputs to fp16); same layouts, tiles and MAC rate as BF16,
+ *           3 more significand bits, 3 fewer exponent bits (finite up to 65504).
  *   F32X3_SPLIT_B : F32X3 with B split ahead of the call by w2l_split_tf32: B is K-major only and points at
  *           [2][N][ldb] fp32, the tf32 hi plane then the lo plane (ldb % 4 == 0, ldb >= K).  Results are bit-identical
  *           to F32X3 on the unsplit B; the kernel loads both planes by TMA and converts nothing, which pays when B (a
@@ -220,13 +223,15 @@ W2L_API int w2l_gemm_tf32_view(void* stream, int a_mn_major, int b_mn_major, int
  * w2l_set_precision is thread-local and selects the kind used by the fp32-operand entry points (w2l_gemm_tf32*,
  * w2l_conv_time_*) and by the fl_compat modules (which cast their GEMM operands in BF16 mode and pre-split their
  * weights in F32 mode). */
-enum { W2L_GEMM_TF32 = 0, W2L_GEMM_F32X3 = 1, W2L_GEMM_BF16 = 2, W2L_GEMM_F32X3_SPLIT_B = 3 };
-enum { W2L_PRECISION_TF32 = 0, W2L_PRECISION_F32 = 1, W2L_PRECISION_BF16 = 2 };
+enum { W2L_GEMM_TF32 = 0, W2L_GEMM_F32X3 = 1, W2L_GEMM_BF16 = 2, W2L_GEMM_F32X3_SPLIT_B = 3, W2L_GEMM_FP16 = 4 };
+/* FP16 is BF16 mode with fp16 GEMM operands: the same layers cast the same operands, everything else is unchanged */
+enum { W2L_PRECISION_TF32 = 0, W2L_PRECISION_F32 = 1, W2L_PRECISION_BF16 = 2, W2L_PRECISION_FP16 = 3 };
 W2L_API int w2l_set_precision(int precision);
 W2L_API int w2l_get_precision(void);
-/* General form: A / B are fp32 (kinds TF32, F32X3) or bf16 (kind BF16) with lda / ldb in ELEMENTS (rows 16-byte aligned:
- * ld % 4 for fp32, ld % 8 for bf16); C is fp32 or bf16 (c_bf16; no accumulate / split-K then); aux (the backward mask
- * source) fp32 or bf16 (aux_bf16).  allow_overlap: operand rows may overlap (im2col views, see w2l_gemm_tf32_view). */
+/* General form: A / B are fp32 (kinds TF32, F32X3), bf16 (kind BF16) or fp16 (kind FP16) with lda / ldb in ELEMENTS (rows
+ * 16-byte aligned: ld % 4 for fp32, ld % 8 for 16-bit); C is fp32 or 16-bit (c_bf16; no accumulate / split-K then); aux
+ * (the backward mask source) fp32 or 16-bit (aux_bf16).  A 16-bit C or aux is fp16 for kind FP16 and bf16 for every other
+ * kind.  allow_overlap: operand rows may overlap (im2col views, see w2l_gemm_tf32_view). */
 W2L_API int w2l_gemm(void* stream, int kind, int a_mn_major, int b_mn_major, int M, int N, int K, const void* A, int lda,
                      const void* B, int ldb, void* C, int ldc, int c_bf16, const float* bias, int act, int accumulate,
                      const void* aux, int ld_aux, int aux_bf16, int aux_mode, float aux_scale, float dropout_p,
@@ -235,6 +240,9 @@ W2L_API int w2l_gemm(void* stream, int kind, int a_mn_major, int b_mn_major, int
  * ld_in, to rows of cols_padded bf16) */
 W2L_API int w2l_cast_bf16(void* stream, long long n, const float* x, void* y);
 W2L_API int w2l_cast_bf16_rows(void* stream, long long rows, int cols, int ld_in, int cols_padded, const float* x, void* y);
+/* the same to fp16 (round to nearest even; beyond 65504 becomes +-inf) */
+W2L_API int w2l_cast_fp16(void* stream, long long n, const float* x, void* y);
+W2L_API int w2l_cast_fp16_rows(void* stream, long long rows, int cols, int ld_in, int cols_padded, const float* x, void* y);
 /* x [rows][cols] fp32 (row stride ld) -> the B planes of W2L_GEMM_F32X3_SPLIT_B, hi = tf32(x), lo = tf32(x - hi) (round to
  * nearest, ties away, as the F32X3 kernel rounds):
  *   transpose = 0: planes [2][rows][cols_padded], plane[r][c] from x[r][c]  (B = x K-major: the forward's weight)
@@ -301,7 +309,8 @@ W2L_API int w2l_weightnorm_bwd(void* stream, int rows, int len, const float* v, 
                                const float* dw, float* dv, float* dg);
 W2L_API int w2l_conv1d_arrange(void* stream, int cin, int cout, int kw, int cin_p, int cout_p, int glu_split, const float* w,
                                const float* bias, float* fwd, float* flip, float* bias_p);
-/* the same with bf16 destination operands (out_bf16 != 0; W2L_PRECISION_BF16): fwd / flip are written as bf16 directly */
+/* the same with 16-bit destination operands, written directly: out_bf16 = 1 bf16 (W2L_PRECISION_BF16), 2 fp16
+ * (W2L_PRECISION_FP16); 0 is fp32 */
 W2L_API int w2l_conv1d_arrange_ex(void* stream, int cin, int cout, int kw, int cin_p, int cout_p, int glu_split, const float* w,
                                   const float* bias, void* fwd, void* flip, float* bias_p, int out_bf16);
 W2L_API int w2l_conv1d_unarrange_grad(void* stream, int cin, int cout, int kw, int cin_p, int cout_p, int glu_split,
@@ -428,6 +437,35 @@ W2L_API int w2l_trainer_set_grad_stream(void* trainer, int on);
 W2L_API int w2l_trainer_set_grad_stream_delay(void* trainer, int us);
 /* precision of the trainer's dense contractions (W2L_PRECISION_*; default: the creating thread's w2l_set_precision) */
 W2L_API int w2l_trainer_set_precision(void* trainer, int precision);
+/* Learning-rate schedule of Train.cpp:1169-1175, 1334-1348, applied on the host at every training step (no launch, no
+ * sync): with curBatch = the step's 1-based update number and curEpoch = the position's epoch,
+ *   lr = lr0 * 0.5^(curEpoch < lr_decay ? 0 : 1 + (curEpoch - lr_decay) / lr_decay_step)
+ *            * (lrcosine ? cos(pi/2 * curBatch / nbatches) : gamma^(curBatch / stepsize)) * min(curBatch / warmup, 1)
+ * in double, rounded to float; lrcrit the same from its lr0.  lr0 / lrcrit0 are w2l_trainer_create's lr / lrcrit (or
+ * w2l_trainer_set_lr's).  Every training step counts, including one whose update the finite guard skips.  Defaults
+ * (flashlight's flag defaults; the factor is then exactly 1): warmup 1, gamma 1, stepsize, nbatches, lr_decay and
+ * lr_decay_step INT64_MAX, lrcosine 0.  warmup = 0 means no warmup.
+ * set_position: the updates already taken (curBatch before the next step) and the epoch (Train.cpp's curEpoch, which is 1
+ * during the first epoch); w2l_trainer_position reads them back; w2l_trainer_lr gives the rates the next step uses. */
+W2L_API int w2l_trainer_set_schedule(void* trainer, long long warmup, double gamma, long long stepsize, int lrcosine, long long nbatches,
+                                     long long lr_decay, long long lr_decay_step);
+W2L_API int w2l_trainer_set_position(void* trainer, long long update, long long epoch);
+W2L_API int w2l_trainer_position(void* trainer, long long* update, long long* epoch);
+W2L_API int w2l_trainer_set_lr(void* trainer, float lr, float lrcrit);
+W2L_API int w2l_trainer_lr(void* trainer, float* lr, float* lrcrit);
+/* Mixed-precision loss scaling (Train.cpp:1135-1140, 1681-1684, 1748-1790, 1806-1818; --fl_amp_use_mixed_precision).
+ * With on = 1, each training step seeds the criterion's loss gradient with the scale (every backward tensor carries it)
+ * and divides it out in the update (gradients / (total_batch * scale)).  A step whose loss is finite and whose gradient
+ * is not, while scale >= min_scale, halves the scale and runs the same batch again on the same dropout seeds and
+ * SpecAugment bands (upstream draws new ones), so a retried step equals a first attempt at the final scale; it reads one
+ * flag from the device per attempt.  Otherwise a non-finite step is skipped and counted as before.  After each step the
+ * scale grows, below max_scale: x2 when the attempt counter (unsigned short, incremented per attempt, wrapping to 0,
+ * reset to 1 by a non-finite gradient) is a multiple of update_interval, else +2.  Reference defaults: 4096, 2000,
+ * 32000, min_scale 1e-4 (flashlight's kAmpMinimumScaleFactorValue).  Loss scaling works in every precision and pays in
+ * fp16.  set_amp resets the counter to 1 and the retry count to 0.  amp_state: the scale the next step starts at, the
+ * counter and the number of retried attempts; host state, no sync. */
+W2L_API int w2l_trainer_set_amp(void* trainer, int on, double initial_scale, int update_interval, double max_scale, double min_scale);
+W2L_API int w2l_trainer_amp_state(void* trainer, void* stream, double* scale, int* counter, long long* retries);
 /* steps whose update was skipped on the device because the loss or a gradient was NaN / Inf (Train.cpp:1686-1698,
  * :1753-1771); synchronises `stream` */
 W2L_API int w2l_trainer_status(void* trainer, void* stream, long long* skipped_steps);
@@ -438,7 +476,9 @@ W2L_API int w2l_trainer_set_flat(void* trainer, void* stream, int which, const f
 W2L_API int w2l_trainer_sync_parameters(void* trainer, void* stream);   /* fl::allReduceParameters, Train.cpp:1078-1079 */
 W2L_API const char* w2l_trainer_describe(void* trainer);
 /* Checkpoints (SURVEY.md §8 f4; the role of Serializer::save / load in Train.cpp:747-800): own little-endian container with
- * the constructor arguments + parameter / momentum arenas of network and criterion; load rebuilds the trainer. */
+ * the constructor arguments + parameter / momentum arenas of network and criterion, the position and the learning-rate
+ * schedule; load rebuilds the trainer.  Files written before the schedule existed load with position 0 and the default
+ * schedule. */
 W2L_API int w2l_trainer_save(void* trainer, void* stream, const char* path);
 W2L_API void* w2l_trainer_load(void* stream, const char* path);
 /* Export for the in-tree streaming inference stack, following the conversions of

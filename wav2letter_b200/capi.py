@@ -27,8 +27,10 @@ EXPORTS = [
     "w2l_fac_viterbi_workspace_size", "w2l_fac_viterbi",
     "w2l_ctc_workspace_size", "w2l_ctc_forward_backward", "w2l_argmax_path", "w2l_linseg_target",
     "w2l_ctc_viterbi_workspace_size", "w2l_ctc_viterbi_target",
-    "w2l_set_precision", "w2l_get_precision", "w2l_gemm", "w2l_cast_bf16", "w2l_cast_bf16_rows", "w2l_split_tf32", "w2l_sgd_step_ex", "w2l_finite_guard",
+    "w2l_set_precision", "w2l_get_precision", "w2l_gemm", "w2l_cast_bf16", "w2l_cast_bf16_rows", "w2l_cast_fp16", "w2l_cast_fp16_rows", "w2l_split_tf32", "w2l_sgd_step_ex", "w2l_finite_guard",
     "w2l_mask_bands", "w2l_trainer_set_precision", "w2l_trainer_set_grad_stream", "w2l_trainer_set_grad_stream_delay", "w2l_delay", "w2l_trainer_status", "w2l_trainer_save", "w2l_trainer_load", "w2l_trainer_export_streaming",
+    "w2l_trainer_set_schedule", "w2l_trainer_set_position", "w2l_trainer_position", "w2l_trainer_set_lr", "w2l_trainer_lr",
+    "w2l_trainer_set_amp", "w2l_trainer_amp_state",
     "w2l_text_create", "w2l_text_destroy", "w2l_text_num_classes", "w2l_text_encode", "w2l_text_prediction2ltr", "w2l_text_target2ltr",
     "w2l_text_ltr2wrd", "w2l_text_align_words", "w2l_edit_distance",
     "w2l_gemm_set_variant", "w2l_gemm_set_tile", "w2l_gemm_tf32", "w2l_gemm_tf32_ex", "w2l_gemm_tf32_view", "w2l_conv_time_workspace_size", "w2l_conv_time_fwd", "w2l_conv_time_dgrad",
@@ -121,11 +123,20 @@ def _load() -> ctypes.CDLL:
     lib.w2l_gemm.argtypes = [vp, i, i, i, i, i, i, vp, i, vp, i, vp, i, i, vp, i, i, vp, i, i, i, f32, f32, u64, i]
     lib.w2l_cast_bf16.argtypes = [vp, ll, vp, vp]
     lib.w2l_cast_bf16_rows.argtypes = [vp, ll, i, i, i, vp, vp]
+    lib.w2l_cast_fp16.argtypes = [vp, ll, vp, vp]
+    lib.w2l_cast_fp16_rows.argtypes = [vp, ll, i, i, i, vp, vp]
     lib.w2l_split_tf32.argtypes = [vp, i, i, i, i, i, vp, vp]
     lib.w2l_sgd_step_ex.argtypes = [vp, ll, vp, vp, vp, f32, f32, f32, f32, f32, vp, i, vp]
     lib.w2l_finite_guard.argtypes = [vp, i, vp, vp, vp]
     lib.w2l_mask_bands.argtypes = [vp, i, i, i, i, vp, vp, i, vp, vp, i, vp, vp, f32]
     lib.w2l_trainer_set_precision.argtypes = [vp, i]
+    lib.w2l_trainer_set_schedule.argtypes = [vp, ll, ctypes.c_double, ll, i, ll, ll, ll]
+    lib.w2l_trainer_set_position.argtypes = [vp, ll, ll]
+    lib.w2l_trainer_position.argtypes = [vp, vp, vp]
+    lib.w2l_trainer_set_lr.argtypes = [vp, ctypes.c_float, ctypes.c_float]
+    lib.w2l_trainer_lr.argtypes = [vp, vp, vp]
+    lib.w2l_trainer_set_amp.argtypes = [vp, i, ctypes.c_double, i, ctypes.c_double, ctypes.c_double]
+    lib.w2l_trainer_amp_state.argtypes = [vp, vp, vp, vp, vp]
     lib.w2l_trainer_set_grad_stream.argtypes = [vp, i]
     lib.w2l_trainer_set_grad_stream_delay.argtypes = [vp, i]
     lib.w2l_delay.argtypes = [vp, i]
@@ -424,12 +435,13 @@ def trace_list() -> list:
     return [(ln.split("\t")[0], float(ln.split("\t")[1])) for ln in buf.value.decode().splitlines()]
 
 
-PRECISIONS = {"tf32": 0, "f32": 1, "fp32": 1, "bf16": 2}
-GEMM_KINDS = {"tf32": 0, "f32x3": 1, "bf16": 2, "f32x3_split_b": 3}
+PRECISIONS = {"tf32": 0, "f32": 1, "fp32": 1, "bf16": 2, "fp16": 3}
+GEMM_KINDS = {"tf32": 0, "f32x3": 1, "bf16": 2, "f32x3_split_b": 3, "fp16": 4}
 
 
 def set_precision(p) -> None:
-    """tf32 (default) | f32 (fp32-accurate 3xTF32 GEMMs and mma.sync time convolutions) | bf16 (bf16 GEMM operands)."""
+    """tf32 (default) | f32 (fp32-accurate 3xTF32 GEMMs and mma.sync time convolutions) | bf16 (bf16 GEMM operands) |
+    fp16 (fp16 GEMM operands)."""
     _check(lib.w2l_set_precision(PRECISIONS[p] if isinstance(p, str) else int(p)))
 
 
@@ -439,18 +451,23 @@ def get_precision() -> int:
 
 def gemm(A, B, kind="tf32", a_mn=False, b_mn=False, bias=None, act=0, out=None, out_bf16=False, accumulate=False, aux=None,
          aux_mode=0, aux_scale=1.0, dropout_p=0.0, seed=0, M=None, N=None, K=None, lda=None, ldb=None, allow_overlap=False):
-    """General wgmma GEMM (w2l_gemm): A/B fp32 (kinds tf32, f32x3) or bfloat16 (kind bf16); C fp32 or bfloat16.
+    """General wgmma GEMM (w2l_gemm): A/B fp32 (kinds tf32, f32x3), bfloat16 (kind bf16) or float16 (kind fp16); C fp32 or
+    16-bit (out_bf16: float16 for kind fp16, bfloat16 otherwise), aux likewise.
     Kind f32x3_split_b: B is the [2][N][ldb] planes of split_tf32 (K is taken from A)."""
     if M is None:
         M, K = (A.shape[1], A.shape[0]) if a_mn else A.shape
         N = B.shape[-2] if B.dim() == 3 else (B.shape[1] if b_mn else B.shape[0])
     lda = A.stride(0) if lda is None else lda
     ldb = B.stride(-2) if ldb is None else ldb
+    kind_id = GEMM_KINDS[kind] if isinstance(kind, str) else int(kind)
+    half = torch.float16 if kind_id == GEMM_KINDS["fp16"] else torch.bfloat16  # the kind's 16-bit C / aux type
     if out is None:
-        out = torch.empty((M, N), dtype=torch.bfloat16 if out_bf16 else torch.float32, device=A.device)
-    _check(lib.w2l_gemm(_stream(), GEMM_KINDS[kind], int(a_mn), int(b_mn), M, N, K, _ptr(A), lda, _ptr(B), ldb, _ptr(out),
-                        out.stride(0), int(out.dtype == torch.bfloat16), _ptr(bias), int(act), int(accumulate), _ptr(aux),
-                        0 if aux is None else aux.stride(0), int(aux is not None and aux.dtype == torch.bfloat16),
+        out = torch.empty((M, N), dtype=half if out_bf16 else torch.float32, device=A.device)
+    if out.dtype not in (torch.float32, half) or (aux is not None and aux.dtype not in (torch.float32, half)):
+        raise TypeError(f"gemm: a 16-bit C or aux of kind {kind} is {half}")
+    _check(lib.w2l_gemm(_stream(), kind_id, int(a_mn), int(b_mn), M, N, K, _ptr(A), lda, _ptr(B), ldb, _ptr(out),
+                        out.stride(0), int(out.dtype == half), _ptr(bias), int(act), int(accumulate), _ptr(aux),
+                        0 if aux is None else aux.stride(0), int(aux is not None and aux.dtype == half),
                         int(aux_mode), float(aux_scale), float(dropout_p), int(seed), int(allow_overlap)))
     return out
 
@@ -459,6 +476,23 @@ def cast_bf16(x):
     x = _req(x, torch.float32, "x")
     y = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
     _check(lib.w2l_cast_bf16(_stream(), x.numel(), _ptr(x), _ptr(y)))
+    return y
+
+
+def cast_fp16(x):
+    x = _req(x, torch.float32, "x")
+    y = torch.empty(x.shape, dtype=torch.float16, device=x.device)
+    _check(lib.w2l_cast_fp16(_stream(), x.numel(), _ptr(x), _ptr(y)))
+    return y
+
+
+def cast_fp16_rows(x, cols_padded):
+    """rows of a 2-D fp32 tensor (rows contiguous) -> [rows][cols_padded] float16, zero-padded columns"""
+    x = _req(x, torch.float32, "x")
+    if x.dim() != 2 or x.stride(1) != 1:
+        raise TypeError("cast_fp16_rows: x must be 2-D with contiguous rows")
+    y = torch.empty((x.shape[0], cols_padded), dtype=torch.float16, device=x.device)
+    _check(lib.w2l_cast_fp16_rows(_stream(), x.shape[0], x.shape[1], x.stride(0), cols_padded, _ptr(x), _ptr(y)))
     return y
 
 

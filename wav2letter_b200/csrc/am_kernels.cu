@@ -778,21 +778,26 @@ __global__ void __launch_bounds__(256) sgd_step_kernel(long long n, float* __res
 // the loop's numerical guards without a host round trip: Train.cpp:1686-1698 (NaN / Inf in the loss) and
 // :1753-1771 (non-finite gradients under mixed precision: skip the update).  guard[0] = this step is bad,
 // guard[1] += 1 per bad step (read by the host whenever it wants).  sq_norm[0 .. n_norm): the step's squared gradient norms.
+// retry (nullable): a step whose loss is finite and whose gradient norm is not is run again at a smaller loss scale:
+// *retry = 1 and it is not counted in guard[1]; otherwise *retry = 0.
 __global__ void finite_guard_kernel(int n_loss, const float* __restrict__ loss, int n_norm, const double* __restrict__ sq_norm,
-                                    int* __restrict__ guard) {
-  __shared__ int bad;
+                                    int* __restrict__ guard, int* __restrict__ retry) {
+  __shared__ int bad_norm, bad_loss;
   if (threadIdx.x == 0) {
-    bad = 0;
-    for (int i = 0; i < n_norm; ++i) bad |= !isfinite(sq_norm[i]);
+    bad_norm = 0;
+    bad_loss = 0;
+    for (int i = 0; i < n_norm; ++i) bad_norm |= !isfinite(sq_norm[i]);
   }
   __syncthreads();
   int b = 0;
   for (int i = threadIdx.x; i < n_loss; i += blockDim.x) b |= !isfinite(loss[i]);
-  if (b) atomicOr(&bad, 1);
+  if (b) atomicOr(&bad_loss, 1);
   __syncthreads();
   if (threadIdx.x == 0) {
+    const int bad = bad_norm | bad_loss, again = retry != nullptr && bad_norm && !bad_loss;
     guard[0] = bad;
-    if (bad) guard[1] += 1;
+    if (bad && !again) guard[1] += 1;
+    if (retry != nullptr) *retry = again;
   }
 }
 
@@ -1174,17 +1179,17 @@ extern "C" int w2l_sgd_step(void* stream_, long long n, float* params, const flo
 }
 // w2l_finite_guard over n_norm squared norms (the trainer keeps the norms of its clipped and unclipped gradients apart)
 namespace w2l {
-int finiteGuard(void* stream_, int n_loss, const float* loss, int n_norm, const double* sq_norm, int* guard) {
+int finiteGuard(void* stream_, int n_loss, const float* loss, int n_norm, const double* sq_norm, int* guard, int* retry) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (n_loss < 0 || (n_loss > 0 && !loss) || n_norm < 0 || (n_norm > 0 && !sq_norm) || !guard)
     return fail(W2L_ERR_INVALID_ARGUMENT, "finite_guard: bad arguments");
-  finite_guard_kernel<<<1, 256, 0, stream>>>(n_loss, loss, n_norm, sq_norm, guard);
+  finite_guard_kernel<<<1, 256, 0, stream>>>(n_loss, loss, n_norm, sq_norm, guard, retry);
   W2L_LAUNCH_CHECK("finite_guard_kernel");
   return W2L_OK;
 }
 }  // namespace w2l
 extern "C" int w2l_finite_guard(void* stream_, int n_loss, const float* loss, const double* sq_norm, int* guard) {
-  return w2l::finiteGuard(stream_, n_loss, loss, sq_norm ? 1 : 0, sq_norm, guard);
+  return w2l::finiteGuard(stream_, n_loss, loss, sq_norm ? 1 : 0, sq_norm, guard, nullptr);
 }
 extern "C" int w2l_mask_bands(void* stream_, int B, int T, int C, int W, const float* x, float* y, int n_f, const int* f0_host,
                               const int* f1_host, int n_t, const int* t0_host, const int* t1_host, float value) {

@@ -73,8 +73,8 @@ void set_profile_events(cudaEvent_t a, cudaEvent_t b) {
 extern "C" {
 int w2l_version(void) { return 200; }
 int w2l_set_precision(int precision) {
-  if (precision != W2L_PRECISION_TF32 && precision != W2L_PRECISION_F32 && precision != W2L_PRECISION_BF16)
-    return w2l::fail(W2L_ERR_INVALID_ARGUMENT, "precision must be W2L_PRECISION_TF32, W2L_PRECISION_F32 or W2L_PRECISION_BF16");
+  if (precision != W2L_PRECISION_TF32 && precision != W2L_PRECISION_F32 && precision != W2L_PRECISION_BF16 && precision != W2L_PRECISION_FP16)
+    return w2l::fail(W2L_ERR_INVALID_ARGUMENT, "precision must be W2L_PRECISION_TF32, W2L_PRECISION_F32, W2L_PRECISION_BF16 or W2L_PRECISION_FP16");
   w2l::set_precision_value(precision);
   return W2L_OK;
 }

@@ -15,7 +15,10 @@
 //                   weight B that would otherwise be converted once per row of output tiles
 //   W2L_GEMM_BF16   bf16 operands in HBM — half the operand bytes, twice the MAC rate
 //                   (configs[2]/[3] "bf16 convs / fp32 loss"; the reference's AMP switch, Train.cpp:211-219)
-// C is fp32 or bf16 (c_bf16); bias / ReLU / dropout / mask / accumulate epilogue.
+//   W2L_GEMM_FP16   fp16 operands in HBM: the BF16 kind with the operand type the reference's AMP switch casts to.  One
+//                   template with BF16 (k16 below): the element type only selects the wgmma type, the tensor map type
+//                   and the type of a 16-bit C / aux
+// C is fp32 or 16-bit (c_bf16: bf16, fp16 for the FP16 kind); bias / ReLU / dropout / mask / accumulate epilogue.
 //
 // Operand storage ("major"):
 //   A K-major : A stored [M][K] (row stride lda)      A MN-major : A stored [K][M]
@@ -52,12 +55,14 @@
 //                  B: one unswizzled box [32 k-rows][BN], converted before use
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
 #include <mutex>
+#include <type_traits>
 
 #include "common.cuh"
 #include "tma_ptx.cuh"
@@ -73,12 +78,29 @@ constexpr int kTileBytes = BM * kRowBytes;  // 16 KB of A per stage
 constexpr int kGemmThreads = 384;
 constexpr int kConvThreads = 96;            // warps 1..3
 constexpr int kConsumerThreads = 256;       // warpgroups 1, 2
-enum { kTf32 = W2L_GEMM_TF32, kF32x3 = W2L_GEMM_F32X3, kBf16 = W2L_GEMM_BF16, kF32x3SplitB = W2L_GEMM_F32X3_SPLIT_B };
+enum { kTf32 = W2L_GEMM_TF32, kF32x3 = W2L_GEMM_F32X3, kBf16 = W2L_GEMM_BF16, kF32x3SplitB = W2L_GEMM_F32X3_SPLIT_B, kFp16 = W2L_GEMM_FP16 };
+// the kinds with 16-bit operands (64 elements of k per 128-byte row, m64nNk16, MN-major operands through the transpose bits)
+__host__ __device__ constexpr bool k16(int mode) { return mode == kBf16 || mode == kFp16; }
+// the 16-bit type of a kind's 16-bit C and aux: fp16 for FP16, bf16 for every other kind
+template <int kMode>
+using Half = typename std::conditional<kMode == kFp16, __half, __nv_bfloat16>::type;
+__device__ __forceinline__ float to_float(__nv_bfloat16 x) { return __bfloat162float(x); }
+__device__ __forceinline__ float to_float(__half x) { return __half2float(x); }
+template <typename H>
+__device__ __forceinline__ H from_float(float x);
+template <>
+__device__ __forceinline__ __nv_bfloat16 from_float<__nv_bfloat16>(float x) { return __float2bfloat16_rn(x); }
+template <>
+__device__ __forceinline__ __half from_float<__half>(float x) { return __float2half_rn(x); }
+__device__ __forceinline__ void from_float2(float x, float y, __nv_bfloat162* d) { *d = __floats2bfloat162_rn(x, y); }
+__device__ __forceinline__ void from_float2(float x, float y, __half2* d) { *d = __floats2half2_rn(x, y); }
+template <typename H>
+using Half2 = typename std::conditional<std::is_same<H, __half>::value, __half2, __nv_bfloat162>::type;
 
 // The raw ring's stages hold the TMA tiles [A | B] ([A | B hi | B lo] for F32X3_SPLIT_B); the converted kinds add a ring
 // of converted B stages, [hi B] or [hi B | lo B] for F32X3.  Unconverted kinds: as many raw stages as fit in 227 KB, at
 // most 6 (4 for F32X3_SPLIT_B).  Converted kinds: 4 raw stages, the rest of the 227 KB for converted stages (at most 4).
-// BN is 128 / 160 / 224 / 256 for unconverted TF32, 128 / 256 for BF16, 128 for the kinds that take A from registers
+// BN is 128 / 160 / 224 / 256 for unconverted TF32, 128 / 256 for BF16 and FP16, 128 for the kinds that take A from registers
 // (accumulators plus two A fragment sets must fit in registers).
 __host__ __device__ constexpr bool converts(int mode, bool a_mn, bool b_mn) { return mode == kF32x3 || (mode == kTf32 && (a_mn || b_mn)); }
 __host__ __device__ constexpr bool a_in_regs(int mode, bool a_mn, bool b_mn) { return converts(mode, a_mn, b_mn) || mode == kF32x3SplitB; }
@@ -147,7 +169,8 @@ __device__ __forceinline__ void convert_tile(const unsigned char* raw, unsigned 
   }
 }
 
-// Epilogue of one accumulator pair: columns col, col + 1 of one row (col is even).
+// Epilogue of one accumulator pair: columns col, col + 1 of one row (col is even).  H: the type of a 16-bit C / aux.
+template <typename H>
 __device__ __forceinline__ void epilogue_pair(const GemmParams& p, int z, int row, int col, float x0, float x1, float b0, float b1, bool vec_c) {
   const bool two = col + 1 < p.N;
   x0 += b0;
@@ -176,9 +199,9 @@ __device__ __forceinline__ void epilogue_pair(const GemmParams& p, int z, int ro
     float m0, m1 = 0.f;
     const size_t ai = (size_t)row * p.ld_aux + col;
     if (p.aux_bf16) {
-      const __nv_bfloat16* a = static_cast<const __nv_bfloat16*>(p.aux) + ai;
-      m0 = __bfloat162float(a[0]);
-      if (two) m1 = __bfloat162float(a[1]);
+      const H* a = static_cast<const H*>(p.aux) + ai;
+      m0 = to_float(a[0]);
+      if (two) m1 = to_float(a[1]);
     } else {
       const float* a = static_cast<const float*>(p.aux) + ai;
       m0 = a[0];
@@ -194,12 +217,12 @@ __device__ __forceinline__ void epilogue_pair(const GemmParams& p, int z, int ro
   }
   const size_t ci = (size_t)row * p.ldc + col;
   if (p.c_bf16) {
-    __nv_bfloat16* dst = static_cast<__nv_bfloat16*>(p.C) + ci;
+    H* dst = static_cast<H*>(p.C) + ci;
     if (two && vec_c) {
-      *reinterpret_cast<__nv_bfloat162*>(dst) = __floats2bfloat162_rn(x0, x1);
+      from_float2(x0, x1, reinterpret_cast<Half2<H>*>(dst));
     } else {
-      dst[0] = __float2bfloat16_rn(x0);
-      if (two) dst[1] = __float2bfloat16_rn(x1);
+      dst[0] = from_float<H>(x0);
+      if (two) dst[1] = from_float<H>(x1);
     }
     return;
   }
@@ -233,16 +256,16 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
                   unsigned int* sched) {  // [claimed, finished CTAs] counters of the dynamic schedule; null: CTA b walks b, b + grid, ...
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  constexpr bool kIsBf16 = kMode == kBf16, kPreSplit = kMode == kF32x3SplitB, kSplit = kMode == kF32x3 || kPreSplit;
+  constexpr bool kIs16 = k16(kMode), kPreSplit = kMode == kF32x3SplitB, kSplit = kMode == kF32x3 || kPreSplit;
   constexpr bool kConv = converts(kMode, kAMn, kBMn), kRegA = a_in_regs(kMode, kAMn, kBMn);
-  constexpr int BKE = kRowBytes / (kIsBf16 ? 2 : 4);  // elements of k per stage: 32 fp32 / 64 bf16
+  constexpr int BKE = kRowBytes / (kIs16 ? 2 : 4);  // elements of k per stage: 32 fp32 / 64 bf16 or fp16
   constexpr int kStages = raw_stages(kMode, kAMn, kBMn, BN), kCvtStages = cvt_stages(kMode, kAMn, kBMn, BN);
   constexpr size_t kRaw = raw_bytes(kMode, BN), kCvt = cvt_bytes(kMode, BN);
   constexpr uint32_t kOperandBytes = (uint32_t)kRaw;
   static_assert(kStages >= 2 && (!kConv || kCvtStages >= 2), "gemm: at least two stages per ring");
   static_assert(!kRegA || BN == 128, "gemm: the kinds that take A from registers run at BN = 128");
   static_assert(!kPreSplit || !kBMn, "gemm: pre-split B planes are K-major");
-  static_assert(!kIsBf16 || !kBMn || BN % 64 == 0, "gemm: MN-major bf16 B is staged in boxes of 64 columns");
+  static_assert(!kIs16 || !kBMn || BN % 64 == 0, "gemm: MN-major 16-bit B is staged in boxes of 64 columns");
   unsigned char* cvt_ring = smem + kStages * kRaw;
   uint64_t* bars = reinterpret_cast<uint64_t*>(cvt_ring + kCvtStages * kCvt);
   uint64_t* full = bars;                       // raw stage landed (TMA transaction count)
@@ -321,7 +344,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
             const int k0 = (kb_begin + kb) * BKE;
             if (!kAMn) {
               tma_load_2d(&map_a, &full[s], sa, k0, m0);  // box {128 B of k, 128 rows}
-            } else if (kIsBf16) {
+            } else if (kIs16) {
 #pragma unroll
               for (int j = 0; j < BM / 64; ++j) tma_load_2d(&map_a, &full[s], sa + j * 8192, m0 + 64 * j, k0);  // box {64 m, 64 k}
             } else {
@@ -333,7 +356,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
               tma_load_3d(&map_b, &full[s], sb + BN * kRowBytes, k0, n0, 1);
             } else if (!kBMn) {
               tma_load_2d(&map_b, &full[s], sb, k0, n0);
-            } else if (kIsBf16) {
+            } else if (kIs16) {
 #pragma unroll
               for (int j = 0; j < BN / 64; ++j) tma_load_2d(&map_b, &full[s], sb + j * 8192, n0 + 64 * j, k0);
             } else {
@@ -476,10 +499,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
 #pragma unroll
           for (int k = 0; k < 4; ++k) {
             const int sc = (kb | k) != 0;
-            if constexpr (kIsBf16) {
+            if constexpr (kIs16) {
               const uint64_t da = kAMn ? make_desc_sw128(a_base + k * 2048, 8192, 1024) : make_desc_sw128(a_base + k * 32, 16, 1024);
               const uint64_t db = kBMn ? make_desc_sw128(b_base + k * 2048, 8192, 1024) : make_desc_sw128(b_base + k * 32, 16, 1024);
-              wg::mma_bf16<BN, kAMn ? 1 : 0, kBMn ? 1 : 0>(acc, da, db, sc);
+              if constexpr (kMode == kFp16) wg::mma_f16<BN, kAMn ? 1 : 0, kBMn ? 1 : 0>(acc, da, db, sc);
+              else wg::mma_bf16<BN, kAMn ? 1 : 0, kBMn ? 1 : 0>(acc, da, db, sc);
             } else {
               wg::mma_tf32<BN>(acc, make_desc_sw128(a_base + k * 32, 16, 1024), make_desc_sw128(b_base + k * 32, 16, 1024), sc);
             }
@@ -502,8 +526,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_consta
         if (col < p.N) {
           const float b0 = p.bias != nullptr ? __ldg(p.bias + col) : 0.f;
           const float b1 = (p.bias != nullptr && col + 1 < p.N) ? __ldg(p.bias + col + 1) : 0.f;
-          if (row0 < p.M) epilogue_pair(p, z, row0, col, acc[4 * j], acc[4 * j + 1], b0, b1, vec_c);
-          if (row0 + 8 < p.M) epilogue_pair(p, z, row0 + 8, col, acc[4 * j + 2], acc[4 * j + 3], b0, b1, vec_c);
+          if (row0 < p.M) epilogue_pair<Half<kMode>>(p, z, row0, col, acc[4 * j], acc[4 * j + 1], b0, b1, vec_c);
+          if (row0 + 8 < p.M) epilogue_pair<Half<kMode>>(p, z, row0 + 8, col, acc[4 * j + 2], acc[4 * j + 3], b0, b1, vec_c);
         }
       }
     }
@@ -559,13 +583,16 @@ int make_map(CUtensorMap* map, int mode, bool raw, const void* ptr, long long ro
              bool swizzle, int planes = 1) {
   EncodeTiledFn fn = encode_fn();
   if (!fn) return fail(W2L_ERR_CUDA, "gemm: cuTensorMapEncodeTiled entry point not found");
-  const int es = mode == kBf16 ? 2 : 4;
+  const int es = k16(mode) ? 2 : 4;
   cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)planes};
   cuuint64_t strides[2] = {(cuuint64_t)ld * es, (cuuint64_t)(rows * ld * es)};
   cuuint32_t box[3] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows, 1};
   cuuint32_t estr[3] = {1, 1, 1};
   // TF32 read directly by wgmma: rounded on load; operands split or converted on chip: the raw fp32 bits
-  const CUtensorMapDataType dt = mode == kBf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : (raw ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_TFLOAT32);
+  const CUtensorMapDataType dt = mode == kBf16   ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                 : mode == kFp16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
+                                 : raw           ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                                 : CU_TENSOR_MAP_DATA_TYPE_TFLOAT32;
   CUresult r = fn(map, dt, planes > 1 ? 3 : 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -576,6 +603,7 @@ int make_map(CUtensorMap* map, int mode, bool raw, const void* ptr, long long ro
 const char* kernel_name(int mode) {
   switch (mode) {
     case kBf16: return "gemm_wgmma_kernel<bf16>";
+    case kFp16: return "gemm_wgmma_kernel<fp16>";
     case kF32x3: return "gemm_wgmma_kernel<f32x3>";
     case kF32x3SplitB: return "gemm_wgmma_kernel<f32x3_split_b>";
     default: return "gemm_wgmma_kernel<tf32>";
@@ -632,7 +660,7 @@ template <int kMode, bool kAMn, bool kBMn>
 int launch_mode(cudaStream_t stream, int bn, const CUtensorMap& ma, const CUtensorMap& mb, const GemmParams& p) {
   if constexpr (a_in_regs(kMode, kAMn, kBMn)) {
     return launch_bn<kMode, kAMn, kBMn, 128>(stream, ma, mb, p);
-  } else if constexpr (kMode == kBf16) {  // 128 or 256 (MN-major B is staged in 64-wide boxes)
+  } else if constexpr (k16(kMode)) {  // 128 or 256 (MN-major B is staged in 64-wide boxes)
     return bn <= 128 ? launch_bn<kMode, kAMn, kBMn, 128>(stream, ma, mb, p) : launch_bn<kMode, kAMn, kBMn, 256>(stream, ma, mb, p);
   } else {
     switch (bn) {
@@ -667,7 +695,7 @@ thread_local int g_force_bn = 0;  // w2l_gemm_set_tile: tests pin the tile width
 int choose_bn(int mode, bool a_mn, bool b_mn, int M, int N, int total_kb, bool plain, int* splits_out) {
   auto allowed = [&](int bn) {
     if (a_in_regs(mode, a_mn, b_mn)) return bn == 128;
-    if (mode == kBf16) return bn == 128 || bn == 256;
+    if (k16(mode)) return bn == 128 || bn == 256;
     return true;
   };
   if (g_force_bn && allowed(g_force_bn)) {
@@ -700,7 +728,7 @@ int gemm_impl(void* stream_, int mode, int a_mn_major, int b_mn_major, int M, in
               void* C, int ldc, int c_bf16, const float* bias, int act, int accumulate, const void* aux, int ld_aux, int aux_bf16,
               int aux_mode, float aux_scale, float dropout_p, unsigned long long seed, bool allow_overlap, bool allow_split_k = true) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (mode != kTf32 && mode != kF32x3 && mode != kBf16 && mode != kF32x3SplitB) return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: unknown operand kind");
+  if (mode != kTf32 && mode != kF32x3 && mode != kBf16 && mode != kF32x3SplitB && mode != kFp16) return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: unknown operand kind");
   if (mode == kF32x3SplitB && b_mn_major) return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: F32X3_SPLIT_B takes K-major B planes");
   if (M <= 0 || N <= 0 || K <= 0) return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: M, N, K must be positive");
   if (!A || !B || !C) return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: null pointer");
@@ -709,40 +737,41 @@ int gemm_impl(void* stream_, int mode, int a_mn_major, int b_mn_major, int M, in
     return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: bad aux mask arguments");
   if (dropout_p < 0.f || dropout_p >= 1.f) return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: dropout_p must be in [0, 1)");
   if (dropout_p > 0.f && N % 4 != 0) return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: dropout needs N % 4 == 0");
-  const int row_align = mode == kBf16 ? 8 : 4;  // elements per 16 bytes
+  const int row_align = k16(mode) ? 8 : 4;  // elements per 16 bytes
   if ((lda % row_align) || (ldb % row_align) || (reinterpret_cast<uintptr_t>(A) & 15) || (reinterpret_cast<uintptr_t>(B) & 15))
-    return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: operand rows must be 16-byte aligned (ld % 4 == 0 for fp32, ld % 8 == 0 for bf16)");
+    return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: operand rows must be 16-byte aligned (ld % 4 == 0 for fp32, ld % 8 == 0 for bf16 / fp16)");
   if (ldc < N || (!allow_overlap && (lda < (a_mn_major ? M : K) || ldb < (b_mn_major ? N : K))))
     return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: leading dimension smaller than the row length");
   if (lda <= 0 || ldb <= 0) return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: non-positive leading dimension");
   if (c_bf16 && accumulate) return fail(W2L_ERR_INVALID_ARGUMENT, "gemm: accumulation needs an fp32 C");
-  const int bke = kRowBytes / (mode == kBf16 ? 2 : 4);
+  const int bke = kRowBytes / (k16(mode) ? 2 : 4);
   const int total_kb = (K + bke - 1) / bke;
   const bool plain = act == 0 && aux_mode == 0 && dropout_p == 0.f && bias == nullptr && !c_bf16;
   int splits = 1;
   const int BN = choose_bn(mode, a_mn_major != 0, b_mn_major != 0, M, N, total_kb, plain && allow_split_k, &splits);
   const bool raw = a_in_regs(mode, a_mn_major != 0, b_mn_major != 0);
-  const bool bf16 = mode == kBf16;
+  const bool half = k16(mode);
   CUtensorMap ma, mb;
   int rc;
-  // K-major: box {128 B of k, tile rows}, 128B swizzle.  MN-major bf16: box {64 m/n, 64 k}, 128B swizzle.  MN-major fp32:
+  // K-major: box {128 B of k, tile rows}, 128B swizzle.  MN-major 16-bit: box {64 m/n, 64 k}, 128B swizzle.  MN-major fp32:
   // A in boxes {8 m, 32 k} (read as register fragments), B in one box {BN, 32 k} (converted in shared memory), unswizzled.
   // Pre-split B: the K-major box of each plane
   if (!a_mn_major)
     rc = make_map(&ma, mode, raw, A, M, K, lda, bke, BM, true);
   else
-    rc = make_map(&ma, mode, raw, A, K, M, lda, bf16 ? 64 : 8, bke, bf16);
+    rc = make_map(&ma, mode, raw, A, K, M, lda, half ? 64 : 8, bke, half);
   if (rc) return rc;
   if (!b_mn_major)
     rc = make_map(&mb, mode, raw, B, N, K, ldb, bke, BN, true, mode == kF32x3SplitB ? 2 : 1);
   else
-    rc = make_map(&mb, mode, raw, B, K, N, ldb, bf16 ? 64 : BN, bke, bf16);
+    rc = make_map(&mb, mode, raw, B, K, N, ldb, half ? 64 : BN, bke, half);
   if (rc) return rc;
   GemmParams p{M, N, K, ldc, act, C, bias, accumulate, aux_mode, ld_aux, aux, aux_scale, dropout_p, seed, splits, c_bf16, aux_bf16, nullptr};
   // split-K: partial tiles in stream-ordered scratch (at most about one tile per SM of partials), then a fixed-order sum
   if (splits > 1) W2L_CUDA_CHECK(cudaMallocAsync(reinterpret_cast<void**>(&p.ws), sizeof(float) * (size_t)splits * M * N, stream));
   switch (mode) {
     case kBf16: rc = launch<kBf16>(stream, a_mn_major, b_mn_major, BN, ma, mb, p); break;
+    case kFp16: rc = launch<kFp16>(stream, a_mn_major, b_mn_major, BN, ma, mb, p); break;
     case kF32x3: rc = launch<kF32x3>(stream, a_mn_major, b_mn_major, BN, ma, mb, p); break;
     case kF32x3SplitB: rc = launch<kF32x3SplitB>(stream, a_mn_major, b_mn_major, BN, ma, mb, p); break;
     default: rc = launch<kTf32>(stream, a_mn_major, b_mn_major, BN, ma, mb, p);
@@ -767,25 +796,55 @@ int gemm_impl(void* stream_, int mode, int a_mn_major, int b_mn_major, int M, in
 // fp32-operand entry points follow the thread's precision setting
 int f32_kind() { return current_precision() == W2L_PRECISION_F32 ? kF32x3 : kTf32; }
 
-__global__ void __launch_bounds__(256) cast_bf16_kernel(long long n4, const float4* __restrict__ x, uint2* __restrict__ y, long long n,
-                                                        const float* __restrict__ xs, __nv_bfloat16* __restrict__ ys) {
+// fp32 -> 16-bit H (round to nearest even): w2l_cast_bf16 / w2l_cast_fp16
+template <typename H>
+__global__ void __launch_bounds__(256) cast_kernel(long long n4, const float4* __restrict__ x, uint2* __restrict__ y, long long n,
+                                                   const float* __restrict__ xs, H* __restrict__ ys) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n4) {
     const float4 v = x[i];
-    const __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
+    Half2<H> a, b;
+    from_float2(v.x, v.y, &a);
+    from_float2(v.z, v.w, &b);
     y[i] = make_uint2(*reinterpret_cast<const uint32_t*>(&a), *reinterpret_cast<const uint32_t*>(&b));
   }
-  if (i < n - 4 * n4) ys[4 * n4 + i] = __float2bfloat16_rn(xs[4 * n4 + i]);
+  if (i < n - 4 * n4) ys[4 * n4 + i] = from_float<H>(xs[4 * n4 + i]);
 }
-// rows of `cols` floats (row stride ld_in) -> rows of cols_p bf16 (row stride cols_p), zero-padded columns
-__global__ void __launch_bounds__(256) cast_bf16_rows_kernel(long long rows, int cols, int ld_in, int cols_p, const float* __restrict__ x,
-                                                             __nv_bfloat16* __restrict__ y) {
+// rows of `cols` floats (row stride ld_in) -> rows of cols_p H (row stride cols_p), zero-padded columns
+template <typename H>
+__global__ void __launch_bounds__(256) cast_rows_kernel(long long rows, int cols, int ld_in, int cols_p, const float* __restrict__ x,
+                                                        H* __restrict__ y) {
   const long long total = rows * cols_p;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const long long r = i / cols_p;
     const int c = (int)(i % cols_p);
-    y[i] = c < cols ? __float2bfloat16_rn(x[r * ld_in + c]) : __float2bfloat16_rn(0.f);
+    y[i] = c < cols ? from_float<H>(x[r * ld_in + c]) : from_float<H>(0.f);
   }
+}
+template <typename H>
+int cast(void* stream_, long long n, const float* x, void* y, const char* name, const char* kname) {
+  if (n <= 0) return W2L_OK;
+  if (!x || !y) return fail(W2L_ERR_INVALID_ARGUMENT, std::string(name) + ": null pointer");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const bool vec = ((reinterpret_cast<uintptr_t>(x) & 15) == 0) && ((reinterpret_cast<uintptr_t>(y) & 7) == 0);
+  const long long n4 = vec ? n / 4 : 0;
+  const long long threads = std::max<long long>(n4, n - 4 * n4);
+  cast_kernel<H><<<(unsigned)((threads + 255) / 256), 256, 0, stream>>>(n4, reinterpret_cast<const float4*>(x), static_cast<uint2*>(y), n, x,
+                                                                        static_cast<H*>(y));
+  W2L_LAUNCH_CHECK(kname);
+  return W2L_OK;
+}
+template <typename H>
+int cast_rows(void* stream_, long long rows, int cols, int ld_in, int cols_padded, const float* x, void* y, const char* name,
+              const char* kname) {
+  if (rows <= 0 || cols <= 0) return W2L_OK;
+  if (!x || !y || cols_padded < cols || ld_in < cols) return fail(W2L_ERR_INVALID_ARGUMENT, std::string(name) + ": bad arguments");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const long long total = rows * cols_padded;
+  const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, (long long)sm_count() * 16);
+  cast_rows_kernel<H><<<grid, 256, 0, stream>>>(rows, cols, ld_in, cols_padded, x, static_cast<H*>(y));
+  W2L_LAUNCH_CHECK(kname);
+  return W2L_OK;
 }
 
 }  // namespace
@@ -841,27 +900,13 @@ extern "C" int w2l_gemm_tf32_view(void* stream_, int a_mn_major, int b_mn_major,
                    0ull, true);
 }
 
-extern "C" int w2l_cast_bf16(void* stream_, long long n, const float* x, void* y) {
-  if (n <= 0) return W2L_OK;
-  if (!x || !y) return fail(W2L_ERR_INVALID_ARGUMENT, "cast_bf16: null pointer");
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  const bool vec = ((reinterpret_cast<uintptr_t>(x) & 15) == 0) && ((reinterpret_cast<uintptr_t>(y) & 7) == 0);
-  const long long n4 = vec ? n / 4 : 0;
-  const long long threads = std::max<long long>(n4, n - 4 * n4);
-  cast_bf16_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, stream>>>(n4, reinterpret_cast<const float4*>(x), static_cast<uint2*>(y), n, x,
-                                                                         static_cast<__nv_bfloat16*>(y));
-  W2L_LAUNCH_CHECK("cast_bf16_kernel");
-  return W2L_OK;
-}
+extern "C" int w2l_cast_bf16(void* stream_, long long n, const float* x, void* y) { return cast<__nv_bfloat16>(stream_, n, x, y, "cast_bf16", "cast_bf16_kernel"); }
 extern "C" int w2l_cast_bf16_rows(void* stream_, long long rows, int cols, int ld_in, int cols_padded, const float* x, void* y) {
-  if (rows <= 0 || cols <= 0) return W2L_OK;
-  if (!x || !y || cols_padded < cols || ld_in < cols) return fail(W2L_ERR_INVALID_ARGUMENT, "cast_bf16_rows: bad arguments");
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  const long long total = rows * cols_padded;
-  const unsigned grid = (unsigned)std::min<long long>((total + 255) / 256, (long long)sm_count() * 16);
-  cast_bf16_rows_kernel<<<grid, 256, 0, stream>>>(rows, cols, ld_in, cols_padded, x, static_cast<__nv_bfloat16*>(y));
-  W2L_LAUNCH_CHECK("cast_bf16_rows_kernel");
-  return W2L_OK;
+  return cast_rows<__nv_bfloat16>(stream_, rows, cols, ld_in, cols_padded, x, y, "cast_bf16_rows", "cast_bf16_rows_kernel");
+}
+extern "C" int w2l_cast_fp16(void* stream_, long long n, const float* x, void* y) { return cast<__half>(stream_, n, x, y, "cast_fp16", "cast_fp16_kernel"); }
+extern "C" int w2l_cast_fp16_rows(void* stream_, long long rows, int cols, int ld_in, int cols_padded, const float* x, void* y) {
+  return cast_rows<__half>(stream_, rows, cols, ld_in, cols_padded, x, y, "cast_fp16_rows", "cast_fp16_rows_kernel");
 }
 extern "C" int w2l_split_tf32(void* stream_, int transpose, int rows, int cols, int ld, int cols_padded, const float* x, float* planes) {
   if (rows <= 0 || cols <= 0) return W2L_OK;

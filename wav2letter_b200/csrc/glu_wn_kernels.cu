@@ -11,6 +11,7 @@
 //                the two halves of the output channels are padded separately so the GLU halves stay aligned.
 // All HBM-bound streaming kernels: float4 where the shapes allow, one pass.
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
 #include "common.cuh"
@@ -82,9 +83,18 @@ __device__ __forceinline__ int out_row(int co, int cout, int cout_p, int glu_spl
 // is 16 contiguous runs of 32*kw floats (coalesced reads); the forward operand is written as 128-byte runs over ci and the
 // flipped operand as 64-byte runs over co.  (The element-wise version scattered 4-byte writes: 4.4 ms per step for the
 // 209 M-parameter conv_glu model; this one moves the same bytes in ~0.6 ms.)  Pitches kwp (odd) and cpitch (= 1 mod 32) keep
-// both transposed read patterns bank-conflict free.  kOutBf16: write bf16 operands directly (W2L_PRECISION_BF16).
+// both transposed read patterns bank-conflict free.  T: the operand type, float or a 16-bit type written directly
+// (W2L_PRECISION_BF16 / W2L_PRECISION_FP16).
 constexpr int kArrCo = 16, kArrCi = 32;
-template <bool kOutBf16>
+template <typename T>
+__device__ __forceinline__ T operand_from(float x);
+template <>
+__device__ __forceinline__ float operand_from<float>(float x) { return x; }
+template <>
+__device__ __forceinline__ __nv_bfloat16 operand_from<__nv_bfloat16>(float x) { return __float2bfloat16_rn(x); }
+template <>
+__device__ __forceinline__ __half operand_from<__half>(float x) { return __float2half_rn(x); }
+template <typename T>
 __global__ void __launch_bounds__(256) conv1d_arrange_kernel(int cin, int cout, int kw, int cin_p, int cout_p, int glu_split,
                                                              const float* __restrict__ w, const float* __restrict__ bias,
                                                              void* __restrict__ fwd_, void* __restrict__ flip_,
@@ -121,10 +131,7 @@ __global__ void __launch_bounds__(256) conv1d_arrange_kernel(int cin, int cout, 
     if (lane < nci) {
       const float x = arr_tile[col * cpitch + lane * kwp + dk];
       const size_t o = (size_t)out_row(co0 + col, cout, cout_p, glu_split) * kw * cin_p + (size_t)dk * cin_p + (ci0 + lane);
-      if (kOutBf16)
-        static_cast<__nv_bfloat16*>(fwd_)[o] = __float2bfloat16_rn(x);
-      else
-        static_cast<float*>(fwd_)[o] = x;
+      static_cast<T*>(fwd_)[o] = operand_from<T>(x);
     }
   }
   // flipped operand: (ci, dk, co) with co fastest: a half warp takes a (ci, dk) pair, its 16 lanes are the output channels
@@ -136,10 +143,7 @@ __global__ void __launch_bounds__(256) conv1d_arrange_kernel(int cin, int cout, 
       if (col < nco) {
         const float x = arr_tile[col * cpitch + cil * kwp + dk];
         const size_t o = (size_t)(ci0 + cil) * kw * cout_p + (size_t)(kw - 1 - dk) * cout_p + orow;
-        if (kOutBf16)
-          static_cast<__nv_bfloat16*>(flip_)[o] = __float2bfloat16_rn(x);
-        else
-          static_cast<float*>(flip_)[o] = x;
+        static_cast<T*>(flip_)[o] = operand_from<T>(x);
       }
     }
   }
@@ -331,13 +335,15 @@ extern "C" int w2l_weightnorm_bwd(void* stream_, int rows, int len, const float*
 }
 static size_t arrange_smem(int kw) { return (size_t)kArrCo * (kArrCi * (kw | 1) + 1) * sizeof(float); }
 
-// out_bf16 != 0: fwd / flip are bf16 operands (W2L_PRECISION_BF16), written directly — no fp32 copy, no cast pass
+// out_bf16 = 1 / 2: fwd / flip are bf16 / fp16 operands (W2L_PRECISION_BF16 / FP16), written directly — no fp32 copy, no
+// cast pass
 extern "C" int w2l_conv1d_arrange_ex(void* stream_, int cin, int cout, int kw, int cin_p, int cout_p, int glu_split, const float* w,
                                      const float* bias, void* fwd, void* flip, float* bias_p, int out_bf16) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (cin <= 0 || cout <= 0 || kw <= 0 || cin_p < cin || cout_p < cout || (cin_p % 4) || (cout_p % 4) || !w || !fwd)
     return fail(W2L_ERR_INVALID_ARGUMENT, "conv1d_arrange: bad arguments (padded channel counts must be multiples of 4)");
   if (glu_split && ((cout % 2) || (cout_p % 8) || cout_p / 2 < cout / 2)) return fail(W2L_ERR_INVALID_ARGUMENT, "conv1d_arrange: bad GLU split padding");
+  if (out_bf16 < 0 || out_bf16 > 2) return fail(W2L_ERR_INVALID_ARGUMENT, "conv1d_arrange: out_bf16 must be 0 (fp32), 1 (bf16) or 2 (fp16)");
   const size_t es = out_bf16 ? 2 : 4;
   W2L_CUDA_CHECK(cudaMemsetAsync(fwd, 0, es * (size_t)cout_p * kw * cin_p, stream));
   if (flip) W2L_CUDA_CHECK(cudaMemsetAsync(flip, 0, es * (size_t)cin_p * kw * cout_p, stream));
@@ -345,13 +351,13 @@ extern "C" int w2l_conv1d_arrange_ex(void* stream_, int cin, int cout, int kw, i
   const size_t smem = arrange_smem(kw);
   if (smem > 200 * 1024) return fail(W2L_ERR_UNSUPPORTED, "conv1d_arrange: kernel width too large");
   dim3 grid((cout + kArrCo - 1) / kArrCo, (cin + kArrCi - 1) / kArrCi);
-  if (out_bf16) {
-    if (smem > 48 * 1024) W2L_CUDA_CHECK(cudaFuncSetAttribute(conv1d_arrange_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    conv1d_arrange_kernel<true><<<grid, 256, smem, stream>>>(cin, cout, kw, cin_p, cout_p, glu_split, w, bias, fwd, flip, bias_p);
-  } else {
-    if (smem > 48 * 1024) W2L_CUDA_CHECK(cudaFuncSetAttribute(conv1d_arrange_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    conv1d_arrange_kernel<false><<<grid, 256, smem, stream>>>(cin, cout, kw, cin_p, cout_p, glu_split, w, bias, fwd, flip, bias_p);
-  }
+  auto run = [&](auto kernel) -> int {
+    if (smem > 48 * 1024) W2L_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<grid, 256, smem, stream>>>(cin, cout, kw, cin_p, cout_p, glu_split, w, bias, fwd, flip, bias_p);
+    return W2L_OK;
+  };
+  const int rc = out_bf16 == 2 ? run(conv1d_arrange_kernel<__half>) : out_bf16 ? run(conv1d_arrange_kernel<__nv_bfloat16>) : run(conv1d_arrange_kernel<float>);
+  if (rc != W2L_OK) return rc;
   W2L_LAUNCH_CHECK("conv1d_arrange_kernel");
   return W2L_OK;
 }

@@ -17,9 +17,10 @@ namespace {
 void cuda(cudaError_t e, const char* what) {
   if (e != cudaSuccess) throw std::runtime_error(std::string("dense operand: ") + what + ": " + cudaGetErrorString(e));
 }
-size_t elemBytes(int kind) { return kind == W2L_GEMM_BF16 ? 2 : 4; }
+bool is16(int kind) { return kind == W2L_GEMM_BF16 || kind == W2L_GEMM_FP16; }
+size_t elemBytes(int kind) { return is16(kind) ? 2 : 4; }
 bool servesInPlace(int kind, int cols, long long len, const float* src, int zeroRows) {
-  return kind != W2L_GEMM_BF16 && zeroRows == 0 && len == cols && src && (reinterpret_cast<uintptr_t>(src) & 15) == 0;
+  return !is16(kind) && zeroRows == 0 && len == cols && src && (reinterpret_cast<uintptr_t>(src) & 15) == 0;
 }
 size_t copyBytes(int kind, long long rows, int cols, long long len, const float* src, int zeroRows) {
   return servesInPlace(kind, cols, len, src, zeroRows) ? 0 : elemBytes(kind) * (size_t)(zeroRows + rows) * (size_t)len;
@@ -30,12 +31,13 @@ Operand rowsOf(void* stream, int kind, long long rows, int cols, long long len, 
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t pitch = elemBytes(kind) * (size_t)len;
   char* body = static_cast<char*>(dst) + (size_t)zeroRows * pitch;
-  const bool bf16 = kind == W2L_GEMM_BF16, padCols = !bf16 && len > cols;  // the bf16 casts write their own pad columns
+  const bool half = is16(kind), padCols = !half && len > cols;  // the 16-bit casts write their own pad columns
   if (zeroRows || padCols) cuda(cudaMemsetAsync(dst, 0, (size_t)(zeroRows + (padCols ? rows : 0)) * pitch, st), "zero padding");
-  if (bf16 && len == cols)
-    check(w2l_cast_bf16(st, rows * cols, src, body));
-  else if (bf16)
-    check(w2l_cast_bf16_rows(st, rows, cols, cols, (int)len, src, body));
+  if (half && len == cols)
+    check(kind == W2L_GEMM_FP16 ? w2l_cast_fp16(st, rows * cols, src, body) : w2l_cast_bf16(st, rows * cols, src, body));
+  else if (half)
+    check(kind == W2L_GEMM_FP16 ? w2l_cast_fp16_rows(st, rows, cols, cols, (int)len, src, body)
+                                : w2l_cast_bf16_rows(st, rows, cols, cols, (int)len, src, body));
   else if (len == cols)
     cuda(cudaMemcpyAsync(body, src, sizeof(float) * (size_t)rows * cols, cudaMemcpyDeviceToDevice, st), "copy");
   else
@@ -45,10 +47,15 @@ Operand rowsOf(void* stream, int kind, long long rows, int cols, long long len, 
 }  // namespace
 
 int rowKind(int precision) {
-  return precision == W2L_PRECISION_BF16 ? W2L_GEMM_BF16 : precision == W2L_PRECISION_F32 ? W2L_GEMM_F32X3 : W2L_GEMM_TF32;
+  switch (precision) {
+    case W2L_PRECISION_BF16: return W2L_GEMM_BF16;
+    case W2L_PRECISION_FP16: return W2L_GEMM_FP16;
+    case W2L_PRECISION_F32: return W2L_GEMM_F32X3;
+    default: return W2L_GEMM_TF32;
+  }
 }
 long long padRow(int kind, long long n) {
-  const long long a = kind == W2L_GEMM_BF16 ? 8 : 4;
+  const long long a = is16(kind) ? 8 : 4;
   return (n + a - 1) / a * a;
 }
 

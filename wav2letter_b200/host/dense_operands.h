@@ -16,7 +16,7 @@ struct Operand {
   bool mnMajor = false;
 };
 
-int rowKind(int precision);               // the precision's kind of row operands: TF32, F32X3 or BF16
+int rowKind(int precision);               // the precision's kind of row operands: TF32, F32X3, BF16 or FP16
 long long padRow(int kind, long long n);  // n padded to whole TMA rows of the kind
 
 // contiguous rows of `cols` floats as rows of padRow(kind, cols) entries behind `zeroRows` zero rows: the source itself

@@ -78,8 +78,8 @@ class StreamingAM(_StreamHandle):
 
     def __init__(self, trainer, max_streams: int, max_chunk: int = 50, precision: str | None = None):
         """Snapshot of `trainer`'s network parameters (training may go on) with state for `max_streams` slots and chunks
-        of at most `max_chunk` feature frames.  precision: None (the thread's w2l_set_precision), "tf32", "f32" or
-        "bf16"."""
+        of at most `max_chunk` feature frames.  precision: None (the thread's w2l_set_precision), "tf32", "f32",
+        "bf16" or "fp16"."""
         saved = capi.get_precision()
         if precision is not None:
             capi.set_precision(precision)
