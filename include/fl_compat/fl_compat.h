@@ -24,6 +24,7 @@
 #include <functional>
 #include <memory>
 #include <random>
+#include <stdexcept>
 #include <string>
 #include <vector>
 
@@ -622,6 +623,75 @@ class LinearSegmentationCriterion : public SequenceCriterion {
   af::array ws_;
 };
 using LinSegCriterion = LinearSegmentationCriterion;
+
+// ---- Seq2Seq (--criterion=seq2seq), DESIGN.md §9 ---------------------------------------------------------------
+// Attentions and windows are descriptions the criterion runs itself (its kernels read keys and values in place from
+// the encoder output); only the types the seq2seq recipes use exist: KeyValueAttention (--attention=keyvalue) and
+// SoftPretrainWindow(std) (--attnWindow=softPretrain --softwstd).
+class AttentionBase {
+ public:
+  virtual ~AttentionBase() = default;
+  virtual std::string prettyString() const = 0;
+};
+class KeyValueAttention : public AttentionBase {
+ public:
+  std::string prettyString() const override { return "KeyValueAttention"; }
+};
+class WindowBase {
+ public:
+  virtual ~WindowBase() = default;
+  virtual std::string prettyString() const = 0;
+};
+class SoftPretrainWindow : public WindowBase {
+ public:
+  explicit SoftPretrainWindow(double std) : std_(std) {
+    if (!(std > 0)) throw std::invalid_argument("SoftPretrainWindow: std must be > 0");
+  }
+  double std() const { return std_; }
+  std::string prettyString() const override { return "SoftPretrainWindow"; }
+
+ private:
+  double std_;
+};
+
+// Seq2SeqCriterion with the constructor arguments of Train.cpp:416-432.  forward({encoder output [2H,T',B], target
+// [U,B] int32, [durations], [target sizes]}) -> {loss [B]}: the sizes are accepted and not used — every utterance spans
+// all T' frames and its target ends at its first pad.  Targets hold tokens, then eos, then pad; an utterance holding a
+// value outside [0, N) (-1 included) is rejected in-band, checked on the device: its loss is NaN and its gradient zero
+// (Train.cpp stops on a NaN loss, :1686-1698; the trainer's finite guard skips the update).  Parameters (layout order): E [N][H], startEmbedding [H], per round and layer
+// W_ih [3H][H], W_hh [3H][H], b_ih [3H], b_hh [3H], then W_o [N][H], b_o [N].  Refused (std::invalid_argument):
+// inputfeeding, a sampling strategy other than "rand", attentions other than KeyValueAttention, windows other than
+// SoftPretrainWindow, attentions.size() != nAttnRound.  viterbiPath is the greedy decode (int32 [maxDecoderOutputLen, B],
+// padded with pad); viterbiPathWithTarget is not supported.
+class Seq2SeqCriterion : public SequenceCriterion {
+ public:
+  Seq2SeqCriterion(int nClass, int hiddenDim, int eos, int pad, int maxDecoderOutputLen,
+                   const std::vector<std::shared_ptr<AttentionBase>>& attentions, std::shared_ptr<WindowBase> window = nullptr,
+                   bool trainWithWindow = false, int pctTeacherForcing = 100, double labelSmooth = 0.0, bool inputFeeding = false,
+                   const std::string& samplingStrategy = "rand", double gumbelTemperature = 1.0, int nRnnLayer = 1, int nAttnRound = 1,
+                   float dropOut = 0.0);
+  std::vector<Variable> forward(const std::vector<Variable>& inputs) override;
+  af::array viterbiPath(const af::array& input, const af::array& inputSize = af::array()) override;
+  af::array viterbiPathWithTarget(const af::array& input, const af::array& target, af::array* index = nullptr) override;
+  // greedy decode of every utterance: tokens [maxDecoderOutputLen, B] int32 (pad after the end), lengths [B] int32
+  af::array decode(const af::array& input, af::array* lengths);
+  void clearWindow() { windowOn_ = false; }
+  void setWindow(bool on) { windowOn_ = on && window_ != nullptr; }  // checkpoint restore
+  bool windowSet() const { return windowOn_; }
+  unsigned long long lastSeed() const { return lastSeed_; }  // the Philox seed the last training forward drew
+  std::string prettyString() const override;
+  int hiddenDim() const { return H_; }
+
+ private:
+  int N_, H_, eos_, pad_, maxLen_, pct_, S_, R_;
+  double ls_;
+  float dropout_;
+  std::shared_ptr<WindowBase> window_;
+  bool trainWithWindow_, windowOn_;
+  unsigned long long lastSeed_ = 0;
+  std::vector<std::shared_ptr<Linear>> ih_;  // the input projections (one per round and layer) and the output layer
+  std::shared_ptr<Linear> out_;
+};
 
 }  // namespace speech
 }  // namespace pkg

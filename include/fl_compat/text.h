@@ -64,6 +64,7 @@ namespace speech {
 
 constexpr const char* kCtcCriterion = "ctc";
 constexpr const char* kAsgCriterion = "asg";
+constexpr const char* kSeq2SeqRNNCriterion = "seq2seq";
 constexpr const char* kBlankToken = "#";
 constexpr const char* kSilToken = "|";
 constexpr int kTargetPadValue = -1;

@@ -186,6 +186,57 @@ W2L_API int w2l_ctc_viterbi_target(void* stream, int B, int T, int N, int L, con
 W2L_API int w2l_linseg_target(void* stream, int B, int T, int L, const int32_t* target, int32_t* out);
 
 /* ----------------------------------------------------------------------------------------
+ * Seq2Seq criterion (--criterion=seq2seq: attention-GRU decoder, DESIGN.md §9), the kernels fl_compat's
+ * Seq2SeqCriterion runs beside the GEMMs of its projections.  Rows r = b*U + u of [B*U][width] row-major, H the hidden
+ * size (--encoderdim), N the dictionary size (eos and pad included), x the encoder output [B][T'][2H] (keys x[.][0:H],
+ * values x[.][H:2H]), target [B][U] int32.  Limits: H a multiple of 32 and <= 1024, 3 <= N <= 65536
+ * (w2l_seq2seq_check; W2L_ERR_UNSUPPORTED outside), and what fits on chip: 8 (H + T') floats for the attention, 16 U
+ * floats for its gradient, the W_hh slice of one CTA for the recurrence.
+ *   embed_fwd   tokens[b][0] = N (startEmbedding), tokens[b][u] = target[b][u-1], replaced with probability
+ *               1 - pct/100 by min(floor(r2 (N-1)), N-2) (Philox block of counter b*U + u under seed: r1 = word x, r2 =
+ *               word y, each (w >> 8) 2^-24; replaced iff r1 < fp32(1 - pct/100)); out[r] = E[tokens[r]] or start.
+ *               Targets are checked on the device: a value outside [0, N) sets bad[b] (int32 [B], nullable, zeroed
+ *               by the caller) and is read as token 0, so nothing outside E is read.
+ *   embed_bwd   dE[n] += sum of din over the rows with token n, dstart likewise (row order; no atomics)
+ *   gru_fwd     one GRU layer over all U steps from h0 (NULL: 0), gi = W_ih x + b_ih precomputed [B*U][3H], gate order
+ *               r, z, n; stash (nullable) [5][B*U][H] = r, z, n, W_hn h + b_hn, h_{u-1}.  One cooperative launch.
+ *   gru_bwd     from dout [B*U][H]: dgi = d(W_ih x + b_ih) and dgh = d(W_hh h + b_hh), both [B*U][3H]; carry [B][H]
+ *               scratch.  dW_hh = dgh^T h_{u-1}, db_hh = colsum dgh are the caller's GEMM / reduction.
+ *   attn_fwd    out = q + sum_t softmax_t(q.k_t / sqrt(H) + w_{u,t}) v_t, with the soft window
+ *               w = -(t - u T'/window_u)^2 / (2 window_std^2) when window_std > 0; attn (nullable) [B*U][T'] the weights
+ *   attn_bwd    from dout = d out: dq (the identity path included) and dx [B][T'][2H] (written), dS [B*U][T'] scratch
+ *   loss        per row: log-softmax over N, (1-ls)(-log p_y) - (ls/N) sum_c log p_c, 0 on rows with target = pad;
+ *               loss[b] = sum over u (in order), rowloss [B*U] scratch; grad != 0 also writes the logit gradient
+ *               dloss[b] (NULL: 1) (p - (1-ls) e_y - ls/N) over the logits, in place, 0 on pad rows.
+ *               An utterance flagged in bad (nullable: embed_fwd's flags) or with a target outside [0, N) gets loss
+ *               NaN and zero gradient: rejected in-band, as the other criteria reject bad labels.
+ *   scale_rows  d[b*U+u][:] *= g[b] / seed_scale
+ *   decode_*    one greedy step: argmax of logits [B][N] (first maximum); eos finishes an utterance (len[b] = step, not
+ *               emitted), another token is written to tokens[b][step] and in[b] = E[token]; done[B] counts finished
+ *               utterances.  init: in = start, tokens = pad, len = maxlen, done = 0 ([B + 1] ints).
+ * ---------------------------------------------------------------------------------------- */
+W2L_API int w2l_seq2seq_check(int H, int N);
+W2L_API int w2l_seq2seq_embed_fwd(void* stream, int B, int U, int H, int N, const int32_t* target, const float* E, const float* start,
+                                  float pct_teacher_forcing, unsigned long long seed, int32_t* tokens, float* out, int32_t* bad);
+W2L_API int w2l_seq2seq_embed_bwd(void* stream, int B, int U, int H, int N, const int32_t* tokens, const float* din, float* dE, float* dstart);
+W2L_API size_t w2l_seq2seq_gru_stash_floats(int B, int U, int H);
+W2L_API int w2l_seq2seq_gru_fwd(void* stream, int B, int U, int H, const float* gi, const float* Whh, const float* bhh, const float* h0,
+                                float* out, float* stash);
+W2L_API int w2l_seq2seq_gru_bwd(void* stream, int B, int U, int H, const float* dout, const float* Whh, const float* stash, float* dgi, float* dgh,
+                                float* carry);
+W2L_API int w2l_seq2seq_attn_fwd(void* stream, int B, int U, int Tp, int H, const float* q, const float* x, int window_u, float window_std,
+                                 float* out, float* attn);
+W2L_API int w2l_seq2seq_attn_bwd(void* stream, int B, int U, int Tp, int H, const float* q, const float* x, const float* attn, const float* dout,
+                                 float* dq, float* dx, float* dS);
+W2L_API int w2l_seq2seq_loss(void* stream, int B, int U, int N, int pad, const int32_t* target, float* logits, float label_smooth,
+                             const float* dloss, int grad, float* rowloss, float* loss, const int32_t* bad);
+W2L_API int w2l_seq2seq_scale_rows(void* stream, int B, int U, int N, const float* g, float seed_scale, float* d);
+W2L_API int w2l_seq2seq_decode_init(void* stream, int B, int H, int maxlen, int pad, const float* start, float* in, int32_t* tokens, int32_t* len,
+                                    int32_t* done);
+W2L_API int w2l_seq2seq_decode_step(void* stream, int B, int N, int H, int step, int eos, const float* logits, const float* E, float* in,
+                                    int32_t* tokens, int maxlen, int32_t* len, int32_t* done);
+
+/* ----------------------------------------------------------------------------------------
  * Dense contraction of the acoustic model (replaces fl::Linear's af::matmul -> cuBLAS and the
  * GEMM inside cuDNN's convolutions; forward at Train.cpp:1470, backward at :1720).
  *   C[m][n] = act( sum_k A(m,k) * B(n,k) + bias[n] ),  fp32 storage, wgmma math in the kind the thread's precision
@@ -414,6 +465,31 @@ W2L_API int w2l_mfsc(void* stream, int B, int max_samples, const float* audio, c
  * ---------------------------------------------------------------------------------------- */
 W2L_API void* w2l_trainer_create(void* stream, const char* arch_text, int n_feat, int n_label, const char* criterion,
                                  int scale_mode, float transdiag, float lr, float lrcrit, float momentum, float maxgradnorm);
+/* The seq2seq criterion (Train.cpp:411-432; DESIGN.md §9): the arch's output is the encoder, 2 * hidden features per
+ * frame; n_label counts the dictionary with eos and pad.  rounds = --decoderattnround, layers = --decoderrnnlayer,
+ * dropout = --decoderdropout, label_smooth = --labelsmooth, pct_teacher_forcing = --pctteacherforcing, window_std =
+ * --softwstd of a SoftPretrainWindow (0: no window), train_with_window = --trainWithWindow.  Targets [U,B] hold tokens,
+ * then eos, then pad; an utterance with a value outside [0, n_label) (-1 included) gets a NaN loss, so the step's
+ * update is skipped and counted (w2l_trainer_status), with no host synchronisation.  Its parameters form the criterion arena: they step with lrcrit
+ * and momentum 0 and are clipped with the network.  In its checkpoints (the same version 2 container) the settings and the
+ * window flag follow the arch text. */
+W2L_API void* w2l_trainer_create_seq2seq(void* stream, const char* arch_text, int n_feat, int n_label, int hidden, int eos, int pad,
+                                         int max_decoder_output_len, int rounds, int layers, float dropout, float label_smooth,
+                                         int pct_teacher_forcing, float window_std, int train_with_window, float lr, float lrcrit, float momentum,
+                                         float maxgradnorm);
+/* features per frame of the network output (n_label; 2 * hidden for seq2seq) */
+W2L_API int w2l_trainer_output_width(void* trainer, int* width);
+/* seq2seq only: {hidden, eos, pad, maxdecoderoutputlen, rounds, layers, window still set} */
+W2L_API int w2l_trainer_seq2seq_config(void* trainer, int* config7);
+/* seq2seq only: clearWindow() after the --pretrainWindow updates (Train.cpp:1885-1910) */
+W2L_API int w2l_trainer_clear_window(void* trainer);
+/* seq2seq only: the Philox seed of the last training forward (substitutions: that seed; the dropout after layer k of the
+ * flattened round-major stack: seed + 1 + k) */
+W2L_API int w2l_trainer_seq2seq_seed(void* trainer, unsigned long long* seed);
+/* seq2seq only: eval-mode network forward, then the greedy decode of every utterance: tokens device int32
+ * [B][maxdecoderoutputlen] padded with pad (capacity elements), lengths device int32 [B] (eos not counted) */
+W2L_API int w2l_trainer_decode(void* trainer, void* stream, int B, int T, const float* features, int32_t* tokens, int32_t* lengths,
+                               long long capacity);
 W2L_API void w2l_trainer_destroy(void* trainer);
 /* train != 0: backward, clip and update; total_batch (the batch summed over ranks, which divides every gradient) must
  * then be finite and > 0, else W2L_ERR_INVALID_ARGUMENT and nothing runs.  train == 0: loss only, total_batch unused. */

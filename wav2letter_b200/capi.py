@@ -45,6 +45,11 @@ EXPORTS = [
     "w2l_stream_run", "w2l_stream_plan",
     "w2l_mfsc_stream_create", "w2l_mfsc_stream_destroy", "w2l_mfsc_stream_state_bytes", "w2l_mfsc_stream_max_frames_out",
     "w2l_mfsc_stream_start", "w2l_mfsc_stream_run",
+    "w2l_seq2seq_check", "w2l_seq2seq_embed_fwd", "w2l_seq2seq_embed_bwd", "w2l_seq2seq_gru_stash_floats", "w2l_seq2seq_gru_fwd",
+    "w2l_seq2seq_gru_bwd", "w2l_seq2seq_attn_fwd", "w2l_seq2seq_attn_bwd", "w2l_seq2seq_loss", "w2l_seq2seq_scale_rows",
+    "w2l_seq2seq_decode_init", "w2l_seq2seq_decode_step",
+    "w2l_trainer_create_seq2seq", "w2l_trainer_output_width", "w2l_trainer_seq2seq_config", "w2l_trainer_clear_window",
+    "w2l_trainer_seq2seq_seed", "w2l_trainer_decode",
 ]
 
 
@@ -162,6 +167,26 @@ def _load() -> ctypes.CDLL:
     lib.w2l_edit_distance.argtypes = [cp, cp, vp]
     lib.w2l_trainer_create.restype = vp
     lib.w2l_trainer_create.argtypes = [vp, ctypes.c_char_p, i, i, ctypes.c_char_p, i, f32, f32, f32, f32, f32]
+    lib.w2l_trainer_create_seq2seq.restype = vp
+    lib.w2l_trainer_create_seq2seq.argtypes = [vp, ctypes.c_char_p, i, i, i, i, i, i, i, i, f32, f32, i, f32, i, f32, f32, f32, f32]
+    lib.w2l_trainer_output_width.argtypes = [vp, vp]
+    lib.w2l_trainer_seq2seq_config.argtypes = [vp, vp]
+    lib.w2l_trainer_clear_window.argtypes = [vp]
+    lib.w2l_trainer_seq2seq_seed.argtypes = [vp, vp]
+    lib.w2l_trainer_decode.argtypes = [vp, vp, i, i, vp, vp, vp, ll]
+    lib.w2l_seq2seq_check.argtypes = [i, i]
+    lib.w2l_seq2seq_embed_fwd.argtypes = [vp, i, i, i, i, vp, vp, vp, f32, u64, vp, vp, vp]
+    lib.w2l_seq2seq_embed_bwd.argtypes = [vp, i, i, i, i, vp, vp, vp, vp]
+    lib.w2l_seq2seq_gru_stash_floats.restype = sz
+    lib.w2l_seq2seq_gru_stash_floats.argtypes = [i, i, i]
+    lib.w2l_seq2seq_gru_fwd.argtypes = [vp, i, i, i, vp, vp, vp, vp, vp, vp]
+    lib.w2l_seq2seq_gru_bwd.argtypes = [vp, i, i, i, vp, vp, vp, vp, vp, vp]
+    lib.w2l_seq2seq_attn_fwd.argtypes = [vp, i, i, i, i, vp, vp, i, f32, vp, vp]
+    lib.w2l_seq2seq_attn_bwd.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, vp, vp, vp]
+    lib.w2l_seq2seq_loss.argtypes = [vp, i, i, i, i, vp, vp, f32, vp, i, vp, vp, vp]
+    lib.w2l_seq2seq_scale_rows.argtypes = [vp, i, i, i, vp, f32, vp]
+    lib.w2l_seq2seq_decode_init.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, vp]
+    lib.w2l_seq2seq_decode_step.argtypes = [vp, i, i, i, i, i, vp, vp, vp, vp, i, vp, vp]
     lib.w2l_trainer_destroy.argtypes = [vp]
     lib.w2l_trainer_destroy.restype = None
     lib.w2l_trainer_step.argtypes = [vp, vp, i, i, vp, i, vp, vp, i, f32]

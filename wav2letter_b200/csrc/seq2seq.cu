@@ -1,0 +1,690 @@
+// seq2seq.cu — the attention-GRU Seq2Seq criterion of the seq2seq_tds recipes (--criterion=seq2seq), sm_90a.
+// The dense projections (each layer's input projection, the output projection and their gradients) are the persistent
+// wgmma GEMM, called by the host layer; this file holds everything else (DESIGN.md §9):
+//   embedding gather with the teacher-forcing substitution, and its deterministic scatter-add;
+//   the GRU recurrence forward and backward through time, one cooperative launch per layer for the whole sequence:
+//     W_hh stays in shared memory (one slice of hidden units per CTA), one grid barrier per step, fp32 throughout;
+//   key-value attention forward (scores, soft window, softmax over T', context, + the query) and backward;
+//   log-softmax + label-smoothed NLL + logit gradient in one pass over each row, written in place;
+//   the greedy decode's per-step argmax and feedback.
+// Layouts: rows r = b * U + u of [B*U][width] row-major; the encoder output x [B][T'][2H] (keys x[.][0:H], values
+// x[.][H:2H]); targets y [B][U] int32; the decoder's input tokens [B][U] with N standing for startEmbedding.
+#include <cooperative_groups.h>
+
+#include "common.cuh"
+
+namespace cg = cooperative_groups;
+
+namespace w2l {
+namespace {
+
+constexpr int kThreads = 256;
+constexpr int kBatchChunk = 16;  // most rows of h (forward) or dgh (backward) the recurrence stages at a time
+constexpr int kUTile = 8;        // decoder steps per attention CTA
+constexpr int kTTile = 8;        // encoder frames per attention-gradient CTA
+constexpr size_t kSmemLimit = 220 * 1024;
+
+__device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-x)); }
+
+// ---- embedding -----------------------------------------------------------------------------------------------
+// tokens[b][0] = N (start); tokens[b][u] = y~[b][u-1]: with counter e = b * U + u, Philox block (e lo, e hi) under the
+// seed, r1 = (word x >> 8) 2^-24, r2 = (word y >> 8) 2^-24; replaced iff r1 < q (q = 1 - pctteacherforcing / 100) by
+// min(floor(r2 * (N - 1)), N - 2), all in fp32 (tests/seq2seq_reference.py models it bit for bit).  A target value outside
+// [0, N) sets bad[b] (the loss then gives the utterance NaN and no gradient) and is read as token 0.
+__global__ void __launch_bounds__(128) embed_fwd_kernel(int U, int H, int N, const int32_t* __restrict__ y, const float* __restrict__ E,
+                                                        const float* __restrict__ start, float q, unsigned long long seed,
+                                                        int32_t* __restrict__ tokens, float* __restrict__ out, int32_t* __restrict__ bad) {
+  const long long row = blockIdx.x;
+  const int u = (int)(row % U);
+  if (threadIdx.x == 0 && bad && (y[row] < 0 || y[row] >= N)) atomicOr(bad + row / U, 1);
+  int tok = N;
+  if (u > 0) {
+    tok = y[row - 1];
+    if (tok < 0 || tok >= N) tok = 0;
+    if (q > 0.f) {
+      const uint4 r = philox4x32((uint32_t)row, (uint32_t)(row >> 32), (uint32_t)seed, (uint32_t)(seed >> 32));
+      const float r1 = (float)(r.x >> 8) * (1.0f / 16777216.0f);
+      if (r1 < q) {
+        const float r2 = (float)(r.y >> 8) * (1.0f / 16777216.0f);
+        tok = min((int)floorf(r2 * (float)(N - 1)), N - 2);
+      }
+    }
+  }
+  if (threadIdx.x == 0) tokens[row] = tok;
+  const float* src = tok == N ? start : E + (size_t)tok * H;
+  for (int h = threadIdx.x; h < H; h += blockDim.x) out[row * H + h] = src[h];
+}
+
+// dE[tok] += sum of d_in over the rows that read E[tok], in row order; the first row of each token does the sum (the
+// same bits every run); tok == N goes to dstart
+__global__ void __launch_bounds__(128) embed_bwd_kernel(long long P, int H, int N, const int32_t* __restrict__ tokens,
+                                                        const float* __restrict__ din, float* __restrict__ dE, float* __restrict__ dstart) {
+  const long long p = blockIdx.x;
+  const int tok = tokens[p];
+  int seen = 0;
+  for (long long k = threadIdx.x; k < p && !seen; k += blockDim.x) seen = tokens[k] == tok;
+  if (__syncthreads_or(seen)) return;
+  float* dst = tok == N ? dstart : dE + (size_t)tok * H;
+  for (int h = threadIdx.x; h < H; h += blockDim.x) {
+    float s = 0.f;
+    for (long long k = p; k < P; ++k)
+      if (tokens[k] == tok) s += din[k * H + h];
+    dst[h] += s;
+  }
+}
+
+// ---- GRU recurrence ------------------------------------------------------------------------------------------
+// CTA c owns hidden units [c J, c J + J).  Forward step u, for rows b:
+//   gh_g = W_hg h_{u-1} + b_hg (g = r, z, n: rows g H + j of W_hh, staged once), r = s(gi_r + gh_r), z = s(gi_z + gh_z),
+//   n = tanh(gi_n + r gh_n), h_u = (1 - z) n + z h_{u-1};  gi already holds W_ih x + b_ih (the GEMM).
+struct GruFwdArgs {
+  int B, U, H, J, BC;  // BC: rows staged at a time (<= kBatchChunk, as many as fit beside the W_hh slice)
+  const float* gi;   // [B*U][3H]
+  const float* Whh;  // [3H][H]
+  const float* bhh;  // [3H]
+  const float* h0;   // [B][H] or null (zeros)
+  float* out;        // [B*U][H]
+  float* stash;      // [5][B*U][H] r, z, n, gh_n, h_{u-1}; or null
+};
+
+__global__ void __launch_bounds__(kThreads, 1) gru_fwd_kernel(GruFwdArgs a) {
+  extern __shared__ float sm[];
+  const int H = a.H, J = a.J, j0 = blockIdx.x * J;
+  const int nj = min(J, H - j0);
+  float* Ws = sm;                       // [3J][H]: local row g J + j = global row g H + j0 + j
+  float* hs = Ws + (size_t)3 * J * H;  // [BC][H]
+  float* gh = hs + (size_t)a.BC * H;   // [BC][3J]
+  for (int i = threadIdx.x; i < 3 * J * H; i += blockDim.x) {
+    const int lr = i / H, k = i % H, g = lr / J, j = lr % J;
+    Ws[i] = j < nj ? a.Whh[((size_t)g * H + j0 + j) * H + k] : 0.f;
+  }
+  cg::grid_group grid = cg::this_grid();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  const size_t plane = (size_t)a.B * a.U * H;
+  for (int u = 0; u < a.U; ++u) {
+    for (int b0 = 0; b0 < a.B; b0 += a.BC) {
+      const int nb = min(a.BC, a.B - b0);
+      __syncthreads();
+      for (int i = threadIdx.x; i < nb * H; i += blockDim.x) {
+        const int b = b0 + i / H, k = i % H;
+        float v = 0.f;
+        if (u > 0)
+          v = __ldcg(a.out + ((size_t)b * a.U + u - 1) * H + k);
+        else if (a.h0)
+          v = a.h0[(size_t)b * H + k];
+        hs[i] = v;
+      }
+      __syncthreads();
+      for (int pr = warp; pr < nb * 3 * J; pr += nw) {
+        const int b = pr / (3 * J), lr = pr % (3 * J);
+        const float* w = Ws + (size_t)lr * H;
+        const float* h = hs + (size_t)b * H;
+        float acc = 0.f;
+        for (int k = lane; k < H; k += 32) acc = fmaf(w[k], h[k], acc);
+        acc = warp_sum(acc);
+        if (lane == 0) gh[pr] = acc;
+      }
+      __syncthreads();
+      for (int i = threadIdx.x; i < nb * nj; i += blockDim.x) {
+        const int bl = i / nj, j = i % nj, jj = j0 + j, b = b0 + bl;
+        const size_t row = (size_t)b * a.U + u;
+        const float* g3 = gh + (size_t)bl * 3 * J;
+        const float* gi = a.gi + row * 3 * H;
+        const float ghr = g3[j] + a.bhh[jj], ghz = g3[J + j] + a.bhh[H + jj], ghn = g3[2 * J + j] + a.bhh[2 * H + jj];
+        const float r = sigmoidf_(gi[jj] + ghr), z = sigmoidf_(gi[H + jj] + ghz);
+        const float n = tanhf(gi[2 * H + jj] + r * ghn);
+        const float hp = hs[(size_t)bl * H + jj];
+        const float hn = (1.f - z) * n + z * hp;
+        a.out[row * H + jj] = hn;
+        if (a.stash) {
+          const size_t o = row * H + jj;
+          a.stash[o] = r;
+          a.stash[plane + o] = z;
+          a.stash[2 * plane + o] = n;
+          a.stash[3 * plane + o] = ghn;
+          a.stash[4 * plane + o] = hp;
+        }
+      }
+    }
+    if (u + 1 < a.U) grid.sync();
+  }
+}
+
+// Backward step u = U-1 .. 0 for the units of this CTA (W_hh's columns j0 .. j0 + J - 1 staged once):
+//   dh = dout_u + z_{u+1} dh_{u+1} + sum_i W_hh[i][j] dgh_{u+1}[i]
+//   dn = dh (1 - z), dz = dh (h_{u-1} - n), da_n = dn (1 - n^2), da_r = da_n gh_n r (1 - r), da_z = dz z (1 - z)
+//   dgi = (da_r, da_z, da_n), dgh = (da_r, da_z, da_n r)
+// carry [B][H] holds z dh between steps (each unit is only ever touched by its own CTA).
+struct GruBwdArgs {
+  int B, U, H, J, BC;
+  const float* dout;   // [B*U][H]
+  const float* Whh;    // [3H][H]
+  const float* stash;  // the forward's
+  float* dgi;          // [B*U][3H]
+  float* dgh;          // [B*U][3H]
+  float* carry;        // [B][H]
+};
+
+__global__ void __launch_bounds__(kThreads, 1) gru_bwd_kernel(GruBwdArgs a) {
+  extern __shared__ float sm[];
+  const int H = a.H, J = a.J, j0 = blockIdx.x * J, H3 = 3 * H;
+  const int nj = min(J, H - j0);
+  float* WT = sm;                              // [J][3H]: WT[j][i] = W_hh[i][j0 + j]
+  float* ds = WT + (size_t)J * H3;     // [BC][3H]: dgh of step u + 1
+  float* rec = ds + (size_t)a.BC * H3;  // [BC][J]
+  for (int i = threadIdx.x; i < J * H3; i += blockDim.x) {
+    const int j = i / H3, r = i % H3;
+    WT[i] = j < nj ? a.Whh[(size_t)r * H + j0 + j] : 0.f;
+  }
+  cg::grid_group grid = cg::this_grid();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  const size_t plane = (size_t)a.B * a.U * H;
+  for (int u = a.U - 1; u >= 0; --u) {
+    const bool last = u == a.U - 1;
+    for (int b0 = 0; b0 < a.B; b0 += a.BC) {
+      const int nb = min(a.BC, a.B - b0);
+      __syncthreads();
+      if (!last) {
+        for (int i = threadIdx.x; i < nb * H3; i += blockDim.x) {
+          const int b = b0 + i / H3, k = i % H3;
+          ds[i] = __ldcg(a.dgh + ((size_t)b * a.U + u + 1) * H3 + k);
+        }
+        __syncthreads();
+        for (int pr = warp; pr < nb * J; pr += nw) {
+          const int b = pr / J, j = pr % J;
+          const float* w = WT + (size_t)j * H3;
+          const float* d = ds + (size_t)b * H3;
+          float acc = 0.f;
+          for (int k = lane; k < H3; k += 32) acc = fmaf(w[k], d[k], acc);
+          acc = warp_sum(acc);
+          if (lane == 0) rec[pr] = acc;
+        }
+        __syncthreads();
+      }
+      for (int i = threadIdx.x; i < nb * nj; i += blockDim.x) {
+        const int bl = i / nj, j = i % nj, jj = j0 + j, b = b0 + bl;
+        const size_t row = (size_t)b * a.U + u, o = row * H + jj;
+        float dh = a.dout[o];
+        if (!last) dh += a.carry[(size_t)b * H + jj] + rec[bl * J + j];
+        const float r = a.stash[o], z = a.stash[plane + o], n = a.stash[2 * plane + o], ghn = a.stash[3 * plane + o],
+                    hp = a.stash[4 * plane + o];
+        const float dn = dh * (1.f - z), dz = dh * (hp - n);
+        const float dan = dn * (1.f - n * n), dar = dan * ghn * r * (1.f - r), daz = dz * z * (1.f - z);
+        float* gi = a.dgi + row * H3;
+        float* gh = a.dgh + row * H3;
+        gi[jj] = dar;
+        gi[H + jj] = daz;
+        gi[2 * H + jj] = dan;
+        gh[jj] = dar;
+        gh[H + jj] = daz;
+        gh[2 * H + jj] = dan * r;
+        a.carry[(size_t)b * H + jj] = dh * z;
+      }
+    }
+    if (u > 0) grid.sync();
+  }
+}
+
+int gruUnits(int H) {
+  const int sms = sm_count();
+  return (H + sms - 1) / sms;
+}
+// the most rows (<= kBatchChunk) whose staging fits beside the W_hh slice: smem(bc) = fixed + bc * perRow floats; 0 if none
+int gruChunk(size_t fixedFloats, size_t perRowFloats) {
+  for (int bc = kBatchChunk; bc >= 1; bc /= 2)
+    if (sizeof(float) * (fixedFloats + bc * perRowFloats) <= kSmemLimit) return bc;
+  return 0;
+}
+
+// ---- key-value attention -------------------------------------------------------------------------------------
+// per (tile of kUTile decoder steps, utterance): s_t = q.k_t / sqrt(H) + w_t, a = softmax_t(s), out = q + sum_t a_t v_t.
+// Window (win_inv2s2 > 0): w_{u,t} = -(t - u T' / U_win)^2 * win_inv2s2, 0-based u and t.
+__device__ __forceinline__ float window_at(int u, int t, int Tp, int Uwin, float inv2s2) {
+  const float c = (float)u * (float)Tp / (float)Uwin;
+  const float d = (float)t - c;
+  return -(d * d) * inv2s2;
+}
+
+__global__ void __launch_bounds__(kThreads) attn_fwd_kernel(int U, int Tp, int H, const float* __restrict__ q, const float* __restrict__ x,
+                                                            float scale, int Uwin, float inv2s2, float* __restrict__ out,
+                                                            float* __restrict__ attn) {
+  extern __shared__ float sm[];
+  float* qs = sm;                       // [kUTile][H]
+  float* ss = qs + (size_t)kUTile * H;  // [kUTile][Tp]
+  const int b = blockIdx.y, u0 = blockIdx.x * kUTile, nu = min(kUTile, U - u0);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  const float* xb = x + (size_t)b * Tp * 2 * H;
+  for (int i = threadIdx.x; i < kUTile * H; i += blockDim.x) qs[i] = i / H < nu ? q[((size_t)b * U + u0) * H + i] : 0.f;
+  __syncthreads();
+  for (int t = warp; t < Tp; t += nw) {
+    float acc[kUTile];
+#pragma unroll
+    for (int i = 0; i < kUTile; ++i) acc[i] = 0.f;
+    const float* k = xb + (size_t)t * 2 * H;
+    for (int h = lane; h < H; h += 32) {
+      const float kv = k[h];
+#pragma unroll
+      for (int i = 0; i < kUTile; ++i) acc[i] = fmaf(qs[i * H + h], kv, acc[i]);
+    }
+#pragma unroll
+    for (int i = 0; i < kUTile; ++i) {
+      const float s = warp_sum(acc[i]) * scale;
+      if (lane == 0) ss[(size_t)i * Tp + t] = inv2s2 > 0.f ? s + window_at(u0 + i, t, Tp, Uwin, inv2s2) : s;
+    }
+  }
+  __syncthreads();
+  for (int i = warp; i < nu; i += nw) {
+    float* s = ss + (size_t)i * Tp;
+    float m = kNegInf;
+    for (int t = lane; t < Tp; t += 32) m = fmaxf(m, s[t]);
+    m = warp_max(m);
+    float z = 0.f;
+    for (int t = lane; t < Tp; t += 32) {
+      const float e = expf(s[t] - m);
+      s[t] = e;
+      z += e;
+    }
+    const float inv = 1.f / warp_sum(z);
+    for (int t = lane; t < Tp; t += 32) {
+      s[t] *= inv;
+      if (attn) attn[((size_t)b * U + u0 + i) * Tp + t] = s[t];
+    }
+  }
+  __syncthreads();
+  for (int h = threadIdx.x; h < H; h += blockDim.x) {
+    float acc[kUTile];
+#pragma unroll
+    for (int i = 0; i < kUTile; ++i) acc[i] = 0.f;
+    for (int t = 0; t < Tp; ++t) {
+      const float v = xb[(size_t)t * 2 * H + H + h];
+#pragma unroll
+      for (int i = 0; i < kUTile; ++i) acc[i] = fmaf(ss[(size_t)i * Tp + t], v, acc[i]);
+    }
+    for (int i = 0; i < nu; ++i) out[((size_t)b * U + u0 + i) * H + h] = qs[i * H + h] + acc[i];
+  }
+}
+
+// dA_t = dout.v_t, dS = a (dA - sum_t a dA), dq = dout + sum_t dS_t k_t / sqrt(H); dS is kept for the key / value side
+__global__ void __launch_bounds__(kThreads) attn_bwd_q_kernel(int U, int Tp, int H, const float* __restrict__ x, const float* __restrict__ attn,
+                                                              const float* __restrict__ dout, float scale, float* __restrict__ dS,
+                                                              float* __restrict__ dq) {
+  extern __shared__ float sm[];
+  float* gs = sm;                       // [kUTile][H]  dout rows
+  float* ss = gs + (size_t)kUTile * H;  // [kUTile][Tp] dA, then dS
+  const int b = blockIdx.y, u0 = blockIdx.x * kUTile, nu = min(kUTile, U - u0);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  const float* xb = x + (size_t)b * Tp * 2 * H;
+  for (int i = threadIdx.x; i < kUTile * H; i += blockDim.x) gs[i] = i / H < nu ? dout[((size_t)b * U + u0) * H + i] : 0.f;
+  __syncthreads();
+  for (int t = warp; t < Tp; t += nw) {
+    float acc[kUTile];
+#pragma unroll
+    for (int i = 0; i < kUTile; ++i) acc[i] = 0.f;
+    const float* v = xb + (size_t)t * 2 * H + H;
+    for (int h = lane; h < H; h += 32) {
+      const float vv = v[h];
+#pragma unroll
+      for (int i = 0; i < kUTile; ++i) acc[i] = fmaf(gs[i * H + h], vv, acc[i]);
+    }
+#pragma unroll
+    for (int i = 0; i < kUTile; ++i) {
+      const float s = warp_sum(acc[i]);
+      if (lane == 0) ss[(size_t)i * Tp + t] = s;
+    }
+  }
+  __syncthreads();
+  for (int i = warp; i < nu; i += nw) {
+    float* s = ss + (size_t)i * Tp;
+    const float* a = attn + ((size_t)b * U + u0 + i) * Tp;
+    float dot = 0.f;
+    for (int t = lane; t < Tp; t += 32) dot = fmaf(a[t], s[t], dot);
+    dot = warp_sum(dot);
+    for (int t = lane; t < Tp; t += 32) {
+      const float d = a[t] * (s[t] - dot);
+      s[t] = d;
+      dS[((size_t)b * U + u0 + i) * Tp + t] = d;
+    }
+  }
+  __syncthreads();
+  for (int h = threadIdx.x; h < H; h += blockDim.x) {
+    float acc[kUTile];
+#pragma unroll
+    for (int i = 0; i < kUTile; ++i) acc[i] = 0.f;
+    for (int t = 0; t < Tp; ++t) {
+      const float k = xb[(size_t)t * 2 * H + h];
+#pragma unroll
+      for (int i = 0; i < kUTile; ++i) acc[i] = fmaf(ss[(size_t)i * Tp + t], k, acc[i]);
+    }
+    for (int i = 0; i < nu; ++i) dq[((size_t)b * U + u0 + i) * H + h] = gs[i * H + h] + acc[i] * scale;
+  }
+}
+
+// per (tile of kTTile frames, utterance): dk_t = sum_u dS_{u,t} q_u / sqrt(H), dv_t = sum_u a_{u,t} dout_u, written to
+// dx[b][t][0:H] and dx[b][t][H:2H]
+__global__ void __launch_bounds__(kThreads) attn_bwd_kv_kernel(int U, int Tp, int H, const float* __restrict__ q, const float* __restrict__ attn,
+                                                               const float* __restrict__ dS, const float* __restrict__ dout, float scale,
+                                                               float* __restrict__ dx) {
+  extern __shared__ float sm[];
+  float* as = sm;                       // [U][kTTile]
+  float* ds = as + (size_t)U * kTTile;  // [U][kTTile]
+  const int b = blockIdx.y, t0 = blockIdx.x * kTTile, nt = min(kTTile, Tp - t0);
+  for (int i = threadIdx.x; i < U * kTTile; i += blockDim.x) {
+    const int u = i / kTTile, j = i % kTTile;
+    const size_t o = ((size_t)b * U + u) * Tp + t0 + j;
+    as[i] = j < nt ? attn[o] : 0.f;
+    ds[i] = j < nt ? dS[o] : 0.f;
+  }
+  __syncthreads();
+  for (int h = threadIdx.x; h < H; h += blockDim.x) {
+    float dk[kTTile], dv[kTTile];
+#pragma unroll
+    for (int j = 0; j < kTTile; ++j) dk[j] = dv[j] = 0.f;
+    for (int u = 0; u < U; ++u) {
+      const size_t r = ((size_t)b * U + u) * H + h;
+      const float qq = q[r], gg = dout[r];
+#pragma unroll
+      for (int j = 0; j < kTTile; ++j) {
+        dk[j] = fmaf(ds[u * kTTile + j], qq, dk[j]);
+        dv[j] = fmaf(as[u * kTTile + j], gg, dv[j]);
+      }
+    }
+    for (int j = 0; j < nt; ++j) {
+      float* o = dx + ((size_t)b * Tp + t0 + j) * 2 * H;
+      o[h] = dk[j] * scale;
+      o[H + h] = dv[j];
+    }
+  }
+}
+
+// ---- loss ----------------------------------------------------------------------------------------------------
+// one CTA per row (b, u): one pass for max / sum exp (online) / sum of logits, then (with grad) the gradient in place:
+//   loss_row = (1 - ls) (lse - x_y) + ls lse - (ls / N) sum_c x_c   (= (1 - ls) nll - (ls / N) sum_c log p_c)
+//   grad_c = g_b (p_c - (1 - ls) [c == y] - ls / N);  pad rows: loss 0, gradient 0
+// Rows of an utterance flagged in bad (nullable), and a row whose target is outside [0, N): loss NaN, gradient 0.
+__global__ void __launch_bounds__(512) loss_kernel(int U, int N, int pad, const int32_t* __restrict__ y, float* __restrict__ logits,
+                                                   float ls, const float* __restrict__ dloss, int grad, float* __restrict__ rowloss,
+                                                   const int32_t* __restrict__ bad) {
+  __shared__ float sm_m[16], sm_s[16], sm_x[16];
+  const long long row = blockIdx.x;
+  const int tgt = y[row];
+  float* x = logits + row * N;
+  const bool invalid = tgt < 0 || tgt >= N || (bad && bad[row / U]);
+  if (tgt == pad || invalid) {
+    if (threadIdx.x == 0) rowloss[row] = invalid ? __int_as_float(0x7fc00000) : 0.f;
+    if (grad)
+      for (int c = threadIdx.x; c < N; c += blockDim.x) x[c] = 0.f;
+    return;
+  }
+  float m = kNegInf, s = 0.f, sx = 0.f;
+  for (int c = threadIdx.x; c < N; c += blockDim.x) {
+    const float v = x[c];
+    if (v > m) {
+      s = s * expf(m - v) + 1.f;
+      m = v;
+    } else {
+      s += expf(v - m);
+    }
+    sx += v;
+  }
+  // merge (m, s) across the warp, then across warps
+  for (int o = 16; o > 0; o >>= 1) {
+    const float m2 = __shfl_xor_sync(0xffffffffu, m, o), s2 = __shfl_xor_sync(0xffffffffu, s, o);
+    const float mm = fmaxf(m, m2);
+    s = (m == kNegInf ? 0.f : s * expf(m - mm)) + (m2 == kNegInf ? 0.f : s2 * expf(m2 - mm));
+    m = mm;
+    sx += __shfl_xor_sync(0xffffffffu, sx, o);
+  }
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  if (lane == 0) {
+    sm_m[warp] = m;
+    sm_s[warp] = s;
+    sm_x[warp] = sx;
+  }
+  __syncthreads();
+  float M = kNegInf;
+  for (int w = 0; w < nw; ++w) M = fmaxf(M, sm_m[w]);
+  float S = 0.f, SX = 0.f;
+  for (int w = 0; w < nw; ++w) {
+    S += sm_m[w] == kNegInf ? 0.f : sm_s[w] * expf(sm_m[w] - M);
+    SX += sm_x[w];
+  }
+  const float lse = M + logf(S);
+  const float xt = x[tgt];
+  if (threadIdx.x == 0) rowloss[row] = (1.f - ls) * (lse - xt) + ls * lse - (ls / (float)N) * SX;
+  if (!grad) return;
+  __syncthreads();  // every thread has read x[tgt]
+  const float g = dloss ? dloss[row / U] : 1.f;
+  const float off = ls / (float)N;
+  for (int c = threadIdx.x; c < N; c += blockDim.x) {
+    const float p = expf(x[c] - lse);
+    x[c] = g * (p - off - (c == tgt ? 1.f - ls : 0.f));
+  }
+}
+
+__global__ void loss_sum_kernel(int B, int U, const float* __restrict__ rowloss, float* __restrict__ loss) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  float s = 0.f;
+  for (int u = 0; u < U; ++u) s += rowloss[(size_t)b * U + u];
+  loss[b] = s;
+}
+
+// rows (b, u) of a [B*U][N] gradient times g[b] / seed_scale (an upstream gradient other than the one the loss kernel
+// was seeded with)
+__global__ void scale_rows_kernel(int U, int N, const float* __restrict__ g, float inv_seed, float* __restrict__ d) {
+  const long long row = blockIdx.x;
+  const float f = g[row / U] * inv_seed;
+  for (int c = threadIdx.x; c < N; c += blockDim.x) d[row * N + c] *= f;
+}
+
+// ---- greedy decode -------------------------------------------------------------------------------------------
+// init: in[b] = startEmbedding, tokens = pad, len = maxlen, done = 0
+__global__ void decode_init_kernel(int B, int H, int maxlen, int pad, const float* __restrict__ start, float* __restrict__ in,
+                                   int32_t* __restrict__ tokens, int32_t* __restrict__ len, int32_t* __restrict__ done) {
+  const int b = blockIdx.x;
+  for (int h = threadIdx.x; h < H; h += blockDim.x) in[(size_t)b * H + h] = start[h];
+  for (int i = threadIdx.x; i < maxlen; i += blockDim.x) tokens[(size_t)b * maxlen + i] = pad;
+  if (threadIdx.x == 0) {
+    len[b] = maxlen;
+    done[b] = 0;
+    if (b == 0) done[B] = 0;
+  }
+}
+
+// step: the argmax of each utterance's logits (first maximum); eos ends the utterance (not emitted), any other token is
+// emitted and fed back as E[token]; done[B] counts finished utterances
+__global__ void __launch_bounds__(256) decode_step_kernel(int N, int H, int step, int eos, const float* __restrict__ logits,
+                                                          const float* __restrict__ E, float* __restrict__ in, int32_t* __restrict__ tokens,
+                                                          int maxlen, int32_t* __restrict__ len, int32_t* __restrict__ done) {
+  __shared__ float bv[8];
+  __shared__ int bi[8];
+  __shared__ int tokS;
+  const int b = blockIdx.x;
+  if (done[b]) return;
+  const float* x = logits + (size_t)b * N;
+  float v = kNegInf;
+  int idx = 0x7fffffff;
+  for (int c = threadIdx.x; c < N; c += blockDim.x)
+    if (x[c] > v) {
+      v = x[c];
+      idx = c;
+    }
+  for (int o = 16; o > 0; o >>= 1) {
+    const float v2 = __shfl_xor_sync(0xffffffffu, v, o);
+    const int i2 = __shfl_xor_sync(0xffffffffu, idx, o);
+    if (v2 > v || (v2 == v && i2 < idx)) {
+      v = v2;
+      idx = i2;
+    }
+  }
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0) {
+    bv[warp] = v;
+    bi[warp] = idx;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float bvv = bv[0];
+    int bii = bi[0];
+    for (int w = 1; w < (int)(blockDim.x >> 5); ++w)
+      if (bv[w] > bvv || (bv[w] == bvv && bi[w] < bii)) {
+        bvv = bv[w];
+        bii = bi[w];
+      }
+    if (bii >= N) bii = 0;  // all logits NaN: token 0
+    tokS = bii;
+    if (bii == eos) {
+      len[b] = step;
+      done[b] = 1;
+      atomicAdd(done + gridDim.x, 1);
+    } else {
+      tokens[(size_t)b * maxlen + step] = bii;
+    }
+  }
+  __syncthreads();
+  const int tok = tokS;
+  if (tok == eos) return;
+  for (int h = threadIdx.x; h < H; h += blockDim.x) in[(size_t)b * H + h] = E[(size_t)tok * H + h];
+}
+
+}  // namespace
+}  // namespace w2l
+
+using namespace w2l;
+
+extern "C" {
+
+W2L_API int w2l_seq2seq_check(int H, int N) {
+  if (H <= 0 || H % 32 != 0 || H > 1024 || N < 3 || N > 65536)
+    return fail(W2L_ERR_UNSUPPORTED, "seq2seq: need H a multiple of 32 and <= 1024, and 3 <= N <= 65536");
+  return W2L_OK;
+}
+
+W2L_API int w2l_seq2seq_embed_fwd(void* stream, int B, int U, int H, int N, const int32_t* target, const float* E, const float* start,
+                                  float pct_teacher_forcing, unsigned long long seed, int32_t* tokens, float* out, int32_t* bad) {
+  if (int rc = w2l_seq2seq_check(H, N)) return rc;
+  if (B <= 0 || U <= 0 || !target || !E || !start || !tokens || !out || !(pct_teacher_forcing >= 0.f && pct_teacher_forcing <= 100.f))
+    return fail(W2L_ERR_INVALID_ARGUMENT, "seq2seq_embed_fwd: bad arguments");
+  const float q = (float)(1.0 - (double)pct_teacher_forcing / 100.0);
+  embed_fwd_kernel<<<(unsigned)((long long)B * U), 128, 0, static_cast<cudaStream_t>(stream)>>>(U, H, N, target, E, start, q, seed, tokens, out, bad);
+  W2L_LAUNCH_CHECK("seq2seq_embed_fwd_kernel");
+  return W2L_OK;
+}
+
+W2L_API int w2l_seq2seq_embed_bwd(void* stream, int B, int U, int H, int N, const int32_t* tokens, const float* din, float* dE, float* dstart) {
+  if (int rc = w2l_seq2seq_check(H, N)) return rc;
+  if (B <= 0 || U <= 0 || !tokens || !din || !dE || !dstart) return fail(W2L_ERR_INVALID_ARGUMENT, "seq2seq_embed_bwd: bad arguments");
+  const long long P = (long long)B * U;
+  embed_bwd_kernel<<<(unsigned)P, 128, 0, static_cast<cudaStream_t>(stream)>>>(P, H, N, tokens, din, dE, dstart);
+  W2L_LAUNCH_CHECK("seq2seq_embed_bwd_kernel");
+  return W2L_OK;
+}
+
+W2L_API size_t w2l_seq2seq_gru_stash_floats(int B, int U, int H) { return (size_t)5 * B * U * H; }
+
+W2L_API int w2l_seq2seq_gru_fwd(void* stream, int B, int U, int H, const float* gi, const float* Whh, const float* bhh, const float* h0,
+                                float* out, float* stash) {
+  if (int rc = w2l_seq2seq_check(H, 3)) return rc;
+  if (B <= 0 || U <= 0 || !gi || !Whh || !bhh || !out) return fail(W2L_ERR_INVALID_ARGUMENT, "seq2seq_gru_fwd: bad arguments");
+  const int J = gruUnits(H), grid = (H + J - 1) / J;
+  const int BC = gruChunk((size_t)3 * J * H, (size_t)H + 3 * J);
+  if (BC == 0) return fail(W2L_ERR_UNSUPPORTED, "seq2seq_gru_fwd: W_hh slice does not fit on chip");
+  const size_t smem = sizeof(float) * ((size_t)3 * J * H + (size_t)BC * (H + 3 * J));
+  W2L_CUDA_CHECK(cudaFuncSetAttribute(gru_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  GruFwdArgs a{B, U, H, J, BC, gi, Whh, bhh, h0, out, stash};
+  void* args[] = {&a};
+  W2L_CUDA_CHECK(cudaLaunchCooperativeKernel((const void*)gru_fwd_kernel, dim3(grid), dim3(kThreads), args, smem, static_cast<cudaStream_t>(stream)));
+  W2L_LAUNCH_CHECK("seq2seq_gru_fwd_kernel");
+  return W2L_OK;
+}
+
+W2L_API int w2l_seq2seq_gru_bwd(void* stream, int B, int U, int H, const float* dout, const float* Whh, const float* stash, float* dgi, float* dgh,
+                                float* carry) {
+  if (int rc = w2l_seq2seq_check(H, 3)) return rc;
+  if (B <= 0 || U <= 0 || !dout || !Whh || !stash || !dgi || !dgh || !carry) return fail(W2L_ERR_INVALID_ARGUMENT, "seq2seq_gru_bwd: bad arguments");
+  const int J = gruUnits(H), grid = (H + J - 1) / J;
+  // at H = 1024 the 96 KB W_hh slice leaves room for 8 rows of dgh (12 KB each), not 16
+  const int BC = gruChunk((size_t)J * 3 * H, (size_t)3 * H + J);
+  if (BC == 0) return fail(W2L_ERR_UNSUPPORTED, "seq2seq_gru_bwd: W_hh slice does not fit on chip");
+  const size_t smem = sizeof(float) * ((size_t)J * 3 * H + (size_t)BC * (3 * H + J));
+  W2L_CUDA_CHECK(cudaFuncSetAttribute(gru_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  GruBwdArgs a{B, U, H, J, BC, dout, Whh, stash, dgi, dgh, carry};
+  void* args[] = {&a};
+  W2L_CUDA_CHECK(cudaLaunchCooperativeKernel((const void*)gru_bwd_kernel, dim3(grid), dim3(kThreads), args, smem, static_cast<cudaStream_t>(stream)));
+  W2L_LAUNCH_CHECK("seq2seq_gru_bwd_kernel");
+  return W2L_OK;
+}
+
+W2L_API int w2l_seq2seq_attn_fwd(void* stream, int B, int U, int Tp, int H, const float* q, const float* x, int window_u, float window_std,
+                                 float* out, float* attn) {
+  if (int rc = w2l_seq2seq_check(H, 3)) return rc;
+  if (B <= 0 || U <= 0 || Tp <= 0 || !q || !x || !out || (window_std > 0.f && window_u <= 0))
+    return fail(W2L_ERR_INVALID_ARGUMENT, "seq2seq_attn_fwd: bad arguments");
+  const size_t smem = sizeof(float) * (size_t)kUTile * (H + Tp);
+  if (smem > kSmemLimit) return fail(W2L_ERR_UNSUPPORTED, "seq2seq_attn_fwd: too many encoder frames");
+  W2L_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const float inv2s2 = window_std > 0.f ? (float)(1.0 / (2.0 * (double)window_std * window_std)) : 0.f;
+  attn_fwd_kernel<<<dim3((U + kUTile - 1) / kUTile, B), kThreads, smem, static_cast<cudaStream_t>(stream)>>>(
+      U, Tp, H, q, x, 1.f / sqrtf((float)H), window_u, inv2s2, out, attn);
+  W2L_LAUNCH_CHECK("seq2seq_attn_fwd_kernel");
+  return W2L_OK;
+}
+
+W2L_API int w2l_seq2seq_attn_bwd(void* stream, int B, int U, int Tp, int H, const float* q, const float* x, const float* attn, const float* dout,
+                                 float* dq, float* dx, float* dS) {
+  if (int rc = w2l_seq2seq_check(H, 3)) return rc;
+  if (B <= 0 || U <= 0 || Tp <= 0 || !q || !x || !attn || !dout || !dq || !dx || !dS) return fail(W2L_ERR_INVALID_ARGUMENT, "seq2seq_attn_bwd: bad arguments");
+  const size_t smem1 = sizeof(float) * (size_t)kUTile * (H + Tp), smem2 = sizeof(float) * (size_t)2 * U * kTTile;
+  if (smem1 > kSmemLimit || smem2 > kSmemLimit) return fail(W2L_ERR_UNSUPPORTED, "seq2seq_attn_bwd: too many frames or decoder steps");
+  W2L_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_q_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
+  W2L_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
+  const float scale = 1.f / sqrtf((float)H);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  attn_bwd_q_kernel<<<dim3((U + kUTile - 1) / kUTile, B), kThreads, smem1, s>>>(U, Tp, H, x, attn, dout, scale, dS, dq);
+  W2L_LAUNCH_CHECK("seq2seq_attn_bwd_q_kernel");
+  attn_bwd_kv_kernel<<<dim3((Tp + kTTile - 1) / kTTile, B), kThreads, smem2, s>>>(U, Tp, H, q, attn, dS, dout, scale, dx);
+  W2L_LAUNCH_CHECK("seq2seq_attn_bwd_kv_kernel");
+  return W2L_OK;
+}
+
+W2L_API int w2l_seq2seq_loss(void* stream, int B, int U, int N, int pad, const int32_t* target, float* logits, float label_smooth,
+                             const float* dloss, int grad, float* rowloss, float* loss, const int32_t* bad) {
+  if (int rc = w2l_seq2seq_check(32, N)) return rc;
+  if (B <= 0 || U <= 0 || pad < 0 || pad >= N || !target || !logits || !rowloss || !loss || !(label_smooth >= 0.f && label_smooth < 1.f))
+    return fail(W2L_ERR_INVALID_ARGUMENT, "seq2seq_loss: bad arguments");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  profile_kind(2);
+  profile_start(s);
+  loss_kernel<<<(unsigned)((long long)B * U), 512, 0, s>>>(U, N, pad, target, logits, label_smooth, dloss, grad, rowloss, bad);
+  profile_stop(s);
+  W2L_LAUNCH_CHECK("seq2seq_loss_kernel");
+  loss_sum_kernel<<<(B + 127) / 128, 128, 0, s>>>(B, U, rowloss, loss);
+  W2L_LAUNCH_CHECK("seq2seq_loss_sum_kernel");
+  return W2L_OK;
+}
+
+W2L_API int w2l_seq2seq_scale_rows(void* stream, int B, int U, int N, const float* g, float seed_scale, float* d) {
+  if (B <= 0 || U <= 0 || N <= 0 || !g || !d || !(seed_scale > 0.f)) return fail(W2L_ERR_INVALID_ARGUMENT, "seq2seq_scale_rows: bad arguments");
+  scale_rows_kernel<<<(unsigned)((long long)B * U), 256, 0, static_cast<cudaStream_t>(stream)>>>(U, N, g, 1.f / seed_scale, d);
+  W2L_LAUNCH_CHECK("seq2seq_scale_rows_kernel");
+  return W2L_OK;
+}
+
+W2L_API int w2l_seq2seq_decode_init(void* stream, int B, int H, int maxlen, int pad, const float* start, float* in, int32_t* tokens, int32_t* len,
+                                    int32_t* done) {
+  if (B <= 0 || H <= 0 || maxlen <= 0 || !start || !in || !tokens || !len || !done) return fail(W2L_ERR_INVALID_ARGUMENT, "seq2seq_decode_init: bad arguments");
+  decode_init_kernel<<<B, 256, 0, static_cast<cudaStream_t>(stream)>>>(B, H, maxlen, pad, start, in, tokens, len, done);
+  W2L_LAUNCH_CHECK("seq2seq_decode_init_kernel");
+  return W2L_OK;
+}
+
+W2L_API int w2l_seq2seq_decode_step(void* stream, int B, int N, int H, int step, int eos, const float* logits, const float* E, float* in,
+                                    int32_t* tokens, int maxlen, int32_t* len, int32_t* done) {
+  if (B <= 0 || N <= 0 || H <= 0 || step < 0 || step >= maxlen || !logits || !E || !in || !tokens || !len || !done)
+    return fail(W2L_ERR_INVALID_ARGUMENT, "seq2seq_decode_step: bad arguments");
+  decode_step_kernel<<<B, 256, 0, static_cast<cudaStream_t>(stream)>>>(N, H, step, eos, logits, E, in, tokens, maxlen, len, done);
+  W2L_LAUNCH_CHECK("seq2seq_decode_step_kernel");
+  return W2L_OK;
+}
+
+}  // extern "C"

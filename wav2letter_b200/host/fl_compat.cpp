@@ -1871,6 +1871,232 @@ af::array LinearSegmentationCriterion::viterbiPathWithTarget(const af::array& in
   return facAlign(N_, params_[0], input, target, index);
 }
 
+// ================================================================================================
+// Seq2SeqCriterion (DESIGN.md §9): an autograd graph of embedding -> R x (S GRU layers -> key-value attention) ->
+// output Linear -> fused log-softmax / NLL.  The projections are fl::Linear's GEMMs (the thread's precision); the
+// recurrence, attention, embedding and loss are csrc/seq2seq.cu.
+// ================================================================================================
+namespace {
+// one GRU layer over the whole sequence: gi = W_ih x + b_ih [B*U][3H] in, h [B*U][H] out
+Variable gruLayer(const Variable& gi, const Variable& whh, const Variable& bhh, int B, int U, int H) {
+  af::array out = af::array::empty(af::dim4(H, U, B));
+  af::array stash = af::array::empty(af::dim4((long long)w2l_seq2seq_gru_stash_floats(B, U, H)));
+  check(w2l_seq2seq_gru_fwd(currentStream(), B, U, H, gi.array().f32(), whh.array().f32(), bhh.array().f32(), nullptr, out.f32(), stash.f32()));
+  return Variable(out, {gi, whh, bhh}, [=](std::vector<Variable>& ins, const Variable& g) {
+    const long long M = (long long)B * U;
+    af::array dgi = af::array::empty(af::dim4(3 * H, U, B));
+    af::array dgh = af::array::empty(af::dim4(3 * H, U, B));
+    af::array carry = af::array::empty(af::dim4(H, B));
+    check(w2l_seq2seq_gru_bwd(currentStream(), B, U, H, g.array().f32(), ins[1].array().f32(), stash.f32(), dgi.f32(), dgh.f32(), carry.f32()));
+    if (ins[1].isCalcGrad()) {
+      // dW_hh [3H][H] = dgh^T h_{u-1} over all rows (the stash's fifth plane), db_hh = column sums: one GEMM, one reduction
+      const af::array hprev = af::array::view(stash, sizeof(float) * (size_t)(4 * M * H), af::dim4(H, U, B), DType::f32);
+      const HeldOperand dyop = rowOperand(dgh, M, 3 * H), xop = rowOperand(hprev, M, H);
+      af::array dw = ins[1].gradStorage();
+      const int accumulate = xop.op.ld == H && !dw.isEmpty() ? 1 : 0;
+      if (!accumulate) dw = af::array::empty(ins[1].dims());
+      check(w2l_gemm(currentStream(), xop.op.kind, 1, 1, 3 * H, H, (int)M, dyop.op.ptr, dyop.op.ld, xop.op.ptr, xop.op.ld, dw.f32(), H, 0, nullptr, 0,
+                     accumulate, nullptr, 0, 0, 0, 1.f, 0.f, 0ull, 0));
+      ins[1].addGrad(Variable(dw, false));
+      af::array db = ins[2].gradStorage();
+      if (db.isEmpty()) db = af::array::zeros(ins[2].dims());
+      check(w2l_colsum_accumulate(currentStream(), (int)M, 3 * H, dgh.f32(), 3 * H, db.f32()));
+      ins[2].addGrad(Variable(db, false));
+    }
+    ins[0].addGrad(Variable(dgi, false), true);
+  });
+}
+// inverted dropout between stacked layers with a given seed: w2l_act_fwd's mask (tests/dropout_reference.py simt_scale)
+Variable seededDropout(const Variable& in, float p, unsigned long long seed) {
+  af::array y = af::array::empty(in.dims());
+  check(w2l_act_fwd(currentStream(), in.elements(), in.array().f32(), 0, p, seed, y.f32()));
+  return Variable(y, {in}, [y, p](std::vector<Variable>& ins, const Variable& g) {
+    af::array d = af::array::empty(y.dims());
+    check(w2l_mask_mul(currentStream(), y.elements(), g.array().f32(), y.f32(), 2, 1.0f / (1.0f - p), d.f32()));
+    ins[0].addGrad(Variable(d, false), true);
+  });
+}
+// h = q + attention(q, x): the round's output, the next round's input
+Variable attentionRound(const Variable& q, const Variable& x, int B, int U, int Tp, int H, float windowStd) {
+  af::array out = af::array::empty(af::dim4(H, U, B));
+  af::array attn = af::array::empty(af::dim4(Tp, U, B));
+  check(w2l_seq2seq_attn_fwd(currentStream(), B, U, Tp, H, q.array().f32(), x.array().f32(), U, windowStd, out.f32(), attn.f32()));
+  return Variable(out, {q, x}, [=](std::vector<Variable>& ins, const Variable& g) {
+    af::array dq = af::array::empty(ins[0].dims());
+    af::array dx = af::array::empty(ins[1].dims());
+    af::array dS = af::array::empty(af::dim4(Tp, U, B));
+    check(w2l_seq2seq_attn_bwd(currentStream(), B, U, Tp, H, ins[0].array().f32(), ins[1].array().f32(), attn.f32(), g.array().f32(), dq.f32(),
+                               dx.f32(), dS.f32()));
+    ins[0].addGrad(Variable(dq, false), true);
+    ins[1].addGrad(Variable(dx, false), true);
+  });
+}
+}  // namespace
+
+Seq2SeqCriterion::Seq2SeqCriterion(int nClass, int hiddenDim, int eos, int pad, int maxDecoderOutputLen,
+                                   const std::vector<std::shared_ptr<AttentionBase>>& attentions, std::shared_ptr<WindowBase> window,
+                                   bool trainWithWindow, int pctTeacherForcing, double labelSmooth, bool inputFeeding,
+                                   const std::string& samplingStrategy, double gumbelTemperature, int nRnnLayer, int nAttnRound, float dropOut)
+    : N_(nClass), H_(hiddenDim), eos_(eos), pad_(pad), maxLen_(maxDecoderOutputLen), pct_(pctTeacherForcing), S_(nRnnLayer), R_(nAttnRound),
+      ls_(labelSmooth), dropout_(dropOut), window_(std::move(window)), trainWithWindow_(trainWithWindow), windowOn_(window_ != nullptr) {
+  (void)gumbelTemperature;  // only the gumbel sampling strategy reads it
+  if (inputFeeding) throw std::invalid_argument("Seq2SeqCriterion: inputfeeding is not supported");
+  if (samplingStrategy != "rand") throw std::invalid_argument("Seq2SeqCriterion: sampling strategy '" + samplingStrategy + "' is not supported (only rand)");
+  if (nAttnRound < 1 || nRnnLayer < 1) throw std::invalid_argument("Seq2SeqCriterion: need at least one attention round and one RNN layer");
+  if ((int)attentions.size() != nAttnRound) throw std::invalid_argument("Seq2SeqCriterion: one attention per attention round");
+  for (const auto& a : attentions)
+    if (!std::dynamic_pointer_cast<KeyValueAttention>(a)) throw std::invalid_argument("Seq2SeqCriterion: only KeyValueAttention is supported");
+  if (window_ && !std::dynamic_pointer_cast<SoftPretrainWindow>(window_))
+    throw std::invalid_argument("Seq2SeqCriterion: only SoftPretrainWindow is supported");
+  if (w2l_seq2seq_check(hiddenDim, nClass) != W2L_OK) throw std::invalid_argument(w2l_last_error());
+  if (eos < 0 || eos >= nClass || pad < 0 || pad >= nClass || eos == pad) throw std::invalid_argument("Seq2SeqCriterion: eos and pad must be two classes");
+  if (maxDecoderOutputLen < 1) throw std::invalid_argument("Seq2SeqCriterion: maxdecoderoutputlen must be >= 1");
+  if (pctTeacherForcing < 0 || pctTeacherForcing > 100) throw std::invalid_argument("Seq2SeqCriterion: pctteacherforcing must be in [0, 100]");
+  if (!(labelSmooth >= 0 && labelSmooth < 1)) throw std::invalid_argument("Seq2SeqCriterion: labelsmooth must be in [0, 1)");
+  if (!(dropOut >= 0 && dropOut < 1)) throw std::invalid_argument("Seq2SeqCriterion: decoderdropout must be in [0, 1)");
+  const int H = hiddenDim;
+  const double bound = std::sqrt(1.0 / (double)H);
+  params_.push_back(Variable(uniformInit(af::dim4(H, nClass), bound, nextSeed()), true));  // E [N][H]
+  params_.push_back(Variable(uniformInit(af::dim4(H), 0.1, nextSeed()), true));           // startEmbedding
+  for (int k = 0; k < R_ * S_; ++k) {
+    auto ih = std::make_shared<Linear>(H, 3 * H), hh = std::make_shared<Linear>(H, 3 * H);
+    params_.push_back(ih->param(0));
+    params_.push_back(hh->param(0));
+    params_.push_back(ih->param(1));
+    params_.push_back(hh->param(1));
+    ih_.push_back(ih);
+  }
+  out_ = std::make_shared<Linear>(H, nClass);
+  params_.push_back(out_->param(0));
+  params_.push_back(out_->param(1));
+}
+std::string Seq2SeqCriterion::prettyString() const {
+  std::ostringstream o;
+  o << "Seq2SeqCriterion (H: " << H_ << ", N: " << N_ << ", rounds: " << R_ << ", layers: " << S_ << ", dropout: " << dropout_
+    << ", labelsmooth: " << ls_ << ", pctteacherforcing: " << pct_ << ", window: " << (window_ ? window_->prettyString() : "none") << ")";
+  return o.str();
+}
+
+std::vector<Variable> Seq2SeqCriterion::forward(const std::vector<Variable>& inputs) {
+  if (inputs.size() < 2 || inputs.size() > 4)
+    throw std::invalid_argument("Seq2SeqCriterion: expects {encoder output, target} and optionally durations and target sizes");
+  const Variable& x = inputs[0];
+  const af::array target = inputs[1].array();
+  if (x.type() != DType::f32) throw std::invalid_argument("Seq2SeqCriterion: encoder output must be f32");
+  if (target.type() != DType::i32) throw std::invalid_argument("Seq2SeqCriterion: target must be s32");
+  const int H = H_, N = N_;
+  if (x.dims(0) != 2 * H)
+    throw std::invalid_argument("Seq2SeqCriterion: encoder output has " + std::to_string(x.dims(0)) + " features; KeyValueAttention needs 2 * encoderdim = " +
+                                std::to_string(2 * H));
+  const int Tp = (int)x.dims(1), B = (int)(x.dims(2) * x.dims(3)), U = (int)target.dims(0);
+  if (target.dims(1) * target.dims(2) * target.dims(3) != B) throw std::invalid_argument("Seq2SeqCriterion: batch size mismatch between encoder output and target");
+  if (U < 1 || Tp < 1) throw std::invalid_argument("Seq2SeqCriterion: empty target or encoder output");
+  const bool train = train_;
+  bool needGrad = train && x.isCalcGrad();
+  for (const auto& p : params_) needGrad = needGrad || (train && p.isCalcGrad());
+  const unsigned long long seed = train ? nextSeed() : 0ull;
+  if (train) lastSeed_ = seed;
+  const bool window = windowOn_ && (!train || trainWithWindow_);
+  const float windowStd = window ? (float)std::static_pointer_cast<SoftPretrainWindow>(window_)->std() : 0.f;
+
+  // decoder inputs: startEmbedding, then E[y~_{u-1}] (teacher forcing with substitution while training)
+  af::array tokens = af::array::empty(af::dim4(U, B), DType::i32);
+  af::array in = af::array::empty(af::dim4(H, U, B));
+  // targets are checked on the device, without a host round trip: an utterance with a value outside [0, N) is flagged
+  // here and the loss kernel gives it NaN and no gradient
+  af::array bad = af::array::zeros(af::dim4(B), DType::i32);
+  check(w2l_seq2seq_embed_fwd(currentStream(), B, U, H, N, target.i32(), params_[0].array().f32(), params_[1].array().f32(), train ? (float)pct_ : 100.f,
+                              seed, tokens.i32(), in.f32(), bad.i32()));
+  Variable h(in, {params_[0], params_[1]}, [=](std::vector<Variable>& ins, const Variable& g) {
+    af::array dE = ins[0].gradStorage(), ds = ins[1].gradStorage();
+    if (dE.isEmpty()) dE = af::array::zeros(ins[0].dims());
+    if (ds.isEmpty()) ds = af::array::zeros(ins[1].dims());
+    check(w2l_seq2seq_embed_bwd(currentStream(), B, U, H, N, tokens.i32(), g.array().f32(), dE.f32(), ds.f32()));
+    ins[0].addGrad(Variable(dE, false));
+    ins[1].addGrad(Variable(ds, false));
+  });
+  for (int r = 0; r < R_; ++r) {
+    Variable cur = h;
+    for (int l = 0; l < S_; ++l) {
+      const int k = r * S_ + l, base = 2 + 4 * k;
+      Variable gi = ih_[k]->forwardWith(cur, params_[base], params_[base + 2]);
+      cur = gruLayer(gi, params_[base + 1], params_[base + 3], B, U, H);
+      // the layer's dropout mask: seed + 1 + k (cuDNN applies dropout to every layer's output but the stack's last)
+      if (train && dropout_ > 0.f && l + 1 < S_) cur = seededDropout(cur, dropout_, seed + 1 + (unsigned long long)k);
+    }
+    h = attentionRound(cur, x, B, U, Tp, H, windowStd);
+  }
+  const int wo = 2 + 4 * R_ * S_;
+  Variable logits = out_->forwardWith(h, params_[wo], params_[wo + 1]);
+  af::array rowloss = af::array::empty(af::dim4(U, B));
+  af::array loss = af::array::empty(af::dim4(B));
+  const float ls = train ? (float)ls_ : 0.f;
+  if (!needGrad) {
+    check(w2l_seq2seq_loss(currentStream(), B, U, N, pad_, target.i32(), logits.array().f32(), ls, nullptr, 0, rowloss.f32(), loss.f32(), bad.i32()));
+    return {Variable(loss, false)};
+  }
+  // loss and logit gradient in one pass; the gradient overwrites the logits (nothing reads them afterwards)
+  const af::array lossSeed = lossGradSeed(B);
+  const float seedScale = g_loss_grad_scale;
+  check(w2l_seq2seq_loss(currentStream(), B, U, N, pad_, target.i32(), logits.array().f32(), ls, lossSeed.isEmpty() ? nullptr : lossSeed.f32(), 1,
+                         rowloss.f32(), loss.f32(), bad.i32()));
+  const af::array dlogits = logits.array();
+  return {Variable(loss, {logits}, [=](std::vector<Variable>& ins, const Variable& g) {
+    if (!g.isOnesSeed()) check(w2l_seq2seq_scale_rows(currentStream(), B, U, N, g.array().f32(), seedScale, dlogits.f32()));
+    ins[0].addGrad(Variable(dlogits, false), true);
+  })};
+}
+
+af::array Seq2SeqCriterion::decode(const af::array& x, af::array* lengths) {
+  const int H = H_, N = N_;
+  if (x.type() != DType::f32 || x.dims(0) != 2 * H)
+    throw std::invalid_argument("Seq2SeqCriterion: encoder output has " + std::to_string(x.dims(0)) + " features; KeyValueAttention needs 2 * encoderdim = " +
+                                std::to_string(2 * H));
+  const int Tp = (int)x.dims(1), B = (int)(x.dims(2) * x.dims(3)), maxLen = maxLen_;
+  af::array in = af::array::empty(af::dim4(H, 1, B));
+  af::array tokens = af::array::empty(af::dim4(maxLen, B), DType::i32);
+  af::array len = af::array::empty(af::dim4(B), DType::i32);
+  af::array done = af::array::empty(af::dim4(B + 1), DType::i32);
+  check(w2l_seq2seq_decode_init(currentStream(), B, H, maxLen, pad_, params_[1].array().f32(), in.f32(), tokens.i32(), len.i32(), done.i32()));
+  // every layer's hidden state, two buffers each (a step reads one and writes the other)
+  std::vector<af::array> state;
+  for (int i = 0; i < 2 * R_ * S_; ++i) state.push_back(af::array::empty(af::dim4(H, 1, B)));
+  auto P = [&](int i) { return fl::noGrad(params_[i].array()); };
+  constexpr int kCheckEvery = 8;  // steps between host reads of the finished count
+  for (int step = 0; step < maxLen; ++step) {
+    Variable h = fl::noGrad(in);
+    for (int r = 0; r < R_; ++r) {
+      Variable cur = h;
+      for (int l = 0; l < S_; ++l) {
+        const int k = r * S_ + l, base = 2 + 4 * k;
+        Variable gi = ih_[k]->forwardWith(cur, P(base), P(base + 2));
+        const af::array& prev = state[2 * k + ((step + 1) & 1)];
+        const af::array& next = state[2 * k + (step & 1)];
+        check(w2l_seq2seq_gru_fwd(currentStream(), B, 1, H, gi.array().f32(), params_[base + 1].array().f32(), params_[base + 3].array().f32(),
+                                  step ? prev.f32() : nullptr, next.f32(), nullptr));
+        cur = fl::noGrad(next);
+      }
+      af::array a = af::array::empty(af::dim4(H, 1, B));
+      check(w2l_seq2seq_attn_fwd(currentStream(), B, 1, Tp, H, cur.array().f32(), x.f32(), 1, 0.f, a.f32(), nullptr));
+      h = fl::noGrad(a);
+    }
+    const int wo = 2 + 4 * R_ * S_;
+    Variable logits = out_->forwardWith(h, P(wo), P(wo + 1));
+    check(w2l_seq2seq_decode_step(currentStream(), B, N, H, step, eos_, logits.array().f32(), params_[0].array().f32(), in.f32(), tokens.i32(), maxLen,
+                                  len.i32(), done.i32()));
+    if ((step + 1) % kCheckEvery == 0 && step + 1 < maxLen) {
+      af::array count = af::array::view(done, sizeof(int32_t) * (size_t)B, af::dim4(1), DType::i32);
+      if (count.scalar<int32_t>() == B) break;
+    }
+  }
+  if (lengths) *lengths = len;
+  return tokens;
+}
+af::array Seq2SeqCriterion::viterbiPath(const af::array& input, const af::array&) { return decode(input, nullptr); }
+af::array Seq2SeqCriterion::viterbiPathWithTarget(const af::array&, const af::array&, af::array*) {
+  throw std::invalid_argument("Seq2SeqCriterion: viterbiPathWithTarget is not supported");
+}
+
 }  // namespace speech
 }  // namespace pkg
 }  // namespace fl

@@ -277,6 +277,11 @@ std::vector<std::string> tknIdx2Ltr(const std::vector<int>& labels, const Dictio
 std::vector<std::string> tknPrediction2Ltr(std::vector<int> tokens, const Dictionary& tokenDict, const std::string& criterion,
                                            const std::string& surround, bool eosToken, int replabel, bool useWordPiece,
                                            const std::string& wordSep) {
+  if (criterion == kSeq2SeqRNNCriterion) {  // a decoded sequence ends at eos; pad fills the rest of its row
+    const int eosIdx = tokenDict.getIndex(lib::text::kEosToken), padIdx = tokenDict.getIndex(lib::text::kPadToken);
+    tokens.erase(std::find(tokens.begin(), tokens.end(), eosIdx), tokens.end());
+    tokens.erase(std::remove(tokens.begin(), tokens.end(), padIdx), tokens.end());
+  }
   if (criterion == kCtcCriterion || criterion == kAsgCriterion) uniq(tokens);
   if (criterion == kCtcCriterion) {
     const int blankIdx = tokenDict.getIndex(kBlankToken);
@@ -288,7 +293,10 @@ std::vector<std::string> tknPrediction2Ltr(std::vector<int> tokens, const Dictio
 }
 std::vector<std::string> tknTarget2Ltr(std::vector<int> tokens, const Dictionary& tokenDict, const std::string& criterion,
                                        const std::string& surround, bool eosToken, int replabel, bool useWordPiece, const std::string& wordSep) {
-  (void)criterion;
+  if (criterion == kSeq2SeqRNNCriterion) {  // targets are padded with the pad index
+    const int padIdx = tokenDict.getIndex(lib::text::kPadToken);
+    tokens.erase(std::remove(tokens.begin(), tokens.end(), padIdx), tokens.end());
+  }
   if (tokens.empty()) return {};
   remapLabels(tokens, tokenDict, surround, eosToken, replabel);
   return tknIdx2Ltr(tokens, tokenDict, useWordPiece, wordSep);
@@ -480,6 +488,10 @@ W2L_API void* w2l_text_create(const char* tokens_text, const char* lexicon_text,
     for (int r = 1; r <= replabel; ++r) t->dict.addEntry("<" + std::to_string(r) + ">");  // Train.cpp:245-247
     t->criterion = criterion ? criterion : "";
     if (t->criterion == fl::pkg::speech::kCtcCriterion) t->dict.addEntry(fl::pkg::speech::kBlankToken);  // blank last, :248-251
+    if (t->criterion == fl::pkg::speech::kSeq2SeqRNNCriterion) {  // eos, then pad, last (:252-257)
+      t->dict.addEntry(fl::lib::text::kEosToken);
+      t->dict.addEntry(fl::lib::text::kPadToken);
+    }
     if (lexicon_text && *lexicon_text) {
       std::istringstream ls(lexicon_text);
       t->lexicon = fl::lib::text::loadWords(ls);
@@ -501,7 +513,9 @@ W2L_API long long w2l_text_encode(void* h, const char* transcript, int32_t* out,
     auto* t = static_cast<TextPipeline*>(h);
     // the reference's own configuration (recipes/slimIPL/src/Train.cpp:296-305): skipUnk = true, letter fallback with the
     // word separator on the left for word pieces, on the right otherwise
-    fl::pkg::speech::TargetGenerationConfig cfg(t->wordsep, 0, t->criterion, t->surround, false, t->replabel, true, t->wordpiece, !t->wordpiece);
+    // seq2seq targets end with eos (eosToken)
+    fl::pkg::speech::TargetGenerationConfig cfg(t->wordsep, 0, t->criterion, t->surround, t->criterion == fl::pkg::speech::kSeq2SeqRNNCriterion, t->replabel, true,
+                                                t->wordpiece, !t->wordpiece);
     const std::vector<int> tgt = fl::pkg::speech::targetFeatures(splitSpace(transcript), t->dict, t->lexicon, cfg);
     if (out && cap >= (long long)tgt.size()) std::copy(tgt.begin(), tgt.end(), out);
     return (long long)tgt.size();
@@ -512,7 +526,7 @@ W2L_API long long w2l_text_prediction2ltr(void* h, const int32_t* path, int n, c
   return guardedText([&]() -> long long {
     auto* t = static_cast<TextPipeline*>(h);
     std::vector<int> v(path, path + n);
-    return putJoined(fl::pkg::speech::tknPrediction2Ltr(v, t->dict, t->criterion, t->surround, false, t->replabel, t->wordpiece, t->wordsep), out, cap);
+    return putJoined(fl::pkg::speech::tknPrediction2Ltr(v, t->dict, t->criterion, t->surround, t->criterion == fl::pkg::speech::kSeq2SeqRNNCriterion, t->replabel, t->wordpiece, t->wordsep), out, cap);
   });
 }
 // padded target row (len entries, negative = padding) -> letters, space-joined
@@ -521,7 +535,7 @@ W2L_API long long w2l_text_target2ltr(void* h, const int32_t* target, int len, c
     auto* t = static_cast<TextPipeline*>(h);
     const int n = fl::pkg::speech::getTargetSize(target, len);
     std::vector<int> v(target, target + n);
-    return putJoined(fl::pkg::speech::tknTarget2Ltr(v, t->dict, t->criterion, t->surround, false, t->replabel, t->wordpiece, t->wordsep), out, cap);
+    return putJoined(fl::pkg::speech::tknTarget2Ltr(v, t->dict, t->criterion, t->surround, t->criterion == fl::pkg::speech::kSeq2SeqRNNCriterion, t->replabel, t->wordpiece, t->wordsep), out, cap);
   });
 }
 // letters (space-joined) -> words (space-joined), split at the word separator

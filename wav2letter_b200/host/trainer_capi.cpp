@@ -71,6 +71,11 @@ struct AmpState {
   unsigned short counter = 1;
   long long retries = 0;  // steps run again at half the scale
 };
+// the Seq2Seq criterion's constructor settings (w2l_trainer_create_seq2seq), kept for checkpoints
+struct Seq2SeqSettings {
+  int hidden = 0, eos = 0, pad = 0, maxLen = 0, rounds = 1, layers = 1, pct = 100, trainWithWindow = 0;
+  float dropout = 0.f, labelSmooth = 0.f, windowStd = 0.f;
+};
 struct Trainer {
   std::shared_ptr<fl::Module> net;
   std::unique_ptr<fl::OverlappedArenaReducer> reducer;  // created at the first distributed step
@@ -90,7 +95,10 @@ struct Trainer {
   long long update = 0;  // training steps taken: Train.cpp's curBatch after the step
   long long epoch = 0;   // Train.cpp's curEpoch (1 while the first epoch runs), set by the caller
   int nFeat, nLabel;
+  int outWidth;  // features per frame of the network output: nLabel, or 2 * hidden for seq2seq
   bool isCtc;
+  std::shared_ptr<Seq2SeqCriterion> s2s;  // set for "seq2seq"
+  Seq2SeqSettings s2sSettings;
   // the criterion's gradient is part of clipGradNorm: Train.cpp runs ctc / asg with clampCrit = true (:1923,1939) and the
   // --linseg warm start with clampCrit = false (:1878), where the transitions step unclipped
   bool clampCrit = true;
@@ -201,8 +209,9 @@ w2l::streaming::TrainerSnapshotSource w2l::streaming::trainerSnapshotSource(void
 
 extern "C" {
 
-W2L_API void* w2l_trainer_create(void* stream, const char* arch_text, int n_feat, int n_label, const char* criterion, int scale_mode,
-                                 float transdiag, float lr, float lrcrit, float momentum, float maxgradnorm) {
+namespace {
+Trainer* createTrainer(void* stream, const char* arch_text, int n_feat, int n_label, const char* criterion, int scale_mode, float transdiag, float lr,
+                       float lrcrit, float momentum, float maxgradnorm, const Seq2SeqSettings* s2s) {
   Trainer* t = nullptr;
   const int rc = guarded([&] {
     w2l::setCurrentStream(stream);
@@ -229,8 +238,19 @@ W2L_API void* w2l_trainer_create(void* stream, const char* arch_text, int n_feat
       tr->crit = lin;
       tr->isCtc = false;
       tr->clampCrit = false;
+    } else if (c == "seq2seq" && s2s) {
+      // Train.cpp:411-432: one KeyValueAttention per round, SoftPretrainWindow(--softwstd) when set
+      std::vector<std::shared_ptr<AttentionBase>> attentions;
+      for (int i = 0; i < s2s->rounds; ++i) attentions.push_back(std::make_shared<KeyValueAttention>());
+      std::shared_ptr<WindowBase> window;
+      if (s2s->windowStd > 0.f) window = std::make_shared<SoftPretrainWindow>(s2s->windowStd);
+      tr->s2s = std::make_shared<Seq2SeqCriterion>(n_label, s2s->hidden, s2s->eos, s2s->pad, s2s->maxLen, attentions, window, s2s->trainWithWindow != 0,
+                                                   s2s->pct, s2s->labelSmooth, false, "rand", 1.0, s2s->layers, s2s->rounds, s2s->dropout);
+      tr->crit = tr->s2s;
+      tr->isCtc = false;
+      tr->s2sSettings = *s2s;
     } else {
-      throw std::invalid_argument("criterion must be 'ctc', 'asg' or 'linseg'");
+      throw std::invalid_argument(s2s ? "criterion must be 'seq2seq'" : "criterion must be 'ctc', 'asg' or 'linseg'");
     }
     tr->netArena = flattenParameters({tr->net});
     if (!tr->crit->params().empty()) tr->critArena = flattenParameters({tr->crit});
@@ -243,6 +263,7 @@ W2L_API void* w2l_trainer_create(void* stream, const char* arch_text, int n_feat
     tr->maxgradnorm = maxgradnorm;
     tr->nFeat = n_feat;
     tr->nLabel = n_label;
+    tr->outWidth = tr->s2s ? 2 * s2s->hidden : n_label;
     tr->archText = arch;
     tr->critName = c;
     tr->scaleMode = scale_mode;
@@ -250,6 +271,58 @@ W2L_API void* w2l_trainer_create(void* stream, const char* arch_text, int n_feat
     t = tr.release();
   });
   return rc == W2L_OK ? t : nullptr;
+}
+}  // namespace
+
+W2L_API void* w2l_trainer_create(void* stream, const char* arch_text, int n_feat, int n_label, const char* criterion, int scale_mode,
+                                 float transdiag, float lr, float lrcrit, float momentum, float maxgradnorm) {
+  return createTrainer(stream, arch_text, n_feat, n_label, criterion, scale_mode, transdiag, lr, lrcrit, momentum, maxgradnorm, nullptr);
+}
+
+W2L_API void* w2l_trainer_create_seq2seq(void* stream, const char* arch_text, int n_feat, int n_label, int hidden, int eos, int pad,
+                                         int max_decoder_output_len, int rounds, int layers, float dropout, float label_smooth,
+                                         int pct_teacher_forcing, float window_std, int train_with_window, float lr, float lrcrit, float momentum,
+                                         float maxgradnorm) {
+  Seq2SeqSettings s;
+  s.hidden = hidden;
+  s.eos = eos;
+  s.pad = pad;
+  s.maxLen = max_decoder_output_len;
+  s.rounds = rounds;
+  s.layers = layers;
+  s.dropout = dropout;
+  s.labelSmooth = label_smooth;
+  s.pct = pct_teacher_forcing;
+  s.windowStd = window_std;
+  s.trainWithWindow = train_with_window;
+  return createTrainer(stream, arch_text, n_feat, n_label, "seq2seq", 0, 0.f, lr, lrcrit, momentum, maxgradnorm, &s);
+}
+
+W2L_API int w2l_trainer_output_width(void* h, int* width) {
+  if (!h || !width) return w2l::fail(W2L_ERR_INVALID_ARGUMENT, "trainer_output_width: null trainer or output");
+  *width = static_cast<Trainer*>(h)->outWidth;
+  return W2L_OK;
+}
+
+W2L_API int w2l_trainer_seq2seq_config(void* h, int* config7) {
+  auto* t = static_cast<Trainer*>(h);
+  if (!t || !t->s2s || !config7) return w2l::fail(W2L_ERR_INVALID_ARGUMENT, "trainer_seq2seq_config: not a seq2seq trainer");
+  const Seq2SeqSettings& s = t->s2sSettings;
+  const int v[7] = {s.hidden, s.eos, s.pad, s.maxLen, s.rounds, s.layers, t->s2s->windowSet() ? 1 : 0};
+  std::copy(v, v + 7, config7);
+  return W2L_OK;
+}
+W2L_API int w2l_trainer_clear_window(void* h) {
+  auto* t = static_cast<Trainer*>(h);
+  if (!t || !t->s2s) return w2l::fail(W2L_ERR_INVALID_ARGUMENT, "trainer_clear_window: not a seq2seq trainer");
+  t->s2s->clearWindow();
+  return W2L_OK;
+}
+W2L_API int w2l_trainer_seq2seq_seed(void* h, unsigned long long* seed) {
+  auto* t = static_cast<Trainer*>(h);
+  if (!t || !t->s2s || !seed) return w2l::fail(W2L_ERR_INVALID_ARGUMENT, "trainer_seq2seq_seed: not a seq2seq trainer");
+  *seed = t->s2s->lastSeed();
+  return W2L_OK;
 }
 
 W2L_API void w2l_trainer_destroy(void* h) { delete static_cast<Trainer*>(h); }
@@ -511,7 +584,7 @@ W2L_API int w2l_trainer_forward(void* h, void* stream, int B, int T, const float
     Variable out = t->net->forward(std::vector<Variable>{fl::input(af::array::wrap(const_cast<float*>(features), af::dim4(T, t->nFeat, 1, B)))}).front();
     if (out.elements() > capacity) throw std::invalid_argument("trainer_forward: output buffer too small");
     af::array::wrap(emissions_out, out.dims()).copyFrom(out.array());
-    if (t_out) *t_out = (int)(out.elements() / ((long long)B * t->nLabel));  // frames of nLabel values per sample
+    if (t_out) *t_out = (int)(out.elements() / ((long long)B * t->outWidth));  // frames of outWidth values per sample
   });
 }
 
@@ -522,6 +595,7 @@ W2L_API int w2l_trainer_align(void* h, void* stream, int B, int T, const float* 
     w2l::setCurrentStream(stream);
     auto* t = static_cast<Trainer*>(h);
     if (B <= 0 || T <= 0 || L <= 0 || !features || !target || !path) throw std::invalid_argument("trainer_align: bad arguments");
+    if (t->s2s) throw std::invalid_argument("trainer_align: forced alignment is not supported for the seq2seq criterion");
     PrecisionScope scope(t->precision);
     t->net->eval();
     Variable out = t->net->forward(std::vector<Variable>{fl::input(af::array::wrap(const_cast<float*>(features), af::dim4(T, t->nFeat, 1, B)))}).front();
@@ -532,6 +606,26 @@ W2L_API int w2l_trainer_align(void* h, void* stream, int B, int T, const float* 
     af::array::wrap(path, p.dims(), w2l::DType::i32).copyFrom(p);
     if (idx) af::array::wrap(idx, index.dims(), w2l::DType::i32).copyFrom(index);
     if (t_out) *t_out = (int)p.dims(0);
+  });
+}
+
+// network forward (eval mode) + the seq2seq criterion's greedy decode: tokens device int32 [B][maxdecoderoutputlen] (pad
+// after each utterance's end), lengths device int32 [B]
+W2L_API int w2l_trainer_decode(void* h, void* stream, int B, int T, const float* features, int32_t* tokens, int32_t* lengths, long long capacity) {
+  return guarded([&] {
+    w2l::setCurrentStream(stream);
+    auto* t = static_cast<Trainer*>(h);
+    if (!t->s2s) throw std::invalid_argument("trainer_decode: only the seq2seq criterion decodes");
+    if (B <= 0 || T <= 0 || !features || !tokens || !lengths) throw std::invalid_argument("trainer_decode: bad arguments");
+    if (capacity < (long long)B * t->s2sSettings.maxLen) throw std::invalid_argument("trainer_decode: token buffer too small");
+    PrecisionScope scope(t->precision);
+    t->net->eval();
+    t->crit->eval();
+    Variable out = t->net->forward(std::vector<Variable>{fl::input(af::array::wrap(const_cast<float*>(features), af::dim4(T, t->nFeat, 1, B)))}).front();
+    af::array len;
+    const af::array tok = t->s2s->decode(out.array(), &len);
+    af::array::wrap(tokens, tok.dims(), w2l::DType::i32).copyFrom(tok);
+    af::array::wrap(lengths, len.dims(), w2l::DType::i32).copyFrom(len);
   });
 }
 
@@ -558,7 +652,10 @@ W2L_API int w2l_trainer_sync_parameters(void* h, void* stream) {  // fl::allRedu
 // position (i64 update, i64 epoch), the learning-rate schedule (i64 warmup, f64 gamma, i64 stepsize, i32 lrcosine,
 // i64 nbatches, i64 lr_decay, i64 lr_decay_step) and the loss scaling (i32 on, f64 scale, i32 update_interval,
 // f64 max_scale, f64 min_scale, i32 counter, i64 retries).  Version 1 files load with position 0, the default schedule and
-// loss scaling off.  Plays
+// loss scaling off.  The constructor arguments depend on the criterion name: for "seq2seq" the arch text is followed by
+// the criterion's settings (i32 hidden, eos, pad, maxdecoderoutputlen, rounds, layers, pctteacherforcing,
+// trainWithWindow; f32 dropout, labelsmooth, softwstd) and i32 "the window is still set"; the other criteria have none,
+// so their files are what they always were.  Plays
 // the role of Serializer::save(path, version, config, network, criterion, netoptim, critoptim) (Train.cpp:747-800).
 
 W2L_API int w2l_trainer_save(void* h, void* stream, const char* path) {
@@ -582,6 +679,12 @@ W2L_API int w2l_trainer_save(void* h, void* stream, const char* path) {
       put<float>(o, t->maxgradnorm);
       putStr(o, t->critName);
       putStr(o, t->archText);
+      if (t->s2s) {  // the seq2seq settings and whether the window is still set
+        const Seq2SeqSettings& s = t->s2sSettings;
+        for (int v : {s.hidden, s.eos, s.pad, s.maxLen, s.rounds, s.layers, s.pct, s.trainWithWindow}) put<int32_t>(o, v);
+        for (float v : {s.dropout, s.labelSmooth, s.windowStd}) put<float>(o, v);
+        put<int32_t>(o, t->s2s->windowSet() ? 1 : 0);
+      }
       putArena(o, t->netArena.values, t->netArena.elements);
       putArena(o, t->netArena.velocity, t->netArena.elements);
       putArena(o, t->critArena.values, t->critArena.elements);
@@ -626,9 +729,19 @@ W2L_API void* w2l_trainer_load(void* stream, const char* path) {
     const int nFeat = get<int32_t>(i), nLabel = get<int32_t>(i), scaleMode = get<int32_t>(i), precision = get<int32_t>(i);
     const float transdiag = get<float>(i), lr = get<float>(i), lrcrit = get<float>(i), momentum = get<float>(i), maxgradnorm = get<float>(i);
     const std::string crit = getStr(i), arch = getStr(i);
-    void* h = w2l_trainer_create(stream, arch.c_str(), nFeat, nLabel, crit.c_str(), scaleMode, transdiag, lr, lrcrit, momentum, maxgradnorm);
+    Seq2SeqSettings s2s;
+    int windowSet = 0;
+    const bool isSeq2seq = crit == "seq2seq";
+    if (isSeq2seq) {
+      for (int* v : {&s2s.hidden, &s2s.eos, &s2s.pad, &s2s.maxLen, &s2s.rounds, &s2s.layers, &s2s.pct, &s2s.trainWithWindow}) *v = get<int32_t>(i);
+      for (float* v : {&s2s.dropout, &s2s.labelSmooth, &s2s.windowStd}) *v = get<float>(i);
+      windowSet = get<int32_t>(i);
+    }
+    void* h = isSeq2seq ? createTrainer(stream, arch.c_str(), nFeat, nLabel, crit.c_str(), scaleMode, transdiag, lr, lrcrit, momentum, maxgradnorm, &s2s)
+                           : w2l_trainer_create(stream, arch.c_str(), nFeat, nLabel, crit.c_str(), scaleMode, transdiag, lr, lrcrit, momentum, maxgradnorm);
     if (!h) throw std::invalid_argument(std::string("checkpoint: cannot rebuild the trainer: ") + w2l_last_error());
     std::unique_ptr<Trainer> t(static_cast<Trainer*>(h));
+    if (t->s2s) t->s2s->setWindow(windowSet != 0);
     t->precision = precision;
     w2l::setCurrentStream(stream);
     getArena(i, t->netArena.values, t->netArena.elements, stream);
@@ -679,6 +792,7 @@ W2L_API int w2l_trainer_export_streaming(void* h, void* stream, const char* outd
   return guarded([&] {
     w2l::setCurrentStream(stream);
     auto* t = static_cast<Trainer*>(h);
+    if (t->s2s) throw std::invalid_argument("export: the streaming export covers ctc and asg models, not the seq2seq criterion");
     const std::string dir = outdir;
     ::mkdir(dir.c_str(), 0755);
     // host copies of the parameters in module order

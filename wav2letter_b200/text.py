@@ -18,6 +18,7 @@ class TextPipeline:
         if not h:
             raise capi.W2LError(1, lib.w2l_last_error().decode())
         self.h = ctypes.c_void_p(h)
+        self.criterion = criterion
 
     def close(self):
         if getattr(self, "h", None):
@@ -41,11 +42,16 @@ class TextPipeline:
         lib.w2l_text_encode(self.h, transcript.encode(), out.ctypes.data_as(ctypes.c_void_p), n)
         return out[:n]
 
+    @property
+    def pad_index(self) -> int:
+        """the value targets are padded with: the pad token's index for seq2seq (the dictionary's last entry), else -1"""
+        return self.num_classes - 1 if self.criterion == "seq2seq" else -1
+
     def encode_batch(self, transcripts) -> np.ndarray:
-        """[B][L] int32 padded with -1 (kTargetPadValue)"""
+        """[B][L] int32 padded with pad_index (-1, kTargetPadValue; the pad token for seq2seq)"""
         rows = [self.encode(t) for t in transcripts]
         L = max(1, max(len(r) for r in rows))
-        out = np.full((len(rows), L), -1, np.int32)
+        out = np.full((len(rows), L), self.pad_index, np.int32)
         for b, r in enumerate(rows):
             out[b, :len(r)] = r
         return out

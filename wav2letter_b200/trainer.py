@@ -17,11 +17,22 @@ from .capi import _check, _ptr, _stream, lib
 class Trainer:
     def __init__(self, arch_text: str, n_feat: int, n_label: int, criterion: str = "ctc", scale_mode="none",
                  transdiag: float = 0.0, lr: float = 0.05, lrcrit: float = 0.0, momentum: float = 0.0,
-                 maxgradnorm: float = 0.0, precision: str | None = None):
-        """precision: None (the thread's w2l_set_precision), "tf32", "f32" (fp32-accurate), "bf16" or "fp16"."""
+                 maxgradnorm: float = 0.0, precision: str | None = None, seq2seq: dict | None = None):
+        """precision: None (the thread's w2l_set_precision), "tf32", "f32" (fp32-accurate), "bf16" or "fp16".
+        criterion "seq2seq" takes its settings from `seq2seq` (Train.cpp's flags): hidden (--encoderdim), eos, pad,
+        maxdecoderoutputlen, and optionally rounds (--decoderattnround, 1), layers (--decoderrnnlayer, 1), dropout
+        (--decoderdropout, 0), labelsmooth (0), pctteacherforcing (100), window_std (--softwstd; 0 = no window) and
+        train_with_window (--trainWithWindow, False); n_label counts the dictionary with eos and pad."""
         mode = capi.SCALE_MODES[scale_mode] if isinstance(scale_mode, str) else int(scale_mode)
-        self.h = lib.w2l_trainer_create(_stream(), arch_text.encode(), n_feat, n_label, criterion.encode(), mode,
-                                        transdiag, lr, lrcrit, momentum, maxgradnorm)
+        if criterion == "seq2seq":
+            s = dict(SEQ2SEQ_DEFAULTS, **(seq2seq or {}))
+            self.h = lib.w2l_trainer_create_seq2seq(_stream(), arch_text.encode(), n_feat, n_label, int(s["hidden"]), int(s["eos"]), int(s["pad"]),
+                                                    int(s["maxdecoderoutputlen"]), int(s["rounds"]), int(s["layers"]), float(s["dropout"]),
+                                                    float(s["labelsmooth"]), int(s["pctteacherforcing"]), float(s["window_std"]),
+                                                    int(bool(s["train_with_window"])), lr, lrcrit, momentum, maxgradnorm)
+        else:
+            self.h = lib.w2l_trainer_create(_stream(), arch_text.encode(), n_feat, n_label, criterion.encode(), mode,
+                                            transdiag, lr, lrcrit, momentum, maxgradnorm)
         if not self.h:
             raise capi.W2LError(1, lib.w2l_last_error().decode())
         self.h = ctypes.c_void_p(self.h)
@@ -153,13 +164,46 @@ class Trainer:
                                     float(total_batch if total_batch is not None else B)))
         return loss_out
 
+    def output_width(self) -> int:
+        """features per frame of the network output: n_label, or 2 * hidden (the encoder) for seq2seq"""
+        w = ctypes.c_int(0)
+        _check(lib.w2l_trainer_output_width(self.h, ctypes.byref(w)))
+        return int(w.value)
+
     def forward(self, features: torch.Tensor) -> torch.Tensor:
         B, _, F, T = features.shape
-        cap = B * (2 * T + 64) * self.n_label  # SAME-padded even kernels grow the frame count by one each
+        width = self.output_width()
+        cap = B * (2 * T + 64) * width  # SAME-padded even kernels grow the frame count by one each
         out = torch.empty(cap, dtype=torch.float32, device=features.device)
         tout = ctypes.c_int(0)
         _check(lib.w2l_trainer_forward(self.h, _stream(), B, T, _ptr(features), _ptr(out), cap, ctypes.byref(tout)))
-        return out[: B * tout.value * self.n_label].view(B, tout.value, self.n_label)
+        return out[: B * tout.value * width].view(B, tout.value, width)
+
+    def seq2seq_config(self) -> dict:
+        """hidden, eos, pad, maxdecoderoutputlen, rounds, layers and whether the window is still set (seq2seq only)"""
+        v = (ctypes.c_int * 7)()
+        _check(lib.w2l_trainer_seq2seq_config(self.h, v))
+        return dict(zip(("hidden", "eos", "pad", "maxdecoderoutputlen", "rounds", "layers", "window_set"), (int(x) for x in v)))
+
+    def clear_window(self):
+        """Seq2SeqCriterion::clearWindow(): after the --pretrainWindow updates, train without the soft window"""
+        _check(lib.w2l_trainer_clear_window(self.h))
+
+    def seq2seq_seed(self) -> int:
+        """the Philox seed the last training step's criterion drew (token substitution; dropout after layer k: seed + 1 + k)"""
+        s = ctypes.c_ulonglong(0)
+        _check(lib.w2l_trainer_seq2seq_seed(self.h, ctypes.byref(s)))
+        return int(s.value)
+
+    def decode(self, features: torch.Tensor):
+        """Greedy decode (seq2seq): eval-mode forward, then argmax token by token from startEmbedding until eos or
+        maxdecoderoutputlen steps.  Returns (tokens CUDA int32 [B, maxdecoderoutputlen] padded with pad, lengths CUDA int32 [B])."""
+        B, _, F, T = features.shape
+        n = self.seq2seq_config()["maxdecoderoutputlen"]
+        tokens = torch.empty((B, n), dtype=torch.int32, device=features.device)
+        lengths = torch.empty(B, dtype=torch.int32, device=features.device)
+        _check(lib.w2l_trainer_decode(self.h, _stream(), B, T, _ptr(features), _ptr(tokens), _ptr(lengths), tokens.numel()))
+        return tokens, lengths
 
     def align(self, features: torch.Tensor, target: torch.Tensor):
         """Forced alignment: eval-mode forward, then the criterion's viterbiPathWithTarget.  features CUDA float
@@ -194,6 +238,9 @@ def nccl_unique_id() -> bytes:
 def init_distributed(rank: int, world: int, uid: bytes):
     _check(lib.w2l_init_distributed(rank, world, ctypes.c_char_p(uid)))
 
+
+# the seq2seq settings' defaults (Train.cpp's flag defaults where they exist)
+SEQ2SEQ_DEFAULTS = dict(rounds=1, layers=1, dropout=0.0, labelsmooth=0.0, pctteacherforcing=100, window_std=0.0, train_with_window=False)
 
 from . import archs  # noqa: E402
 
