@@ -662,9 +662,23 @@ class SoftPretrainWindow : public WindowBase {
 // W_ih [3H][H], W_hh [3H][H], b_ih [3H], b_hh [3H], then W_o [N][H], b_o [N].  Refused (std::invalid_argument):
 // inputfeeding, a sampling strategy other than "rand", attentions other than KeyValueAttention, windows other than
 // SoftPretrainWindow, attentions.size() != nAttnRound.  viterbiPath is the greedy decode (int32 [maxDecoderOutputLen, B],
-// padded with pad); viterbiPathWithTarget is not supported.
+// padded with pad); viterbiPathWithTarget is not supported.  beamSearch / beamPath are the criterion's token-level beam
+// search over its own log-probabilities (no LM, no length normalisation, no window), as local_prior_match's
+// batchBeamSearch calls it; beamSearchBatch searches whole batches on the device and serves both.
 class Seq2SeqCriterion : public SequenceCriterion {
  public:
+  // a hypothesis of the beam search: its score (sum of log-probabilities, eos included when completed) and its tokens
+  // (eos excluded).  There is no decoder state: the search starts only from the single empty hypothesis.
+  struct CandidateHypo {
+    float score = 0.f;
+    std::vector<int> path;
+  };
+  // device results of beamSearchBatch: tokens int32 [maxLen, K, B] padded with pad, lengths int32 [K, B], scores f32
+  // [K, B], counts int32 [B] (<= K); slots at or beyond counts[b] hold pad, length 0 and score -inf
+  struct BeamResult {
+    af::array tokens, lengths, scores, counts;
+  };
+
   Seq2SeqCriterion(int nClass, int hiddenDim, int eos, int pad, int maxDecoderOutputLen,
                    const std::vector<std::shared_ptr<AttentionBase>>& attentions, std::shared_ptr<WindowBase> window = nullptr,
                    bool trainWithWindow = false, int pctTeacherForcing = 100, double labelSmooth = 0.0, bool inputFeeding = false,
@@ -675,6 +689,16 @@ class Seq2SeqCriterion : public SequenceCriterion {
   af::array viterbiPathWithTarget(const af::array& input, const af::array& target, af::array* index = nullptr) override;
   // greedy decode of every utterance: tokens [maxDecoderOutputLen, B] int32 (pad after the end), lengths [B] int32
   af::array decode(const af::array& input, af::array* lengths);
+  // beam search of every utterance of input [2H, T', B] with beamSize in [1, 16] (std::invalid_argument outside) for at
+  // most maxLen steps: the completions if there are any (sorted by score if more than beamSize ever completed, else in
+  // completion order), otherwise the live beam at length maxLen
+  BeamResult beamSearchBatch(const af::array& input, int beamSize, int maxLen);
+  // one utterance [2H, T', 1] from the single empty hypothesis ({CandidateHypo{}}; any other beam throws
+  // std::invalid_argument): at most beamSize hypotheses
+  std::vector<CandidateHypo> beamSearch(const af::array& input, std::vector<CandidateHypo> beam, int beamSize, int maxLen);
+  // beamSearch(input, {CandidateHypo{}}, beamSize, maxDecoderOutputLen)[0].path as int32 [length] (an empty array for
+  // an empty path)
+  af::array beamPath(const af::array& input, int beamSize = 10);
   void clearWindow() { windowOn_ = false; }
   void setWindow(bool on) { windowOn_ = on && window_ != nullptr; }  // checkpoint restore
   bool windowSet() const { return windowOn_; }
@@ -683,6 +707,10 @@ class Seq2SeqCriterion : public SequenceCriterion {
   int hiddenDim() const { return H_; }
 
  private:
+  // one eval-mode decoder step over B * U rows (U query rows per utterance of x): every round and layer from the states
+  // prev[k] (empty: zeros) into next[k], attention without the window, then the output Linear: logits [N, 1, B * U]
+  Variable decoderStep(const af::array& x, int B, int U, const af::array& in, const std::vector<af::array>& prev,
+                       const std::vector<af::array>& next);
   int N_, H_, eos_, pad_, maxLen_, pct_, S_, R_;
   double ls_;
   float dropout_;

@@ -214,6 +214,18 @@ W2L_API int w2l_linseg_target(void* stream, int B, int T, int L, const int32_t* 
  *   decode_*    one greedy step: argmax of logits [B][N] (first maximum); eos finishes an utterance (len[b] = step, not
  *               emitted), another token is written to tokens[b][step] and in[b] = E[token]; done[B] counts finished
  *               utterances.  init: in = start, tokens = pad, len = maxlen, done = 0 ([B + 1] ints).
+ *   beam_*      the beam search of DESIGN.md §9 over B utterances x K slots, decoder rows r = b*K + slot, 1 <= K <= 16
+ *               (W2L_ERR_UNSUPPORTED outside).  ws: beam_workspace_size(B, K, maxlen) bytes; its first int32 counts
+ *               the utterances whose search has stopped early (the host reads it between steps).
+ *               init: in [B*K][H] = start, slot 0 of each utterance live with score 0.
+ *               step: from logits [B*K][N] of the live rows: scores s = score + log_softmax(logits) in fp32, each row's
+ *               best 2K (s desc, class asc), then per utterance the walk over the merged ranks (eos at rank < K
+ *               completes the hypothesis, at rank >= K is dropped; other classes extend the beam up to K), the K-cap
+ *               (stable sort of the completions, keep K) and the early stop (K-th completion > best live score).  Then
+ *               state[l][r] = next[l][b*K + parent(r)] for l < layers (each [B*K][H]) and in[r] = E[token(r)].
+ *               finish: tokens [B][K][maxlen] padded with pad, lengths and scores [B][K], counts [B] (<= K): the
+ *               completions if there are any (sorted if the cap ever applied, else in completion order), else the
+ *               live beam at length steps; slots at or beyond counts[b] hold pad, length 0 and score -inf.
  * ---------------------------------------------------------------------------------------- */
 W2L_API int w2l_seq2seq_check(int H, int N);
 W2L_API int w2l_seq2seq_embed_fwd(void* stream, int B, int U, int H, int N, const int32_t* target, const float* E, const float* start,
@@ -235,6 +247,12 @@ W2L_API int w2l_seq2seq_decode_init(void* stream, int B, int H, int maxlen, int 
                                     int32_t* done);
 W2L_API int w2l_seq2seq_decode_step(void* stream, int B, int N, int H, int step, int eos, const float* logits, const float* E, float* in,
                                     int32_t* tokens, int maxlen, int32_t* len, int32_t* done);
+W2L_API size_t w2l_seq2seq_beam_workspace_size(int B, int K, int maxlen);
+W2L_API int w2l_seq2seq_beam_init(void* stream, int B, int K, int H, int maxlen, const float* start, float* in, void* ws, size_t ws_bytes);
+W2L_API int w2l_seq2seq_beam_step(void* stream, int B, int K, int N, int H, int layers, int step, int maxlen, int eos, const float* logits,
+                                  const float* E, float* in, float* state, const float* next, void* ws, size_t ws_bytes);
+W2L_API int w2l_seq2seq_beam_finish(void* stream, int B, int K, int maxlen, int steps, int pad, const void* ws, size_t ws_bytes, int32_t* tokens,
+                                    int32_t* lengths, float* scores, int32_t* counts);
 
 /* ----------------------------------------------------------------------------------------
  * Dense contraction of the acoustic model (replaces fl::Linear's af::matmul -> cuBLAS and the
@@ -490,6 +508,11 @@ W2L_API int w2l_trainer_seq2seq_seed(void* trainer, unsigned long long* seed);
  * [B][maxdecoderoutputlen] padded with pad (capacity elements), lengths device int32 [B] (eos not counted) */
 W2L_API int w2l_trainer_decode(void* trainer, void* stream, int B, int T, const float* features, int32_t* tokens, int32_t* lengths,
                                long long capacity);
+/* seq2seq only: eval-mode network forward, then Seq2SeqCriterion::beamSearchBatch with beam K (1..16) and max_len steps
+ * (0: maxdecoderoutputlen): tokens device int32 [B][K][max_len] (capacity elements) padded with pad, lengths int32 and
+ * scores float [B][K], counts int32 [B]; slots at or beyond counts[b] hold pad, length 0 and score -inf */
+W2L_API int w2l_trainer_beam_search(void* trainer, void* stream, int B, int T, const float* features, int beam, int max_len, int32_t* tokens,
+                                    int32_t* lengths, float* scores, int32_t* counts, long long capacity);
 W2L_API void w2l_trainer_destroy(void* trainer);
 /* train != 0: backward, clip and update; total_batch (the batch summed over ranks, which divides every gradient) must
  * then be finite and > 0, else W2L_ERR_INVALID_ARGUMENT and nothing runs.  train == 0: loss only, total_batch unused. */

@@ -48,8 +48,9 @@ EXPORTS = [
     "w2l_seq2seq_check", "w2l_seq2seq_embed_fwd", "w2l_seq2seq_embed_bwd", "w2l_seq2seq_gru_stash_floats", "w2l_seq2seq_gru_fwd",
     "w2l_seq2seq_gru_bwd", "w2l_seq2seq_attn_fwd", "w2l_seq2seq_attn_bwd", "w2l_seq2seq_loss", "w2l_seq2seq_scale_rows",
     "w2l_seq2seq_decode_init", "w2l_seq2seq_decode_step",
+    "w2l_seq2seq_beam_workspace_size", "w2l_seq2seq_beam_init", "w2l_seq2seq_beam_step", "w2l_seq2seq_beam_finish",
     "w2l_trainer_create_seq2seq", "w2l_trainer_output_width", "w2l_trainer_seq2seq_config", "w2l_trainer_clear_window",
-    "w2l_trainer_seq2seq_seed", "w2l_trainer_decode",
+    "w2l_trainer_seq2seq_seed", "w2l_trainer_decode", "w2l_trainer_beam_search",
 ]
 
 
@@ -174,6 +175,7 @@ def _load() -> ctypes.CDLL:
     lib.w2l_trainer_clear_window.argtypes = [vp]
     lib.w2l_trainer_seq2seq_seed.argtypes = [vp, vp]
     lib.w2l_trainer_decode.argtypes = [vp, vp, i, i, vp, vp, vp, ll]
+    lib.w2l_trainer_beam_search.argtypes = [vp, vp, i, i, vp, i, i, vp, vp, vp, vp, ll]
     lib.w2l_seq2seq_check.argtypes = [i, i]
     lib.w2l_seq2seq_embed_fwd.argtypes = [vp, i, i, i, i, vp, vp, vp, f32, u64, vp, vp, vp]
     lib.w2l_seq2seq_embed_bwd.argtypes = [vp, i, i, i, i, vp, vp, vp, vp]
@@ -187,6 +189,11 @@ def _load() -> ctypes.CDLL:
     lib.w2l_seq2seq_scale_rows.argtypes = [vp, i, i, i, vp, f32, vp]
     lib.w2l_seq2seq_decode_init.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, vp]
     lib.w2l_seq2seq_decode_step.argtypes = [vp, i, i, i, i, i, vp, vp, vp, vp, i, vp, vp]
+    lib.w2l_seq2seq_beam_workspace_size.restype = sz
+    lib.w2l_seq2seq_beam_workspace_size.argtypes = [i, i, i]
+    lib.w2l_seq2seq_beam_init.argtypes = [vp, i, i, i, i, vp, vp, vp, sz]
+    lib.w2l_seq2seq_beam_step.argtypes = [vp, i, i, i, i, i, i, i, i, vp, vp, vp, vp, vp, vp, sz]
+    lib.w2l_seq2seq_beam_finish.argtypes = [vp, i, i, i, i, i, vp, sz, vp, vp, vp, vp]
     lib.w2l_trainer_destroy.argtypes = [vp]
     lib.w2l_trainer_destroy.restype = None
     lib.w2l_trainer_step.argtypes = [vp, vp, i, i, vp, i, vp, vp, i, f32]

@@ -6,7 +6,9 @@
 //     W_hh stays in shared memory (one slice of hidden units per CTA), one grid barrier per step, fp32 throughout;
 //   key-value attention forward (scores, soft window, softmax over T', context, + the query) and backward;
 //   log-softmax + label-smoothed NLL + logit gradient in one pass over each row, written in place;
-//   the greedy decode's per-step argmax and feedback.
+//   the greedy decode's per-step argmax and feedback;
+//   the beam search's per-step selection (each row's best 2K candidates, the per-utterance walk, the state permutation)
+//   and its final backtrace.
 // Layouts: rows r = b * U + u of [B*U][width] row-major; the encoder output x [B][T'][2H] (keys x[.][0:H], values
 // x[.][H:2H]); targets y [B][U] int32; the decoder's input tokens [B][U] with N standing for startEmbedding.
 #include <cooperative_groups.h>
@@ -547,6 +549,338 @@ __global__ void __launch_bounds__(256) decode_step_kernel(int N, int H, int step
   for (int h = threadIdx.x; h < H; h += blockDim.x) in[(size_t)b * H + h] = E[(size_t)tok * H + h];
 }
 
+// ---- beam search ---------------------------------------------------------------------------------------------
+// B utterances x K hypothesis slots = B K decoder rows (row = b K + slot).  Per step: topk (each live row's best 2K
+// candidates), merge (one warp per utterance applies the walk of DESIGN.md §9), advance (states and inputs by parent).
+constexpr int kMaxBeam = 16;
+
+// the workspace, carved from one caller buffer (w2l_seq2seq_beam_workspace_size); count comes first
+struct BeamWs {
+  int32_t* count;      // [1]     finished utterances
+  int32_t* done;       // [B]     the search of b has stopped early
+  int32_t* live;       // [B]     live slots (the beam's width)
+  int32_t* ncomp;      // [B]     completions held (<= K after each step)
+  float* score;        // [B K]   live scores (-inf on dead slots)
+  float* compScore;    // [B 2K]  completions: score, step, slot
+  int32_t* compStep;   // [B 2K]
+  int32_t* compSlot;   // [B 2K]
+  float* topScore;     // [B K 2K] each row's best 2K candidates, best first
+  int32_t* topIdx;     // [B K 2K]
+  int32_t* hist;       // [maxlen][B K][2] (parent slot, token) of every slot after each step
+  size_t bytes;
+};
+
+BeamWs beam_ws(void* base, int B, int K, int maxlen) {
+  BeamWs w{};
+  char* p = static_cast<char*>(base);
+  size_t off = 0;
+  auto take = [&](size_t n) {
+    char* q = p ? p + off : nullptr;
+    off += (n * 4 + 15) / 16 * 16;
+    return q;
+  };
+  const size_t BK = (size_t)B * K;
+  w.count = (int32_t*)take(1);
+  w.done = (int32_t*)take(B);
+  w.live = (int32_t*)take(B);
+  w.ncomp = (int32_t*)take(B);
+  w.score = (float*)take(BK);
+  w.compScore = (float*)take(2 * BK);
+  w.compStep = (int32_t*)take(2 * BK);
+  w.compSlot = (int32_t*)take(2 * BK);
+  w.topScore = (float*)take(2 * BK * K);
+  w.topIdx = (int32_t*)take(2 * BK * K);
+  w.hist = (int32_t*)take(2 * BK * maxlen);
+  w.bytes = off;
+  return w;
+}
+
+// fp32 score -> unsigned key in the same order (NaN lowest)
+__device__ __forceinline__ unsigned order_key(float s) {
+  const unsigned u = __float_as_uint(s);
+  if (s != s) return 0u;
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+
+// init: in = start on every row, slot 0 live with score 0, the other slots dead
+__global__ void beam_init_kernel(int B, int K, int H, const float* __restrict__ start, float* __restrict__ in, BeamWs w) {
+  const int row = blockIdx.x, b = row / K, slot = row % K;
+  for (int h = threadIdx.x; h < H; h += blockDim.x) in[(size_t)row * H + h] = start[h];
+  if (threadIdx.x == 0) {
+    w.score[row] = slot == 0 ? 0.f : kNegInf;
+    if (slot == 0) {
+      w.done[b] = 0;
+      w.live[b] = 1;
+      w.ncomp[b] = 0;
+      if (b == 0) w.count[0] = 0;
+    }
+  }
+}
+
+// topk: per live row, lse of the logits, candidate scores s_c = score + (x_c - lse) in fp32, then the best
+// M = min(2K, N) by (s desc, c asc): a radix select of the M-th largest key (4 passes of 8 bits), one ordered pass that
+// takes every key above it and the lowest-index ties at it, and a rank sort of the M taken
+__global__ void __launch_bounds__(256) beam_topk_kernel(int K, int N, const float* __restrict__ logits, BeamWs w) {
+  __shared__ float sm_m[8], sm_s[8];
+  __shared__ unsigned hist[256];
+  __shared__ unsigned selKey[2 * kMaxBeam];
+  __shared__ int selIdx[2 * kMaxBeam];
+  __shared__ int warpEq[8];
+  __shared__ unsigned sPrefix;
+  __shared__ int sNeed, sTaken;
+  const int row = blockIdx.x, b = row / K, slot = row % K;
+  if (w.done[b] || slot >= w.live[b]) return;
+  const float* x = logits + (size_t)row * N;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
+  float m = kNegInf, s = 0.f;
+  for (int c = threadIdx.x; c < N; c += blockDim.x) {
+    const float v = x[c];
+    if (v > m) {
+      s = s * expf(m - v) + 1.f;
+      m = v;
+    } else {
+      s += expf(v - m);
+    }
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    const float m2 = __shfl_xor_sync(0xffffffffu, m, o), s2 = __shfl_xor_sync(0xffffffffu, s, o);
+    const float mm = fmaxf(m, m2);
+    s = (m == kNegInf ? 0.f : s * expf(m - mm)) + (m2 == kNegInf ? 0.f : s2 * expf(m2 - mm));
+    m = mm;
+  }
+  if (lane == 0) {
+    sm_m[warp] = m;
+    sm_s[warp] = s;
+  }
+  __syncthreads();
+  float M_ = kNegInf;
+  for (int i = 0; i < nw; ++i) M_ = fmaxf(M_, sm_m[i]);
+  float S = 0.f;
+  for (int i = 0; i < nw; ++i) S += sm_m[i] == kNegInf ? 0.f : sm_s[i] * expf(sm_m[i] - M_);
+  const float lse = M_ + logf(S);
+  const float base = w.score[row];
+  auto score_of = [&](int c) { return base + (x[c] - lse); };
+  const int M = min(2 * K, N);
+  // radix select: the key T with count(key > T) < M <= count(key >= T); sNeed ends as the ties at T to take
+  if (threadIdx.x == 0) {
+    sPrefix = 0u;
+    sNeed = M;
+  }
+  unsigned mask = 0u;
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    __syncthreads();
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) hist[i] = 0u;
+    __syncthreads();
+    const unsigned prefix = sPrefix;
+    for (int c = threadIdx.x; c < N; c += blockDim.x) {
+      const unsigned k = order_key(score_of(c));
+      if ((k & mask) == prefix) atomicAdd(&hist[(k >> shift) & 255u], 1u);
+    }
+    __syncthreads();
+    if (warp == 0) {  // digits from 255 down, 8 per lane: the digit where the running count reaches sNeed
+      const int need = sNeed;
+      unsigned cnt = 0;
+      for (int i = 0; i < 8; ++i) cnt += hist[255 - 8 * lane - i];
+      unsigned incl = cnt;
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+      }
+      const unsigned before = incl - cnt;
+      if (before < (unsigned)need && (unsigned)need <= incl) {
+        unsigned run = before;
+        for (int i = 0; i < 8; ++i) {
+          const int d = 255 - 8 * lane - i;
+          if (run + hist[d] >= (unsigned)need) {
+            sPrefix = prefix | ((unsigned)d << shift);
+            sNeed = need - (int)run;
+            break;
+          }
+          run += hist[d];
+        }
+      }
+    }
+    mask |= 255u << shift;
+  }
+  __syncthreads();
+  const unsigned T = sPrefix;
+  const int needEq = sNeed;
+  if (threadIdx.x == 0) sTaken = 0;
+  int eqSeen = 0;  // ties at T met so far in index order (every thread keeps the same count)
+  for (int c0 = 0; c0 < N; c0 += blockDim.x) {
+    const int c = c0 + threadIdx.x;
+    const unsigned k = c < N ? order_key(score_of(c)) : 0u;
+    const bool eq = c < N && k == T;
+    const unsigned bal = __ballot_sync(0xffffffffu, eq);
+    __syncthreads();
+    if (lane == 0) warpEq[warp] = __popc(bal);
+    __syncthreads();
+    int rank = eqSeen + __popc(bal & ((1u << lane) - 1u));
+    for (int i = 0; i < warp; ++i) rank += warpEq[i];
+    for (int i = 0; i < nw; ++i) eqSeen += warpEq[i];
+    if (c < N && (k > T || (eq && rank < needEq))) {
+      const int at = atomicAdd(&sTaken, 1);
+      selKey[at] = k;
+      selIdx[at] = c;
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x < M) {
+    const unsigned k = selKey[threadIdx.x];
+    const int c = selIdx[threadIdx.x];
+    int r = 0;
+    for (int i = 0; i < M; ++i) r += selKey[i] > k || (selKey[i] == k && selIdx[i] < c);
+    const size_t o = (size_t)row * 2 * K + r;
+    w.topScore[o] = score_of(c);
+    w.topIdx[o] = c;
+  }
+}
+
+// merge: one warp per utterance.  Lane l < live holds a cursor into row l's sorted list; each rank j the warp takes the
+// best head (key desc, flat index l N + c asc).  eos at j < K completes hypothesis l (its path, score with log p(eos));
+// eos at j >= K is dropped; another token extends the new beam, until it holds K.  Then the K-cap (stable sort of the
+// completions by score, keep K) and the early stop (K-th completion above the best live score).
+__global__ void __launch_bounds__(32) beam_merge_kernel(int K, int N, int step, int eos, BeamWs w) {
+  __shared__ float cs[2 * kMaxBeam];
+  __shared__ int cst[2 * kMaxBeam], csl[2 * kMaxBeam];
+  const int b = blockIdx.x, lane = threadIdx.x;
+  if (w.done[b]) return;
+  const int live = w.live[b], M = min(2 * K, N);
+  const float* ts = w.topScore + (size_t)b * K * 2 * K;
+  const int* ti = w.topIdx + (size_t)b * K * 2 * K;
+  int cur = 0;  // this lane's cursor
+  int nc = w.ncomp[b], n = 0;
+  float best = kNegInf;
+  int2* hist = reinterpret_cast<int2*>(w.hist) + ((size_t)step * gridDim.x + b) * K;
+  for (int i = lane; i < nc; i += 32) {
+    cs[i] = w.compScore[(size_t)b * 2 * K + i];
+    cst[i] = w.compStep[(size_t)b * 2 * K + i];
+    csl[i] = w.compSlot[(size_t)b * 2 * K + i];
+  }
+  __syncwarp();
+  for (int j = 0; n < K; ++j) {
+    const bool valid = lane < live && cur < M;
+    float sc = valid ? ts[lane * 2 * K + cur] : 0.f;
+    unsigned key = valid ? order_key(sc) : 0u;
+    int flat = valid ? lane * N + ti[lane * 2 * K + cur] : 0x7fffffff;
+    int have = valid, src = lane;
+    for (int o = 16; o > 0; o >>= 1) {
+      const int h2 = __shfl_xor_sync(0xffffffffu, have, o);
+      const unsigned k2 = __shfl_xor_sync(0xffffffffu, key, o);
+      const int f2 = __shfl_xor_sync(0xffffffffu, flat, o);
+      const float s2 = __shfl_xor_sync(0xffffffffu, sc, o);
+      const int l2 = __shfl_xor_sync(0xffffffffu, src, o);
+      if (h2 && (!have || k2 > key || (k2 == key && f2 < flat))) {
+        have = 1;
+        key = k2;
+        flat = f2;
+        sc = s2;
+        src = l2;
+      }
+    }
+    if (!have) break;  // every list is exhausted
+    if (lane == src) ++cur;
+    const int parent = flat / N, tok = flat - parent * N;
+    if (tok == eos) {
+      if (j < K) {
+        if (lane == 0) {
+          cs[nc] = sc;
+          cst[nc] = step;
+          csl[nc] = parent;
+        }
+        ++nc;
+      }
+    } else {
+      if (lane == 0) {
+        hist[n] = make_int2(parent, tok);
+        w.score[(size_t)b * K + n] = sc;
+      }
+      if (n == 0) best = sc;
+      ++n;
+    }
+    __syncwarp();
+  }
+  if (lane == 0) {
+    for (int i = n; i < K; ++i) {  // dead slots follow slot 0 (never selected: their rows are skipped)
+      hist[i] = hist[0];
+      w.score[(size_t)b * K + i] = kNegInf;
+    }
+    w.live[b] = n;
+    bool stop = n == 0;
+    if (nc >= K) {  // insertion sort is stable: equal scores keep their completion order
+      for (int i = 1; i < nc; ++i) {
+        const float s = cs[i];
+        const int st = cst[i], sl = csl[i];
+        int p = i - 1;
+        for (; p >= 0 && order_key(cs[p]) < order_key(s); --p) {
+          cs[p + 1] = cs[p];
+          cst[p + 1] = cst[p];
+          csl[p + 1] = csl[p];
+        }
+        cs[p + 1] = s;
+        cst[p + 1] = st;
+        csl[p + 1] = sl;
+      }
+      nc = K;
+      stop = stop || cs[K - 1] > best;
+    }
+    for (int i = 0; i < nc; ++i) {
+      w.compScore[(size_t)b * 2 * K + i] = cs[i];
+      w.compStep[(size_t)b * 2 * K + i] = cst[i];
+      w.compSlot[(size_t)b * 2 * K + i] = csl[i];
+    }
+    w.ncomp[b] = nc;
+    if (stop) {
+      w.done[b] = 1;
+      atomicAdd(w.count, 1);
+    }
+  }
+}
+
+// advance: blockIdx.y < layers: state[y][row] = next[y][b K + parent]; blockIdx.y == layers: in[row] = E[token]
+__global__ void beam_advance_kernel(int K, int H, int layers, int step, const float* __restrict__ E, float* __restrict__ in,
+                                    float* __restrict__ state, const float* __restrict__ next, BeamWs w) {
+  const int row = blockIdx.x, b = row / K, y = blockIdx.y;
+  if (w.done[b]) return;
+  const int2 e = reinterpret_cast<const int2*>(w.hist)[(size_t)step * gridDim.x + row];
+  const size_t plane = (size_t)gridDim.x * H;
+  const float* src = y < layers ? next + y * plane + ((size_t)b * K + e.x) * H : E + (size_t)e.y * H;
+  float* dst = y < layers ? state + y * plane + (size_t)row * H : in + (size_t)row * H;
+  for (int h = threadIdx.x; h < H; h += blockDim.x) dst[h] = src[h];
+}
+
+// finish: the completions if there are any, else the live beam (length `steps`), each path traced back through hist
+__global__ void beam_finish_kernel(int K, int maxlen, int steps, int pad, BeamWs w, int32_t* __restrict__ tokens, int32_t* __restrict__ lengths,
+                                   float* __restrict__ scores, int32_t* __restrict__ counts) {
+  const int b = blockIdx.x, k = threadIdx.x, B = gridDim.x;
+  if (k >= K) return;
+  const int nc = w.ncomp[b], cnt = nc > 0 ? nc : w.live[b];
+  int32_t* out = tokens + ((size_t)b * K + k) * maxlen;
+  int len = 0;
+  float sc = kNegInf;
+  if (k < cnt) {
+    int slot = k;
+    if (nc > 0) {
+      sc = w.compScore[(size_t)b * 2 * K + k];
+      len = w.compStep[(size_t)b * 2 * K + k];
+      slot = w.compSlot[(size_t)b * 2 * K + k];
+    } else {
+      sc = w.score[(size_t)b * K + k];
+      len = steps;
+    }
+    const int2* hist = reinterpret_cast<const int2*>(w.hist);
+    for (int t = len - 1; t >= 0; --t) {
+      const int2 e = hist[((size_t)t * B + b) * K + slot];
+      out[t] = e.y;
+      slot = e.x;
+    }
+  }
+  for (int t = len; t < maxlen; ++t) out[t] = pad;
+  lengths[(size_t)b * K + k] = len;
+  scores[(size_t)b * K + k] = sc;
+  if (k == 0) counts[b] = cnt;
+}
+
 }  // namespace
 }  // namespace w2l
 
@@ -684,6 +1018,53 @@ W2L_API int w2l_seq2seq_decode_step(void* stream, int B, int N, int H, int step,
     return fail(W2L_ERR_INVALID_ARGUMENT, "seq2seq_decode_step: bad arguments");
   decode_step_kernel<<<B, 256, 0, static_cast<cudaStream_t>(stream)>>>(N, H, step, eos, logits, E, in, tokens, maxlen, len, done);
   W2L_LAUNCH_CHECK("seq2seq_decode_step_kernel");
+  return W2L_OK;
+}
+
+W2L_API size_t w2l_seq2seq_beam_workspace_size(int B, int K, int maxlen) {
+  if (B <= 0 || K <= 0 || maxlen <= 0) return 0;
+  return beam_ws(nullptr, B, K, maxlen).bytes;
+}
+
+static int beam_args(const char* who, int B, int K, int maxlen, const void* ws, size_t ws_bytes) {
+  if (K < 1 || K > kMaxBeam) return fail(W2L_ERR_UNSUPPORTED, std::string(who) + ": beam size must be in [1, 16]");
+  if (B <= 0 || maxlen <= 0 || !ws) return fail(W2L_ERR_INVALID_ARGUMENT, std::string(who) + ": bad arguments");
+  if (ws_bytes < beam_ws(nullptr, B, K, maxlen).bytes) return fail(W2L_ERR_WORKSPACE, std::string(who) + ": workspace too small");
+  return W2L_OK;
+}
+
+W2L_API int w2l_seq2seq_beam_init(void* stream, int B, int K, int H, int maxlen, const float* start, float* in, void* ws, size_t ws_bytes) {
+  if (int rc = beam_args("seq2seq_beam_init", B, K, maxlen, ws, ws_bytes)) return rc;
+  if (H <= 0 || !start || !in) return fail(W2L_ERR_INVALID_ARGUMENT, "seq2seq_beam_init: bad arguments");
+  beam_init_kernel<<<B * K, 128, 0, static_cast<cudaStream_t>(stream)>>>(B, K, H, start, in, beam_ws(ws, B, K, maxlen));
+  W2L_LAUNCH_CHECK("seq2seq_beam_init_kernel");
+  return W2L_OK;
+}
+
+W2L_API int w2l_seq2seq_beam_step(void* stream, int B, int K, int N, int H, int layers, int step, int maxlen, int eos, const float* logits,
+                                  const float* E, float* in, float* state, const float* next, void* ws, size_t ws_bytes) {
+  if (int rc = beam_args("seq2seq_beam_step", B, K, maxlen, ws, ws_bytes)) return rc;
+  if (int rc = w2l_seq2seq_check(H, N)) return rc;
+  if (layers <= 0 || step < 0 || step >= maxlen || eos < 0 || eos >= N || !logits || !E || !in || !state || !next)
+    return fail(W2L_ERR_INVALID_ARGUMENT, "seq2seq_beam_step: bad arguments");
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const BeamWs w = beam_ws(ws, B, K, maxlen);
+  beam_topk_kernel<<<B * K, 256, 0, s>>>(K, N, logits, w);
+  W2L_LAUNCH_CHECK("seq2seq_beam_topk_kernel");
+  beam_merge_kernel<<<B, 32, 0, s>>>(K, N, step, eos, w);
+  W2L_LAUNCH_CHECK("seq2seq_beam_merge_kernel");
+  beam_advance_kernel<<<dim3(B * K, layers + 1), 128, 0, s>>>(K, H, layers, step, E, in, state, next, w);
+  W2L_LAUNCH_CHECK("seq2seq_beam_advance_kernel");
+  return W2L_OK;
+}
+
+W2L_API int w2l_seq2seq_beam_finish(void* stream, int B, int K, int maxlen, int steps, int pad, const void* ws, size_t ws_bytes, int32_t* tokens,
+                                    int32_t* lengths, float* scores, int32_t* counts) {
+  if (int rc = beam_args("seq2seq_beam_finish", B, K, maxlen, ws, ws_bytes)) return rc;
+  if (steps < 1 || steps > maxlen || !tokens || !lengths || !scores || !counts) return fail(W2L_ERR_INVALID_ARGUMENT, "seq2seq_beam_finish: bad arguments");
+  beam_finish_kernel<<<B, 32, 0, static_cast<cudaStream_t>(stream)>>>(K, maxlen, steps, pad, beam_ws(const_cast<void*>(ws), B, K, maxlen), tokens,
+                                                                       lengths, scores, counts);
+  W2L_LAUNCH_CHECK("seq2seq_beam_finish_kernel");
   return W2L_OK;
 }
 

@@ -2047,12 +2047,42 @@ std::vector<Variable> Seq2SeqCriterion::forward(const std::vector<Variable>& inp
   })};
 }
 
-af::array Seq2SeqCriterion::decode(const af::array& x, af::array* lengths) {
-  const int H = H_, N = N_;
+namespace {
+constexpr int kCheckEvery = 8;  // decode steps between host reads of the finished count
+
+void checkEncoderOutput(const af::array& x, int H) {
   if (x.type() != DType::f32 || x.dims(0) != 2 * H)
     throw std::invalid_argument("Seq2SeqCriterion: encoder output has " + std::to_string(x.dims(0)) + " features; KeyValueAttention needs 2 * encoderdim = " +
                                 std::to_string(2 * H));
-  const int Tp = (int)x.dims(1), B = (int)(x.dims(2) * x.dims(3)), maxLen = maxLen_;
+}
+}  // namespace
+
+Variable Seq2SeqCriterion::decoderStep(const af::array& x, int B, int U, const af::array& in, const std::vector<af::array>& prev,
+                                       const std::vector<af::array>& next) {
+  const int H = H_, Tp = (int)x.dims(1), rows = B * U;
+  auto P = [&](int i) { return fl::noGrad(params_[i].array()); };
+  Variable h = fl::noGrad(in);
+  for (int r = 0; r < R_; ++r) {
+    Variable cur = h;
+    for (int l = 0; l < S_; ++l) {
+      const int k = r * S_ + l, base = 2 + 4 * k;
+      Variable gi = ih_[k]->forwardWith(cur, P(base), P(base + 2));
+      check(w2l_seq2seq_gru_fwd(currentStream(), rows, 1, H, gi.array().f32(), params_[base + 1].array().f32(), params_[base + 3].array().f32(),
+                                prev[k].isEmpty() ? nullptr : prev[k].f32(), next[k].f32(), nullptr));
+      cur = fl::noGrad(next[k]);
+    }
+    af::array a = af::array::empty(af::dim4(H, 1, rows));
+    check(w2l_seq2seq_attn_fwd(currentStream(), B, U, Tp, H, cur.array().f32(), x.f32(), 1, 0.f, a.f32(), nullptr));
+    h = fl::noGrad(a);
+  }
+  const int wo = 2 + 4 * R_ * S_;
+  return out_->forwardWith(h, P(wo), P(wo + 1));
+}
+
+af::array Seq2SeqCriterion::decode(const af::array& x, af::array* lengths) {
+  const int H = H_, N = N_;
+  checkEncoderOutput(x, H);
+  const int B = (int)(x.dims(2) * x.dims(3)), maxLen = maxLen_;
   af::array in = af::array::empty(af::dim4(H, 1, B));
   af::array tokens = af::array::empty(af::dim4(maxLen, B), DType::i32);
   af::array len = af::array::empty(af::dim4(B), DType::i32);
@@ -2061,27 +2091,13 @@ af::array Seq2SeqCriterion::decode(const af::array& x, af::array* lengths) {
   // every layer's hidden state, two buffers each (a step reads one and writes the other)
   std::vector<af::array> state;
   for (int i = 0; i < 2 * R_ * S_; ++i) state.push_back(af::array::empty(af::dim4(H, 1, B)));
-  auto P = [&](int i) { return fl::noGrad(params_[i].array()); };
-  constexpr int kCheckEvery = 8;  // steps between host reads of the finished count
+  std::vector<af::array> prev(R_ * S_), next(R_ * S_);
   for (int step = 0; step < maxLen; ++step) {
-    Variable h = fl::noGrad(in);
-    for (int r = 0; r < R_; ++r) {
-      Variable cur = h;
-      for (int l = 0; l < S_; ++l) {
-        const int k = r * S_ + l, base = 2 + 4 * k;
-        Variable gi = ih_[k]->forwardWith(cur, P(base), P(base + 2));
-        const af::array& prev = state[2 * k + ((step + 1) & 1)];
-        const af::array& next = state[2 * k + (step & 1)];
-        check(w2l_seq2seq_gru_fwd(currentStream(), B, 1, H, gi.array().f32(), params_[base + 1].array().f32(), params_[base + 3].array().f32(),
-                                  step ? prev.f32() : nullptr, next.f32(), nullptr));
-        cur = fl::noGrad(next);
-      }
-      af::array a = af::array::empty(af::dim4(H, 1, B));
-      check(w2l_seq2seq_attn_fwd(currentStream(), B, 1, Tp, H, cur.array().f32(), x.f32(), 1, 0.f, a.f32(), nullptr));
-      h = fl::noGrad(a);
+    for (int k = 0; k < R_ * S_; ++k) {
+      prev[k] = step ? state[2 * k + ((step + 1) & 1)] : af::array();
+      next[k] = state[2 * k + (step & 1)];
     }
-    const int wo = 2 + 4 * R_ * S_;
-    Variable logits = out_->forwardWith(h, P(wo), P(wo + 1));
+    Variable logits = decoderStep(x, B, 1, in, prev, next);
     check(w2l_seq2seq_decode_step(currentStream(), B, N, H, step, eos_, logits.array().f32(), params_[0].array().f32(), in.f32(), tokens.i32(), maxLen,
                                   len.i32(), done.i32()));
     if ((step + 1) % kCheckEvery == 0 && step + 1 < maxLen) {
@@ -2091,6 +2107,63 @@ af::array Seq2SeqCriterion::decode(const af::array& x, af::array* lengths) {
   }
   if (lengths) *lengths = len;
   return tokens;
+}
+
+Seq2SeqCriterion::BeamResult Seq2SeqCriterion::beamSearchBatch(const af::array& x, int beamSize, int maxLen) {
+  const int H = H_, N = N_, K = beamSize, layers = R_ * S_;
+  checkEncoderOutput(x, H);
+  if (K < 1 || K > 16) throw std::invalid_argument("Seq2SeqCriterion: beam size must be in [1, 16]");
+  if (maxLen < 1) throw std::invalid_argument("Seq2SeqCriterion: the beam search needs maxLen >= 1");
+  const int B = (int)(x.dims(2) * x.dims(3)), BK = B * K;
+  af::array in = af::array::empty(af::dim4(H, 1, BK));
+  // state: what each slot's next step starts from (zeros at the first step); out: what the step's GRUs write.  The
+  // advance after each step permutes out into state by parent.
+  af::array state = af::array::zeros(af::dim4(H, BK, layers)), out = af::array::empty(af::dim4(H, BK, layers));
+  std::vector<af::array> prev, next;
+  for (int k = 0; k < layers; ++k) {
+    const size_t off = sizeof(float) * (size_t)k * BK * H;
+    prev.push_back(af::array::view(state, off, af::dim4(H, 1, BK), DType::f32));
+    next.push_back(af::array::view(out, off, af::dim4(H, 1, BK), DType::f32));
+  }
+  const size_t wsBytes = w2l_seq2seq_beam_workspace_size(B, K, maxLen);
+  af::array ws = af::array::empty(af::dim4((long long)wsBytes), DType::u8);
+  check(w2l_seq2seq_beam_init(currentStream(), B, K, H, maxLen, params_[1].array().f32(), in.f32(), ws.ptr(), wsBytes));
+  int steps = 0;
+  while (steps < maxLen) {
+    Variable logits = decoderStep(x, B, K, in, prev, next);
+    check(w2l_seq2seq_beam_step(currentStream(), B, K, N, H, layers, steps, maxLen, eos_, logits.array().f32(), params_[0].array().f32(), in.f32(),
+                                state.f32(), out.f32(), ws.ptr(), wsBytes));
+    ++steps;
+    if (steps % kCheckEvery == 0 && steps < maxLen && af::array::view(ws, 0, af::dim4(1), DType::i32).scalar<int32_t>() == B) break;
+  }
+  BeamResult r{af::array::empty(af::dim4(maxLen, K, B), DType::i32), af::array::empty(af::dim4(K, B), DType::i32), af::array::empty(af::dim4(K, B)),
+               af::array::empty(af::dim4(B), DType::i32)};
+  check(w2l_seq2seq_beam_finish(currentStream(), B, K, maxLen, steps, pad_, ws.ptr(), wsBytes, r.tokens.i32(), r.lengths.i32(), r.scores.f32(),
+                                r.counts.i32()));
+  return r;
+}
+
+std::vector<Seq2SeqCriterion::CandidateHypo> Seq2SeqCriterion::beamSearch(const af::array& input, std::vector<CandidateHypo> beam, int beamSize,
+                                                                          int maxLen) {
+  if (beam.size() != 1 || !beam[0].path.empty() || beam[0].score != 0.f)
+    throw std::invalid_argument("Seq2SeqCriterion::beamSearch: only the single empty initial hypothesis is supported");
+  if (input.dims(2) * input.dims(3) != 1) throw std::invalid_argument("Seq2SeqCriterion::beamSearch: one utterance [2H, T', 1] at a time");
+  const BeamResult r = beamSearchBatch(input, beamSize, maxLen);
+  const std::vector<int32_t> tokens = r.tokens.host<int32_t>(), lengths = r.lengths.host<int32_t>();
+  const std::vector<float> scores = r.scores.host<float>();
+  const int count = r.counts.scalar<int32_t>();
+  std::vector<CandidateHypo> out(count);
+  for (int k = 0; k < count; ++k) {
+    out[k].score = scores[k];
+    out[k].path.assign(tokens.begin() + (size_t)k * maxLen, tokens.begin() + (size_t)k * maxLen + lengths[k]);
+  }
+  return out;
+}
+
+af::array Seq2SeqCriterion::beamPath(const af::array& input, int beamSize) {
+  const std::vector<int> path = beamSearch(input, {CandidateHypo{}}, beamSize, maxLen_)[0].path;
+  if (path.empty()) return af::array();
+  return af::array::fromHost(path.data(), af::dim4((long long)path.size()), DType::i32);
 }
 af::array Seq2SeqCriterion::viterbiPath(const af::array& input, const af::array&) { return decode(input, nullptr); }
 af::array Seq2SeqCriterion::viterbiPathWithTarget(const af::array&, const af::array&, af::array*) {

@@ -629,6 +629,31 @@ W2L_API int w2l_trainer_decode(void* h, void* stream, int B, int T, const float*
   });
 }
 
+// network forward (eval mode) + the seq2seq criterion's beam search: tokens device int32 [B][beam][max_len] (pad after
+// each hypothesis), lengths / scores [B][beam], counts [B]
+W2L_API int w2l_trainer_beam_search(void* h, void* stream, int B, int T, const float* features, int beam, int max_len, int32_t* tokens,
+                                    int32_t* lengths, float* scores, int32_t* counts, long long capacity) {
+  return guarded([&] {
+    w2l::setCurrentStream(stream);
+    auto* t = static_cast<Trainer*>(h);
+    if (!t->s2s) throw std::invalid_argument("trainer_beam_search: only the seq2seq criterion has a beam search");
+    if (B <= 0 || T <= 0 || max_len < 0 || !features || !tokens || !lengths || !scores || !counts)
+      throw std::invalid_argument("trainer_beam_search: bad arguments");
+    if (beam < 1 || beam > 16) throw std::invalid_argument("trainer_beam_search: beam size must be in [1, 16]");
+    const int L = max_len ? max_len : t->s2sSettings.maxLen;
+    if (capacity < (long long)B * beam * L) throw std::invalid_argument("trainer_beam_search: token buffer too small");
+    PrecisionScope scope(t->precision);
+    t->net->eval();
+    t->crit->eval();
+    Variable out = t->net->forward(std::vector<Variable>{fl::input(af::array::wrap(const_cast<float*>(features), af::dim4(T, t->nFeat, 1, B)))}).front();
+    const Seq2SeqCriterion::BeamResult r = t->s2s->beamSearchBatch(out.array(), beam, L);
+    af::array::wrap(tokens, r.tokens.dims(), w2l::DType::i32).copyFrom(r.tokens);
+    af::array::wrap(lengths, r.lengths.dims(), w2l::DType::i32).copyFrom(r.lengths);
+    af::array::wrap(scores, r.scores.dims(), w2l::DType::f32).copyFrom(r.scores);
+    af::array::wrap(counts, r.counts.dims(), w2l::DType::i32).copyFrom(r.counts);
+  });
+}
+
 W2L_API int w2l_trainer_time_stride(void* h) { return timeStride(static_cast<Trainer*>(h)->net); }
 
 W2L_API int w2l_nccl_unique_id(void* out128) {

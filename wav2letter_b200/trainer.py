@@ -205,6 +205,24 @@ class Trainer:
         _check(lib.w2l_trainer_decode(self.h, _stream(), B, T, _ptr(features), _ptr(tokens), _ptr(lengths), tokens.numel()))
         return tokens, lengths
 
+    def beam_search(self, features: torch.Tensor, beam_size: int = 4, max_len: int | None = None):
+        """Beam search (seq2seq): eval-mode forward, then Seq2SeqCriterion::beamSearchBatch over the batch with beam_size
+        in [1, 16] for at most max_len steps (None: maxdecoderoutputlen).  Returns CUDA tensors (tokens int32 [B, K, L]
+        padded with pad, lengths int32 [B, K], scores float32 [B, K], counts int32 [B]): per utterance the completed
+        hypotheses if any (best first once more than K completed, else in completion order), otherwise the live beam at
+        length L.  Slots at or beyond counts[b] hold pad, length 0 and score -inf."""
+        B, _, F, T = features.shape
+        L = int(max_len) if max_len is not None else self.seq2seq_config()["maxdecoderoutputlen"]
+        K = int(beam_size)
+        dev = features.device
+        tokens = torch.empty((B, max(K, 1), max(L, 1)), dtype=torch.int32, device=dev)
+        lengths = torch.empty((B, max(K, 1)), dtype=torch.int32, device=dev)
+        scores = torch.empty((B, max(K, 1)), dtype=torch.float32, device=dev)
+        counts = torch.empty(B, dtype=torch.int32, device=dev)
+        _check(lib.w2l_trainer_beam_search(self.h, _stream(), B, T, _ptr(features), K, L, _ptr(tokens), _ptr(lengths), _ptr(scores),
+                                           _ptr(counts), tokens.numel()))
+        return tokens, lengths, scores, counts
+
     def align(self, features: torch.Tensor, target: torch.Tensor):
         """Forced alignment: eval-mode forward, then the criterion's viterbiPathWithTarget.  features CUDA float
         [B,1,F,T], target CUDA int32 [B,L] (-1 padded).  Returns (path, idx), CUDA int32 [B,T']: the token per output
