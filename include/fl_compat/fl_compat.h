@@ -655,14 +655,18 @@ class SoftPretrainWindow : public WindowBase {
 };
 
 // Seq2SeqCriterion with the constructor arguments of Train.cpp:416-432.  forward({encoder output [2H,T',B], target
-// [U,B] int32, [durations], [target sizes]}) -> {loss [B]}: the sizes are accepted and not used — every utterance spans
-// all T' frames and its target ends at its first pad.  Targets hold tokens, then eos, then pad; an utterance holding a
+// [U,B] int32, [durations], [target sizes]}) -> {loss [B]}.  Durations [B] (s32, or f32 holding whole numbers) are the
+// input frame counts of a padded batch: utterance b attends to encoder frames t < T'_b = ceil(d_b T' / max d) only.
+// Target sizes [B] s32 (tokens plus eos) centre the soft window at u T'_b / U_b.  Absent or empty: T' and U.  A target
+// ends at its first pad either way.  Bad sizes (d_b <= 0, no positive duration, a target size outside [1, U]) are
+// rejected in-band like bad targets.  Targets hold tokens, then eos, then pad; an utterance holding a
 // value outside [0, N) (-1 included) is rejected in-band, checked on the device: its loss is NaN and its gradient zero
 // (Train.cpp stops on a NaN loss, :1686-1698; the trainer's finite guard skips the update).  Parameters (layout order): E [N][H], startEmbedding [H], per round and layer
 // W_ih [3H][H], W_hh [3H][H], b_ih [3H], b_hh [3H], then W_o [N][H], b_o [N].  Refused (std::invalid_argument):
 // inputfeeding, a sampling strategy other than "rand", attentions other than KeyValueAttention, windows other than
-// SoftPretrainWindow, attentions.size() != nAttnRound.  viterbiPath is the greedy decode (int32 [maxDecoderOutputLen, B],
-// padded with pad); viterbiPathWithTarget is not supported.  beamSearch / beamPath are the criterion's token-level beam
+// SoftPretrainWindow, attentions.size() != nAttnRound.  viterbiPath(input, inputSize) is the greedy decode (int32
+// [maxDecoderOutputLen, B], padded with pad), each utterance over its T'_b frames when inputSize holds its durations;
+// viterbiPathWithTarget is not supported.  beamSearch / beamPath are the criterion's token-level beam
 // search over its own log-probabilities (no LM, no length normalisation, no window), as local_prior_match's
 // batchBeamSearch calls it; beamSearchBatch searches whole batches on the device and serves both.
 class Seq2SeqCriterion : public SequenceCriterion {
@@ -689,10 +693,14 @@ class Seq2SeqCriterion : public SequenceCriterion {
   af::array viterbiPathWithTarget(const af::array& input, const af::array& target, af::array* index = nullptr) override;
   // greedy decode of every utterance: tokens [maxDecoderOutputLen, B] int32 (pad after the end), lengths [B] int32
   af::array decode(const af::array& input, af::array* lengths);
+  // the same over each utterance's T'_b frames, from inputSizes [B] (durations as forward takes them; empty: T')
+  af::array decode(const af::array& input, af::array* lengths, const af::array& inputSizes);
   // beam search of every utterance of input [2H, T', B] with beamSize in [1, 16] (std::invalid_argument outside) for at
   // most maxLen steps: the completions if there are any (sorted by score if more than beamSize ever completed, else in
   // completion order), otherwise the live beam at length maxLen
   BeamResult beamSearchBatch(const af::array& input, int beamSize, int maxLen);
+  // the same over each utterance's T'_b frames, from inputSizes [B] (durations as forward takes them; empty: T')
+  BeamResult beamSearchBatch(const af::array& input, int beamSize, int maxLen, const af::array& inputSizes);
   // one utterance [2H, T', 1] from the single empty hypothesis ({CandidateHypo{}}; any other beam throws
   // std::invalid_argument): at most beamSize hypotheses
   std::vector<CandidateHypo> beamSearch(const af::array& input, std::vector<CandidateHypo> beam, int beamSize, int maxLen);
@@ -708,9 +716,10 @@ class Seq2SeqCriterion : public SequenceCriterion {
 
  private:
   // one eval-mode decoder step over B * U rows (U query rows per utterance of x): every round and layer from the states
-  // prev[k] (empty: zeros) into next[k], attention without the window, then the output Linear: logits [N, 1, B * U]
+  // prev[k] (empty: zeros) into next[k], attention without the window over frames t < tps[b] (empty: T'), then the
+  // output Linear: logits [N, 1, B * U]
   Variable decoderStep(const af::array& x, int B, int U, const af::array& in, const std::vector<af::array>& prev,
-                       const std::vector<af::array>& next);
+                       const std::vector<af::array>& next, const af::array& tps);
   int N_, H_, eos_, pad_, maxLen_, pct_, S_, R_;
   double ls_;
   float dropout_;

@@ -205,6 +205,15 @@ W2L_API int w2l_linseg_target(void* stream, int B, int T, int L, const int32_t* 
  *   attn_fwd    out = q + sum_t softmax_t(q.k_t / sqrt(H) + w_{u,t}) v_t, with the soft window
  *               w = -(t - u T'/window_u)^2 / (2 window_std^2) when window_std > 0; attn (nullable) [B*U][T'] the weights
  *   attn_bwd    from dout = d out: dq (the identity path included) and dx [B][T'][2H] (written), dS [B*U][T'] scratch
+ *   sizes       per-utterance bounds of a padded batch (DESIGN.md §9), one launch: from durations [B] (the input frame
+ *               counts; int32, or float32 holding whole numbers when durations_f32 = 1; NULL: every T'_b = T')
+ *               T'_b = ceil(d_b T' / max d) in double clamped to [1, T'], into tp_sizes [B]; from target_sizes [B] int32
+ *               (NULL: U) U_b into u_sizes [B].  Rejected in-band, with no host synchronisation: d_b <= 0 or not whole,
+ *               no positive duration at all, a target size outside [1, U] set bad[b] (nullable); the bound stays in range.
+ *   attn_fwd_sized / attn_bwd_sized   attn_fwd / attn_bwd over frames t < tp_sizes[b] of utterance b (device int32
+ *               [B], nullable: T'), with the window centred at u T'_b / U_b, U_b = u_sizes[b] (nullable: window_u).
+ *               Nothing at t >= T'_b is read: attn holds 0 there and dx is written as 0.  With both NULL they are
+ *               attn_fwd / attn_bwd, bit for bit.
  *   loss        per row: log-softmax over N, (1-ls)(-log p_y) - (ls/N) sum_c log p_c, 0 on rows with target = pad;
  *               loss[b] = sum over u (in order), rowloss [B*U] scratch; grad != 0 also writes the logit gradient
  *               dloss[b] (NULL: 1) (p - (1-ls) e_y - ls/N) over the logits, in place, 0 on pad rows.
@@ -240,6 +249,12 @@ W2L_API int w2l_seq2seq_attn_fwd(void* stream, int B, int U, int Tp, int H, cons
                                  float* out, float* attn);
 W2L_API int w2l_seq2seq_attn_bwd(void* stream, int B, int U, int Tp, int H, const float* q, const float* x, const float* attn, const float* dout,
                                  float* dq, float* dx, float* dS);
+W2L_API int w2l_seq2seq_sizes(void* stream, int B, int Tp, int U, const void* durations, int durations_f32, const int32_t* target_sizes,
+                              int32_t* tp_sizes, int32_t* u_sizes, int32_t* bad);
+W2L_API int w2l_seq2seq_attn_fwd_sized(void* stream, int B, int U, int Tp, int H, const float* q, const float* x, const int32_t* tp_sizes,
+                                       const int32_t* u_sizes, int window_u, float window_std, float* out, float* attn);
+W2L_API int w2l_seq2seq_attn_bwd_sized(void* stream, int B, int U, int Tp, int H, const float* q, const float* x, const float* attn, const float* dout,
+                                       const int32_t* tp_sizes, float* dq, float* dx, float* dS);
 W2L_API int w2l_seq2seq_loss(void* stream, int B, int U, int N, int pad, const int32_t* target, float* logits, float label_smooth,
                              const float* dloss, int grad, float* rowloss, float* loss, const int32_t* bad);
 W2L_API int w2l_seq2seq_scale_rows(void* stream, int B, int U, int N, const float* g, float seed_scale, float* d);
@@ -518,6 +533,18 @@ W2L_API void w2l_trainer_destroy(void* trainer);
  * then be finite and > 0, else W2L_ERR_INVALID_ARGUMENT and nothing runs.  train == 0: loss only, total_batch unused. */
 W2L_API int w2l_trainer_step(void* trainer, void* stream, int B, int T, const float* features, int L, const int32_t* target,
                              float* loss_out, int train, float total_batch);
+/* Padded batches of the seq2seq criterion (DESIGN.md §9): the step, decode and beam search above with the durations and
+ * target sizes Train.cpp passes it.  input_sizes [B] device int32 (nullable) are the input frame counts of each
+ * utterance: the attention of utterance b covers encoder frames t < T'_b = ceil(d_b T' / max d); target_sizes [B]
+ * device int32 (nullable, step only) count tokens plus eos and centre the soft window at u T'_b / U_b.  Bad sizes give
+ * that utterance a NaN loss (the update is skipped and counted), checked on the device.  Both NULL: the unsized call,
+ * bit for bit.  A ctc, asg or linseg trainer given sizes returns W2L_ERR_INVALID_ARGUMENT: Train.cpp gives them none. */
+W2L_API int w2l_trainer_step_sized(void* trainer, void* stream, int B, int T, const float* features, int L, const int32_t* target,
+                                   const int32_t* input_sizes, const int32_t* target_sizes, float* loss_out, int train, float total_batch);
+W2L_API int w2l_trainer_decode_sized(void* trainer, void* stream, int B, int T, const float* features, const int32_t* input_sizes, int32_t* tokens,
+                                     int32_t* lengths, long long capacity);
+W2L_API int w2l_trainer_beam_search_sized(void* trainer, void* stream, int B, int T, const float* features, const int32_t* input_sizes, int beam,
+                                          int max_len, int32_t* tokens, int32_t* lengths, float* scores, int32_t* counts, long long capacity);
 W2L_API int w2l_trainer_forward(void* trainer, void* stream, int B, int T, const float* features, float* emissions_out,
                                 long long capacity, int* t_out);
 /* Forced alignment: the eval-mode network forward of w2l_trainer_forward, then the criterion's viterbiPathWithTarget on

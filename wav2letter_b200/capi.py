@@ -51,6 +51,8 @@ EXPORTS = [
     "w2l_seq2seq_beam_workspace_size", "w2l_seq2seq_beam_init", "w2l_seq2seq_beam_step", "w2l_seq2seq_beam_finish",
     "w2l_trainer_create_seq2seq", "w2l_trainer_output_width", "w2l_trainer_seq2seq_config", "w2l_trainer_clear_window",
     "w2l_trainer_seq2seq_seed", "w2l_trainer_decode", "w2l_trainer_beam_search",
+    "w2l_seq2seq_sizes", "w2l_seq2seq_attn_fwd_sized", "w2l_seq2seq_attn_bwd_sized", "w2l_trainer_step_sized", "w2l_trainer_decode_sized",
+    "w2l_trainer_beam_search_sized",
 ]
 
 
@@ -185,6 +187,12 @@ def _load() -> ctypes.CDLL:
     lib.w2l_seq2seq_gru_bwd.argtypes = [vp, i, i, i, vp, vp, vp, vp, vp, vp]
     lib.w2l_seq2seq_attn_fwd.argtypes = [vp, i, i, i, i, vp, vp, i, f32, vp, vp]
     lib.w2l_seq2seq_attn_bwd.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, vp, vp, vp]
+    lib.w2l_seq2seq_sizes.argtypes = [vp, i, i, i, vp, i, vp, vp, vp, vp]
+    lib.w2l_seq2seq_attn_fwd_sized.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, i, f32, vp, vp]
+    lib.w2l_seq2seq_attn_bwd_sized.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.w2l_trainer_step_sized.argtypes = [vp, vp, i, i, vp, i, vp, vp, vp, vp, i, f32]
+    lib.w2l_trainer_decode_sized.argtypes = [vp, vp, i, i, vp, vp, vp, vp, ll]
+    lib.w2l_trainer_beam_search_sized.argtypes = [vp, vp, i, i, vp, vp, i, i, vp, vp, vp, vp, ll]
     lib.w2l_seq2seq_loss.argtypes = [vp, i, i, i, i, vp, vp, f32, vp, i, vp, vp, vp]
     lib.w2l_seq2seq_scale_rows.argtypes = [vp, i, i, i, vp, f32, vp]
     lib.w2l_seq2seq_decode_init.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, vp]

@@ -9,6 +9,7 @@
 //   the greedy decode's per-step argmax and feedback;
 //   the beam search's per-step selection (each row's best 2K candidates, the per-utterance walk, the state permutation)
 //   and its final backtrace.
+// Padded batches: per-utterance frame counts T'_b and target sizes U_b (one size kernel) bound the attention.
 // Layouts: rows r = b * U + u of [B*U][width] row-major; the encoder output x [B][T'][2H] (keys x[.][0:H], values
 // x[.][H:2H]); targets y [B][U] int32; the decoder's input tokens [B][U] with N standing for startEmbedding.
 #include <cooperative_groups.h>
@@ -238,9 +239,67 @@ int gruChunk(size_t fixedFloats, size_t perRowFloats) {
   return 0;
 }
 
+// ---- per-utterance sizes -------------------------------------------------------------------------------------
+// T'_b = ceil(d_b T' / max_b' d_b') in double, clamped to [1, T'] (T' without durations); U_b = the target size (U
+// without sizes).  Rejected in-band through bad[b]: d_b <= 0 or not a whole number, no positive duration at all (every
+// utterance), a target size outside [1, U].  A rejected utterance keeps a bound in range, so the kernels stay defined.
+__global__ void __launch_bounds__(256) sizes_kernel(int B, int Tp, int U, const void* __restrict__ dur, int durF32,
+                                                    const int32_t* __restrict__ tsz, int32_t* __restrict__ tps, int32_t* __restrict__ ups,
+                                                    int32_t* __restrict__ bad) {
+  __shared__ double sm[8];
+  auto duration = [&](int b, bool& ok) {
+    double d;
+    if (durF32) {
+      const float f = static_cast<const float*>(dur)[b];
+      ok = isfinite(f) && f == floorf(f);
+      d = ok ? (double)f : 0.0;
+    } else {
+      d = (double)static_cast<const int32_t*>(dur)[b];
+      ok = true;
+    }
+    ok = ok && d > 0.0;
+    return d;
+  };
+  double m = 0.0;
+  if (dur)
+    for (int b = threadIdx.x; b < B; b += blockDim.x) {
+      bool ok;
+      const double d = duration(b, ok);
+      if (ok) m = fmax(m, d);
+    }
+  for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = m;
+  __syncthreads();
+  double dmax = 0.0;
+  for (int w = 0; w < (int)(blockDim.x >> 5); ++w) dmax = fmax(dmax, sm[w]);
+  for (int b = threadIdx.x; b < B; b += blockDim.x) {
+    bool reject = false;
+    int tb = Tp, ub = U;
+    if (dur) {
+      bool ok;
+      const double d = duration(b, ok);
+      if (ok && dmax > 0.0)
+        tb = (int)fmin(fmax(ceil(d * (double)Tp / dmax), 1.0), (double)Tp);
+      else
+        reject = true;
+    }
+    if (tsz) {
+      const int v = tsz[b];
+      if (v >= 1 && v <= U)
+        ub = v;
+      else
+        reject = true;
+    }
+    tps[b] = tb;
+    ups[b] = ub;
+    if (reject && bad) bad[b] = 1;
+  }
+}
+
 // ---- key-value attention -------------------------------------------------------------------------------------
 // per (tile of kUTile decoder steps, utterance): s_t = q.k_t / sqrt(H) + w_t, a = softmax_t(s), out = q + sum_t a_t v_t.
-// Window (win_inv2s2 > 0): w_{u,t} = -(t - u T' / U_win)^2 * win_inv2s2, 0-based u and t.
+// Window (win_inv2s2 > 0): w_{u,t} = -(t - u T'_b / U_b)^2 * win_inv2s2, 0-based u and t.  With per-utterance sizes
+// (tps / ups, nullable: T' and U_win) only frames t < T'_b take part: nothing past them is read, their weights are 0.
 __device__ __forceinline__ float window_at(int u, int t, int Tp, int Uwin, float inv2s2) {
   const float c = (float)u * (float)Tp / (float)Uwin;
   const float d = (float)t - c;
@@ -248,17 +307,18 @@ __device__ __forceinline__ float window_at(int u, int t, int Tp, int Uwin, float
 }
 
 __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(int U, int Tp, int H, const float* __restrict__ q, const float* __restrict__ x,
-                                                            float scale, int Uwin, float inv2s2, float* __restrict__ out,
-                                                            float* __restrict__ attn) {
+                                                            float scale, int Uwin, float inv2s2, const int32_t* __restrict__ tps,
+                                                            const int32_t* __restrict__ ups, float* __restrict__ out, float* __restrict__ attn) {
   extern __shared__ float sm[];
   float* qs = sm;                       // [kUTile][H]
   float* ss = qs + (size_t)kUTile * H;  // [kUTile][Tp]
   const int b = blockIdx.y, u0 = blockIdx.x * kUTile, nu = min(kUTile, U - u0);
+  const int Tb = tps ? tps[b] : Tp, Ub = ups ? ups[b] : Uwin;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
   const float* xb = x + (size_t)b * Tp * 2 * H;
   for (int i = threadIdx.x; i < kUTile * H; i += blockDim.x) qs[i] = i / H < nu ? q[((size_t)b * U + u0) * H + i] : 0.f;
   __syncthreads();
-  for (int t = warp; t < Tp; t += nw) {
+  for (int t = warp; t < Tb; t += nw) {
     float acc[kUTile];
 #pragma unroll
     for (int i = 0; i < kUTile; ++i) acc[i] = 0.f;
@@ -271,33 +331,35 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(int U, int Tp, int H
 #pragma unroll
     for (int i = 0; i < kUTile; ++i) {
       const float s = warp_sum(acc[i]) * scale;
-      if (lane == 0) ss[(size_t)i * Tp + t] = inv2s2 > 0.f ? s + window_at(u0 + i, t, Tp, Uwin, inv2s2) : s;
+      if (lane == 0) ss[(size_t)i * Tp + t] = inv2s2 > 0.f ? s + window_at(u0 + i, t, Tb, Ub, inv2s2) : s;
     }
   }
   __syncthreads();
   for (int i = warp; i < nu; i += nw) {
     float* s = ss + (size_t)i * Tp;
     float m = kNegInf;
-    for (int t = lane; t < Tp; t += 32) m = fmaxf(m, s[t]);
+    for (int t = lane; t < Tb; t += 32) m = fmaxf(m, s[t]);
     m = warp_max(m);
     float z = 0.f;
-    for (int t = lane; t < Tp; t += 32) {
+    for (int t = lane; t < Tb; t += 32) {
       const float e = expf(s[t] - m);
       s[t] = e;
       z += e;
     }
     const float inv = 1.f / warp_sum(z);
-    for (int t = lane; t < Tp; t += 32) {
+    for (int t = lane; t < Tb; t += 32) {
       s[t] *= inv;
       if (attn) attn[((size_t)b * U + u0 + i) * Tp + t] = s[t];
     }
+    if (attn)
+      for (int t = Tb + lane; t < Tp; t += 32) attn[((size_t)b * U + u0 + i) * Tp + t] = 0.f;
   }
   __syncthreads();
   for (int h = threadIdx.x; h < H; h += blockDim.x) {
     float acc[kUTile];
 #pragma unroll
     for (int i = 0; i < kUTile; ++i) acc[i] = 0.f;
-    for (int t = 0; t < Tp; ++t) {
+    for (int t = 0; t < Tb; ++t) {
       const float v = xb[(size_t)t * 2 * H + H + h];
 #pragma unroll
       for (int i = 0; i < kUTile; ++i) acc[i] = fmaf(ss[(size_t)i * Tp + t], v, acc[i]);
@@ -306,19 +368,21 @@ __global__ void __launch_bounds__(kThreads) attn_fwd_kernel(int U, int Tp, int H
   }
 }
 
-// dA_t = dout.v_t, dS = a (dA - sum_t a dA), dq = dout + sum_t dS_t k_t / sqrt(H); dS is kept for the key / value side
+// dA_t = dout.v_t, dS = a (dA - sum_t a dA), dq = dout + sum_t dS_t k_t / sqrt(H), over t < T'_b; dS is kept for the
+// key / value side
 __global__ void __launch_bounds__(kThreads) attn_bwd_q_kernel(int U, int Tp, int H, const float* __restrict__ x, const float* __restrict__ attn,
-                                                              const float* __restrict__ dout, float scale, float* __restrict__ dS,
-                                                              float* __restrict__ dq) {
+                                                              const float* __restrict__ dout, float scale, const int32_t* __restrict__ tps,
+                                                              float* __restrict__ dS, float* __restrict__ dq) {
   extern __shared__ float sm[];
   float* gs = sm;                       // [kUTile][H]  dout rows
   float* ss = gs + (size_t)kUTile * H;  // [kUTile][Tp] dA, then dS
   const int b = blockIdx.y, u0 = blockIdx.x * kUTile, nu = min(kUTile, U - u0);
+  const int Tb = tps ? tps[b] : Tp;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
   const float* xb = x + (size_t)b * Tp * 2 * H;
   for (int i = threadIdx.x; i < kUTile * H; i += blockDim.x) gs[i] = i / H < nu ? dout[((size_t)b * U + u0) * H + i] : 0.f;
   __syncthreads();
-  for (int t = warp; t < Tp; t += nw) {
+  for (int t = warp; t < Tb; t += nw) {
     float acc[kUTile];
 #pragma unroll
     for (int i = 0; i < kUTile; ++i) acc[i] = 0.f;
@@ -339,9 +403,9 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_q_kernel(int U, int Tp, int
     float* s = ss + (size_t)i * Tp;
     const float* a = attn + ((size_t)b * U + u0 + i) * Tp;
     float dot = 0.f;
-    for (int t = lane; t < Tp; t += 32) dot = fmaf(a[t], s[t], dot);
+    for (int t = lane; t < Tb; t += 32) dot = fmaf(a[t], s[t], dot);
     dot = warp_sum(dot);
-    for (int t = lane; t < Tp; t += 32) {
+    for (int t = lane; t < Tb; t += 32) {
       const float d = a[t] * (s[t] - dot);
       s[t] = d;
       dS[((size_t)b * U + u0 + i) * Tp + t] = d;
@@ -352,7 +416,7 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_q_kernel(int U, int Tp, int
     float acc[kUTile];
 #pragma unroll
     for (int i = 0; i < kUTile; ++i) acc[i] = 0.f;
-    for (int t = 0; t < Tp; ++t) {
+    for (int t = 0; t < Tb; ++t) {
       const float k = xb[(size_t)t * 2 * H + h];
 #pragma unroll
       for (int i = 0; i < kUTile; ++i) acc[i] = fmaf(ss[(size_t)i * Tp + t], k, acc[i]);
@@ -362,19 +426,24 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_q_kernel(int U, int Tp, int
 }
 
 // per (tile of kTTile frames, utterance): dk_t = sum_u dS_{u,t} q_u / sqrt(H), dv_t = sum_u a_{u,t} dout_u, written to
-// dx[b][t][0:H] and dx[b][t][H:2H]
+// dx[b][t][0:H] and dx[b][t][H:2H]; frames t >= T'_b get 0, and a tile wholly past T'_b reads nothing
 __global__ void __launch_bounds__(kThreads) attn_bwd_kv_kernel(int U, int Tp, int H, const float* __restrict__ q, const float* __restrict__ attn,
                                                                const float* __restrict__ dS, const float* __restrict__ dout, float scale,
-                                                               float* __restrict__ dx) {
+                                                               const int32_t* __restrict__ tps, float* __restrict__ dx) {
   extern __shared__ float sm[];
   float* as = sm;                       // [U][kTTile]
   float* ds = as + (size_t)U * kTTile;  // [U][kTTile]
   const int b = blockIdx.y, t0 = blockIdx.x * kTTile, nt = min(kTTile, Tp - t0);
+  const int nv = max(0, min(nt, (tps ? tps[b] : Tp) - t0));  // frames of the tile inside the utterance
+  if (nv == 0) {
+    for (int i = threadIdx.x; i < nt * 2 * H; i += blockDim.x) dx[((size_t)b * Tp + t0) * 2 * H + i] = 0.f;
+    return;
+  }
   for (int i = threadIdx.x; i < U * kTTile; i += blockDim.x) {
     const int u = i / kTTile, j = i % kTTile;
     const size_t o = ((size_t)b * U + u) * Tp + t0 + j;
-    as[i] = j < nt ? attn[o] : 0.f;
-    ds[i] = j < nt ? dS[o] : 0.f;
+    as[i] = j < nv ? attn[o] : 0.f;
+    ds[i] = j < nv ? dS[o] : 0.f;
   }
   __syncthreads();
   for (int h = threadIdx.x; h < H; h += blockDim.x) {
@@ -390,10 +459,15 @@ __global__ void __launch_bounds__(kThreads) attn_bwd_kv_kernel(int U, int Tp, in
         dv[j] = fmaf(as[u * kTTile + j], gg, dv[j]);
       }
     }
-    for (int j = 0; j < nt; ++j) {
+    for (int j = 0; j < nv; ++j) {
       float* o = dx + ((size_t)b * Tp + t0 + j) * 2 * H;
       o[h] = dk[j] * scale;
       o[H + h] = dv[j];
+    }
+    for (int j = nv; j < nt; ++j) {
+      float* o = dx + ((size_t)b * Tp + t0 + j) * 2 * H;
+      o[h] = 0.f;
+      o[H + h] = 0.f;
     }
   }
 }
@@ -949,23 +1023,37 @@ W2L_API int w2l_seq2seq_gru_bwd(void* stream, int B, int U, int H, const float* 
   return W2L_OK;
 }
 
-W2L_API int w2l_seq2seq_attn_fwd(void* stream, int B, int U, int Tp, int H, const float* q, const float* x, int window_u, float window_std,
-                                 float* out, float* attn) {
+W2L_API int w2l_seq2seq_sizes(void* stream, int B, int Tp, int U, const void* durations, int durations_f32, const int32_t* target_sizes,
+                              int32_t* tp_sizes, int32_t* u_sizes, int32_t* bad) {
+  if (B <= 0 || Tp <= 0 || U <= 0 || (durations_f32 != 0 && durations_f32 != 1) || !tp_sizes || !u_sizes)
+    return fail(W2L_ERR_INVALID_ARGUMENT, "seq2seq_sizes: bad arguments");
+  sizes_kernel<<<1, 256, 0, static_cast<cudaStream_t>(stream)>>>(B, Tp, U, durations, durations_f32, target_sizes, tp_sizes, u_sizes, bad);
+  W2L_LAUNCH_CHECK("seq2seq_sizes_kernel");
+  return W2L_OK;
+}
+
+W2L_API int w2l_seq2seq_attn_fwd_sized(void* stream, int B, int U, int Tp, int H, const float* q, const float* x, const int32_t* tp_sizes,
+                                       const int32_t* u_sizes, int window_u, float window_std, float* out, float* attn) {
   if (int rc = w2l_seq2seq_check(H, 3)) return rc;
-  if (B <= 0 || U <= 0 || Tp <= 0 || !q || !x || !out || (window_std > 0.f && window_u <= 0))
+  if (B <= 0 || U <= 0 || Tp <= 0 || !q || !x || !out || (window_std > 0.f && window_u <= 0 && !u_sizes))
     return fail(W2L_ERR_INVALID_ARGUMENT, "seq2seq_attn_fwd: bad arguments");
   const size_t smem = sizeof(float) * (size_t)kUTile * (H + Tp);
   if (smem > kSmemLimit) return fail(W2L_ERR_UNSUPPORTED, "seq2seq_attn_fwd: too many encoder frames");
   W2L_CUDA_CHECK(cudaFuncSetAttribute(attn_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const float inv2s2 = window_std > 0.f ? (float)(1.0 / (2.0 * (double)window_std * window_std)) : 0.f;
   attn_fwd_kernel<<<dim3((U + kUTile - 1) / kUTile, B), kThreads, smem, static_cast<cudaStream_t>(stream)>>>(
-      U, Tp, H, q, x, 1.f / sqrtf((float)H), window_u, inv2s2, out, attn);
+      U, Tp, H, q, x, 1.f / sqrtf((float)H), window_u, inv2s2, tp_sizes, u_sizes, out, attn);
   W2L_LAUNCH_CHECK("seq2seq_attn_fwd_kernel");
   return W2L_OK;
 }
 
-W2L_API int w2l_seq2seq_attn_bwd(void* stream, int B, int U, int Tp, int H, const float* q, const float* x, const float* attn, const float* dout,
-                                 float* dq, float* dx, float* dS) {
+W2L_API int w2l_seq2seq_attn_fwd(void* stream, int B, int U, int Tp, int H, const float* q, const float* x, int window_u, float window_std,
+                                 float* out, float* attn) {
+  return w2l_seq2seq_attn_fwd_sized(stream, B, U, Tp, H, q, x, nullptr, nullptr, window_u, window_std, out, attn);
+}
+
+W2L_API int w2l_seq2seq_attn_bwd_sized(void* stream, int B, int U, int Tp, int H, const float* q, const float* x, const float* attn, const float* dout,
+                                       const int32_t* tp_sizes, float* dq, float* dx, float* dS) {
   if (int rc = w2l_seq2seq_check(H, 3)) return rc;
   if (B <= 0 || U <= 0 || Tp <= 0 || !q || !x || !attn || !dout || !dq || !dx || !dS) return fail(W2L_ERR_INVALID_ARGUMENT, "seq2seq_attn_bwd: bad arguments");
   const size_t smem1 = sizeof(float) * (size_t)kUTile * (H + Tp), smem2 = sizeof(float) * (size_t)2 * U * kTTile;
@@ -974,11 +1062,16 @@ W2L_API int w2l_seq2seq_attn_bwd(void* stream, int B, int U, int Tp, int H, cons
   W2L_CUDA_CHECK(cudaFuncSetAttribute(attn_bwd_kv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
   const float scale = 1.f / sqrtf((float)H);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  attn_bwd_q_kernel<<<dim3((U + kUTile - 1) / kUTile, B), kThreads, smem1, s>>>(U, Tp, H, x, attn, dout, scale, dS, dq);
+  attn_bwd_q_kernel<<<dim3((U + kUTile - 1) / kUTile, B), kThreads, smem1, s>>>(U, Tp, H, x, attn, dout, scale, tp_sizes, dS, dq);
   W2L_LAUNCH_CHECK("seq2seq_attn_bwd_q_kernel");
-  attn_bwd_kv_kernel<<<dim3((Tp + kTTile - 1) / kTTile, B), kThreads, smem2, s>>>(U, Tp, H, q, attn, dS, dout, scale, dx);
+  attn_bwd_kv_kernel<<<dim3((Tp + kTTile - 1) / kTTile, B), kThreads, smem2, s>>>(U, Tp, H, q, attn, dS, dout, scale, tp_sizes, dx);
   W2L_LAUNCH_CHECK("seq2seq_attn_bwd_kv_kernel");
   return W2L_OK;
+}
+
+W2L_API int w2l_seq2seq_attn_bwd(void* stream, int B, int U, int Tp, int H, const float* q, const float* x, const float* attn, const float* dout,
+                                 float* dq, float* dx, float* dS) {
+  return w2l_seq2seq_attn_bwd_sized(stream, B, U, Tp, H, q, x, attn, dout, nullptr, dq, dx, dS);
 }
 
 W2L_API int w2l_seq2seq_loss(void* stream, int B, int U, int N, int pad, const int32_t* target, float* logits, float label_smooth,

@@ -1916,17 +1916,38 @@ Variable seededDropout(const Variable& in, float p, unsigned long long seed) {
     ins[0].addGrad(Variable(d, false), true);
   });
 }
+// per-utterance bounds of a padded batch: tps / ups [B] int32 on the device (both empty without sizes)
+struct Bounds {
+  af::array tps, ups;
+  const int32_t* tp() const { return tps.isEmpty() ? nullptr : tps.i32(); }
+  const int32_t* up() const { return ups.isEmpty() ? nullptr : ups.i32(); }
+};
+bool absent(const af::array& a) { return a.isEmpty() || a.elements() == 0; }
+// durations (s32, or f32 holding whole numbers) and target sizes (s32), each absent when empty; bad sizes set bad[b]
+// on the device (nullable)
+Bounds sizeBounds(const af::array& durations, const af::array& targetSizes, int B, int Tp, int U, int32_t* bad) {
+  if (absent(durations) && absent(targetSizes)) return {};
+  if (!absent(durations) && (durations.elements() != B || (durations.type() != DType::i32 && durations.type() != DType::f32)))
+    throw std::invalid_argument("Seq2SeqCriterion: durations must be s32 or f32 with one entry per utterance");
+  if (!absent(targetSizes) && (targetSizes.elements() != B || targetSizes.type() != DType::i32))
+    throw std::invalid_argument("Seq2SeqCriterion: target sizes must be s32 with one entry per utterance");
+  Bounds r{af::array::empty(af::dim4(B), DType::i32), af::array::empty(af::dim4(B), DType::i32)};
+  check(w2l_seq2seq_sizes(currentStream(), B, Tp, U, absent(durations) ? nullptr : durations.ptr(), !absent(durations) && durations.type() == DType::f32,
+                          absent(targetSizes) ? nullptr : targetSizes.i32(), r.tps.i32(), r.ups.i32(), bad));
+  return r;
+}
 // h = q + attention(q, x): the round's output, the next round's input
-Variable attentionRound(const Variable& q, const Variable& x, int B, int U, int Tp, int H, float windowStd) {
+Variable attentionRound(const Variable& q, const Variable& x, int B, int U, int Tp, int H, float windowStd, const Bounds& bounds) {
   af::array out = af::array::empty(af::dim4(H, U, B));
   af::array attn = af::array::empty(af::dim4(Tp, U, B));
-  check(w2l_seq2seq_attn_fwd(currentStream(), B, U, Tp, H, q.array().f32(), x.array().f32(), U, windowStd, out.f32(), attn.f32()));
+  check(w2l_seq2seq_attn_fwd_sized(currentStream(), B, U, Tp, H, q.array().f32(), x.array().f32(), bounds.tp(), bounds.up(), U, windowStd, out.f32(),
+                                   attn.f32()));
   return Variable(out, {q, x}, [=](std::vector<Variable>& ins, const Variable& g) {
     af::array dq = af::array::empty(ins[0].dims());
     af::array dx = af::array::empty(ins[1].dims());
     af::array dS = af::array::empty(af::dim4(Tp, U, B));
-    check(w2l_seq2seq_attn_bwd(currentStream(), B, U, Tp, H, ins[0].array().f32(), ins[1].array().f32(), attn.f32(), g.array().f32(), dq.f32(),
-                               dx.f32(), dS.f32()));
+    check(w2l_seq2seq_attn_bwd_sized(currentStream(), B, U, Tp, H, ins[0].array().f32(), ins[1].array().f32(), attn.f32(), g.array().f32(),
+                                     bounds.tp(), dq.f32(), dx.f32(), dS.f32()));
     ins[0].addGrad(Variable(dq, false), true);
     ins[1].addGrad(Variable(dx, false), true);
   });
@@ -2005,6 +2026,8 @@ std::vector<Variable> Seq2SeqCriterion::forward(const std::vector<Variable>& inp
   // targets are checked on the device, without a host round trip: an utterance with a value outside [0, N) is flagged
   // here and the loss kernel gives it NaN and no gradient
   af::array bad = af::array::zeros(af::dim4(B), DType::i32);
+  const Bounds bounds = sizeBounds(inputs.size() > 2 && !inputs[2].isEmpty() ? inputs[2].array() : af::array(),
+                                   inputs.size() > 3 && !inputs[3].isEmpty() ? inputs[3].array() : af::array(), B, Tp, U, bad.i32());
   check(w2l_seq2seq_embed_fwd(currentStream(), B, U, H, N, target.i32(), params_[0].array().f32(), params_[1].array().f32(), train ? (float)pct_ : 100.f,
                               seed, tokens.i32(), in.f32(), bad.i32()));
   Variable h(in, {params_[0], params_[1]}, [=](std::vector<Variable>& ins, const Variable& g) {
@@ -2024,7 +2047,7 @@ std::vector<Variable> Seq2SeqCriterion::forward(const std::vector<Variable>& inp
       // the layer's dropout mask: seed + 1 + k (cuDNN applies dropout to every layer's output but the stack's last)
       if (train && dropout_ > 0.f && l + 1 < S_) cur = seededDropout(cur, dropout_, seed + 1 + (unsigned long long)k);
     }
-    h = attentionRound(cur, x, B, U, Tp, H, windowStd);
+    h = attentionRound(cur, x, B, U, Tp, H, windowStd, bounds);
   }
   const int wo = 2 + 4 * R_ * S_;
   Variable logits = out_->forwardWith(h, params_[wo], params_[wo + 1]);
@@ -2058,7 +2081,7 @@ void checkEncoderOutput(const af::array& x, int H) {
 }  // namespace
 
 Variable Seq2SeqCriterion::decoderStep(const af::array& x, int B, int U, const af::array& in, const std::vector<af::array>& prev,
-                                       const std::vector<af::array>& next) {
+                                       const std::vector<af::array>& next, const af::array& tps) {
   const int H = H_, Tp = (int)x.dims(1), rows = B * U;
   auto P = [&](int i) { return fl::noGrad(params_[i].array()); };
   Variable h = fl::noGrad(in);
@@ -2072,17 +2095,21 @@ Variable Seq2SeqCriterion::decoderStep(const af::array& x, int B, int U, const a
       cur = fl::noGrad(next[k]);
     }
     af::array a = af::array::empty(af::dim4(H, 1, rows));
-    check(w2l_seq2seq_attn_fwd(currentStream(), B, U, Tp, H, cur.array().f32(), x.f32(), 1, 0.f, a.f32(), nullptr));
+    check(w2l_seq2seq_attn_fwd_sized(currentStream(), B, U, Tp, H, cur.array().f32(), x.f32(), tps.isEmpty() ? nullptr : tps.i32(), nullptr, 1, 0.f,
+                                     a.f32(), nullptr));
     h = fl::noGrad(a);
   }
   const int wo = 2 + 4 * R_ * S_;
   return out_->forwardWith(h, P(wo), P(wo + 1));
 }
 
-af::array Seq2SeqCriterion::decode(const af::array& x, af::array* lengths) {
+af::array Seq2SeqCriterion::decode(const af::array& x, af::array* lengths) { return decode(x, lengths, af::array()); }
+
+af::array Seq2SeqCriterion::decode(const af::array& x, af::array* lengths, const af::array& inputSizes) {
   const int H = H_, N = N_;
   checkEncoderOutput(x, H);
   const int B = (int)(x.dims(2) * x.dims(3)), maxLen = maxLen_;
+  const af::array tps = sizeBounds(inputSizes, af::array(), B, (int)x.dims(1), 1, nullptr).tps;
   af::array in = af::array::empty(af::dim4(H, 1, B));
   af::array tokens = af::array::empty(af::dim4(maxLen, B), DType::i32);
   af::array len = af::array::empty(af::dim4(B), DType::i32);
@@ -2097,7 +2124,7 @@ af::array Seq2SeqCriterion::decode(const af::array& x, af::array* lengths) {
       prev[k] = step ? state[2 * k + ((step + 1) & 1)] : af::array();
       next[k] = state[2 * k + (step & 1)];
     }
-    Variable logits = decoderStep(x, B, 1, in, prev, next);
+    Variable logits = decoderStep(x, B, 1, in, prev, next, tps);
     check(w2l_seq2seq_decode_step(currentStream(), B, N, H, step, eos_, logits.array().f32(), params_[0].array().f32(), in.f32(), tokens.i32(), maxLen,
                                   len.i32(), done.i32()));
     if ((step + 1) % kCheckEvery == 0 && step + 1 < maxLen) {
@@ -2110,11 +2137,16 @@ af::array Seq2SeqCriterion::decode(const af::array& x, af::array* lengths) {
 }
 
 Seq2SeqCriterion::BeamResult Seq2SeqCriterion::beamSearchBatch(const af::array& x, int beamSize, int maxLen) {
+  return beamSearchBatch(x, beamSize, maxLen, af::array());
+}
+
+Seq2SeqCriterion::BeamResult Seq2SeqCriterion::beamSearchBatch(const af::array& x, int beamSize, int maxLen, const af::array& inputSizes) {
   const int H = H_, N = N_, K = beamSize, layers = R_ * S_;
   checkEncoderOutput(x, H);
   if (K < 1 || K > 16) throw std::invalid_argument("Seq2SeqCriterion: beam size must be in [1, 16]");
   if (maxLen < 1) throw std::invalid_argument("Seq2SeqCriterion: the beam search needs maxLen >= 1");
   const int B = (int)(x.dims(2) * x.dims(3)), BK = B * K;
+  const af::array tps = sizeBounds(inputSizes, af::array(), B, (int)x.dims(1), 1, nullptr).tps;
   af::array in = af::array::empty(af::dim4(H, 1, BK));
   // state: what each slot's next step starts from (zeros at the first step); out: what the step's GRUs write.  The
   // advance after each step permutes out into state by parent.
@@ -2130,7 +2162,7 @@ Seq2SeqCriterion::BeamResult Seq2SeqCriterion::beamSearchBatch(const af::array& 
   check(w2l_seq2seq_beam_init(currentStream(), B, K, H, maxLen, params_[1].array().f32(), in.f32(), ws.ptr(), wsBytes));
   int steps = 0;
   while (steps < maxLen) {
-    Variable logits = decoderStep(x, B, K, in, prev, next);
+    Variable logits = decoderStep(x, B, K, in, prev, next, tps);
     check(w2l_seq2seq_beam_step(currentStream(), B, K, N, H, layers, steps, maxLen, eos_, logits.array().f32(), params_[0].array().f32(), in.f32(),
                                 state.f32(), out.f32(), ws.ptr(), wsBytes));
     ++steps;
@@ -2165,7 +2197,7 @@ af::array Seq2SeqCriterion::beamPath(const af::array& input, int beamSize) {
   if (path.empty()) return af::array();
   return af::array::fromHost(path.data(), af::dim4((long long)path.size()), DType::i32);
 }
-af::array Seq2SeqCriterion::viterbiPath(const af::array& input, const af::array&) { return decode(input, nullptr); }
+af::array Seq2SeqCriterion::viterbiPath(const af::array& input, const af::array& inputSize) { return decode(input, nullptr, inputSize); }
 af::array Seq2SeqCriterion::viterbiPathWithTarget(const af::array&, const af::array&, af::array*) {
   throw std::invalid_argument("Seq2SeqCriterion: viterbiPathWithTarget is not supported");
 }

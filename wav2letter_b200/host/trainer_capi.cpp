@@ -366,13 +366,22 @@ W2L_API int w2l_trainer_param_layout(void* h, int which, int max_params, long lo
 // One step.  features: device [T,F,1,B] (ArrayFire layout, T fastest), target: device [L,B] int32 (-1 padded),
 // loss_out: device [B].  train != 0 runs backward + all-reduce + clip + SGD.  total_batch = sum of B over ranks; with
 // train != 0 it must be finite and > 0 (the gradients are divided by it), else W2L_ERR_INVALID_ARGUMENT before any launch.
-W2L_API int w2l_trainer_step(void* h, void* stream, int B, int T, const float* features, int L, const int32_t* target,
-                             float* loss_out, int train, float total_batch) {
+namespace {
+// a device int32 [B] size array, or empty for NULL
+af::array sizesArray(const int32_t* p, int B) { return p ? af::array::wrap(const_cast<int32_t*>(p), af::dim4(B), w2l::DType::i32) : af::array(); }
+}  // namespace
+
+// input_sizes / target_sizes: device int32 [B] (nullable), the durations and target sizes Train.cpp passes the seq2seq
+// criterion (:1473-1476); the other criteria take none
+W2L_API int w2l_trainer_step_sized(void* h, void* stream, int B, int T, const float* features, int L, const int32_t* target,
+                                   const int32_t* input_sizes, const int32_t* target_sizes, float* loss_out, int train, float total_batch) {
   return guarded([&] {
     if (train && !(std::isfinite(total_batch) && total_batch > 0.f))
       throw std::invalid_argument("trainer_step: total_batch must be finite and > 0 for a training step");
-    w2l::setCurrentStream(stream);
     auto* t = static_cast<Trainer*>(h);
+    const bool sized = input_sizes || target_sizes;
+    if (sized && !t->s2s) throw std::invalid_argument("trainer_step: input and target sizes are taken by the seq2seq criterion only");
+    w2l::setCurrentStream(stream);
     PrecisionScope scope(t->precision);
     if (train) {
       t->net->train();
@@ -399,7 +408,9 @@ W2L_API int w2l_trainer_step(void* h, void* stream, int B, int T, const float* f
       Variable output = t->net->forward(std::vector<Variable>{input}).front();
       // [crit] Train.cpp:1675
       Variable tgt = fl::noGrad(af::array::wrap(const_cast<int32_t*>(target), af::dim4(L, B), w2l::DType::i32));
-      Variable loss = t->crit->forward({output, tgt}).front();
+      Variable loss = (sized ? t->crit->forward({output, tgt, fl::noGrad(sizesArray(input_sizes, B)), fl::noGrad(sizesArray(target_sizes, B))})
+                             : t->crit->forward({output, tgt}))
+                          .front();
       if (loss_out) af::array::wrap(loss_out, af::dim4(B)).copyFrom(loss.array());
       if (!train) return;
       // [bwd]  zeroGrad; loss.backward()   Train.cpp:1718-1720
@@ -477,6 +488,11 @@ W2L_API int w2l_trainer_step(void* h, void* stream, int B, int T, const float* f
       break;
     }
   });
+}
+
+W2L_API int w2l_trainer_step(void* h, void* stream, int B, int T, const float* features, int L, const int32_t* target,
+                             float* loss_out, int train, float total_batch) {
+  return w2l_trainer_step_sized(h, stream, B, T, features, L, target, nullptr, nullptr, loss_out, train, total_batch);
 }
 
 W2L_API int w2l_trainer_set_schedule(void* h, long long warmup, double gamma, long long stepsize, int lrcosine, long long nbatches, long long lr_decay,
@@ -611,7 +627,8 @@ W2L_API int w2l_trainer_align(void* h, void* stream, int B, int T, const float* 
 
 // network forward (eval mode) + the seq2seq criterion's greedy decode: tokens device int32 [B][maxdecoderoutputlen] (pad
 // after each utterance's end), lengths device int32 [B]
-W2L_API int w2l_trainer_decode(void* h, void* stream, int B, int T, const float* features, int32_t* tokens, int32_t* lengths, long long capacity) {
+W2L_API int w2l_trainer_decode_sized(void* h, void* stream, int B, int T, const float* features, const int32_t* input_sizes, int32_t* tokens,
+                                     int32_t* lengths, long long capacity) {
   return guarded([&] {
     w2l::setCurrentStream(stream);
     auto* t = static_cast<Trainer*>(h);
@@ -623,16 +640,19 @@ W2L_API int w2l_trainer_decode(void* h, void* stream, int B, int T, const float*
     t->crit->eval();
     Variable out = t->net->forward(std::vector<Variable>{fl::input(af::array::wrap(const_cast<float*>(features), af::dim4(T, t->nFeat, 1, B)))}).front();
     af::array len;
-    const af::array tok = t->s2s->decode(out.array(), &len);
+    const af::array tok = t->s2s->decode(out.array(), &len, sizesArray(input_sizes, B));
     af::array::wrap(tokens, tok.dims(), w2l::DType::i32).copyFrom(tok);
     af::array::wrap(lengths, len.dims(), w2l::DType::i32).copyFrom(len);
   });
 }
+W2L_API int w2l_trainer_decode(void* h, void* stream, int B, int T, const float* features, int32_t* tokens, int32_t* lengths, long long capacity) {
+  return w2l_trainer_decode_sized(h, stream, B, T, features, nullptr, tokens, lengths, capacity);
+}
 
 // network forward (eval mode) + the seq2seq criterion's beam search: tokens device int32 [B][beam][max_len] (pad after
 // each hypothesis), lengths / scores [B][beam], counts [B]
-W2L_API int w2l_trainer_beam_search(void* h, void* stream, int B, int T, const float* features, int beam, int max_len, int32_t* tokens,
-                                    int32_t* lengths, float* scores, int32_t* counts, long long capacity) {
+W2L_API int w2l_trainer_beam_search_sized(void* h, void* stream, int B, int T, const float* features, const int32_t* input_sizes, int beam,
+                                          int max_len, int32_t* tokens, int32_t* lengths, float* scores, int32_t* counts, long long capacity) {
   return guarded([&] {
     w2l::setCurrentStream(stream);
     auto* t = static_cast<Trainer*>(h);
@@ -646,12 +666,16 @@ W2L_API int w2l_trainer_beam_search(void* h, void* stream, int B, int T, const f
     t->net->eval();
     t->crit->eval();
     Variable out = t->net->forward(std::vector<Variable>{fl::input(af::array::wrap(const_cast<float*>(features), af::dim4(T, t->nFeat, 1, B)))}).front();
-    const Seq2SeqCriterion::BeamResult r = t->s2s->beamSearchBatch(out.array(), beam, L);
+    const Seq2SeqCriterion::BeamResult r = t->s2s->beamSearchBatch(out.array(), beam, L, sizesArray(input_sizes, B));
     af::array::wrap(tokens, r.tokens.dims(), w2l::DType::i32).copyFrom(r.tokens);
     af::array::wrap(lengths, r.lengths.dims(), w2l::DType::i32).copyFrom(r.lengths);
     af::array::wrap(scores, r.scores.dims(), w2l::DType::f32).copyFrom(r.scores);
     af::array::wrap(counts, r.counts.dims(), w2l::DType::i32).copyFrom(r.counts);
   });
+}
+W2L_API int w2l_trainer_beam_search(void* h, void* stream, int B, int T, const float* features, int beam, int max_len, int32_t* tokens,
+                                    int32_t* lengths, float* scores, int32_t* counts, long long capacity) {
+  return w2l_trainer_beam_search_sized(h, stream, B, T, features, nullptr, beam, max_len, tokens, lengths, scores, counts, capacity);
 }
 
 W2L_API int w2l_trainer_time_stride(void* h) { return timeStride(static_cast<Trainer*>(h)->net); }

@@ -152,16 +152,24 @@ class Trainer:
         _check(lib.w2l_trainer_set_flat(self.h, _stream(), which, _ptr(flat.contiguous())))
 
     def step(self, features: torch.Tensor, target: torch.Tensor, train: bool = True, total_batch: float | None = None,
-             loss_out: torch.Tensor | None = None) -> torch.Tensor:
+             loss_out: torch.Tensor | None = None, input_sizes=None, target_sizes=None) -> torch.Tensor:
         """features: CUDA float [B,1,F,T] contiguous (== ArrayFire [T,F,1,B]); target CUDA int32 [B,L].
         total_batch: the batch summed over ranks (default B); every gradient is divided by it.  A training step raises
-        W2LError (code 1) before running anything unless it is finite and > 0; an eval step does not use it."""
+        W2LError (code 1) before running anything unless it is finite and > 0; an eval step does not use it.
+        input_sizes / target_sizes (seq2seq only; a list or a CUDA int32 tensor of B entries): the input frame counts of a
+        padded batch (the counts features.mfsc returns) and the target sizes (tokens plus eos).  Utterance b then attends
+        to its first ceil(d_b T' / max d) encoder frames, and the soft window follows its own diagonal."""
         B, _, F, T = features.shape
         L = target.shape[1]
+        isz, tsz = size_arg(input_sizes, B, "input_sizes"), size_arg(target_sizes, B, "target_sizes")
         if loss_out is None:
             loss_out = torch.empty(B, dtype=torch.float32, device=features.device)
-        _check(lib.w2l_trainer_step(self.h, _stream(), B, T, _ptr(features), L, _ptr(target), _ptr(loss_out), int(train),
-                                    float(total_batch if total_batch is not None else B)))
+        tb = float(total_batch if total_batch is not None else B)
+        if isz is None and tsz is None:
+            _check(lib.w2l_trainer_step(self.h, _stream(), B, T, _ptr(features), L, _ptr(target), _ptr(loss_out), int(train), tb))
+        else:
+            _check(lib.w2l_trainer_step_sized(self.h, _stream(), B, T, _ptr(features), L, _ptr(target), _ptr(isz), _ptr(tsz), _ptr(loss_out),
+                                              int(train), tb))
         return loss_out
 
     def output_width(self) -> int:
@@ -195,23 +203,29 @@ class Trainer:
         _check(lib.w2l_trainer_seq2seq_seed(self.h, ctypes.byref(s)))
         return int(s.value)
 
-    def decode(self, features: torch.Tensor):
+    def decode(self, features: torch.Tensor, input_sizes=None):
         """Greedy decode (seq2seq): eval-mode forward, then argmax token by token from startEmbedding until eos or
-        maxdecoderoutputlen steps.  Returns (tokens CUDA int32 [B, maxdecoderoutputlen] padded with pad, lengths CUDA int32 [B])."""
+        maxdecoderoutputlen steps.  Returns (tokens CUDA int32 [B, maxdecoderoutputlen] padded with pad, lengths CUDA int32 [B]).
+        input_sizes: as in step, so that each utterance of a padded batch decodes over its own frames."""
         B, _, F, T = features.shape
+        isz = size_arg(input_sizes, B, "input_sizes")
         n = self.seq2seq_config()["maxdecoderoutputlen"]
         tokens = torch.empty((B, n), dtype=torch.int32, device=features.device)
         lengths = torch.empty(B, dtype=torch.int32, device=features.device)
-        _check(lib.w2l_trainer_decode(self.h, _stream(), B, T, _ptr(features), _ptr(tokens), _ptr(lengths), tokens.numel()))
+        if isz is None:
+            _check(lib.w2l_trainer_decode(self.h, _stream(), B, T, _ptr(features), _ptr(tokens), _ptr(lengths), tokens.numel()))
+        else:
+            _check(lib.w2l_trainer_decode_sized(self.h, _stream(), B, T, _ptr(features), _ptr(isz), _ptr(tokens), _ptr(lengths), tokens.numel()))
         return tokens, lengths
 
-    def beam_search(self, features: torch.Tensor, beam_size: int = 4, max_len: int | None = None):
+    def beam_search(self, features: torch.Tensor, beam_size: int = 4, max_len: int | None = None, input_sizes=None):
         """Beam search (seq2seq): eval-mode forward, then Seq2SeqCriterion::beamSearchBatch over the batch with beam_size
         in [1, 16] for at most max_len steps (None: maxdecoderoutputlen).  Returns CUDA tensors (tokens int32 [B, K, L]
         padded with pad, lengths int32 [B, K], scores float32 [B, K], counts int32 [B]): per utterance the completed
         hypotheses if any (best first once more than K completed, else in completion order), otherwise the live beam at
-        length L.  Slots at or beyond counts[b] hold pad, length 0 and score -inf."""
+        length L.  Slots at or beyond counts[b] hold pad, length 0 and score -inf.  input_sizes: as in decode."""
         B, _, F, T = features.shape
+        isz = size_arg(input_sizes, B, "input_sizes")
         L = int(max_len) if max_len is not None else self.seq2seq_config()["maxdecoderoutputlen"]
         K = int(beam_size)
         dev = features.device
@@ -219,8 +233,12 @@ class Trainer:
         lengths = torch.empty((B, max(K, 1)), dtype=torch.int32, device=dev)
         scores = torch.empty((B, max(K, 1)), dtype=torch.float32, device=dev)
         counts = torch.empty(B, dtype=torch.int32, device=dev)
-        _check(lib.w2l_trainer_beam_search(self.h, _stream(), B, T, _ptr(features), K, L, _ptr(tokens), _ptr(lengths), _ptr(scores),
-                                           _ptr(counts), tokens.numel()))
+        if isz is None:
+            _check(lib.w2l_trainer_beam_search(self.h, _stream(), B, T, _ptr(features), K, L, _ptr(tokens), _ptr(lengths), _ptr(scores),
+                                               _ptr(counts), tokens.numel()))
+        else:
+            _check(lib.w2l_trainer_beam_search_sized(self.h, _stream(), B, T, _ptr(features), _ptr(isz), K, L, _ptr(tokens), _ptr(lengths),
+                                                     _ptr(scores), _ptr(counts), tokens.numel()))
         return tokens, lengths, scores, counts
 
     def align(self, features: torch.Tensor, target: torch.Tensor):
@@ -245,6 +263,29 @@ class Trainer:
 
     def sync_parameters(self):
         _check(lib.w2l_trainer_sync_parameters(self.h, _stream()))
+
+
+def size_arg(sizes, B: int, name: str):
+    """None, or the per-utterance sizes as a contiguous CUDA int32 tensor of B entries: from a list / tuple of whole
+    numbers, or a CUDA int32 tensor as it is.  Their values are checked on the device (a bad one gives that utterance a
+    NaN loss); their form is checked here, before anything runs."""
+    if sizes is None:
+        return None
+    if isinstance(sizes, torch.Tensor):
+        if not sizes.is_cuda or sizes.dtype != torch.int32 or not sizes.is_contiguous() or sizes.dim() != 1:
+            raise TypeError(f"{name}: expected a contiguous 1-d CUDA tensor of torch.int32")
+        t = sizes
+    else:
+        vals = list(sizes)
+        if not all(isinstance(v, (int, np.integer)) and not isinstance(v, bool) for v in vals):
+            raise TypeError(f"{name}: expected whole numbers")
+        if any(v < -(1 << 31) or v >= (1 << 31) for v in vals):
+            raise ValueError(f"{name}: values must fit in int32")
+        t = None
+    n = t.numel() if t is not None else len(vals)
+    if n != B:
+        raise ValueError(f"{name}: {n} entries for a batch of {B}")
+    return t if t is not None else torch.tensor(vals, dtype=torch.int32, device="cuda")
 
 
 def nccl_unique_id() -> bytes:
