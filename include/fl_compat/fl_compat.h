@@ -624,6 +624,12 @@ class LinearSegmentationCriterion : public SequenceCriterion {
 };
 using LinSegCriterion = LinearSegmentationCriterion;
 
+// slimIPL's soft-label loss (recipes/slimIPL/src/Train.cpp:1663-1673), one fused kernel (w2l_soft_label_loss):
+//   softScale * -mean over frames and utterances of sum_c softmax(teacher)[c] * logSoftmax(student)[c]
+// student: the network output [N,T',B] f32; teacher: the teacher's output of the same shape (no gradient flows into it;
+// another shape throws std::invalid_argument).  Returns a [1] loss whose backward adds the fused gradient to student.
+Variable softLabelLoss(const Variable& student, const Variable& teacher, double softScale);
+
 // ---- Seq2Seq (--criterion=seq2seq), DESIGN.md §9 ---------------------------------------------------------------
 // Attentions and windows are descriptions the criterion runs itself (its kernels read keys and values in place from
 // the encoder output); only the types the seq2seq recipes use exist: KeyValueAttention (--attention=keyvalue) and

@@ -270,6 +270,19 @@ W2L_API int w2l_seq2seq_beam_finish(void* stream, int B, int K, int maxlen, int 
                                     int32_t* lengths, float* scores, int32_t* counts);
 
 /* ----------------------------------------------------------------------------------------
+ * slimIPL (recipes/slimIPL/src/Train.cpp; DESIGN.md §7).
+ * w2l_soft_label_loss: student and teacher are fp32 logits [rows][N] (rows = B T'; any N, any float alignment).
+ *   loss_out (one float) = -scale / rows * sum_rows sum_c p_c (z_c - lse(z)),  p = softmax(teacher row), z = student row
+ *   d_student (nullable: loss only) = scale / rows * (softmax(z) - p), written, not accumulated; exactly 0 where a teacher
+ *   row has the bits of its student row.  ws: device scratch of `rows` floats.  Deterministic (no atomics).
+ * w2l_ema_update: ema = ema * d + params * (1 - d) over n floats, d and 1 - d each rounded once from decay, every product
+ *   and the sum rounded once (no fma).
+ * ---------------------------------------------------------------------------------------- */
+W2L_API int w2l_soft_label_loss(void* stream, long long rows, int N, const float* student, const float* teacher, float scale, float* loss_out,
+                                float* d_student, float* ws);
+W2L_API int w2l_ema_update(void* stream, long long n, float* ema, const float* params, double decay);
+
+/* ----------------------------------------------------------------------------------------
  * Dense contraction of the acoustic model (replaces fl::Linear's af::matmul -> cuBLAS and the
  * GEMM inside cuDNN's convolutions; forward at Train.cpp:1470, backward at :1720).
  *   C[m][n] = act( sum_k A(m,k) * B(n,k) + bias[n] ),  fp32 storage, wgmma math in the kind the thread's precision
@@ -547,6 +560,32 @@ W2L_API int w2l_trainer_beam_search_sized(void* trainer, void* stream, int B, in
                                           int max_len, int32_t* tokens, int32_t* lengths, float* scores, int32_t* counts, long long capacity);
 W2L_API int w2l_trainer_forward(void* trainer, void* stream, int B, int T, const float* features, float* emissions_out,
                                 long long capacity, int* t_out);
+/* slimIPL (recipes/slimIPL/src/Train.cpp; DESIGN.md §7).
+ * set_ema (--slimIPL_ema / --slimIPL_ema_decay): on = 1 builds the teacher, a second network from the same arch text or
+ * plugin with its own value arena, copied from the network as it is now (a second call restarts it from the network);
+ * on = 0 drops it.  Every training call (step, step_sized, step_soft) then runs ema = ema * decay + net * (1 - decay)
+ * once after the optimizer (w2l_ema_update), also after a skipped update and once per batch under mixed-precision
+ * retries; eval steps do not.  Only the network is averaged.  Without a teacher, "the teacher" below is the network.
+ * w2l_trainer_ema reads the setting back.  num_params / param_layout / get_flat / set_flat take which = 2 for the
+ * teacher's values (get_flat: what = 0 only).
+ * forward_teacher: w2l_trainer_forward of the network (teacher = 0) or of the teacher (soft pseudo-labels, :1413-1415).
+ * viterbi_path: eval-mode forward of the network or teacher, then crit->viterbiPath (:1362-1407): CTC the per-frame
+ * argmax, ASG / LinSeg the FCC Viterbi path, seq2seq the greedy decode.  path device int32 [B][T'] (seq2seq
+ * [B][maxdecoderoutputlen], padded with pad; capacity elements); T' (or maxdecoderoutputlen) through t_out.  input_sizes:
+ * seq2seq only, as in step_sized; the CTC and ASG paths cover all T' frames of a padded batch, as Train.cpp's.
+ * step_soft: a training step whose loss is the soft-label loss (w2l_soft_label_loss, :1663-1673) of the train-mode
+ * output against teacher_logits, device [B][t_teacher][output width] (another shape: W2L_ERR_INVALID_ARGUMENT), scaled
+ * by soft_scale (--slimIPL_soft_scale); loss_out receives one float.  Backward, all-reduce, clip, finite guard, loss
+ * scaling and update are the step's; the criterion gets a zero gradient.  total_batch: the world size (the loss is one
+ * scalar per rank, :1743-1747). */
+W2L_API int w2l_trainer_set_ema(void* trainer, void* stream, int on, double decay);
+W2L_API int w2l_trainer_ema(void* trainer, int* on, double* decay);
+W2L_API int w2l_trainer_forward_teacher(void* trainer, void* stream, int B, int T, const float* features, int teacher, float* emissions_out,
+                                        long long capacity, int* t_out);
+W2L_API int w2l_trainer_viterbi_path(void* trainer, void* stream, int B, int T, const float* features, const int32_t* input_sizes, int teacher,
+                                     int32_t* path, long long capacity, int* t_out);
+W2L_API int w2l_trainer_step_soft(void* trainer, void* stream, int B, int T, const float* features, const float* teacher_logits, int t_teacher,
+                                  float soft_scale, float* loss_out, float total_batch);
 /* Forced alignment: the eval-mode network forward of w2l_trainer_forward, then the criterion's viterbiPathWithTarget on
  * its emissions.  path / idx: device int32 [B][T'] (capacity elements each; idx nullable), T' through t_out.  CTC:
  * w2l_ctc_viterbi_target, idx = extended-target state.  ASG / LinSeg: w2l_fac_viterbi with the criterion's transitions,
@@ -595,7 +634,7 @@ W2L_API int w2l_trainer_amp_state(void* trainer, void* stream, double* scale, in
 /* steps whose update was skipped on the device because the loss or a gradient was NaN / Inf (Train.cpp:1686-1698,
  * :1753-1771); synchronises `stream` */
 W2L_API int w2l_trainer_status(void* trainer, void* stream, long long* skipped_steps);
-W2L_API long long w2l_trainer_num_params(void* trainer, int which /*0 network, 1 criterion*/);
+W2L_API long long w2l_trainer_num_params(void* trainer, int which /*0 network, 1 criterion, 2 teacher*/);
 W2L_API int w2l_trainer_param_layout(void* trainer, int which, int max_params, long long* elements, long long* dims4);
 W2L_API int w2l_trainer_get_flat(void* trainer, void* stream, int which, int what /*0 values, 1 gradients*/, float* out);
 W2L_API int w2l_trainer_set_flat(void* trainer, void* stream, int which, const float* in);
@@ -604,7 +643,8 @@ W2L_API const char* w2l_trainer_describe(void* trainer);
 /* Checkpoints (SURVEY.md §8 f4; the role of Serializer::save / load in Train.cpp:747-800): own little-endian container with
  * the constructor arguments + parameter / momentum arenas of network and criterion, the position and the learning-rate
  * schedule; load rebuilds the trainer.  Files written before the schedule existed load with position 0 and the default
- * schedule. */
+ * schedule.  A trainer with a teacher writes version 4 (version 2 followed by the decay and the teacher's values); one
+ * without writes version 2 as before. */
 W2L_API int w2l_trainer_save(void* trainer, void* stream, const char* path);
 W2L_API void* w2l_trainer_load(void* stream, const char* path);
 /* Export for the in-tree streaming inference stack, following the conversions of

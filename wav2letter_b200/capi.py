@@ -53,6 +53,8 @@ EXPORTS = [
     "w2l_trainer_seq2seq_seed", "w2l_trainer_decode", "w2l_trainer_beam_search",
     "w2l_seq2seq_sizes", "w2l_seq2seq_attn_fwd_sized", "w2l_seq2seq_attn_bwd_sized", "w2l_trainer_step_sized", "w2l_trainer_decode_sized",
     "w2l_trainer_beam_search_sized",
+    "w2l_soft_label_loss", "w2l_ema_update", "w2l_trainer_set_ema", "w2l_trainer_ema", "w2l_trainer_forward_teacher",
+    "w2l_trainer_viterbi_path", "w2l_trainer_step_soft",
 ]
 
 
@@ -206,6 +208,13 @@ def _load() -> ctypes.CDLL:
     lib.w2l_trainer_destroy.restype = None
     lib.w2l_trainer_step.argtypes = [vp, vp, i, i, vp, i, vp, vp, i, f32]
     lib.w2l_trainer_forward.argtypes = [vp, vp, i, i, vp, vp, ll, vp]
+    lib.w2l_soft_label_loss.argtypes = [vp, ll, i, vp, vp, f32, vp, vp, vp]
+    lib.w2l_ema_update.argtypes = [vp, ll, vp, vp, ctypes.c_double]
+    lib.w2l_trainer_set_ema.argtypes = [vp, vp, i, ctypes.c_double]
+    lib.w2l_trainer_ema.argtypes = [vp, vp, vp]
+    lib.w2l_trainer_forward_teacher.argtypes = [vp, vp, i, i, vp, i, vp, ll, vp]
+    lib.w2l_trainer_viterbi_path.argtypes = [vp, vp, i, i, vp, vp, i, vp, ll, vp]
+    lib.w2l_trainer_step_soft.argtypes = [vp, vp, i, i, vp, vp, i, f32, vp, f32]
     lib.w2l_trainer_align.argtypes = [vp, vp, i, i, vp, i, vp, vp, vp, ll, vp]
     lib.w2l_trainer_time_stride.argtypes = [vp]
     lib.w2l_trainer_num_params.restype = ll
@@ -668,3 +677,33 @@ def layernorm_bwd(a, r, dy, gain, mr, branch_mode=0, branch_scale=1.0):
                                  _ptr(d_res), int(branch_mode), float(branch_scale), _ptr(dgain), _ptr(dbias),
                                  _ptr(scratch)))
     return d_branch, d_res, dgain, dbias
+
+
+def soft_label_loss(student, teacher, scale=1.0, need_grad=True, d_student=None):
+    """slimIPL's soft-label loss (w2l_soft_label_loss) over logits [..., N] (rows = every leading index): returns
+    (loss float32 [1] = -scale / rows * sum_rows sum_c softmax(teacher)_c logSoftmax(student)_c,
+    d_student = scale / rows * (softmax(student) - softmax(teacher)) or None).  d_student: an output buffer of the
+    student's shape (any float alignment)."""
+    student = _req(student, torch.float32, "student")
+    teacher = _req(teacher, torch.float32, "teacher")
+    if student.shape != teacher.shape:
+        raise ValueError(f"soft_label_loss: teacher shape {tuple(teacher.shape)} != student shape {tuple(student.shape)}")
+    N = student.shape[-1]
+    rows = student.numel() // N
+    loss = torch.empty(1, dtype=torch.float32, device=student.device)
+    ws = torch.empty(rows, dtype=torch.float32, device=student.device)
+    if need_grad and d_student is None:
+        d_student = torch.empty_like(student)
+    d = _req(d_student, torch.float32, "d_student") if need_grad else None
+    _check(lib.w2l_soft_label_loss(_stream(), rows, N, _ptr(student), _ptr(teacher), float(scale), _ptr(loss), _ptr(d), _ptr(ws)))
+    return loss, d
+
+
+def ema_update(ema, params, decay):
+    """in place: ema = ema * decay + params * (1 - decay) (w2l_ema_update), float32 tensors of the same size"""
+    ema = _req(ema, torch.float32, "ema")
+    params = _req(params, torch.float32, "params")
+    if ema.numel() != params.numel():
+        raise ValueError("ema_update: sizes differ")
+    _check(lib.w2l_ema_update(_stream(), ema.numel(), _ptr(ema), _ptr(params), float(decay)))
+    return ema

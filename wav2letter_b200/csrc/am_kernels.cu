@@ -356,24 +356,6 @@ __device__ __forceinline__ void ln_moments(float K, double S, double Q, long lon
   rstd = (float)(1.0 / sqrt(var + (double)eps));
 }
 
-// CTA totals of the per-thread values v[0..K): warp sums, then thread 0 adds the NW warps' sums in warp order (no atomics,
-// the same bits every run).  The totals are left in thread 0's v.
-template <int NW, class T, int K>
-__device__ __forceinline__ void cta_sum(T (&v)[K]) {
-  __shared__ T red[K][NW];
-#pragma unroll
-  for (int k = 0; k < K; ++k) {
-    v[k] = warp_sum(v[k]);
-    if ((threadIdx.x & 31) == 0) red[k][threadIdx.x >> 5] = v[k];
-  }
-  __syncthreads();
-  if (threadIdx.x == 0)
-#pragma unroll
-    for (int k = 0; k < K; ++k) {
-      v[k] = 0;
-      for (int w = 0; w < NW; ++w) v[k] += red[k][w];
-    }
-}
 // CTA partial (sum, sum of squares / products) -> out[0..1]; the consumer kernel adds the CTAs' partials in a fixed order
 // (no zero-fill of the scratch, no atomics, deterministic)
 __device__ __forceinline__ void block_sum2_store(double s, double q, double* out) {

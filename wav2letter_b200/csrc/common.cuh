@@ -102,6 +102,24 @@ __device__ __forceinline__ double warp_sum(double v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
+// CTA totals of the per-thread values v[0..K): warp sums, then thread 0 adds the NW warps' sums in warp order (no atomics,
+// the same bits every run).  The totals are left in thread 0's v.
+template <int NW, class T, int K>
+__device__ __forceinline__ void cta_sum(T (&v)[K]) {
+  __shared__ T red[K][NW];
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    v[k] = warp_sum(v[k]);
+    if ((threadIdx.x & 31) == 0) red[k][threadIdx.x >> 5] = v[k];
+  }
+  __syncthreads();
+  if (threadIdx.x == 0)
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+      v[k] = 0;
+      for (int w = 0; w < NW; ++w) v[k] += red[k][w];
+    }
+}
 
 // ---- one V-wide chunk of a memory-bound pass: V = 4 (float4: 16-byte aligned, lengths multiples of 4) or V = 1 ----------
 template <int V> struct VecOf { using type = float; };

@@ -1850,6 +1850,29 @@ af::array ConnectionistTemporalClassificationCriterion::viterbiPathWithTarget(co
   return path;
 }
 
+Variable softLabelLoss(const Variable& student, const Variable& teacher, double softScale) {
+  if (student.type() != DType::f32 || teacher.type() != DType::f32 || student.dims() != teacher.dims())
+    throw std::invalid_argument("softLabelLoss: teacher must have the student's shape " + student.dims().str() + ", got " + teacher.dims().str());
+  const int N = (int)student.dims(0);
+  const long long rows = student.elements() / N;
+  af::array loss = af::array::empty(af::dim4(1));
+  af::array ws = af::array::empty(af::dim4(rows));
+  if (!student.isCalcGrad()) {
+    check(w2l_soft_label_loss(currentStream(), rows, N, student.array().f32(), teacher.array().f32(), (float)softScale, loss.f32(), nullptr, ws.f32()));
+    return Variable(loss, false);
+  }
+  // loss and gradient in one kernel; under loss scaling the gradient carries the scale, as the criteria's fused backward
+  const af::array d = af::array::empty(student.dims());
+  check(w2l_soft_label_loss(currentStream(), rows, N, student.array().f32(), teacher.array().f32(), (float)softScale, loss.f32(), d.f32(), ws.f32()));
+  const af::array seed = lossGradSeed(1);
+  const float seedScale = g_loss_grad_scale;
+  if (!seed.isEmpty()) check(w2l_seq2seq_scale_rows(currentStream(), 1, (int)rows, N, seed.f32(), 1.f, d.f32()));
+  return Variable(loss, {student}, [=](std::vector<Variable>& ins, const Variable& g) {
+    if (!g.isOnesSeed()) check(w2l_seq2seq_scale_rows(currentStream(), 1, (int)rows, N, g.array().f32(), seedScale, d.f32()));
+    ins[0].addGrad(Variable(d, false), true);
+  });
+}
+
 LinearSegmentationCriterion::LinearSegmentationCriterion(int N, CriterionScaleMode scalemode) : N_(N), scaleMode_(scalemode) {
   params_.push_back(Variable(af::array::zeros(af::dim4(N, N)), true));
 }

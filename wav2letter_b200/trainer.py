@@ -128,6 +128,7 @@ class Trainer:
         return lib.w2l_trainer_describe(self.h).decode()
 
     def num_params(self, which: int = 0) -> int:
+        """which: 0 the network, 1 the criterion, 2 the teacher (set_ema; without one, the network)"""
         return int(lib.w2l_trainer_num_params(self.h, which))
 
     def layout(self, which: int = 0):
@@ -178,14 +179,65 @@ class Trainer:
         _check(lib.w2l_trainer_output_width(self.h, ctypes.byref(w)))
         return int(w.value)
 
-    def forward(self, features: torch.Tensor) -> torch.Tensor:
+    def forward(self, features: torch.Tensor, teacher: bool = False) -> torch.Tensor:
+        """eval-mode network output [B, T', width]; teacher=True: the teacher's (set_ema; without one, the network's),
+        slimIPL's soft pseudo-labels"""
         B, _, F, T = features.shape
         width = self.output_width()
         cap = B * (2 * T + 64) * width  # SAME-padded even kernels grow the frame count by one each
         out = torch.empty(cap, dtype=torch.float32, device=features.device)
         tout = ctypes.c_int(0)
-        _check(lib.w2l_trainer_forward(self.h, _stream(), B, T, _ptr(features), _ptr(out), cap, ctypes.byref(tout)))
+        if teacher:
+            _check(lib.w2l_trainer_forward_teacher(self.h, _stream(), B, T, _ptr(features), 1, _ptr(out), cap, ctypes.byref(tout)))
+        else:
+            _check(lib.w2l_trainer_forward(self.h, _stream(), B, T, _ptr(features), _ptr(out), cap, ctypes.byref(tout)))
         return out[: B * tout.value * width].view(B, tout.value, width)
+
+    def set_ema(self, decay: float | None = 0.999):
+        """slimIPL's teacher (--slimIPL_ema --slimIPL_ema_decay): a second copy of the network, started from the network as
+        it is now, that every later training step moves by ema = ema * decay + net * (1 - decay).  None drops it."""
+        _check(lib.w2l_trainer_set_ema(self.h, _stream(), 0 if decay is None else 1, 0.0 if decay is None else float(decay)))
+
+    def ema(self) -> float | None:
+        """the teacher's decay, or None without a teacher"""
+        on, d = ctypes.c_int(0), ctypes.c_double(0)
+        _check(lib.w2l_trainer_ema(self.h, ctypes.byref(on), ctypes.byref(d)))
+        return float(d.value) if on.value else None
+
+    def viterbi_path(self, features: torch.Tensor, teacher: bool = False, input_sizes=None) -> torch.Tensor:
+        """crit->viterbiPath of the eval-mode output of the network or (teacher=True) the teacher: CUDA int32 [B, T'] (CTC
+        per-frame argmax, ASG / LinSeg FCC Viterbi) or [B, maxdecoderoutputlen] (seq2seq greedy decode, padded with pad).
+        input_sizes: seq2seq only, as in step."""
+        B, _, F, T = features.shape
+        isz = size_arg(input_sizes, B, "input_sizes")
+        try:
+            maxlen = self.seq2seq_config()["maxdecoderoutputlen"]
+        except capi.W2LError:  # not seq2seq: one token per output frame
+            maxlen = 0
+        cap = B * max(2 * T + 64, maxlen)
+        path = torch.empty(cap, dtype=torch.int32, device=features.device)
+        tout = ctypes.c_int(0)
+        _check(lib.w2l_trainer_viterbi_path(self.h, _stream(), B, T, _ptr(features), _ptr(isz), int(bool(teacher)), _ptr(path), cap,
+                                            ctypes.byref(tout)))
+        return path[: B * tout.value].view(B, tout.value)
+
+    def step_soft(self, features: torch.Tensor, teacher_logits: torch.Tensor, soft_scale: float = 1.0, total_batch: float | None = None,
+                  loss_out: torch.Tensor | None = None) -> torch.Tensor:
+        """slimIPL's training step on an unlabelled batch with soft pseudo-labels (--slimIPL_use_soft): the loss is
+        soft_scale * -mean over frames of sum_c softmax(teacher_logits)_c logSoftmax(output)_c, teacher_logits CUDA float32
+        [B, T', width] as forward returns it.  total_batch defaults to the world size (the loss is one scalar per rank).
+        Returns the loss, CUDA float32 [1]."""
+        B, _, F, T = features.shape
+        teacher_logits = capi._req(teacher_logits, torch.float32, "teacher_logits")
+        if teacher_logits.dim() != 3 or teacher_logits.shape[0] != B or teacher_logits.shape[2] != self.output_width():
+            raise ValueError(f"teacher_logits: expected [B={B}, T', {self.output_width()}], got {tuple(teacher_logits.shape)}")
+        if loss_out is None:
+            loss_out = torch.empty(1, dtype=torch.float32, device=features.device)
+        if total_batch is None:
+            total_batch = torch.distributed.get_world_size() if torch.distributed.is_available() and torch.distributed.is_initialized() else 1
+        _check(lib.w2l_trainer_step_soft(self.h, _stream(), B, T, _ptr(features), _ptr(teacher_logits), teacher_logits.shape[1],
+                                         float(soft_scale), _ptr(loss_out), float(total_batch)))
+        return loss_out
 
     def seq2seq_config(self) -> dict:
         """hidden, eos, pad, maxdecoderoutputlen, rounds, layers and whether the window is still set (seq2seq only)"""
