@@ -190,8 +190,8 @@ W2L_API int w2l_linseg_target(void* stream, int B, int T, int L, const int32_t* 
  * Seq2SeqCriterion runs beside the GEMMs of its projections.  Rows r = b*U + u of [B*U][width] row-major, H the hidden
  * size (--encoderdim), N the dictionary size (eos and pad included), x the encoder output [B][T'][2H] (keys x[.][0:H],
  * values x[.][H:2H]), target [B][U] int32.  Limits: H a multiple of 32 and <= 1024, 3 <= N <= 65536
- * (w2l_seq2seq_check; W2L_ERR_UNSUPPORTED outside), and what fits on chip: 8 (H + T') floats for the attention, 16 U
- * floats for its gradient, the W_hh slice of one CTA for the recurrence.
+ * (w2l_seq2seq_check; W2L_ERR_UNSUPPORTED outside), and what fits in 220 KB of shared memory: 8 (H + T') floats for
+ * the attention (T' <= 7040 - H), 16 U floats for its gradient (U <= 3520), the W_hh slice of one CTA for the recurrence.
  *   embed_fwd   tokens[b][0] = N (startEmbedding), tokens[b][u] = target[b][u-1], replaced with probability
  *               1 - pct/100 by min(floor(r2 (N-1)), N-2) (Philox block of counter b*U + u under seed: r1 = word x, r2 =
  *               word y, each (w >> 8) 2^-24; replaced iff r1 < fp32(1 - pct/100)); out[r] = E[tokens[r]] or start.
