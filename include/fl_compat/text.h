@@ -116,6 +116,39 @@ std::string alignWords(const std::vector<int>& target, const std::vector<int>& f
 }  // namespace speech
 }  // namespace pkg
 
+class EditDistanceMeter;
+
+namespace pkg {
+namespace speech {
+
+// evalOutput's scoring (Train.cpp:837-869) for a whole batch on the GPU (w2l_text_edit_counts, csrc/text_eval.cu), with
+// the counts tknPrediction2Ltr / tknTarget2Ltr / tkn2Wrd / EditDistanceMeter::add give utterance by utterance.  Built once
+// from the token dictionary and the flags the host functions take; works on the current stream (w2l::currentStream).
+class DeviceEditScorer {
+ public:
+  DeviceEditScorer(const lib::text::Dictionary& tokenDict, const std::string& criterion, const std::string& surround, int replabel,
+                   bool useWordPiece, const std::string& wordSep);
+  ~DeviceEditScorer();
+  DeviceEditScorer(const DeviceEditScorer&) = delete;
+  DeviceEditScorer& operator=(const DeviceEditScorer&) = delete;
+  // paths: device int32 [B][nPath] (criterion->viterbiPath's [T', B]), targets: device int32 [B][L] (padded as the
+  // dataset pads).  Adds every utterance's letter counts to tknMeter and word counts to wrdMeter after one read-back.
+  // Where the host functions would throw (a token outside the dictionary) it throws std::invalid_argument and adds
+  // nothing; beyond w2l_text_edit_counts' limit likewise.
+  void add(const int32_t* paths, int B, int nPath, const int32_t* targets, int L, EditDistanceMeter& tknMeter, EditDistanceMeter& wrdMeter);
+  // the same on the arrays themselves: viterbiPath [T', B] and the target [L, B]
+  template <class Array>
+  void add(const Array& viterbiPath, const Array& target, EditDistanceMeter& tknMeter, EditDistanceMeter& wrdMeter) {
+    add(viterbiPath.i32(), (int)viterbiPath.dims(1), (int)viterbiPath.dims(0), target.i32(), (int)target.dims(0), tknMeter, wrdMeter);
+  }
+
+ private:
+  void* dev_ = nullptr;  // w2l_text_device_create's tables
+};
+
+}  // namespace speech
+}  // namespace pkg
+
 // fl::EditDistanceMeter (mtr.tknEdit / mtr.wrdEdit, Train.cpp:868-869): Levenshtein alignment of hypothesis vs reference
 class EditDistanceMeter {
  public:

@@ -773,6 +773,35 @@ W2L_API long long w2l_text_align_words(void* text, const int32_t* target, int le
 /* out4 += {reference length, deletions, insertions, substitutions} of one (hypothesis, reference) pair */
 W2L_API int w2l_edit_distance(const char* hyp, const char* ref, long long* out4);
 
+/* ----------------------------------------------------------------------------------------
+ * The same scoring on the device, for a whole batch (csrc/text_eval.cu; DESIGN.md §10).
+ *   w2l_text_device_create  device tables of a w2l_text_create handle, built once with its own Dictionary and splitWrd:
+ *                           each token's role (replabel <k>, or unspellable), its letters (CSR of letter ids: the
+ *                           splitWrd code points with --usewordpiece, else the whole token), each letter's bytes, the
+ *                           blank / eos / pad / <SIL> / surround indices and the separator's letter id.  Synchronises
+ *                           `stream` once.  NULL on error.  The text handle may be destroyed afterwards.
+ *   w2l_text_edit_counts    counts[B][8] = {reference letters, deletions, insertions, substitutions, reference words,
+ *                           deletions, insertions, substitutions} of hypothesis row b of paths[B][n_path] (its first
+ *                           path_lengths[b] entries when path_lengths is non-NULL) against target row b of targets[B][L],
+ *                           exactly as w2l_text_prediction2ltr / target2ltr / ltr2wrd / w2l_edit_distance give them.
+ *                           Where the host pipeline throws (a token outside the dictionary reaches the letters, a path
+ *                           length outside [0, n_path]) that utterance's eight counts are -1.  Two kernels, no host sync.
+ *                           Limit: n_path and L each times (1 + replabel) times the longest token's letter count
+ *                           <= 1 048 576, else W2L_ERR_UNSUPPORTED and nothing is launched.
+ *   w2l_text_edit_workspace_size   its workspace in bytes (0 outside the limit, with the error text set).
+ * ---------------------------------------------------------------------------------------- */
+W2L_API void* w2l_text_device_create(void* text, void* stream);
+W2L_API void w2l_text_device_destroy(void* dev_text);
+W2L_API size_t w2l_text_edit_workspace_size(void* dev_text, int B, int n_path, int L);
+W2L_API int w2l_text_edit_counts(void* dev_text, void* stream, int B, int n_path, const int32_t* paths, const int32_t* path_lengths, int L,
+                                 const int32_t* targets, int32_t* counts, void* ws, size_t ws_bytes);
+/* Train.cpp's test() for one batch (:965-980 with evalOutput :829-872): the eval-mode forward, the criterion's eval loss
+ * into loss[B] (the bits of w2l_trainer_step with train = 0), the criterion's viterbiPath (CTC argmax, ASG / LinSeg FCC
+ * Viterbi, seq2seq greedy decode with input_sizes) and w2l_text_edit_counts of it against target into counts[B][8].
+ * input_sizes / target_sizes as in w2l_trainer_step_sized (seq2seq only).  The only host read is the greedy decode's. */
+W2L_API int w2l_trainer_evaluate(void* trainer, void* stream, void* dev_text, int B, int T, const float* features, int L, const int32_t* target,
+                                 const int32_t* input_sizes, const int32_t* target_sizes, float* loss, int32_t* counts);
+
 #ifdef __cplusplus
 }
 #endif

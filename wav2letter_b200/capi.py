@@ -55,6 +55,7 @@ EXPORTS = [
     "w2l_trainer_beam_search_sized",
     "w2l_soft_label_loss", "w2l_ema_update", "w2l_trainer_set_ema", "w2l_trainer_ema", "w2l_trainer_forward_teacher",
     "w2l_trainer_viterbi_path", "w2l_trainer_step_soft",
+    "w2l_text_device_create", "w2l_text_device_destroy", "w2l_text_edit_workspace_size", "w2l_text_edit_counts", "w2l_trainer_evaluate",
 ]
 
 
@@ -170,6 +171,14 @@ def _load() -> ctypes.CDLL:
     lib.w2l_text_align_words.restype = ll
     lib.w2l_text_align_words.argtypes = [vp, vp, i, vp, i, ctypes.c_double, cp, vp, ll]
     lib.w2l_edit_distance.argtypes = [cp, cp, vp]
+    lib.w2l_text_device_create.restype = vp
+    lib.w2l_text_device_create.argtypes = [vp, vp]
+    lib.w2l_text_device_destroy.argtypes = [vp]
+    lib.w2l_text_device_destroy.restype = None
+    lib.w2l_text_edit_workspace_size.restype = sz
+    lib.w2l_text_edit_workspace_size.argtypes = [vp, i, i, i]
+    lib.w2l_text_edit_counts.argtypes = [vp, vp, i, i, vp, vp, i, vp, vp, vp, sz]
+    lib.w2l_trainer_evaluate.argtypes = [vp, vp, vp, i, i, vp, i, vp, vp, vp, vp, vp]
     lib.w2l_trainer_create.restype = vp
     lib.w2l_trainer_create.argtypes = [vp, ctypes.c_char_p, i, i, ctypes.c_char_p, i, f32, f32, f32, f32, f32]
     lib.w2l_trainer_create_seq2seq.restype = vp

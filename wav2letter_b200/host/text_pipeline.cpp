@@ -12,10 +12,14 @@
 #include <sstream>
 #include <stdexcept>
 
+#include <cuda_runtime.h>
+
+#include "text_tables.h"
 #include "w2l_b200.h"
 
 namespace w2l {
 int fail(int code, const std::string& msg);
+void* currentStream();
 }
 
 namespace fl {
@@ -387,6 +391,105 @@ std::string alignWords(const std::vector<int>& target, const std::vector<int>& f
   return line;
 }
 
+// The tables of csrc/text_eval.cu, built with this file's own Dictionary and splitWrd so that the device and the
+// functions above agree on every letter: token roles, letters (tknIdx2Ltr's strings, one id per distinct string), each
+// letter's bytes, and the indices tknPrediction2Ltr / remapLabels look up (getIndex throws where they would on every call)
+w2l::TextTablesHost buildTextTables(const Dictionary& d, const std::string& criterion, const std::string& surround, int replabel, bool useWordPiece,
+                                    const std::string& wordSep) {
+  w2l::TextTablesHost tb;
+  tb.criterion = criterion == kCtcCriterion ? w2l::kTextCtc
+                 : criterion == kAsgCriterion ? w2l::kTextAsg
+                 : criterion == kSeq2SeqRNNCriterion ? w2l::kTextSeq2Seq
+                                                     : w2l::kTextOther;
+  tb.replabel = std::max(replabel, 0);
+  if (tb.criterion == w2l::kTextCtc) tb.blank = d.getIndex(kBlankToken);
+  if (tb.criterion == w2l::kTextSeq2Seq) {
+    tb.eos = d.getIndex(lib::text::kEosToken);
+    tb.pad = d.getIndex(lib::text::kPadToken);
+  }
+  if (d.contains(kSilToken)) tb.sil = d.getIndex(kSilToken);
+  if (!surround.empty()) tb.surround = d.getIndex(surround);
+  const int N = (int)d.indexSize();
+  if (tb.replabel > 127) throw std::invalid_argument("text device tables: replabel above 127");
+  tb.role.assign((size_t)N, 0);
+  for (int r = 1; r <= tb.replabel; ++r) tb.role[(size_t)d.getIndex("<" + std::to_string(r) + ">")] = (int8_t)r;
+  std::unordered_map<std::string, int> letterId;
+  std::vector<std::string> letters;
+  tb.ltrOff.push_back(0);
+  for (int v = 0; v < N; ++v) {
+    const std::string tok = d.getEntry(v);
+    std::vector<std::string> spelled;
+    if (useWordPiece) {
+      try {
+        spelled = lib::text::splitWrd(tok);
+      } catch (const std::exception&) {
+        if (tb.role[(size_t)v] == 0) tb.role[(size_t)v] = -1;  // tknIdx2Ltr throws on this token
+      }
+    } else {
+      spelled.push_back(tok);
+    }
+    for (const auto& str : spelled) {
+      auto it = letterId.emplace(str, (int)letters.size()).first;
+      if (it->second == (int)letters.size()) letters.push_back(str);
+      tb.ltr.push_back(it->second);
+    }
+    tb.ltrOff.push_back((int32_t)tb.ltr.size());
+  }
+  if (!wordSep.empty()) {
+    auto it = letterId.find(wordSep);
+    if (it != letterId.end()) tb.sep = it->second;
+  }
+  tb.byteOff.push_back(0);
+  for (const auto& str : letters) {
+    tb.bytes.insert(tb.bytes.end(), str.begin(), str.end());
+    tb.byteOff.push_back((int32_t)tb.bytes.size());
+  }
+  return tb;
+}
+
+namespace {
+void cudaOrThrow(cudaError_t e, const char* what) {
+  if (e != cudaSuccess) throw std::runtime_error(std::string("DeviceEditScorer: ") + what + ": " + cudaGetErrorString(e));
+}
+}  // namespace
+
+DeviceEditScorer::DeviceEditScorer(const Dictionary& tokenDict, const std::string& criterion, const std::string& surround, int replabel, bool useWordPiece,
+                                   const std::string& wordSep) {
+  dev_ = w2l::textDeviceUpload(buildTextTables(tokenDict, criterion, surround, replabel, useWordPiece, wordSep), w2l::currentStream());
+  if (!dev_) throw std::runtime_error(std::string("DeviceEditScorer: ") + w2l_last_error());
+}
+DeviceEditScorer::~DeviceEditScorer() { w2l_text_device_destroy(dev_); }
+
+void DeviceEditScorer::add(const int32_t* paths, int B, int nPath, const int32_t* targets, int L, EditDistanceMeter& tknMeter, EditDistanceMeter& wrdMeter) {
+  if (B <= 0) return;
+  void* stream = w2l::currentStream();
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const size_t wsBytes = w2l_text_edit_workspace_size(dev_, B, nPath, L);
+  if (!wsBytes) {
+    const int rc = w2l_text_edit_counts(dev_, stream, B, nPath, paths, nullptr, L, targets, nullptr, nullptr, 0);  // its error text
+    throw std::invalid_argument("DeviceEditScorer: " + std::string(w2l_last_error()) + " (code " + std::to_string(rc) + ")");
+  }
+  const size_t countBytes = (size_t)B * 8 * sizeof(int32_t), off = (countBytes + 255) / 256 * 256;
+  void* mem = nullptr;
+  cudaOrThrow(cudaMallocAsync(&mem, off + wsBytes, s), "cudaMallocAsync");
+  int32_t* counts = static_cast<int32_t*>(mem);
+  std::vector<int32_t> host((size_t)B * 8);
+  const int rc = w2l_text_edit_counts(dev_, stream, B, nPath, paths, nullptr, L, targets, counts, static_cast<char*>(mem) + off, wsBytes);
+  const std::string err = rc == W2L_OK ? "" : w2l_last_error();
+  cudaError_t e = rc == W2L_OK ? cudaMemcpyAsync(host.data(), counts, countBytes, cudaMemcpyDeviceToHost, s) : cudaSuccess;
+  cudaFreeAsync(mem, s);
+  if (rc != W2L_OK) throw std::invalid_argument("DeviceEditScorer: " + err);
+  cudaOrThrow(e, "cudaMemcpyAsync");
+  cudaOrThrow(cudaStreamSynchronize(s), "cudaStreamSynchronize");  // the one read-back of the batch
+  for (int b = 0; b < B; ++b)
+    if (host[(size_t)b * 8] < 0) throw std::invalid_argument("DeviceEditScorer: utterance " + std::to_string(b) + " has a token outside the dictionary");
+  for (int b = 0; b < B; ++b) {
+    const int32_t* c = &host[(size_t)b * 8];
+    tknMeter.add(c[0], c[1], c[2], c[3]);
+    wrdMeter.add(c[4], c[5], c[6], c[7]);
+  }
+}
+
 }  // namespace speech
 }  // namespace pkg
 
@@ -560,6 +663,17 @@ W2L_API long long w2l_text_align_words(void* h, const int32_t* target, int len, 
     if (out && cap >= need) std::memcpy(out, line.c_str(), (size_t)need);
     return need;
   });
+}
+// device tables of the handle for w2l_text_edit_counts (csrc/text_eval.cu)
+W2L_API void* w2l_text_device_create(void* h, void* stream) {
+  void* dev = nullptr;
+  guardedText([&]() -> long long {
+    auto* t = static_cast<TextPipeline*>(h);
+    if (!t) throw std::invalid_argument("text_device_create: null text pipeline");
+    dev = w2l::textDeviceUpload(fl::pkg::speech::buildTextTables(t->dict, t->criterion, t->surround, t->replabel, t->wordpiece, t->wordsep), stream);
+    return dev ? 0 : -1;
+  });
+  return dev;
 }
 // EditDistanceMeter::add on one (hypothesis, reference) pair of space-joined token strings: out4 += {n, ndel, nins, nsub}
 W2L_API int w2l_edit_distance(const char* hyp, const char* ref, long long* out4) {

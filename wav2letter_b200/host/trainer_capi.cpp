@@ -511,6 +511,16 @@ namespace {
 af::array sizesArray(const int32_t* p, int B) { return p ? af::array::wrap(const_cast<int32_t*>(p), af::dim4(B), w2l::DType::i32) : af::array(); }
 }  // namespace
 
+namespace {
+// the criterion's loss of the network output (Train.cpp:1664-1676), with the seq2seq sizes when given: the one loss both
+// the step and w2l_trainer_evaluate compute
+Variable criterionLoss(Trainer* t, const Variable& output, int B, int L, const int32_t* target, const int32_t* input_sizes, const int32_t* target_sizes) {
+  Variable tgt = fl::noGrad(af::array::wrap(const_cast<int32_t*>(target), af::dim4(L, B), w2l::DType::i32));
+  if (!input_sizes && !target_sizes) return t->crit->forward({output, tgt}).front();
+  return t->crit->forward({output, tgt, fl::noGrad(sizesArray(input_sizes, B)), fl::noGrad(sizesArray(target_sizes, B))}).front();
+}
+}  // namespace
+
 // input_sizes / target_sizes: device int32 [B] (nullable), the durations and target sizes Train.cpp passes the seq2seq
 // criterion (:1473-1476); the other criteria take none
 W2L_API int w2l_trainer_step_sized(void* h, void* stream, int B, int T, const float* features, int L, const int32_t* target,
@@ -521,12 +531,8 @@ W2L_API int w2l_trainer_step_sized(void* h, void* stream, int B, int T, const fl
     auto* t = static_cast<Trainer*>(h);
     const bool sized = input_sizes || target_sizes;
     if (sized && !t->s2s) throw std::invalid_argument("trainer_step: input and target sizes are taken by the seq2seq criterion only");
-    runStep(t, stream, B, T, features, [&](const Variable& output) {
-      Variable tgt = fl::noGrad(af::array::wrap(const_cast<int32_t*>(target), af::dim4(L, B), w2l::DType::i32));
-      return (sized ? t->crit->forward({output, tgt, fl::noGrad(sizesArray(input_sizes, B)), fl::noGrad(sizesArray(target_sizes, B))})
-                    : t->crit->forward({output, tgt}))
-          .front();
-    }, loss_out, train, total_batch);
+    runStep(t, stream, B, T, features, [&](const Variable& output) { return criterionLoss(t, output, B, L, target, input_sizes, target_sizes); },
+            loss_out, train, total_batch);
   });
 }
 
@@ -683,6 +689,37 @@ W2L_API int w2l_trainer_viterbi_path(void* h, void* stream, int B, int T, const 
     af::array::wrap(path, p.dims(), w2l::DType::i32).copyFrom(p);
     if (t_out) *t_out = (int)p.dims(0);
   });
+}
+
+// test() for one batch (Train.cpp:965-980, evalOutput :829-872): one eval-mode forward feeds both the criterion's loss,
+// as the eval step computes it, and its viterbiPath, which the device scoring turns into counts[B][8]
+W2L_API int w2l_trainer_evaluate(void* h, void* stream, void* dev_text, int B, int T, const float* features, int L, const int32_t* target,
+                                 const int32_t* input_sizes, const int32_t* target_sizes, float* loss, int32_t* counts) {
+  int rc = W2L_OK;
+  const int g = guarded([&] {
+    w2l::setCurrentStream(stream);
+    auto* t = static_cast<Trainer*>(h);
+    if (!t || !dev_text || B <= 0 || T <= 0 || L <= 0 || !features || !target || !loss || !counts)
+      throw std::invalid_argument("trainer_evaluate: bad arguments");
+    const bool sized = input_sizes || target_sizes;
+    if (sized && !t->s2s) throw std::invalid_argument("trainer_evaluate: input and target sizes are taken by the seq2seq criterion only");
+    PrecisionScope scope(t->precision);
+    Variable output;  // the eval step's own forward and loss; the path is decoded from that same output
+    runStep(t, stream, B, T, features, [&](const Variable& o) {
+      output = o;
+      return criterionLoss(t, o, B, L, target, input_sizes, target_sizes);
+    }, loss, 0, 1.f);
+    const af::array p = t->crit->viterbiPath(output.array(), sizesArray(input_sizes, B));
+    const int nPath = (int)p.dims(0);
+    const size_t bytes = w2l_text_edit_workspace_size(dev_text, B, nPath, L);
+    if (!bytes) {
+      rc = w2l_text_edit_counts(dev_text, stream, B, nPath, p.i32(), nullptr, L, target, counts, nullptr, 0);  // the limit's error
+      return;
+    }
+    const af::array ws = af::array::empty(af::dim4((long long)bytes), w2l::DType::u8);
+    rc = w2l_text_edit_counts(dev_text, stream, B, nPath, p.i32(), nullptr, L, target, counts, ws.ptr(), bytes);
+  });
+  return g != W2L_OK ? g : rc;
 }
 
 // --slimIPL_ema: on = 1 builds the teacher, a second network from the same arch text or plugin with its own value arena,

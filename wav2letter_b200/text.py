@@ -5,6 +5,7 @@ from __future__ import annotations
 import ctypes
 
 import numpy as np
+import torch
 
 from . import capi
 from .capi import lib
@@ -21,9 +22,44 @@ class TextPipeline:
         self.criterion = criterion
 
     def close(self):
+        if getattr(self, "dev", None):
+            lib.w2l_text_device_destroy(self.dev)
+            self.dev = None
         if getattr(self, "h", None):
             lib.w2l_text_destroy(self.h)
             self.h = None
+
+    def to_device(self):
+        """builds (once) the device tables w2l_text_edit_counts and Trainer.evaluate read; returns their handle"""
+        if getattr(self, "dev", None) is None:
+            d = lib.w2l_text_device_create(self.h, capi._stream())
+            if not d:
+                raise capi.W2LError(1, lib.w2l_last_error().decode())
+            self.dev = ctypes.c_void_p(d)
+        return self.dev
+
+    def edit_counts(self, paths, targets, path_lengths=None):
+        """evalOutput's scoring of a batch on the GPU: paths CUDA int32 [B, n] (viterbi_path / decode rows, a beam_search
+        row, slimIPL teacher paths), targets CUDA int32 [B, L] (padded as encode_batch pads), path_lengths None or CUDA
+        int32 [B] (row b is then its first path_lengths[b] entries).  Returns CUDA int32 [B, 8]: {reference letters,
+        deletions, insertions, substitutions} for letters, then the same for words, equal to prediction2ltr / target2ltr
+        / ltr2wrd / EditDistanceMeter on every row; -1 in all eight where those raise (a token outside the dictionary)."""
+        paths = capi._req(paths, torch.int32, "paths")
+        targets = capi._req(targets, torch.int32, "targets")
+        path_lengths = capi._req(path_lengths, torch.int32, "path_lengths")
+        if paths.dim() != 2 or targets.dim() != 2 or paths.shape[0] != targets.shape[0]:
+            raise ValueError(f"paths [B, n] and targets [B, L] expected, got {tuple(paths.shape)} and {tuple(targets.shape)}")
+        B, n = paths.shape
+        L = targets.shape[1]
+        if path_lengths is not None and tuple(path_lengths.shape) != (B,):
+            raise ValueError(f"path_lengths: expected [{B}], got {tuple(path_lengths.shape)}")
+        dev = self.to_device()
+        counts = torch.empty((B, 8), dtype=torch.int32, device=paths.device)
+        nbytes = lib.w2l_text_edit_workspace_size(dev, B, n, L)
+        ws = torch.empty(max(int(nbytes), 1), dtype=torch.uint8, device=paths.device)
+        capi._check(lib.w2l_text_edit_counts(dev, capi._stream(), B, n, capi._ptr(paths), capi._ptr(path_lengths), L, capi._ptr(targets),
+                                             capi._ptr(counts), capi._ptr(ws), int(nbytes)))
+        return counts
 
     __del__ = close
 
@@ -106,3 +142,32 @@ class EditDistanceMeter:
 
     def raw(self):
         return tuple(int(v) for v in self.acc)
+
+
+class ErrorRates:
+    """Sums the counts of edit_counts / Trainer.evaluate batch by batch on the device (mtr.tknEdit and mtr.wrdEdit) and
+    reports them as EditDistanceMeter.value() does.  Rows of -1 (utterances the host pipeline would refuse) are counted
+    in `rejected` and left out of the sums.  Summing across ranks is the caller's: all-reduce `sums` before reading."""
+
+    def __init__(self, device="cuda"):
+        self.sums = torch.zeros(9, dtype=torch.int64, device=device)  # 8 counts, then rejected rows
+
+    def add(self, counts: torch.Tensor):
+        ok = counts[:, 0] >= 0
+        self.sums[:8] += (counts.to(torch.int64) * ok.unsqueeze(1)).sum(0)
+        self.sums[8] += (~ok).sum()
+
+    def _value(self, n, ndel, nins, nsub):
+        d = float(max(n, 1))
+        return [100.0 * (ndel + nins + nsub) / d, n, 100.0 * nins / d, 100.0 * ndel / d, 100.0 * nsub / d]
+
+    def value(self):
+        """(token meter value, word meter value, rejected rows); each value is [error %, n, ins %, del %, sub %]"""
+        s = [int(v) for v in self.sums.tolist()]
+        return self._value(*s[0:4]), self._value(*s[4:8]), s[8]
+
+    def ter(self) -> float:
+        return self.value()[0][0]
+
+    def wer(self) -> float:
+        return self.value()[1][0]

@@ -221,6 +221,25 @@ class Trainer:
                                             ctypes.byref(tout)))
         return path[: B * tout.value].view(B, tout.value)
 
+    def evaluate(self, features: torch.Tensor, target: torch.Tensor, text, input_sizes=None, target_sizes=None):
+        """Train.cpp's test() on one batch: the eval-mode forward, the criterion's loss (the bits of step(train=False)), its
+        viterbi path (as viterbi_path) and the device scoring of that path against target (TextPipeline.edit_counts).
+        text: the batch's TextPipeline.  input_sizes / target_sizes: seq2seq only, as in step.  Returns CUDA tensors
+        (loss float32 [B], counts int32 [B, 8]); nothing is read back to the host but the greedy decode's own polls."""
+        from .text import TextPipeline
+
+        if not isinstance(text, TextPipeline):
+            raise TypeError("text: expected a TextPipeline")
+        B, _, F, T = features.shape
+        target = capi._req(target, torch.int32, "target")
+        L = target.shape[1]
+        isz, tsz = size_arg(input_sizes, B, "input_sizes"), size_arg(target_sizes, B, "target_sizes")
+        loss = torch.empty(B, dtype=torch.float32, device=features.device)
+        counts = torch.empty((B, 8), dtype=torch.int32, device=features.device)
+        _check(lib.w2l_trainer_evaluate(self.h, _stream(), text.to_device(), B, T, _ptr(features), L, _ptr(target), _ptr(isz), _ptr(tsz),
+                                        _ptr(loss), _ptr(counts)))
+        return loss, counts
+
     def step_soft(self, features: torch.Tensor, teacher_logits: torch.Tensor, soft_scale: float = 1.0, total_batch: float | None = None,
                   loss_out: torch.Tensor | None = None) -> torch.Tensor:
         """slimIPL's training step on an unlabelled batch with soft pseudo-labels (--slimIPL_use_soft): the loss is
