@@ -70,6 +70,11 @@ W2L_API const char* w2l_last_error(void);
  * (bench.py's "gpu_launches" claim) */
 W2L_API long long w2l_launch_count(void);
 W2L_API void w2l_reset_launch_count(void);
+/* the process-wide seed stream that parameter initialisation, dropout and SpecAugment draw from (flashlight's
+ * fl::setSeed): read it, and set it back, so that what one part of a program creates does not change the initial
+ * parameters of trainers created after it */
+W2L_API unsigned long long w2l_get_seed(void);
+W2L_API void w2l_set_seed(unsigned long long seed);
 /* Measurement hook (bench.py's roofline leg): while set (non-NULL cudaEvent_t handles), every
  * call on this thread records `start` right before and `stop` right after its DOMINANT kernel
  * (asg_chains_kernel, ctc_chains_kernel, the GEMM of a dense op) on the call's stream, so that
@@ -558,6 +563,8 @@ W2L_API int w2l_trainer_decode_sized(void* trainer, void* stream, int B, int T, 
                                      int32_t* lengths, long long capacity);
 W2L_API int w2l_trainer_beam_search_sized(void* trainer, void* stream, int B, int T, const float* features, const int32_t* input_sizes, int beam,
                                           int max_len, int32_t* tokens, int32_t* lengths, float* scores, int32_t* counts, long long capacity);
+/* eval-mode network output [B][T'][width] into emissions_out (capacity floats); T' through t_out.  A buffer smaller than
+ * B T' width returns W2L_ERR_INVALID_ARGUMENT with nothing written to it, and t_out still set: call again with that size. */
 W2L_API int w2l_trainer_forward(void* trainer, void* stream, int B, int T, const float* features, float* emissions_out,
                                 long long capacity, int* t_out);
 /* slimIPL (recipes/slimIPL/src/Train.cpp; DESIGN.md §7).

@@ -19,7 +19,7 @@ TERM_FCC, TERM_FAC, TERM_ASG = 1, 2, 3
 
 # every entry point include/w2l_b200.h declares (tests check the library exports all of them)
 EXPORTS = [
-    "w2l_version", "w2l_last_error", "w2l_launch_count", "w2l_reset_launch_count", "w2l_set_profile_events", "w2l_set_profile_event_list", "w2l_profile_events_used", "w2l_trace_begin", "w2l_trace_end", "w2l_trace_list",
+    "w2l_version", "w2l_last_error", "w2l_launch_count", "w2l_reset_launch_count", "w2l_get_seed", "w2l_set_seed", "w2l_set_profile_events", "w2l_set_profile_event_list", "w2l_profile_events_used", "w2l_trace_begin", "w2l_trace_end", "w2l_trace_list",
     "w2l_asg_workspace_size", "w2l_asg_forward_backward",
     "w2l_asg64_workspace_size", "w2l_asg64_forward_backward",
     "w2l_fcc_viterbi_workspace_size", "w2l_fcc_viterbi",
@@ -74,6 +74,8 @@ def _load() -> ctypes.CDLL:
     vp, i, sz = ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t
     lib.w2l_last_error.restype = ctypes.c_char_p
     lib.w2l_launch_count.restype = ctypes.c_longlong
+    lib.w2l_get_seed.restype = ctypes.c_ulonglong
+    lib.w2l_set_seed.argtypes = [ctypes.c_ulonglong]
     lib.w2l_set_profile_events.argtypes = [vp, vp]
     lib.w2l_set_profile_event_list.argtypes = [i, vp, vp, i]
     lib.w2l_trace_begin.argtypes = [vp, i]

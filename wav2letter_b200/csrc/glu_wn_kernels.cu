@@ -344,12 +344,13 @@ extern "C" int w2l_conv1d_arrange_ex(void* stream_, int cin, int cout, int kw, i
     return fail(W2L_ERR_INVALID_ARGUMENT, "conv1d_arrange: bad arguments (padded channel counts must be multiples of 4)");
   if (glu_split && ((cout % 2) || (cout_p % 8) || cout_p / 2 < cout / 2)) return fail(W2L_ERR_INVALID_ARGUMENT, "conv1d_arrange: bad GLU split padding");
   if (out_bf16 < 0 || out_bf16 > 2) return fail(W2L_ERR_INVALID_ARGUMENT, "conv1d_arrange: out_bf16 must be 0 (fp32), 1 (bf16) or 2 (fp16)");
+  // every rejection comes before the destinations are touched
+  const size_t smem = arrange_smem(kw);
+  if (smem > 200 * 1024) return fail(W2L_ERR_UNSUPPORTED, "conv1d_arrange: kernel width too large");
   const size_t es = out_bf16 ? 2 : 4;
   W2L_CUDA_CHECK(cudaMemsetAsync(fwd, 0, es * (size_t)cout_p * kw * cin_p, stream));
   if (flip) W2L_CUDA_CHECK(cudaMemsetAsync(flip, 0, es * (size_t)cin_p * kw * cout_p, stream));
   if (bias_p) W2L_CUDA_CHECK(cudaMemsetAsync(bias_p, 0, sizeof(float) * (size_t)cout_p, stream));
-  const size_t smem = arrange_smem(kw);
-  if (smem > 200 * 1024) return fail(W2L_ERR_UNSUPPORTED, "conv1d_arrange: kernel width too large");
   dim3 grid((cout + kArrCo - 1) / kArrCo, (cin + kArrCi - 1) / kArrCi);
   auto run = [&](auto kernel) -> int {
     if (smem > 48 * 1024) W2L_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

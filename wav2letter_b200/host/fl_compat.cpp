@@ -2228,3 +2228,6 @@ af::array Seq2SeqCriterion::viterbiPathWithTarget(const af::array&, const af::ar
 }  // namespace speech
 }  // namespace pkg
 }  // namespace fl
+
+extern "C" W2L_API unsigned long long w2l_get_seed(void) { return fl::g_seed_counter.load(); }
+extern "C" W2L_API void w2l_set_seed(unsigned long long seed) { fl::g_seed_counter.store(seed); }

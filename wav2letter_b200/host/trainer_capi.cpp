@@ -661,9 +661,10 @@ W2L_API int w2l_trainer_forward_teacher(void* h, void* stream, int B, int T, con
     auto* t = static_cast<Trainer*>(h);
     PrecisionScope scope(t->precision);
     Variable out = evalForward(t, teacher, B, T, features);
+    // frames of outWidth values per sample, reported also when the buffer is too small: the caller learns the size it needs
+    if (t_out) *t_out = (int)(out.elements() / ((long long)B * t->outWidth));
     if (out.elements() > capacity) throw std::invalid_argument("trainer_forward: output buffer too small");
     af::array::wrap(emissions_out, out.dims()).copyFrom(out.array());
-    if (t_out) *t_out = (int)(out.elements() / ((long long)B * t->outWidth));  // frames of outWidth values per sample
   });
 }
 W2L_API int w2l_trainer_forward(void* h, void* stream, int B, int T, const float* features, float* emissions_out, long long capacity,

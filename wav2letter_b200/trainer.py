@@ -185,12 +185,20 @@ class Trainer:
         B, _, F, T = features.shape
         width = self.output_width()
         cap = B * (2 * T + 64) * width  # SAME-padded even kernels grow the frame count by one each
-        out = torch.empty(cap, dtype=torch.float32, device=features.device)
         tout = ctypes.c_int(0)
-        if teacher:
-            _check(lib.w2l_trainer_forward_teacher(self.h, _stream(), B, T, _ptr(features), 1, _ptr(out), cap, ctypes.byref(tout)))
-        else:
-            _check(lib.w2l_trainer_forward(self.h, _stream(), B, T, _ptr(features), _ptr(out), cap, ctypes.byref(tout)))
+
+        def run(cap):
+            out = torch.empty(cap, dtype=torch.float32, device=features.device)
+            if teacher:
+                rc = lib.w2l_trainer_forward_teacher(self.h, _stream(), B, T, _ptr(features), 1, _ptr(out), cap, ctypes.byref(tout))
+            else:
+                rc = lib.w2l_trainer_forward(self.h, _stream(), B, T, _ptr(features), _ptr(out), cap, ctypes.byref(tout))
+            return rc, out
+
+        rc, out = run(cap)
+        if rc != 0 and B * tout.value * width > cap:  # explicit padding (e.g. 170 frames a side) outgrew the guess: the exact size
+            rc, out = run(B * tout.value * width)
+        _check(rc)
         return out[: B * tout.value * width].view(B, tout.value, width)
 
     def set_ema(self, decay: float | None = 0.999):
