@@ -675,13 +675,16 @@ W2L_API int w2l_trainer_export_streaming(void* trainer, void* stream, const char
  * on the host: a run call neither reads from the device nor synchronises, and returns the output frame counts at once.
  * Calls on one handle must be ordered (one CUDA stream, or the caller's synchronisation).
  *
- *   w2l_stream_create   snapshots the trainer's network parameters (training may go on), takes the calling thread's
+ *   w2l_stream_create   snapshots the trainer's network parameters and its criterion (kind; ASG / LinSeg transitions)
+ *                       (training may go on), takes the calling thread's
  *                       w2l_set_precision, and allocates all state and per-call buffers for max_streams slots (at most
  *                       1024) and chunks of at most max_chunk frames.  Accepts exactly the archs the export accepts,
  *                       with its error text.  NULL on failure (w2l_last_error).
- *   w2l_stream_state_bytes   device bytes of carried state per slot (two planes of the held frames of every convolution)
+ *   w2l_stream_state_bytes   device bytes of carried state per slot (two planes of the held frames of every convolution,
+ *                       and for ASG / LinSeg the Viterbi scores and the backpointers of the uncommitted frames)
  *   w2l_stream_max_frames_out  the most output frames one call can give a stream (sizes the emission buffer)
- *   w2l_stream_start    resets the n slots (host int slots[n]) and holds their left padding; a running slot forgets its past
+ *   w2l_stream_start    resets the n slots (host int slots[n]) and holds their left padding; a running slot forgets its
+ *                       past, its path included
  *   w2l_stream_run      slots[n], frames_in[n] (host ints, each <= Tc <= max_chunk), features device [n][1][nFeat][Tc]
  *                       (ArrayFire [Tc,nFeat,1,n], the trainer's layout); emissions device [n][T'max][nLabel] with
  *                       T'max = max frames_out, rows t >= frames_out[i] of stream i unspecified; capacity in floats;
@@ -689,6 +692,22 @@ W2L_API int w2l_trainer_export_streaming(void* trainer, void* stream, const char
  *                       slot stays finished until the next start.  Errors (W2L_ERR_INVALID_ARGUMENT): a slot out of range
  *                       or listed twice, a slot not started or already finished, a chunk longer than Tc, Tc > max_chunk,
  *                       too small a capacity.
+ *   w2l_stream_run_path   w2l_stream_run, then the criterion's viterbiPath of the call's output frames, carried per
+ *                       slot (w2l_stream_run is this call without a path).  path device int32 [n][P] with
+ *                       P = w2l_stream_max_path_out, path_capacity in ints (>= n * P); path_info device int32 [n][3]:
+ *                       {stream frame index of the first entry committed in this call, entries committed in this call,
+ *                       forced frames so far}.  emissions may be NULL (nothing is copied out; capacity is then unused).
+ *                       Per stream, the entries of every call and of finish put end to end are, bit for bit, the
+ *                       criterion's viterbiPath of its emissions put end to end, whatever the chunking and the other
+ *                       streams: CTC w2l_argmax_path (every frame commits at once); ASG / LinSeg w2l_fcc_viterbi (N <= 32)
+ *                       or w2l_fcc_viterbi64 (N <= 64), carried un-re-centred, committing each call every frame up to the
+ *                       newest one at which all N states' traced-back paths agree, and on finish the rest along the
+ *                       first-maximum end state.  The one exception: a slot holding more than 1024 uncommitted frames
+ *                       commits its oldest along the current first-maximum state's path, and counts them as forced.
+ *                       A path covers the output frames of the calls that asked for one.  Neither reads from the device
+ *                       nor synchronises.  W2L_ERR_UNSUPPORTED: the criterion has no streaming path (ASG / LinSeg over
+ *                       64 tokens); W2L_ERR_INVALID_ARGUMENT as w2l_stream_run, and a path_capacity below n * P.
+ *   w2l_stream_max_path_out  P: the most path entries one call can commit per stream (0: no streaming path)
  *   w2l_stream_plan     host only: the frame bookkeeping of one stream over n_calls calls of frames_host[k] frames (the
  *                       last one finishing when finish_last), for every convolution c of the arch: conv_spec_host
  *                       [c][4] = {kw, stride, pad_left, pad_right}, frames_out_host[k][max_convs] and tails_host
@@ -701,6 +720,10 @@ W2L_API int w2l_stream_max_frames_out(void* s);
 W2L_API int w2l_stream_start(void* s, void* stream, int n, const int* slots);
 W2L_API int w2l_stream_run(void* s, void* stream, int n, const int* slots, const int* frames_in, const float* features, int Tc, int finish,
                            float* emissions, long long capacity, int* frames_out);
+W2L_API int w2l_stream_run_path(void* s, void* stream, int n, const int* slots, const int* frames_in, const float* features, int Tc,
+                                int finish, float* emissions, long long capacity, int* frames_out, int32_t* path, long long path_capacity,
+                                int32_t* path_info);
+W2L_API int w2l_stream_max_path_out(void* s);
 W2L_API int w2l_stream_plan(const char* arch_text, int n_feat, int n_label, int n_calls, const int* frames_host, int finish_last,
                             int max_convs, int* n_convs, int* conv_spec_host, int* frames_out_host, int* tails_host);
 /* ----------------------------------------------------------------------------------------

@@ -42,7 +42,7 @@ EXPORTS = [
     "w2l_trainer_describe", "w2l_nccl_unique_id", "w2l_init_distributed", "w2l_trainer_align", "w2l_trainer_time_stride",
     "w2l_mfsc_num_frames", "w2l_mfsc_workspace_size", "w2l_mfsc",
     "w2l_stream_create", "w2l_stream_destroy", "w2l_stream_state_bytes", "w2l_stream_max_frames_out", "w2l_stream_start",
-    "w2l_stream_run", "w2l_stream_plan",
+    "w2l_stream_run", "w2l_stream_run_path", "w2l_stream_max_path_out", "w2l_stream_plan",
     "w2l_mfsc_stream_create", "w2l_mfsc_stream_destroy", "w2l_mfsc_stream_state_bytes", "w2l_mfsc_stream_max_frames_out",
     "w2l_mfsc_stream_start", "w2l_mfsc_stream_run",
     "w2l_seq2seq_check", "w2l_seq2seq_embed_fwd", "w2l_seq2seq_embed_bwd", "w2l_seq2seq_gru_stash_floats", "w2l_seq2seq_gru_fwd",
@@ -251,6 +251,8 @@ def _load() -> ctypes.CDLL:
     lib.w2l_stream_max_frames_out.argtypes = [vp]
     lib.w2l_stream_start.argtypes = [vp, vp, i, vp]
     lib.w2l_stream_run.argtypes = [vp, vp, i, vp, vp, vp, i, i, vp, ctypes.c_longlong, vp]
+    lib.w2l_stream_run_path.argtypes = [vp, vp, i, vp, vp, vp, i, i, vp, ctypes.c_longlong, vp, vp, ctypes.c_longlong, vp]
+    lib.w2l_stream_max_path_out.argtypes = [vp]
     lib.w2l_stream_plan.argtypes = [ctypes.c_char_p, i, i, i, vp, i, i, vp, vp, vp, vp]
     lib.w2l_mfsc_stream_create.restype = vp
     lib.w2l_mfsc_stream_create.argtypes = [vp, i, i, i, i, i, i, i]

@@ -6,18 +6,99 @@
 //   w2l_fac_viterbi : forced alignment (upstream ForceAlignmentCriterion::viterbiPath).
 //   w2l_argmax_path : CTCLoss::viterbiPath (per-frame argmax, first maximum wins).
 //   w2l_linseg_target: LinearSegmentationCriterion target stretch (Train.cpp:589-617).
+//   the streaming path (host/stream_capi.cpp, w2l_stream_run_path): the FCC Viterbi above carried across calls
+//                     with partial traceback, through the same per-frame step; CTC through argmax_path_kernel.
 // The file is compiled with -fmad=false: only adds and compares are on the value path, but the
 // flag makes the no-contraction guarantee explicit.
 #include <cuda_runtime.h>
 
 #include "common.cuh"
+#include "../host/stream_internal.h"
 
 namespace w2l {
 namespace {
 
 __host__ __device__ inline size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
 
-// ---- FCC Viterbi: one warp per sample, lane i = states i + 32 s (s < NW / 32) ------------------------------
+// ---- FCC Viterbi building blocks: lane i holds states i + 32 s (s < NW / 32) ----------------------------------
+// Both the batch decoder and the carried streaming path below take every frame through fcc_step, so their values and
+// backpointers are the same bits.
+template <int NW>
+__device__ __forceinline__ void fcc_load_trans(int N, int lane, const float* __restrict__ trans, float (&tr)[NW / 32][NW]) {
+#pragma unroll
+  for (int s = 0; s < NW / 32; ++s)
+#pragma unroll
+    for (int j = 0; j < NW; ++j) tr[s][j] = (lane + 32 * s < N && j < N) ? trans[(lane + 32 * s) * N + j] : kNegInf;
+}
+
+// one frame of the max-plus recursion: alpha_i <- max_j (alpha_j + trans[i][j]) + e_i, fp32 add then compare, j
+// ascending, strict '>' so the first maximum wins; state i's argmax j goes to bp[i].  vec: NW floats of shared memory
+// that no lane reads between the previous call and this one (callers alternate two buffers).
+template <int NW>
+__device__ __forceinline__ void fcc_step(int N, int lane, float (&alpha)[NW / 32], const float (&tr)[NW / 32][NW], const float (&e)[NW / 32],
+                                         float* vec, uint8_t* bp) {
+  constexpr int S = NW / 32;
+#pragma unroll
+  for (int s = 0; s < S; ++s) vec[lane + 32 * s] = alpha[s];
+  __syncwarp();
+  float best[S];
+  int arg[S];
+#pragma unroll
+  for (int s = 0; s < S; ++s) {
+    best[s] = kNegInf;
+    arg[s] = 0;
+  }
+  const float4* v4 = reinterpret_cast<const float4*>(vec);
+#pragma unroll
+  for (int q = 0; q < NW / 4; ++q) {
+    const float4 v = v4[q];
+    const float vv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const int j = 4 * q + r;
+      if (j < N) {
+#pragma unroll
+        for (int s = 0; s < S; ++s) {
+          const float val = __fadd_rn(vv[r], tr[s][j]);
+          if (val > best[s]) {
+            best[s] = val;
+            arg[s] = j;
+          }
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int s = 0; s < S; ++s) {
+    alpha[s] = __fadd_rn(best[s], e[s]);
+    bp[lane + 32 * s] = (uint8_t)arg[s];
+  }
+}
+
+// the first maximum over the N states (a lane's lower state first, then lanes), on every lane
+template <int NW>
+__device__ __forceinline__ int fcc_first_max(int N, int lane, const float (&alpha)[NW / 32]) {
+  float bv = lane < N ? alpha[0] : kNegInf;
+  int bi = lane;
+#pragma unroll
+  for (int s = 1; s < NW / 32; ++s)
+    if (lane + 32 * s < N && alpha[s] > bv) {
+      bv = alpha[s];
+      bi = lane + 32 * s;
+    }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (ov > bv || (ov == bv && oi < bi)) {
+      bv = ov;
+      bi = oi;
+    }
+  }
+  return bi;
+}
+
+// ---- FCC Viterbi: one warp per sample --------------------------------------------------------------------------
 // backpointers: uint8 [T][NW] in shared memory when they fit, else in the global workspace.
 // NW = 32 serves w2l_fcc_viterbi (N <= 32), NW = 64 w2l_fcc_viterbi64 (N <= 64); every state takes its candidates j in
 // ascending order with the same add and strict compare, so both widths are bit-exact with the reference.
@@ -34,71 +115,19 @@ __global__ void __launch_bounds__(32) fcc_viterbi_kernel(int T, int N, const flo
                            : bp_global + (size_t)b * T * NW;
   const float* eb = emis + (size_t)b * T * N;
   float tr[S][NW];
-#pragma unroll
-  for (int s = 0; s < S; ++s)
-#pragma unroll
-    for (int j = 0; j < NW; ++j) tr[s][j] = (lane + 32 * s < N && j < N) ? trans[(lane + 32 * s) * N + j] : kNegInf;
+  fcc_load_trans<NW>(N, lane, trans, tr);
   float alpha[S];
 #pragma unroll
   for (int s = 0; s < S; ++s) alpha[s] = lane + 32 * s < N ? eb[lane + 32 * s] : kNegInf;
   int buf = 0;
   for (int t = 1; t < T; ++t) {
+    float e[S];
 #pragma unroll
-    for (int s = 0; s < S; ++s) vec[buf * NW + lane + 32 * s] = alpha[s];
-    __syncwarp();
-    float e[S], best[S];
-    int arg[S];
-#pragma unroll
-    for (int s = 0; s < S; ++s) {
-      e[s] = lane + 32 * s < N ? eb[(size_t)t * N + lane + 32 * s] : kNegInf;
-      best[s] = kNegInf;
-      arg[s] = 0;
-    }
-    const float4* v4 = reinterpret_cast<const float4*>(vec + buf * NW);
-#pragma unroll
-    for (int q = 0; q < NW / 4; ++q) {
-      const float4 v = v4[q];
-      const float vv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-      for (int r = 0; r < 4; ++r) {
-        const int j = 4 * q + r;
-        if (j < N) {
-#pragma unroll
-          for (int s = 0; s < S; ++s) {
-            const float val = __fadd_rn(vv[r], tr[s][j]);
-            if (val > best[s]) {
-              best[s] = val;
-              arg[s] = j;
-            }
-          }
-        }
-      }
-    }
-#pragma unroll
-    for (int s = 0; s < S; ++s) {
-      alpha[s] = __fadd_rn(best[s], e[s]);
-      bp[(size_t)t * NW + lane + 32 * s] = (uint8_t)arg[s];
-    }
+    for (int s = 0; s < S; ++s) e[s] = lane + 32 * s < N ? eb[(size_t)t * N + lane + 32 * s] : kNegInf;
+    fcc_step<NW>(N, lane, alpha, tr, e, vec + buf * NW, bp + (size_t)t * NW);
     buf ^= 1;
   }
-  // final state: first maximum over states (a lane's lower state first, then lanes)
-  float bv = lane < N ? alpha[0] : kNegInf;
-  int bi = lane;
-#pragma unroll
-  for (int s = 1; s < S; ++s)
-    if (lane + 32 * s < N && alpha[s] > bv) {
-      bv = alpha[s];
-      bi = lane + 32 * s;
-    }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-    if (ov > bv || (ov == bv && oi < bi)) {
-      bv = ov;
-      bi = oi;
-    }
-  }
+  const int bi = fcc_first_max<NW>(N, lane, alpha);
   __syncwarp();
   int32_t* pb = path + (size_t)b * T;
   if (bp_in_smem) {
@@ -122,6 +151,120 @@ __global__ void __launch_bounds__(32) fcc_viterbi_kernel(int T, int N, const flo
         pb[t - 1] = pos;
       }
     }
+  }
+}
+
+// ---- the streaming path: FCC Viterbi carried across calls, with partial traceback (DESIGN.md §4) ----------------
+// One warp per stream.  A slot holds alpha (un-re-centred, as above), a header and a ring of the backpointers of its
+// pending frames (frames not yet committed; pending frame k lives in ring row (head + k) % ring).  The header's ints:
+// seen (the slot has had its first frame, whose alpha is its emissions), pending, head, committed, forced.
+constexpr int kSlotHeaderBytes = 32;
+
+template <int NW>
+__global__ void __launch_bounds__(32) stream_viterbi_kernel(const __grid_constant__ streaming::StreamPathArgs a) {
+  constexpr int S = NW / 32;
+  __shared__ __align__(16) float vec[2 * NW];
+  const int i = blockIdx.x, lane = threadIdx.x, N = a.N, R = a.ring;
+  unsigned char* slot = a.state + (size_t)a.slot[i] * a.slotBytes;
+  float* alpha_g = reinterpret_cast<float*>(slot);
+  int* hdr = reinterpret_cast<int*>(slot + 4 * NW);
+  uint8_t* ring = slot + 4 * NW + kSlotHeaderBytes;
+  int seen = hdr[0], pending = hdr[1], head = hdr[2];
+  const int committed = hdr[3];
+  int forced = hdr[4];
+  float tr[S][NW];
+  fcc_load_trans<NW>(N, lane, a.trans, tr);
+  float alpha[S];
+#pragma unroll
+  for (int s = 0; s < S; ++s) alpha[s] = alpha_g[lane + 32 * s];
+  // 1. advance alpha over the new frames, appending their backpointers
+  const float* eb = a.emis + (size_t)i * a.T * N;
+  const int fresh = a.frames[i];
+  int buf = 0;
+  for (int t = 0; t < fresh; ++t) {
+    float e[S];
+#pragma unroll
+    for (int s = 0; s < S; ++s) e[s] = lane + 32 * s < N ? eb[(size_t)t * N + lane + 32 * s] : kNegInf;
+    if (seen) {
+      fcc_step<NW>(N, lane, alpha, tr, e, vec + buf * NW, ring + (size_t)((head + pending) % R) * NW);
+      buf ^= 1;
+    } else {  // the stream's first frame: its backpointers are never read
+#pragma unroll
+      for (int s = 0; s < S; ++s) alpha[s] = e[s];
+      seen = 1;
+    }
+    ++pending;
+  }
+#pragma unroll
+  for (int s = 0; s < S; ++s) alpha_g[lane + 32 * s] = alpha[s];
+  __syncwarp();  // the ring rows each lane wrote are read by the others from here on
+  int32_t* out = a.path + (size_t)i * a.P;
+  int done = 0;
+  // frames 0 .. count - 1 of the pending ones, frame count - 1 in state `last`; lane 0 traces back and writes them
+  auto commit = [&](int count, int last) {
+    if (lane == 0) {
+      int st = last;
+      for (int k = count - 1; k >= 0; --k) {
+        out[done + k] = st;
+        if (k > 0) st = ring[(size_t)((head + k) % R) * NW + st];
+      }
+    }
+    head = (head + count) % R;
+    pending -= count;
+    done += count;
+  };
+  // 2. trace every state back to the newest frame at which all N agree: every frame up to it is on the final path
+  if (pending > 0) {
+    int pos[S];
+#pragma unroll
+    for (int s = 0; s < S; ++s) pos[s] = lane + 32 * s;
+    for (int k = pending - 1; k >= 0; --k) {
+      const int first = __shfl_sync(0xffffffffu, pos[0], 0);
+      bool same = true;
+#pragma unroll
+      for (int s = 0; s < S; ++s) same = same && (lane + 32 * s >= N || pos[s] == first);
+      if (__ballot_sync(0xffffffffu, same) == 0xffffffffu) {
+        commit(k + 1, first);
+        break;
+      }
+      if (k == 0) break;
+      const uint8_t* row = ring + (size_t)((head + k) % R) * NW;
+#pragma unroll
+      for (int s = 0; s < S; ++s)
+        if (lane + 32 * s < N) pos[s] = row[pos[s]];
+    }
+  }
+  // 3. finish: everything along the first-maximum end state's path; otherwise, past the bound, the oldest frames along it
+  if (pending > 0 && (a.finish || pending > a.maxPending)) {
+    const int count = a.finish ? pending : pending - a.maxPending;
+    int st = fcc_first_max<NW>(N, lane, alpha);
+    if (lane == 0)
+      for (int k = pending - 1; k >= count; --k) st = ring[(size_t)((head + k) % R) * NW + st];
+    st = __shfl_sync(0xffffffffu, st, 0);
+    if (!a.finish) forced += count;
+    commit(count, st);
+  }
+  if (lane == 0) {
+    a.info[3 * i] = committed;
+    a.info[3 * i + 1] = done;
+    a.info[3 * i + 2] = forced;
+    hdr[0] = seen;
+    hdr[1] = pending;
+    hdr[2] = head;
+    hdr[3] = committed + done;
+    hdr[4] = forced;
+  }
+}
+
+// CTC: every output frame commits at once; argmax_path_kernel's rows [n][T] go to path [n][P]
+__global__ void __launch_bounds__(256) stream_place_kernel(const __grid_constant__ streaming::StreamPlaceArgs a) {
+  const int i = blockIdx.y;
+  const int f = a.frames[i];
+  for (int k = blockIdx.x * blockDim.x + threadIdx.x; k < f; k += gridDim.x * blockDim.x) a.path[(size_t)i * a.P + k] = a.rows[(size_t)i * a.T + k];
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    a.info[3 * i] = a.base[i];
+    a.info[3 * i + 1] = f;
+    a.info[3 * i + 2] = 0;
   }
 }
 
@@ -357,3 +500,38 @@ extern "C" int w2l_linseg_target(void* stream_, int B, int T, int L, const int32
   W2L_LAUNCH_CHECK("linseg_target_kernel");
   return W2L_OK;
 }
+
+namespace w2l {
+namespace streaming {
+
+size_t streamViterbiSlotBytes(int nw, int ring) { return align16((size_t)4 * nw + kSlotHeaderBytes + (size_t)ring * nw); }
+
+int launchStreamViterbi(void* stream_, int nw, const StreamPathArgs& a) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (a.n <= 0 || a.n > kMaxCallStreams || a.N <= 0 || a.N > nw || (nw != 32 && nw != 64) || a.ring <= a.maxPending)
+    return fail(W2L_ERR_INVALID_ARGUMENT, "stream viterbi: bad sizes");
+  if (nw == 32)
+    stream_viterbi_kernel<32><<<a.n, 32, 0, stream>>>(a);
+  else
+    stream_viterbi_kernel<64><<<a.n, 32, 0, stream>>>(a);
+  W2L_LAUNCH_CHECK("stream_viterbi_kernel");
+  return W2L_OK;
+}
+
+int launchStreamArgmax(void* stream_, int N, const float* emis, const StreamPlaceArgs& a) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (a.n <= 0 || a.n > kMaxCallStreams || N <= 0 || a.T < 0) return fail(W2L_ERR_INVALID_ARGUMENT, "stream argmax: bad sizes");
+  if (a.T > 0) {
+    const long long nframes = (long long)a.n * a.T;
+    const int blocks = (int)std::min<long long>((nframes + 7) / 8, sm_count() * 8);
+    argmax_path_kernel<<<blocks, 256, 0, stream>>>(nframes, N, emis, a.rows);
+    W2L_LAUNCH_CHECK("argmax_path_kernel");
+  }
+  dim3 grid((unsigned)std::max(1, std::min((a.T + 255) / 256, 16)), (unsigned)a.n);
+  stream_place_kernel<<<grid, 256, 0, stream>>>(a);
+  W2L_LAUNCH_CHECK("stream_place_kernel");
+  return W2L_OK;
+}
+
+}  // namespace streaming
+}  // namespace w2l

@@ -11,7 +11,9 @@
 // depends on the other streams in the call, and a stream's emissions must not).  Rows past a
 // stream's valid frames are slack: computed, finite, never read as data (every layer after a convolution is per
 // frame).  All frame counts follow from integer arithmetic on the host, so a call neither reads from the device nor
-// synchronises.  DESIGN.md §4.
+// synchronises.  w2l_stream_run_path then runs the criterion's viterbiPath over the call's output (CTC argmax; ASG /
+// LinSeg FCC Viterbi carried per slot, csrc/criterion_viterbi.cu), so a caller can take tokens instead of emissions.
+// DESIGN.md §4.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -115,6 +117,9 @@ using namespace w2l::streaming;
 
 namespace {
 namespace dense = w2l::dense;
+// Pending frames a slot's FCC Viterbi may hold before its oldest are committed along the best path (DESIGN.md §4)
+constexpr int kMaxPendingFrames = 1024;
+enum class PathKind { None, Ctc, Fcc };
 long long up4(long long n) { return (n + 3) / 4 * 4; }
 
 // a Linear layer: its weight as the forward GEMM's B operand, made once at create
@@ -151,6 +156,15 @@ struct Stream {
   void* convWs = nullptr;
   size_t convWsBytes = 0;
   int maxOut = 0;  // bound on the output frames of one call
+  // the criterion's path (w2l_stream_run_path): CTC places argmax rows, ASG / LinSeg carry FCC Viterbi in pathState
+  PathKind pathKind = PathKind::None;
+  int pathNW = 0;                      // FCC: states per warp, 32 or 64
+  int maxPathOut = 0;                  // path entries one call can commit per stream
+  float* trans = nullptr;              // FCC: the criterion's N x N transitions, copied at create
+  unsigned char* pathState = nullptr;  // FCC: [slot][pathSlotBytes]
+  long long pathSlotBytes = 0;
+  int32_t* argmaxRows = nullptr;       // CTC: [max_streams][maxOut]
+  std::vector<int> ctcCommitted;       // CTC: per slot, frames the path has been given since start
 };
 
 // C[M][nout] = act(A[M][nin] W^T + bias)
@@ -163,6 +177,139 @@ void linear(Stream* s, cudaStream_t st, const DenseLayer& d, long long M, const 
 // count, which depends on the other streams in the call, and the two kernels round mean / rstd differently
 void layerNorm(Stream* s, cudaStream_t st, long long rows, int F, const float* a, const float* r, const float* gain, const float* bias, float* y) {
   w2l::check(w2l_layernorm_rows_fwd(st, rows, F, 1e-5f, a, r, gain, bias, y, s->meanRstd));
+}
+// One call: the network over every stream's new frames, then, when path is set, the criterion's path of its output.
+// emissions may be null when path is set; the output then stays in the activation buffers.
+void runStream(void* h, void* stream, int n, const int* slots, const int* frames_in, const float* features, int Tc, int finish, float* emissions,
+               long long capacity, int* frames_out, int32_t* path, long long path_capacity, int32_t* path_info) {
+  Stream* s = handleOf<Stream>(h, "stream");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  s->slots.check(n, slots, true);
+  if (!frames_in || !frames_out) throw std::invalid_argument("stream_run: null frame-count array");
+  if (Tc < 0 || Tc > s->maxChunk) throw std::invalid_argument("stream_run: Tc must be in [0, max_chunk]");
+  int most = 0;
+  for (int i = 0; i < n; ++i) {
+    if (frames_in[i] < 0 || frames_in[i] > Tc)
+      throw std::invalid_argument("stream_run: the chunk of slot " + std::to_string(slots[i]) + " is longer than Tc (or negative)");
+    most = std::max(most, frames_in[i]);
+  }
+  if (most > 0 && !features) throw std::invalid_argument("stream_run: null features");
+  const int W = s->nFeat;
+  const Plan p = s->slots.plan(n, slots, frames_in, finish != 0);
+  if (emissions && (long long)n * p.tOutMax * s->nLabel > capacity) throw std::invalid_argument("stream_run: emission buffer too small (capacity)");
+  if (p.tOutMax > 0 && !emissions && !path) throw std::invalid_argument("stream_run: null emissions");
+  if (!path != !path_info) throw std::invalid_argument("stream_run_path: path and path_info go together");
+  if (path && path_capacity < (long long)n * s->maxPathOut) throw std::invalid_argument("stream_run_path: path buffer too small (path_capacity)");
+  PrecisionScope scope(s->precision);
+  // [n][1][F][Tc] (ArrayFire [Tc,F,1,n]) -> [n][Tc][F]: frames of W groups of one channel
+  if (most > 0) w2l::check(w2l_transpose_input(st, n, W, Tc, features, s->xT));
+  const float* cur = s->xT;
+  int curFrames = Tc;  // frame stride of every stream in `cur`
+  bool live = true;    // the padded batch has frames
+  auto pick = [&](std::initializer_list<const float*> busy) {
+    for (float* a : s->act)
+      if (std::find(busy.begin(), busy.end(), a) == busy.end()) return a;
+    throw std::logic_error("stream: no free activation buffer");
+  };
+  const auto& layers = s->arch.layers;
+  size_t ci = 0;  // the convolution's index among the state buffers
+  for (size_t li = 0; li < layers.size(); ++li) {
+    const Layer& l = layers[li];
+    const int feat = l.curC * W;
+    if (l.op == Op::Conv || l.op == Op::Tds) {
+      const int win = p.winFrames[ci], tout = p.outFrames[ci];
+      if (win > 0) w2l::check(launchWindow(st, s->slots.window(p, ci, cur, curFrames, s->win, win)));
+      ++ci;
+      live = tout > 0;
+      curFrames = tout;
+      if (!live) continue;
+      const size_t pidx = s->paramBase[li];
+      const float* w = s->params[pidx];
+      const float* b = s->params[pidx + 1];
+      const long long rows = (long long)n * tout;
+      const int fout = l.cout * W;
+      if (l.op == Op::Conv) {
+        // a ReLU right after the convolution runs in its epilogue, as in the training network
+        const bool relu = li + 1 < layers.size() && layers[li + 1].op == Op::Relu;
+        float* y = pick({cur});
+        w2l::check(w2l_conv_time_fwd(st, n, win, tout, W, l.cin, l.cout, l.kw, l.stride, 0, s->win, w, b, nullptr, y, relu ? 1 : 0, 0.f, 0ull,
+                                     s->convWs, s->convWsBytes));
+        cur = y;
+        if (relu) ++li;
+        continue;
+      }
+      // TDS: LN1(x + relu(conv x)) -> LN2(z + W2 relu(W1 z + b1) + b2); the residual x of output frame j is window
+      // frame j + padL (the convolution reads frames j .. j + kw - 1 of the window)
+      float* y1 = pick({cur});
+      w2l::check(w2l_conv_time_fwd(st, n, win, tout, W, l.cin, l.cout, l.kw, 1, 0, s->win, w, b, nullptr, y1, 1, 0.f, 0ull, s->convWs, s->convWsBytes));
+      float* res = pick({cur, y1});
+      cuda(cudaMemcpy2DAsync(res, sizeof(float) * (size_t)tout * feat, s->win + (size_t)l.padL * feat, sizeof(float) * (size_t)win * feat,
+                             sizeof(float) * (size_t)tout * feat, (size_t)n, cudaMemcpyDeviceToDevice, st),
+           "stream: residual");
+      float* z = pick({cur, y1, res});
+      layerNorm(s, st, rows, fout, y1, res, s->params[pidx + 2], s->params[pidx + 3], z);
+      linear(s, st, s->dense[s->denseOf[li]], rows, z, s->hidden, 1);
+      linear(s, st, s->dense[s->denseOf[li] + 1], rows, s->hidden, y1, 0);
+      layerNorm(s, st, rows, fout, y1, z, s->params[pidx + 8], s->params[pidx + 9], res);
+      cur = res;
+      continue;
+    }
+    if (!live) continue;
+    const long long rows = (long long)n * curFrames;
+    const size_t pidx = s->paramBase[li];
+    if (l.op == Op::Relu) {
+      float* y = pick({cur});
+      w2l::check(w2l_act_fwd(st, rows * feat, cur, 1, 0.f, 0ull, y));
+      cur = y;
+    } else if (l.op == Op::LayerNorm) {
+      float* y = pick({cur});
+      layerNorm(s, st, rows, feat, cur, nullptr, s->params[pidx], s->params[pidx + 1], y);
+      cur = y;
+    } else if (l.op == Op::Linear) {
+      float* y = li + 1 == layers.size() && emissions ? emissions : pick({cur});
+      linear(s, st, s->dense[s->denseOf[li]], rows, cur, y, 0);
+      cur = y;
+    }
+  }
+  if (live && emissions && cur != emissions)
+    cuda(cudaMemcpyAsync(emissions, cur, sizeof(float) * (size_t)n * p.tOutMax * s->nLabel, cudaMemcpyDeviceToDevice, st), "stream: emissions");
+  // the criterion's path over the call's [n][T'max][N] emissions in `cur` (rows t >= framesOut[i] are not read)
+  if (path && s->pathKind == PathKind::Ctc) {
+    StreamPlaceArgs a;
+    a.rows = s->argmaxRows;
+    a.path = path;
+    a.info = path_info;
+    a.T = live ? p.tOutMax : 0;
+    a.P = s->maxPathOut;
+    a.n = n;
+    for (int i = 0; i < n; ++i) {
+      a.frames[i] = p.framesOut[i];
+      a.base[i] = s->ctcCommitted[slots[i]];
+    }
+    w2l::check(launchStreamArgmax(st, s->nLabel, cur, a));
+    for (int i = 0; i < n; ++i) s->ctcCommitted[slots[i]] += p.framesOut[i];
+  } else if (path) {
+    StreamPathArgs a;
+    a.emis = cur;
+    a.trans = s->trans;
+    a.state = s->pathState;
+    a.slotBytes = s->pathSlotBytes;
+    a.path = path;
+    a.info = path_info;
+    a.T = live ? p.tOutMax : 0;
+    a.N = s->nLabel;
+    a.P = s->maxPathOut;
+    a.n = n;
+    a.finish = finish ? 1 : 0;
+    a.maxPending = kMaxPendingFrames;
+    a.ring = s->maxPathOut;
+    for (int i = 0; i < n; ++i) {
+      a.slot[i] = slots[i];
+      a.frames[i] = live ? p.framesOut[i] : 0;
+    }
+    w2l::check(launchStreamViterbi(st, s->pathNW, a));
+  }
+  s->slots.commit(p, frames_out);
 }
 }  // namespace
 
@@ -207,6 +354,7 @@ W2L_API void* w2l_stream_create(void* trainer, void* stream, int max_streams, in
     if (max_chunk <= 0 || max_chunk > 32767) throw std::invalid_argument("stream_create: max_chunk must be in [1, 32767] frames");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const TrainerSnapshotSource src = trainerSnapshotSource(trainer);
+    if (src.criterion == "seq2seq") throw std::invalid_argument("stream_create: the seq2seq criterion has no streaming model");
     auto s = std::make_unique<Stream>();
     s->arch = parseArch(src.arch, src.nFeat, src.nLabel);
     s->slots = SlotTable("stream", max_streams, convBuffers(s->arch));
@@ -292,6 +440,22 @@ W2L_API void* w2l_stream_create(void* trainer, void* stream, int max_streams, in
     if (ci == 0) throw std::invalid_argument("stream_create: the arch has no convolution, nothing to stream");
     if (feat != src.nLabel) throw std::invalid_argument("stream_create: the last layer does not produce NLABEL values per frame");
     s->maxOut = fresh;
+    // the criterion: CTC needs no slot state; ASG / LinSeg over up to 64 tokens carry their Viterbi per slot
+    if (src.criterion == "ctc") {
+      s->pathKind = PathKind::Ctc;
+      s->maxPathOut = s->maxOut;
+      s->argmaxRows = s->mem.alloc<int32_t>((size_t)max_streams * s->maxOut);
+      s->ctcCommitted.assign(max_streams, 0);
+    } else if ((src.criterion == "asg" || src.criterion == "linseg") && src.trans && src.nLabel <= 64) {
+      s->pathKind = PathKind::Fcc;
+      s->pathNW = src.nLabel <= 32 ? 32 : 64;
+      s->maxPathOut = kMaxPendingFrames + s->maxOut;
+      s->pathSlotBytes = (long long)streamViterbiSlotBytes(s->pathNW, s->maxPathOut);
+      s->pathState = s->mem.alloc<unsigned char>((size_t)max_streams * s->pathSlotBytes);
+      s->trans = s->mem.alloc<float>((size_t)src.nLabel * src.nLabel);
+      cuda(cudaMemcpyAsync(s->trans, src.trans, sizeof(float) * (size_t)src.nLabel * src.nLabel, cudaMemcpyDeviceToDevice, st), "stream: transitions");
+      cuda(cudaMemsetAsync(s->pathState, 0, (size_t)max_streams * s->pathSlotBytes, st), "stream: path state");
+    }
     // state and per-call buffers, all up front
     s->slots.state = s->mem.alloc<float>((size_t)max_streams * (size_t)s->slots.slotFloats());
     s->xT = s->mem.alloc<float>((size_t)max_streams * max_chunk * W);
@@ -314,7 +478,13 @@ W2L_API void w2l_stream_destroy(void* h) { delete static_cast<Stream*>(h); }
 
 W2L_API long long w2l_stream_state_bytes(void* h) {
   if (!h) return -1;
-  return (long long)sizeof(float) * static_cast<Stream*>(h)->slots.slotFloats();
+  const Stream* s = static_cast<Stream*>(h);
+  return (long long)sizeof(float) * s->slots.slotFloats() + s->pathSlotBytes;
+}
+
+W2L_API int w2l_stream_max_path_out(void* h) {
+  if (!h) return -1;
+  return static_cast<Stream*>(h)->maxPathOut;
 }
 
 W2L_API int w2l_stream_max_frames_out(void* h) {
@@ -327,104 +497,22 @@ W2L_API int w2l_stream_start(void* h, void* stream, int n, const int* slots) {
     Stream* s = handleOf<Stream>(h, "stream");
     s->slots.check(n, slots, false);
     w2l::check(launchZeroSlots(stream, s->slots.state, s->slots.slotFloats(), n, slots));
+    if (s->pathState) w2l::check(launchZeroSlots(stream, reinterpret_cast<float*>(s->pathState), s->pathSlotBytes / 4, n, slots));
+    for (int i = 0; i < n && !s->ctcCommitted.empty(); ++i) s->ctcCommitted[slots[i]] = 0;
     s->slots.start(n, slots);
   });
 }
 
 W2L_API int w2l_stream_run(void* h, void* stream, int n, const int* slots, const int* frames_in, const float* features, int Tc, int finish,
                            float* emissions, long long capacity, int* frames_out) {
-  return guarded([&] {
-    Stream* s = handleOf<Stream>(h, "stream");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    s->slots.check(n, slots, true);
-    if (!frames_in || !frames_out) throw std::invalid_argument("stream_run: null frame-count array");
-    if (Tc < 0 || Tc > s->maxChunk) throw std::invalid_argument("stream_run: Tc must be in [0, max_chunk]");
-    int most = 0;
-    for (int i = 0; i < n; ++i) {
-      if (frames_in[i] < 0 || frames_in[i] > Tc)
-        throw std::invalid_argument("stream_run: the chunk of slot " + std::to_string(slots[i]) + " is longer than Tc (or negative)");
-      most = std::max(most, frames_in[i]);
-    }
-    if (most > 0 && !features) throw std::invalid_argument("stream_run: null features");
-    const int W = s->nFeat;
-    const Plan p = s->slots.plan(n, slots, frames_in, finish != 0);
-    if ((long long)n * p.tOutMax * s->nLabel > capacity) throw std::invalid_argument("stream_run: emission buffer too small (capacity)");
-    if (p.tOutMax > 0 && !emissions) throw std::invalid_argument("stream_run: null emissions");
-    PrecisionScope scope(s->precision);
-    // [n][1][F][Tc] (ArrayFire [Tc,F,1,n]) -> [n][Tc][F]: frames of W groups of one channel
-    if (most > 0) w2l::check(w2l_transpose_input(st, n, W, Tc, features, s->xT));
-    const float* cur = s->xT;
-    int curFrames = Tc;  // frame stride of every stream in `cur`
-    bool live = true;    // the padded batch has frames
-    auto pick = [&](std::initializer_list<const float*> busy) {
-      for (float* a : s->act)
-        if (std::find(busy.begin(), busy.end(), a) == busy.end()) return a;
-      throw std::logic_error("stream: no free activation buffer");
-    };
-    const auto& layers = s->arch.layers;
-    size_t ci = 0;  // the convolution's index among the state buffers
-    for (size_t li = 0; li < layers.size(); ++li) {
-      const Layer& l = layers[li];
-      const int feat = l.curC * W;
-      if (l.op == Op::Conv || l.op == Op::Tds) {
-        const int win = p.winFrames[ci], tout = p.outFrames[ci];
-        if (win > 0) w2l::check(launchWindow(st, s->slots.window(p, ci, cur, curFrames, s->win, win)));
-        ++ci;
-        live = tout > 0;
-        curFrames = tout;
-        if (!live) continue;
-        const size_t pidx = s->paramBase[li];
-        const float* w = s->params[pidx];
-        const float* b = s->params[pidx + 1];
-        const long long rows = (long long)n * tout;
-        const int fout = l.cout * W;
-        if (l.op == Op::Conv) {
-          // a ReLU right after the convolution runs in its epilogue, as in the training network
-          const bool relu = li + 1 < layers.size() && layers[li + 1].op == Op::Relu;
-          float* y = pick({cur});
-          w2l::check(w2l_conv_time_fwd(st, n, win, tout, W, l.cin, l.cout, l.kw, l.stride, 0, s->win, w, b, nullptr, y, relu ? 1 : 0, 0.f, 0ull,
-                                       s->convWs, s->convWsBytes));
-          cur = y;
-          if (relu) ++li;
-          continue;
-        }
-        // TDS: LN1(x + relu(conv x)) -> LN2(z + W2 relu(W1 z + b1) + b2); the residual x of output frame j is window
-        // frame j + padL (the convolution reads frames j .. j + kw - 1 of the window)
-        float* y1 = pick({cur});
-        w2l::check(w2l_conv_time_fwd(st, n, win, tout, W, l.cin, l.cout, l.kw, 1, 0, s->win, w, b, nullptr, y1, 1, 0.f, 0ull, s->convWs, s->convWsBytes));
-        float* res = pick({cur, y1});
-        cuda(cudaMemcpy2DAsync(res, sizeof(float) * (size_t)tout * feat, s->win + (size_t)l.padL * feat, sizeof(float) * (size_t)win * feat,
-                               sizeof(float) * (size_t)tout * feat, (size_t)n, cudaMemcpyDeviceToDevice, st),
-             "stream: residual");
-        float* z = pick({cur, y1, res});
-        layerNorm(s, st, rows, fout, y1, res, s->params[pidx + 2], s->params[pidx + 3], z);
-        linear(s, st, s->dense[s->denseOf[li]], rows, z, s->hidden, 1);
-        linear(s, st, s->dense[s->denseOf[li] + 1], rows, s->hidden, y1, 0);
-        layerNorm(s, st, rows, fout, y1, z, s->params[pidx + 8], s->params[pidx + 9], res);
-        cur = res;
-        continue;
-      }
-      if (!live) continue;
-      const long long rows = (long long)n * curFrames;
-      const size_t pidx = s->paramBase[li];
-      if (l.op == Op::Relu) {
-        float* y = pick({cur});
-        w2l::check(w2l_act_fwd(st, rows * feat, cur, 1, 0.f, 0ull, y));
-        cur = y;
-      } else if (l.op == Op::LayerNorm) {
-        float* y = pick({cur});
-        layerNorm(s, st, rows, feat, cur, nullptr, s->params[pidx], s->params[pidx + 1], y);
-        cur = y;
-      } else if (l.op == Op::Linear) {
-        float* y = li + 1 == layers.size() ? emissions : pick({cur});
-        linear(s, st, s->dense[s->denseOf[li]], rows, cur, y, 0);
-        cur = y;
-      }
-    }
-    if (live && cur != emissions)
-      cuda(cudaMemcpyAsync(emissions, cur, sizeof(float) * (size_t)n * p.tOutMax * s->nLabel, cudaMemcpyDeviceToDevice, st), "stream: emissions");
-    s->slots.commit(p, frames_out);
-  });
+  return guarded([&] { runStream(h, stream, n, slots, frames_in, features, Tc, finish, emissions, capacity, frames_out, nullptr, 0, nullptr); });
+}
+
+W2L_API int w2l_stream_run_path(void* h, void* stream, int n, const int* slots, const int* frames_in, const float* features, int Tc, int finish,
+                                float* emissions, long long capacity, int* frames_out, int32_t* path, long long path_capacity, int32_t* path_info) {
+  if (h && (path || path_info) && static_cast<Stream*>(h)->pathKind == PathKind::None)
+    return w2l::fail(W2L_ERR_UNSUPPORTED, "stream_run_path: the criterion has no streaming path (CTC, or ASG / LinSeg over at most 64 tokens)");
+  return guarded([&] { runStream(h, stream, n, slots, frames_in, features, Tc, finish, emissions, capacity, frames_out, path, path_capacity, path_info); });
 }
 
 }  // extern "C"

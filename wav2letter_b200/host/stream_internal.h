@@ -7,6 +7,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cstdint>
 #include <stdexcept>
 #include <string>
 #include <utility>
@@ -82,11 +83,13 @@ struct Arch {
 // Walks the arch text with the export's checks and error text (std::invalid_argument / std::logic_error).
 Arch parseArch(const std::string& archText, int nFeat, int nLabel);
 
-// what the stream runtime needs of a trainer: the arch, the sizes, the precision and the parameters in module order
+// what the stream runtime needs of a trainer: the arch, the sizes, the precision, the parameters in module order and the
+// criterion ("ctc", "asg", "linseg" or "seq2seq") with its N x N transitions (ASG / LinSeg, else null)
 struct TrainerSnapshotSource {
-  std::string arch;
+  std::string arch, criterion;
   int nFeat = 0, nLabel = 0, precision = 0;
   std::vector<std::pair<const float*, long long>> params;  // device pointer, elements
+  const float* trans = nullptr;
 };
 TrainerSnapshotSource trainerSnapshotSource(void* trainer);
 
@@ -104,6 +107,38 @@ struct WindowArgs {
 int launchWindow(void* stream, const WindowArgs& a);
 // zero both planes of the n slots' state (slotFloats each): start
 int launchZeroSlots(void* stream, float* state, long long slotFloats, int n, const int* slots);
+
+// ---- the criterion's path of the streaming acoustic model (csrc/criterion_viterbi.cu) ---------------------------
+// ASG / LinSeg: the FCC Viterbi recursion carried across calls, one warp per stream, NW = 32 or 64 states per warp.  A
+// slot is streamViterbiSlotBytes(NW, ring) bytes (zero = started): alpha, a header and a ring of `ring` rows of NW
+// backpointers, ring >= maxPending + the most frames one call brings.  Per stream the call appends frames[i] frames
+// of emis, commits every frame all states' paths agree on, then on finish the rest along the first-maximum end state,
+// otherwise, past maxPending pending frames, the oldest ones along it (counted as forced).  The committed labels go to
+// path[i][0..), {first committed frame, committed, forced so far} to info[i][3].
+struct StreamPathArgs {
+  const float* emis;   // [n][T][N]
+  const float* trans;  // [N][N], trans[to][from]
+  unsigned char* state;
+  long long slotBytes;
+  int32_t* path;  // [n][P]
+  int32_t* info;  // [n][3]
+  int T, N, P, n, finish, maxPending, ring;
+  int slot[kMaxCallStreams];
+  int frames[kMaxCallStreams];
+};
+size_t streamViterbiSlotBytes(int nw, int ring);
+int launchStreamViterbi(void* stream, int nw, const StreamPathArgs& a);
+// CTC: argmax_path_kernel over the n * T rows of emis into rows, then each stream's frames[i] labels to path[i][0..)
+// and {base[i], frames[i], 0} to info[i][3]
+struct StreamPlaceArgs {
+  int32_t* rows;  // [n][T]
+  int32_t* path;  // [n][P]
+  int32_t* info;  // [n][3]
+  int T, P, n;
+  int frames[kMaxCallStreams];
+  int base[kMaxCallStreams];
+};
+int launchStreamArgmax(void* stream, int N, const float* emis, const StreamPlaceArgs& a);
 
 // ---- the slot model of both streaming runtimes (host/stream_slots.cpp) -----------------------------------------
 // One state buffer: a convolution's input frames of F floats, held under the buffer rule of

@@ -210,6 +210,12 @@ w2l::streaming::TrainerSnapshotSource w2l::streaming::trainerSnapshotSource(void
   s.nLabel = t->nLabel;
   s.precision = t->precision;
   for (auto& p : t->net->params()) s.params.emplace_back(p.array().f32(), p.elements());
+  s.criterion = t->critName;
+  if (!t->isCtc && !t->s2s) {  // ASG, and LinSeg sharing its transitions: the first parameter in the criterion arena
+    auto cp = t->crit->params();
+    if (cp.empty() || cp[0].elements() != (long long)t->nLabel * t->nLabel) throw std::runtime_error("stream: invalid criterion parameters for ASG");
+    s.trans = cp[0].array().f32();
+  }
   return s;
 }
 

@@ -4,8 +4,10 @@
 A trained streaming TDS network run chunk by chunk over many concurrent streams, as the in-tree inference library
 runs it.  Per stream, the emissions of every `run` and of `finish`, put end to end, do not change by a bit with the
 chunking or with the other streams in a call, and match the eval-mode `Trainer.forward` of the whole utterance in
-frame count and up to the rounding of the LayerNorm statistics.  The harness owns the tensors; the frame arithmetic
-and every kernel run inside libw2l_b200.so.
+frame count and up to the rounding of the LayerNorm statistics.  `run(..., path=True)` also gives each stream its
+criterion's viterbiPath, committed chunk by chunk (CTC argmax; ASG / LinSeg FCC Viterbi carried across calls), which
+TextPipeline turns into letters and words like a whole-utterance path.  The harness owns the tensors; the frame
+arithmetic and every kernel run inside libw2l_b200.so.
 """
 from __future__ import annotations
 
@@ -91,9 +93,16 @@ class StreamingAM(_StreamHandle):
         self.n_label = trainer.n_label
         self._open(h)
 
-    def run(self, slots, features: torch.Tensor | None = None, frames=None, finish: bool = False):
+    def run(self, slots, features: torch.Tensor | None = None, frames=None, finish: bool = False, path: bool = False, emissions: bool = True):
         """features: CUDA float [n,1,F,Tc] contiguous (the trainer's layout), frames: valid frames per stream (default
-        Tc).  Returns (emissions [n,T'max,N], frames_out list): rows t >= frames_out[i] of stream i are unspecified."""
+        Tc).  Returns (emissions [n,T'max,N], frames_out list): rows t >= frames_out[i] of stream i are unspecified.
+
+        path=True also runs the criterion's viterbiPath, carried per slot (w2l_stream_run_path), and returns (emissions,
+        frames_out, path, path_info): path CUDA int32 [n, max_path_out], of which stream i committed its first
+        path_info[i, 1] entries in this call, path_info CUDA int32 [n, 3] = {stream frame index of the first entry
+        committed in this call, entries committed, forced frames so far}.  Per stream the committed entries of every
+        call put end to end are the criterion's viterbiPath of its emissions put end to end (forced frames aside).
+        emissions=False (with path=True) copies no emissions out and returns None in their place."""
         n = len(slots)
         if features is None:
             Tc, fptr = 0, None
@@ -101,8 +110,29 @@ class StreamingAM(_StreamHandle):
             if not features.is_cuda or features.dtype != torch.float32 or not features.is_contiguous() or features.shape[0] != n:
                 raise TypeError("features must be a contiguous CUDA float32 tensor [n,1,F,Tc]")
             Tc, fptr = int(features.shape[3]), _ptr(features)
-        out, tmax, frames_out = self._run(slots, fptr, Tc, frames, finish, self.n_label)
-        return out.view(n, tmax, self.n_label), frames_out
+        if not path:
+            if not emissions:
+                raise ValueError("run: emissions=False needs path=True")
+            out, tmax, frames_out = self._run(slots, fptr, Tc, frames, finish, self.n_label)
+            return out.view(n, tmax, self.n_label), frames_out
+        counts = [Tc] * n if frames is None else frames
+        cap = n * self.max_frames_out * self.n_label if emissions else 0
+        out = torch.empty(max(cap, 1), dtype=torch.float32, device="cuda") if emissions else None
+        P = self.max_path_out
+        p = torch.empty((n, max(P, 1)), dtype=torch.int32, device="cuda")
+        info = torch.empty((n, 3), dtype=torch.int32, device="cuda")
+        fo = (ctypes.c_int * n)()
+        _check(lib.w2l_stream_run_path(self.h, _stream(), n, _ints(slots), _ints(counts), fptr, Tc, int(finish), _ptr(out) if emissions else None, cap,
+                                       fo, _ptr(p), n * P, _ptr(info)))
+        frames_out = list(fo)
+        tmax = max(frames_out) if frames_out else 0
+        e = out[: n * tmax * self.n_label].view(n, tmax, self.n_label) if emissions else None
+        return e, frames_out, p[:, :P], info
+
+    @property
+    def max_path_out(self) -> int:
+        """the most path entries one call can commit per stream (0: the criterion has no streaming path)"""
+        return int(lib.w2l_stream_max_path_out(self.h))
 
 
 class StreamingFeatures(_StreamHandle):
