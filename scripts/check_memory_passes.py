@@ -15,7 +15,6 @@ that start one float into their allocation, at lengths that are and are not mult
       (B = 16, 600 frames, 800 features) and conv_glu-sized WeightNorm / GLU rows.  Needs a CUDA device.
 """
 import argparse
-import ctypes
 import json
 import os
 import sys
@@ -46,7 +45,7 @@ def passes(torch, capi):
         dy = buf(B * R, off)
         gain, bias = (torch.tensor([1.7], device="cuda"), torch.tensor([-0.3], device="cuda")) if affine else (None, None)
         y, mr = buf(B * R, off, 0.0), torch.empty(2 * B, device="cuda")
-        scratch = torch.empty(160 * B, dtype=torch.float64, device="cuda")
+        scratch = capi.layernorm_scratch(B, "cuda")
         capi._check(lib.w2l_layernorm_fwd(S(), B, R, 1e-5, P(a), P(r), P(gain), P(bias), P(y), P(mr), P(scratch)))
         out = [y, mr]
         for mode in (0, 1, 2):
@@ -79,7 +78,7 @@ def passes(torch, capi):
 
     def axpy(n, off):
         x, y = buf(n, off), buf(n, off)
-        capi._check(lib.w2l_axpy(ctypes.c_void_p(S()), ctypes.c_longlong(n), ctypes.c_float(0.37), P(x), P(y)))
+        capi._check(lib.w2l_axpy(S(), n, 0.37, P(x), P(y)))
         return [y]
 
     def colsum(M, N, ld, off):
@@ -125,7 +124,7 @@ def timed(torch, capi):
     a, r, dy, y, d_b, d_r = (torch.randn(B * R, device="cuda") for _ in range(6))
     G, F = 16 * 600, 800  # the same activations as per-frame groups (per-row LayerNorm)
     mr, gain, bias = torch.empty(2 * G, device="cuda"), torch.ones(1, device="cuda"), torch.zeros(1, device="cuda")
-    dg, db, scratch = torch.zeros(1, device="cuda"), torch.zeros(1, device="cuda"), torch.empty(160 * G, dtype=torch.float64, device="cuda")
+    dg, db, scratch = torch.zeros(1, device="cuda"), torch.zeros(1, device="cuda"), capi.layernorm_scratch(G, "cuda")
     rows, ln = 1000, 12000
     v, w, dv = (torch.randn(rows * ln, device="cuda") for _ in range(3))
     g, inv, dgn = torch.rand(rows, device="cuda") + 0.5, torch.empty(rows, device="cuda"), torch.zeros(rows, device="cuda")
@@ -142,7 +141,7 @@ def timed(torch, capi):
     yield "weightnorm_bwd", lambda: lib.w2l_weightnorm_bwd(S(), rows, ln, P(v), P(g), P(inv), P(w), P(dv), P(dgn))
     yield "glu_fwd", lambda: lib.w2l_glu_fwd(S(), gr, H, P(x), P(gy), 0.2, 5)
     yield "glu_bwd", lambda: lib.w2l_glu_bwd(S(), gr, H, P(x), P(gdy), P(gdx), 0.2, 5)
-    yield "axpy", lambda: lib.w2l_axpy(ctypes.c_void_p(S()), ctypes.c_longlong(n), ctypes.c_float(0.5), P(pg), P(pv))
+    yield "axpy", lambda: lib.w2l_axpy(S(), n, 0.5, P(pg), P(pv))
     yield "colsum_accumulate", lambda: lib.w2l_colsum_accumulate(S(), G, F, P(a), F, P(colsum_out))
     yield "sq_norm_accumulate", lambda: lib.w2l_sq_norm_accumulate(S(), n, P(pg), P(sq))
     yield "sgd_step_ex", lambda: lib.w2l_sgd_step_ex(S(), n, P(p), P(pg), P(pv), 1e-6, 0.9, 0.0, 1.0, 1.0, P(sq), 0, None)

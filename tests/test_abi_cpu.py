@@ -1,9 +1,8 @@
-"""CPU-side checks of the C ABI: the library loads, exports every symbol include/w2l_b200.h
-declares, reports workspace sizes, and rejects bad arguments with the documented codes —
+"""CPU-side checks of the C ABI: the library loads, binds every prototype include/w2l_b200.h
+declares with the types it states, reports workspace sizes, and rejects bad arguments with the documented codes —
 no kernel is launched, so they run without a GPU."""
 import ctypes
 import os
-import re
 
 import numpy as np
 import pytest
@@ -11,19 +10,57 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def header_symbols():
-    txt = open(os.path.join(ROOT, "include", "w2l_b200.h")).read()
-    return sorted(set(re.findall(r"W2L_API\s+[\w\s\*]+?\b(w2l_\w+)\s*\(", txt)))
-
-
-def test_library_exports_every_declared_symbol():
+def test_library_binds_every_declared_prototype():
     from wav2letter_b200 import capi
 
-    syms = header_symbols()
-    assert len(syms) >= 14
-    for s in syms:
+    txt = open(os.path.join(ROOT, "include", "w2l_b200.h")).read()
+    assert len(capi.PROTOTYPES) >= 14
+    assert len(capi.PROTOTYPES) == txt.count("W2L_API ") - txt.count("#define W2L_API ")  # the reader saw every declaration
+    for s, (restype, argtypes) in capi.PROTOTYPES.items():
         assert hasattr(capi.lib, s), f"{s} declared in include/w2l_b200.h but not exported"
-    assert sorted(capi.EXPORTS) == syms
+        fn = getattr(capi.lib, s)
+        assert fn.restype is restype and tuple(fn.argtypes) == argtypes, s
+
+
+def test_prototype_types():
+    """literal signatures, so that a reader that maps every function the same wrong way cannot pass"""
+    from ctypes import c_char_p, c_double, c_float, c_int, c_longlong, c_size_t, c_ulonglong, c_void_p
+
+    from wav2letter_b200 import capi
+
+    P = capi.PROTOTYPES
+    vp, i = c_void_p, c_int
+    assert P["w2l_gemm"] == (c_int, (vp, i, i, i, i, i, i, vp, i, vp, i, vp, i, i, vp, i, i, vp, i, i, i,
+                                     c_float, c_float, c_ulonglong, c_int))
+    assert P["w2l_fill"] == (c_int, (c_void_p, c_longlong, c_float, c_void_p))
+    assert P["w2l_set_seed"][1] == (c_ulonglong,)
+    assert P["w2l_ema_update"][1][-1] is c_double
+    assert P["w2l_trainer_create"][1][1] is c_char_p  # const char* arch_text
+    for name, restype in (("w2l_last_error", c_char_p), ("w2l_trainer_describe", c_char_p), ("w2l_launch_count", c_longlong),
+                          ("w2l_stream_state_bytes", c_longlong), ("w2l_asg_workspace_size", c_size_t),
+                          ("w2l_trainer_create", c_void_p), ("w2l_trainer_destroy", None)):
+        assert P[name][0] is restype, name
+
+
+@pytest.mark.parametrize("decl", ["W2L_API int w2l_x(int32_t n);", "W2L_API int* w2l_x(void);", "W2L_API int w2l_x(int);",
+                                  "W2L_API int w2l_x(float v[]);", "W2L_API int w2l_x(int (*cb)(int));"])
+def test_header_reader_refuses_what_it_cannot_bind(decl):
+    """a type outside the table, or a declaration the reader cannot parse, stops the import instead of going unbound"""
+    from wav2letter_b200 import capi
+
+    with pytest.raises(ImportError, match="w2l_x"):
+        capi._read_header("/* a */\n" + decl + "\nW2L_API int w2l_ok(void);")
+
+
+def test_header_constants():
+    from wav2letter_b200 import capi
+
+    assert (capi.W2L_OK, capi.W2L_ERR_UNSUPPORTED, capi.W2L_TERM_ASG, capi.W2L_SCALE_TARGET_SZ_SQRT, capi.W2L_GEMM_F32X3_SPLIT_B,
+            capi.W2L_PRECISION_FP16, capi.W2L_LN_MAX_PARTS) == (0, 4, 3, 4, 3, 3, 80)
+    assert capi.PRECISIONS == {"tf32": 0, "f32": 1, "fp32": 1, "bf16": 2, "fp16": 3}
+    assert capi.GEMM_KINDS == {"tf32": 0, "f32x3": 1, "bf16": 2, "f32x3_split_b": 3, "fp16": 4}
+    assert capi.SCALE_MODES == {"none": 0, "input_sz": 1, "input_sz_sqrt": 2, "target_sz": 3, "target_sz_sqrt": 4}
+    assert (capi.TERM_FCC, capi.TERM_FAC, capi.TERM_ASG) == (1, 2, 3)
 
 
 def test_golden_fixture_matches_oracle():

@@ -119,12 +119,12 @@ def test_utterance_normalisation_and_padding():
     assert np.isfinite(out).all()
 
 
-def test_abi_symbols_and_argument_errors():
+def test_abi_prototypes_and_argument_errors():
     from wav2letter_b200 import capi
 
     lib = capi.lib
     for s in ("w2l_mfsc_num_frames", "w2l_mfsc_workspace_size", "w2l_mfsc"):
-        assert s in capi.EXPORTS and hasattr(lib, s)
+        assert s in capi.PROTOTYPES and hasattr(lib, s)
     one = ctypes.c_void_p(256)  # never dereferenced: validation fails first
     n = (ctypes.c_int32 * 2)(16000, 8000)
     need = lib.w2l_mfsc_workspace_size(2, 16000, FS, 25, 10, 80)

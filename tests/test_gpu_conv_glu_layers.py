@@ -39,16 +39,6 @@ def _keep_seed_stream():
 OUT_TYPES = {"f32": (0, torch.float32), "bf16": (1, torch.bfloat16), "fp16": (2, torch.float16)}  # operand type per mode
 NAN_BITS = {torch.float32: 0x7FC00001, torch.bfloat16: 0x7FC1, torch.float16: 0x7E01}
 INT_VIEW = {torch.float32: torch.int32, torch.bfloat16: torch.int16, torch.float16: torch.int16}
-W2L_ERR_INVALID_ARGUMENT, W2L_ERR_UNSUPPORTED = 1, 4
-
-
-def _lib():
-    from wav2letter_b200 import capi
-
-    vp, i, ll = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong
-    arr = ctypes.CFUNCTYPE(i, vp, i, i, i, i, i, i, vp, vp, vp, vp, vp, i)(("w2l_conv1d_arrange_ex", capi.lib))
-    unarr = ctypes.CFUNCTYPE(i, vp, i, i, i, i, i, i, vp, vp, ll, vp, vp)(("w2l_conv1d_unarrange_grad", capi.lib))
-    return capi, arr, unarr
 
 
 def _p(t):
@@ -84,13 +74,16 @@ def sizes(kind, cin, cout, glu, xin, xout):
     return cin_p + xin, cout_p + xout
 
 
-def run_arrange(arr, w, bias, cin_p, cout_p, glu, mode, flip=True):
+def run_arrange(w, bias, cin_p, cout_p, glu, mode, flip=True):
+    from wav2letter_b200 import capi
+
     cout, cin, kw = w.shape
     out, dt = OUT_TYPES[mode]
     fwd = nan_filled((cout_p, kw * cin_p), dt)
     fl = nan_filled((cin_p, kw * cout_p), dt) if flip else None
     bias_p = nan_filled((cout_p,), torch.float32) if bias is not None else None
-    rc = arr(torch.cuda.current_stream().cuda_stream, cin, cout, kw, cin_p, cout_p, int(glu), _p(w), _p(bias), _p(fwd), _p(fl), _p(bias_p), out)
+    rc = capi.lib.w2l_conv1d_arrange_ex(torch.cuda.current_stream().cuda_stream, cin, cout, kw, cin_p, cout_p, int(glu), _p(w), _p(bias),
+                                        _p(fwd), _p(fl), _p(bias_p), out)
     torch.cuda.synchronize()
     return rc, fwd, fl, bias_p
 
@@ -100,14 +93,13 @@ def run_arrange(arr, w, bias, cin_p, cout_p, glu, mode, flip=True):
 # ------------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("shape", ALL_SHAPES, ids=shape_id)
 def test_arrange_bits(shape):
-    _, arr, _ = _lib()
     cin, cout, kw, glu, xin, xout = shape
     g = torch.Generator(device="cuda").manual_seed(cin * 7919 + cout * 31 + kw)
     w = torch.randn(cout, cin, kw, device="cuda", generator=g)
     bias = torch.randn(cout, device="cuda", generator=g)
     for mode, (_, dt) in OUT_TYPES.items():
         cin_p, cout_p = sizes(mode, cin, cout, glu, xin, xout)
-        rc, fwd, flip, bias_p = run_arrange(arr, w, bias, cin_p, cout_p, glu, mode)
+        rc, fwd, flip, bias_p = run_arrange(w, bias, cin_p, cout_p, glu, mode)
         assert rc == 0
         rf, rfl, rb = arrange(w, bias, cin_p, cout_p, glu)  # fp32 moves: exact
         assert same_bits(fwd, rf.to(dt)), f"{mode}: forward operand differs at {int((fwd.float() != rf.to(dt).float()).sum())} entries"
@@ -118,19 +110,21 @@ def test_arrange_bits(shape):
 @pytest.mark.parametrize("mode", list(OUT_TYPES))
 def test_arrange_without_flip_or_bias(mode):
     """flip = NULL writes the forward operand alone; bias = NULL leaves bias_p to the zero fill"""
-    _, arr, _ = _lib()
+    from wav2letter_b200 import capi
+
     cin, cout, kw, glu = 65, 42, 9, True
     g = torch.Generator(device="cuda").manual_seed(5)
     w = torch.randn(cout, cin, kw, device="cuda", generator=g)
     cin_p, cout_p = sizes(mode, cin, cout, glu, 0, 0)
     _, dt = OUT_TYPES[mode]
     rf, rfl, _ = arrange(w, None, cin_p, cout_p, glu)
-    rc, fwd, flip, _ = run_arrange(arr, w, None, cin_p, cout_p, glu, mode, flip=False)
+    rc, fwd, flip, _ = run_arrange(w, None, cin_p, cout_p, glu, mode, flip=False)
     assert rc == 0 and flip is None and same_bits(fwd, rf.to(dt))
     bias_p = nan_filled((cout_p,), torch.float32)
     fwd = nan_filled((cout_p, kw * cin_p), dt)
     flip = nan_filled((cin_p, kw * cout_p), dt)
-    rc = arr(torch.cuda.current_stream().cuda_stream, cin, cout, kw, cin_p, cout_p, 1, _p(w), None, _p(fwd), _p(flip), _p(bias_p), OUT_TYPES[mode][0])
+    rc = capi.lib.w2l_conv1d_arrange_ex(torch.cuda.current_stream().cuda_stream, cin, cout, kw, cin_p, cout_p, 1, _p(w), None, _p(fwd),
+                                        _p(flip), _p(bias_p), OUT_TYPES[mode][0])
     torch.cuda.synchronize()
     assert rc == 0 and same_bits(fwd, rf.to(dt)) and same_bits(flip, rfl.to(dt))
     assert same_bits(bias_p, torch.zeros_like(bias_p))
@@ -138,11 +132,12 @@ def test_arrange_without_flip_or_bias(mode):
 
 @pytest.mark.parametrize("case", ["kw100", "odd_glu_cout", "glu_cout_p_not_x8", "out_type_3"])
 def test_arrange_rejections_write_nothing(case):
-    capi, arr, unarr = _lib()
-    cin, cout, kw, glu, cout_p, out, code = {"kw100": (8, 8, 100, 1, 8, 0, W2L_ERR_UNSUPPORTED),
-                                             "odd_glu_cout": (8, 7, 3, 1, 8, 0, W2L_ERR_INVALID_ARGUMENT),
-                                             "glu_cout_p_not_x8": (8, 6, 3, 1, 12, 0, W2L_ERR_INVALID_ARGUMENT),
-                                             "out_type_3": (8, 8, 3, 1, 8, 3, W2L_ERR_INVALID_ARGUMENT)}[case]
+    from wav2letter_b200 import capi
+
+    cin, cout, kw, glu, cout_p, out, code = {"kw100": (8, 8, 100, 1, 8, 0, capi.W2L_ERR_UNSUPPORTED),
+                                             "odd_glu_cout": (8, 7, 3, 1, 8, 0, capi.W2L_ERR_INVALID_ARGUMENT),
+                                             "glu_cout_p_not_x8": (8, 6, 3, 1, 12, 0, capi.W2L_ERR_INVALID_ARGUMENT),
+                                             "out_type_3": (8, 8, 3, 1, 8, 3, capi.W2L_ERR_INVALID_ARGUMENT)}[case]
     w = torch.randn(cout, cin, kw, device="cuda")
     bias = torch.randn(cout, device="cuda")
     fwd = nan_filled((cout_p, kw * cin), torch.float32)
@@ -150,7 +145,8 @@ def test_arrange_rejections_write_nothing(case):
     bias_p = nan_filled((cout_p,), torch.float32)
     torch.cuda.synchronize()
     launches = capi.launch_count()
-    rc = arr(torch.cuda.current_stream().cuda_stream, cin, cout, kw, cin, cout_p, glu, _p(w), _p(bias), _p(fwd), _p(flip), _p(bias_p), out)
+    rc = capi.lib.w2l_conv1d_arrange_ex(torch.cuda.current_stream().cuda_stream, cin, cout, kw, cin, cout_p, glu, _p(w), _p(bias), _p(fwd),
+                                        _p(flip), _p(bias_p), out)
     torch.cuda.synchronize()
     assert rc == code, capi.lib.w2l_last_error().decode()
     assert capi.launch_count() == launches
@@ -158,9 +154,10 @@ def test_arrange_rejections_write_nothing(case):
         assert same_bits(t, nan_filled(t.shape, torch.float32)), "a rejected call wrote its destination"
     if case == "kw100":
         dw = torch.zeros_like(w)
-        rc = unarr(torch.cuda.current_stream().cuda_stream, cin, cout, kw, cin, cout_p, glu, _p(fwd), _p(dw), 0, None, None)
+        rc = capi.lib.w2l_conv1d_unarrange_grad(torch.cuda.current_stream().cuda_stream, cin, cout, kw, cin, cout_p, glu, _p(fwd), _p(dw), 0,
+                                                None, None)
         torch.cuda.synchronize()
-        assert rc == W2L_ERR_UNSUPPORTED and capi.launch_count() == launches and not dw.count_nonzero()
+        assert rc == capi.W2L_ERR_UNSUPPORTED and capi.launch_count() == launches and not dw.count_nonzero()
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -169,7 +166,8 @@ def test_arrange_rejections_write_nothing(case):
 @pytest.mark.parametrize("shape", ALL_SHAPES, ids=shape_id)
 def test_unarrange_bits(shape):
     """dw += unarrange(dfwd): one fp32 addition per element, in the padding of the f32 / tf32 and the bf16 / fp16 modes"""
-    _, _, unarr = _lib()
+    from wav2letter_b200 import capi
+
     cin, cout, kw, glu, xin, xout = shape
     g = torch.Generator(device="cuda").manual_seed(cin * 104729 + cout * 13 + kw)
     for kind in ("f32", "bf16"):
@@ -180,7 +178,8 @@ def test_unarrange_bits(shape):
         dfwd = dfwd.view(cout_p, kw * cin_p)
         dw = torch.randn(cout, cin, kw, device="cuda", generator=g)
         want = dw + unarrange(dfwd, cin, cout, kw, cin_p, cout_p, glu)
-        rc = unarr(torch.cuda.current_stream().cuda_stream, cin, cout, kw, cin_p, cout_p, int(glu), _p(dfwd), _p(dw), 0, None, None)
+        rc = capi.lib.w2l_conv1d_unarrange_grad(torch.cuda.current_stream().cuda_stream, cin, cout, kw, cin_p, cout_p, int(glu), _p(dfwd),
+                                                _p(dw), 0, None, None)
         torch.cuda.synchronize()
         assert rc == 0
         assert same_bits(dw, want), f"{kind}: {int((dw != want).sum())} of {dw.numel()} weight-gradient elements differ"
@@ -198,7 +197,8 @@ def bias_grad_depth(rows):
 def test_bias_grad(rows, cout, glu):
     """|dbias - ref| <= gamma_n (|dbias0| + sum |dy|) per channel, n the summation depth (Higham's gamma_n = n u / (1 - n u));
     NaN in dy's padded columns never reaches dbias; two runs give the same bits"""
-    _, _, unarr = _lib()
+    from wav2letter_b200 import capi
+
     cin, kw = 4, 1
     cin_p, cout_p = sizes("bf16", cin, cout, glu, 0, 0)
     g = torch.Generator(device="cuda").manual_seed(rows + cout)
@@ -210,8 +210,8 @@ def test_bias_grad(rows, cout, glu):
 
     def run(dy_, with_dbias=True):
         dw, db = torch.zeros(cout, cin, kw, device="cuda"), dbias0.clone()
-        rc = unarr(torch.cuda.current_stream().cuda_stream, cin, cout, kw, cin_p, cout_p, int(glu), _p(dfwd), _p(dw), rows, _p(dy_),
-                   _p(db) if with_dbias else None)
+        rc = capi.lib.w2l_conv1d_unarrange_grad(torch.cuda.current_stream().cuda_stream, cin, cout, kw, cin_p, cout_p, int(glu), _p(dfwd),
+                                                _p(dw), rows, _p(dy_), _p(db) if with_dbias else None)
         torch.cuda.synchronize()
         assert rc == 0
         assert same_bits(dw, unarrange(dfwd, cin, cout, kw, cin_p, cout_p, glu)), "the weight part of the call went wrong"

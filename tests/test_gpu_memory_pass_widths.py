@@ -2,8 +2,6 @@
 WeightNorm at a row length that is a multiple of 4, and the LayerNorm backward on buffers that start one float into their
 allocation (which forces V = 1).  Both against float64 torch, with the tolerances of test_gpu_am_kernels.py and
 test_gpu_convglu.py.  GLU and axpy add in the same order at both widths, so their two instances must agree bit for bit."""
-import ctypes
-
 import pytest
 import torch
 import torch.nn.functional as F
@@ -62,7 +60,7 @@ def test_layernorm_bwd_scalar_chunks(B, R):
     yr.backward(dy.double())
     d_branch, d_res = shifted(torch.zeros((B, R), device="cuda"), 1), shifted(torch.zeros((B, R), device="cuda"), 1)
     dgain, dbias = torch.zeros(1, device="cuda"), torch.zeros(1, device="cuda")
-    scratch = torch.empty(160 * B, dtype=torch.float64, device="cuda")
+    scratch = capi.layernorm_scratch(B, "cuda")
     capi._check(capi.lib.w2l_layernorm_bwd(capi._stream(), B, R, capi._ptr(a), capi._ptr(r), capi._ptr(dy), capi._ptr(gain), capi._ptr(mr),
                                            capi._ptr(d_branch), capi._ptr(d_res), 1, 1.25, capi._ptr(dgain), capi._ptr(dbias),
                                            capi._ptr(scratch)))
@@ -99,7 +97,7 @@ def test_axpy_widths_agree():
     outs = []
     for off in (0, 1):
         xs, ys = shifted(x, off), shifted(y, off)
-        capi._check(capi.lib.w2l_axpy(ctypes.c_void_p(capi._stream()), ctypes.c_longlong(n), ctypes.c_float(0.37), capi._ptr(xs), capi._ptr(ys)))
+        capi._check(capi.lib.w2l_axpy(capi._stream(), n, 0.37, capi._ptr(xs), capi._ptr(ys)))
         outs.append(ys)
     assert torch.equal(outs[0], outs[1])
     assert rel(outs[0], y.double() + 0.37 * x.double()) < 1e-6

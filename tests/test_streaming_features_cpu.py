@@ -55,12 +55,12 @@ def speech(n, seed):
     return 2000 * (0.55 + 0.45 * np.sin(2 * np.pi * t / 0.37)) * x + rng.normal(0, 100, n)
 
 
-def test_symbols_in_header_exports_and_library():
+def test_symbols_in_header_prototypes_and_library():
     from wav2letter_b200 import capi
 
     header = open(os.path.join(ROOT, "include", "w2l_b200.h")).read()
     for s in SYMBOLS:
-        assert s + "(" in header and s in capi.EXPORTS and hasattr(capi.lib, s)
+        assert s + "(" in header and s in capi.PROTOTYPES and hasattr(capi.lib, s)
 
 
 def test_create_rejects_bad_arguments_before_any_cuda_call():

@@ -1,5 +1,9 @@
 """ctypes binding of include/w2l_b200.h for the Python harness (tests, bench, smoke).
 
+The header is the one statement of the C ABI: at import, every `W2L_API` prototype in it sets the
+restype / argtypes of its function in `lib` (PROTOTYPES), and its integer constants (enum entries,
+`#define NAME <integer>`) become attributes of this module (W2L_OK, W2L_GEMM_FP16, W2L_LN_MAX_PARTS, ...).
+
 Every function takes CUDA torch tensors, checks dtype/contiguity, and passes raw device
 pointers and the current CUDA stream to the C ABI.  Workspaces are torch byte tensors owned
 by the caller side (cached per size here), exactly as the C ABI demands.
@@ -8,55 +12,46 @@ from __future__ import annotations
 
 import ctypes
 import os
+import re
 
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libw2l_b200.so")
+HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "w2l_b200.h")
 
-SCALE_MODES = {"none": 0, "input_sz": 1, "input_sz_sqrt": 2, "target_sz": 3, "target_sz_sqrt": 4}
-TERM_FCC, TERM_FAC, TERM_ASG = 1, 2, 3
+# C type -> ctypes type.  Parameters: `const char*` is a string, every other pointer a c_void_p.
+_SCALARS = {"int": ctypes.c_int, "size_t": ctypes.c_size_t, "long long": ctypes.c_longlong,
+            "unsigned long long": ctypes.c_ulonglong, "float": ctypes.c_float, "double": ctypes.c_double}
+_RETURNS = dict(_SCALARS, **{"void": None, "void*": ctypes.c_void_p, "const char*": ctypes.c_char_p})
 
-# every entry point include/w2l_b200.h declares (tests check the library exports all of them)
-EXPORTS = [
-    "w2l_version", "w2l_last_error", "w2l_launch_count", "w2l_reset_launch_count", "w2l_get_seed", "w2l_set_seed", "w2l_set_profile_events", "w2l_set_profile_event_list", "w2l_profile_events_used", "w2l_trace_begin", "w2l_trace_end", "w2l_trace_list",
-    "w2l_asg_workspace_size", "w2l_asg_forward_backward",
-    "w2l_asg64_workspace_size", "w2l_asg64_forward_backward",
-    "w2l_fcc_viterbi_workspace_size", "w2l_fcc_viterbi",
-    "w2l_fcc_viterbi64_workspace_size", "w2l_fcc_viterbi64",
-    "w2l_fac_viterbi_workspace_size", "w2l_fac_viterbi",
-    "w2l_ctc_workspace_size", "w2l_ctc_forward_backward", "w2l_argmax_path", "w2l_linseg_target",
-    "w2l_ctc_viterbi_workspace_size", "w2l_ctc_viterbi_target",
-    "w2l_set_precision", "w2l_get_precision", "w2l_gemm", "w2l_cast_bf16", "w2l_cast_bf16_rows", "w2l_cast_fp16", "w2l_cast_fp16_rows", "w2l_split_tf32", "w2l_sgd_step_ex", "w2l_finite_guard",
-    "w2l_mask_bands", "w2l_trainer_set_precision", "w2l_trainer_set_grad_stream", "w2l_trainer_set_grad_stream_delay", "w2l_delay", "w2l_trainer_status", "w2l_trainer_save", "w2l_trainer_load", "w2l_trainer_export_streaming",
-    "w2l_trainer_set_schedule", "w2l_trainer_set_position", "w2l_trainer_position", "w2l_trainer_set_lr", "w2l_trainer_lr",
-    "w2l_trainer_set_amp", "w2l_trainer_amp_state",
-    "w2l_text_create", "w2l_text_destroy", "w2l_text_num_classes", "w2l_text_encode", "w2l_text_prediction2ltr", "w2l_text_target2ltr",
-    "w2l_text_ltr2wrd", "w2l_text_align_words", "w2l_edit_distance",
-    "w2l_gemm_set_variant", "w2l_gemm_set_tile", "w2l_gemm_tf32", "w2l_gemm_tf32_ex", "w2l_gemm_tf32_view", "w2l_conv_time_workspace_size", "w2l_conv_time_fwd", "w2l_conv_time_dgrad",
-    "w2l_conv_time_wgrad", "w2l_layernorm_fwd", "w2l_layernorm_rows_fwd", "w2l_layernorm_bwd", "w2l_colsum_accumulate", "w2l_sq_norm_accumulate",
-    "w2l_sgd_step", "w2l_weightnorm_fwd", "w2l_weightnorm_bwd", "w2l_conv1d_arrange", "w2l_conv1d_arrange_ex", "w2l_conv1d_unarrange_grad",
-    "w2l_glu_fwd", "w2l_glu_bwd", "w2l_prelu_fwd", "w2l_prelu_bwd", "w2l_transpose_input", "w2l_axpy", "w2l_fill", "w2l_act_fwd", "w2l_mask_mul",
-    "w2l_trainer_create", "w2l_trainer_destroy", "w2l_trainer_step", "w2l_trainer_forward", "w2l_trainer_num_params",
-    "w2l_trainer_param_layout", "w2l_trainer_get_flat", "w2l_trainer_set_flat", "w2l_trainer_sync_parameters",
-    "w2l_trainer_describe", "w2l_nccl_unique_id", "w2l_init_distributed", "w2l_trainer_align", "w2l_trainer_time_stride",
-    "w2l_mfsc_num_frames", "w2l_mfsc_workspace_size", "w2l_mfsc",
-    "w2l_stream_create", "w2l_stream_destroy", "w2l_stream_state_bytes", "w2l_stream_max_frames_out", "w2l_stream_start",
-    "w2l_stream_run", "w2l_stream_run_path", "w2l_stream_max_path_out", "w2l_stream_plan",
-    "w2l_mfsc_stream_create", "w2l_mfsc_stream_destroy", "w2l_mfsc_stream_state_bytes", "w2l_mfsc_stream_max_frames_out",
-    "w2l_mfsc_stream_start", "w2l_mfsc_stream_run",
-    "w2l_seq2seq_check", "w2l_seq2seq_embed_fwd", "w2l_seq2seq_embed_bwd", "w2l_seq2seq_gru_stash_floats", "w2l_seq2seq_gru_fwd",
-    "w2l_seq2seq_gru_bwd", "w2l_seq2seq_attn_fwd", "w2l_seq2seq_attn_bwd", "w2l_seq2seq_loss", "w2l_seq2seq_scale_rows",
-    "w2l_seq2seq_decode_init", "w2l_seq2seq_decode_step",
-    "w2l_seq2seq_beam_workspace_size", "w2l_seq2seq_beam_init", "w2l_seq2seq_beam_step", "w2l_seq2seq_beam_finish",
-    "w2l_trainer_create_seq2seq", "w2l_trainer_output_width", "w2l_trainer_seq2seq_config", "w2l_trainer_clear_window",
-    "w2l_trainer_seq2seq_seed", "w2l_trainer_decode", "w2l_trainer_beam_search",
-    "w2l_seq2seq_sizes", "w2l_seq2seq_attn_fwd_sized", "w2l_seq2seq_attn_bwd_sized", "w2l_trainer_step_sized", "w2l_trainer_decode_sized",
-    "w2l_trainer_beam_search_sized",
-    "w2l_soft_label_loss", "w2l_ema_update", "w2l_trainer_set_ema", "w2l_trainer_ema", "w2l_trainer_forward_teacher",
-    "w2l_trainer_viterbi_path", "w2l_trainer_step_soft",
-    "w2l_text_device_create", "w2l_text_device_destroy", "w2l_text_edit_workspace_size", "w2l_text_edit_counts", "w2l_trainer_evaluate",
-]
+
+def _param(ctype: str):
+    return ctypes.c_char_p if ctype == "const char*" else ctypes.c_void_p if ctype.endswith("*") else _SCALARS[ctype]
+
+
+def _read_header(text: str):
+    """({name: (restype, argtypes)} of every W2L_API declaration, {name: value} of every integer constant).
+    A declaration that is not `ret name(type name, ...);` over the mapped types raises ImportError, so none goes unbound."""
+    text = re.sub(r"/\*.*?\*/|//[^\n]*", " ", text, flags=re.S)
+    prototypes = {}
+    for decl in re.findall(r"(?<!#define )\bW2L_API\b[^;]*;", text):
+        decl = " ".join(decl.replace("*", "* ").split()).replace(" *", "*")  # single spaces, pointers written `T*`
+        m = re.fullmatch(r"W2L_API (.+) (w2l_\w+) ?\((.*)\);", decl)
+        try:
+            params = [] if m.group(3) == "void" else [re.fullmatch(r"(.+) \w+", p.strip()).group(1) for p in m.group(3).split(",")]
+            prototypes[m.group(2)] = (_RETURNS[m.group(1)], tuple(map(_param, params)))
+        except (AttributeError, KeyError):  # a regex did not match, or a type outside _SCALARS / _RETURNS
+            raise ImportError(f"{HEADER_PATH}: cannot bind `{decl}`: not a prototype over the types capi.py maps") from None
+    constants = {}
+    for body in re.findall(r"\benum\s*\{([^}]*)\}", text):
+        for entry in filter(str.strip, body.split(",")):
+            m = re.fullmatch(r"\s*(\w+)\s*=\s*(-?\d+)\s*", entry)
+            if not m:
+                raise ImportError(f"{HEADER_PATH}: cannot read the enum entry `{entry.strip()}`")
+            constants[m.group(1)] = int(m.group(2))
+    constants.update((n, int(v)) for n, v in re.findall(r"^\s*#define\s+(\w+)\s+(-?\d+)\s*$", text, re.M))
+    return prototypes, constants
 
 
 class W2LError(RuntimeError):
@@ -65,208 +60,29 @@ class W2LError(RuntimeError):
         self.code = code
 
 
-def _load() -> ctypes.CDLL:
+def _load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
             "(there is no CPU / PyTorch fallback for the hot path)")
+    if not os.path.exists(HEADER_PATH):
+        raise ImportError(f"{HEADER_PATH} is missing: the signatures of {os.path.basename(LIB_PATH)} are read from it "
+                          "(it is part of the source tree)")
     lib = ctypes.CDLL(LIB_PATH)
-    vp, i, sz = ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t
-    lib.w2l_last_error.restype = ctypes.c_char_p
-    lib.w2l_launch_count.restype = ctypes.c_longlong
-    lib.w2l_get_seed.restype = ctypes.c_ulonglong
-    lib.w2l_set_seed.argtypes = [ctypes.c_ulonglong]
-    lib.w2l_set_profile_events.argtypes = [vp, vp]
-    lib.w2l_set_profile_event_list.argtypes = [i, vp, vp, i]
-    lib.w2l_trace_begin.argtypes = [vp, i]
-    lib.w2l_trace_end.restype = ctypes.c_longlong
-    lib.w2l_trace_end.argtypes = [ctypes.c_char_p, ctypes.c_longlong]
-    lib.w2l_trace_list.restype = ctypes.c_longlong
-    lib.w2l_trace_list.argtypes = [ctypes.c_char_p, ctypes.c_longlong]
-    lib.w2l_asg_workspace_size.restype = sz
-    lib.w2l_asg_workspace_size.argtypes = [i, i, i, i]
-    lib.w2l_asg_forward_backward.argtypes = [vp, i, i, i, i, i, i, vp, vp, vp, vp, vp, vp, vp, vp, sz]
-    lib.w2l_fcc_viterbi_workspace_size.restype = sz
-    lib.w2l_fcc_viterbi_workspace_size.argtypes = [i, i, i]
-    lib.w2l_fcc_viterbi.argtypes = [vp, i, i, i, vp, vp, vp, vp, sz]
-    lib.w2l_asg64_workspace_size.restype = sz
-    lib.w2l_asg64_workspace_size.argtypes = [i, i, i, i]
-    lib.w2l_asg64_forward_backward.argtypes = [vp, i, i, i, i, i, i, vp, vp, vp, vp, vp, vp, vp, vp, sz]
-    lib.w2l_fcc_viterbi64_workspace_size.restype = sz
-    lib.w2l_fcc_viterbi64_workspace_size.argtypes = [i, i, i]
-    lib.w2l_fcc_viterbi64.argtypes = [vp, i, i, i, vp, vp, vp, vp, sz]
-    lib.w2l_fac_viterbi_workspace_size.restype = sz
-    lib.w2l_fac_viterbi_workspace_size.argtypes = [i, i, i, i]
-    lib.w2l_fac_viterbi.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, vp, vp, sz]
-    lib.w2l_ctc_workspace_size.restype = sz
-    lib.w2l_ctc_workspace_size.argtypes = [i, i, i, i]
-    lib.w2l_ctc_forward_backward.argtypes = [vp, i, i, i, i, i, vp, vp, vp, vp, vp, vp, sz]
-    lib.w2l_argmax_path.argtypes = [vp, i, i, i, vp, vp]
-    lib.w2l_linseg_target.argtypes = [vp, i, i, i, vp, vp]
-    lib.w2l_ctc_viterbi_workspace_size.restype = sz
-    lib.w2l_ctc_viterbi_workspace_size.argtypes = [i, i, i, i]
-    lib.w2l_ctc_viterbi_target.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, vp, sz]
-    lib.w2l_gemm_tf32.argtypes = [vp, i, i, i, i, i, vp, i, vp, i, vp, i, vp, i]
-    f32, u64, ll = ctypes.c_float, ctypes.c_ulonglong, ctypes.c_longlong
-    ll = ctypes.c_longlong
-    lib.w2l_weightnorm_fwd.argtypes = [vp, i, i, vp, vp, vp, vp]
-    lib.w2l_weightnorm_bwd.argtypes = [vp, i, i, vp, vp, vp, vp, vp, vp]
-    lib.w2l_conv1d_arrange.argtypes = [vp, i, i, i, i, i, i, vp, vp, vp, vp, vp]
-    lib.w2l_conv1d_unarrange_grad.argtypes = [vp, i, i, i, i, i, i, vp, vp, ll, vp, vp]
-    lib.w2l_glu_fwd.argtypes = [vp, ll, i, vp, vp, f32, u64]
-    lib.w2l_glu_bwd.argtypes = [vp, ll, i, vp, vp, vp, f32, u64]
-    lib.w2l_prelu_fwd.argtypes = [vp, ll, vp, vp, vp, f32, u64]
-    lib.w2l_prelu_bwd.argtypes = [vp, ll, vp, vp, vp, vp, vp, f32, u64]
-    lib.w2l_act_fwd.argtypes = [vp, ll, vp, i, f32, u64, vp]
-    lib.w2l_mask_mul.argtypes = [vp, ll, vp, vp, i, f32, vp]
-    lib.w2l_gemm_tf32_view.argtypes = [vp, i, i, i, i, i, vp, i, vp, i, vp, i, vp, i, i]
-    lib.w2l_gemm_tf32_ex.argtypes = [vp, i, i, i, i, i, vp, i, vp, i, vp, i, vp, i, i, vp, i, i, f32, f32, u64]
-    lib.w2l_conv_time_workspace_size.restype = sz
-    lib.w2l_conv_time_workspace_size.argtypes = [i, i, i, i, i]
-    lib.w2l_conv_time_fwd.argtypes = [vp, i, i, i, i, i, i, i, i, i, vp, vp, vp, vp, vp, i, f32, u64, vp, sz]
-    lib.w2l_conv_time_dgrad.argtypes = [vp, i, i, i, i, i, i, i, i, i, vp, vp, vp, vp, vp, sz]
-    lib.w2l_conv_time_wgrad.argtypes = [vp, i, i, i, i, i, i, i, i, i, vp, vp, vp, vp, vp, sz]
-    lib.w2l_layernorm_fwd.argtypes = [vp, i, ll, f32, vp, vp, vp, vp, vp, vp, vp]
-    lib.w2l_layernorm_rows_fwd.argtypes = [vp, ll, i, f32, vp, vp, vp, vp, vp, vp]
-    lib.w2l_layernorm_bwd.argtypes = [vp, i, ll, vp, vp, vp, vp, vp, vp, vp, i, f32, vp, vp, vp]
-    lib.w2l_colsum_accumulate.argtypes = [vp, i, i, vp, i, vp]
-    lib.w2l_sq_norm_accumulate.argtypes = [vp, ll, vp, vp]
-    lib.w2l_sgd_step.argtypes = [vp, ll, vp, vp, vp, f32, f32, f32, f32, f32, vp]
-    lib.w2l_set_precision.argtypes = [i]
-    lib.w2l_gemm.argtypes = [vp, i, i, i, i, i, i, vp, i, vp, i, vp, i, i, vp, i, i, vp, i, i, i, f32, f32, u64, i]
-    lib.w2l_cast_bf16.argtypes = [vp, ll, vp, vp]
-    lib.w2l_cast_bf16_rows.argtypes = [vp, ll, i, i, i, vp, vp]
-    lib.w2l_cast_fp16.argtypes = [vp, ll, vp, vp]
-    lib.w2l_cast_fp16_rows.argtypes = [vp, ll, i, i, i, vp, vp]
-    lib.w2l_split_tf32.argtypes = [vp, i, i, i, i, i, vp, vp]
-    lib.w2l_sgd_step_ex.argtypes = [vp, ll, vp, vp, vp, f32, f32, f32, f32, f32, vp, i, vp]
-    lib.w2l_finite_guard.argtypes = [vp, i, vp, vp, vp]
-    lib.w2l_mask_bands.argtypes = [vp, i, i, i, i, vp, vp, i, vp, vp, i, vp, vp, f32]
-    lib.w2l_trainer_set_precision.argtypes = [vp, i]
-    lib.w2l_trainer_set_schedule.argtypes = [vp, ll, ctypes.c_double, ll, i, ll, ll, ll]
-    lib.w2l_trainer_set_position.argtypes = [vp, ll, ll]
-    lib.w2l_trainer_position.argtypes = [vp, vp, vp]
-    lib.w2l_trainer_set_lr.argtypes = [vp, ctypes.c_float, ctypes.c_float]
-    lib.w2l_trainer_lr.argtypes = [vp, vp, vp]
-    lib.w2l_trainer_set_amp.argtypes = [vp, i, ctypes.c_double, i, ctypes.c_double, ctypes.c_double]
-    lib.w2l_trainer_amp_state.argtypes = [vp, vp, vp, vp, vp]
-    lib.w2l_trainer_set_grad_stream.argtypes = [vp, i]
-    lib.w2l_trainer_set_grad_stream_delay.argtypes = [vp, i]
-    lib.w2l_delay.argtypes = [vp, i]
-    lib.w2l_trainer_status.argtypes = [vp, vp, vp]
-    cp = ctypes.c_char_p
-    lib.w2l_trainer_save.argtypes = [vp, vp, cp]
-    lib.w2l_trainer_load.restype = vp
-    lib.w2l_trainer_load.argtypes = [vp, cp]
-    lib.w2l_trainer_export_streaming.argtypes = [vp, vp, cp, cp]
-    lib.w2l_text_create.restype = vp
-    lib.w2l_text_create.argtypes = [cp, cp, cp, i, cp, i, cp]
-    lib.w2l_text_destroy.argtypes = [vp]
-    lib.w2l_text_destroy.restype = None
-    lib.w2l_text_num_classes.argtypes = [vp]
-    for fn in (lib.w2l_text_encode, lib.w2l_text_prediction2ltr, lib.w2l_text_target2ltr, lib.w2l_text_ltr2wrd):
-        fn.restype = ll
-    lib.w2l_text_encode.argtypes = [vp, cp, vp, ll]
-    lib.w2l_text_prediction2ltr.argtypes = [vp, vp, i, vp, ll]
-    lib.w2l_text_target2ltr.argtypes = [vp, vp, i, vp, ll]
-    lib.w2l_text_ltr2wrd.argtypes = [vp, cp, vp, ll]
-    lib.w2l_text_align_words.restype = ll
-    lib.w2l_text_align_words.argtypes = [vp, vp, i, vp, i, ctypes.c_double, cp, vp, ll]
-    lib.w2l_edit_distance.argtypes = [cp, cp, vp]
-    lib.w2l_text_device_create.restype = vp
-    lib.w2l_text_device_create.argtypes = [vp, vp]
-    lib.w2l_text_device_destroy.argtypes = [vp]
-    lib.w2l_text_device_destroy.restype = None
-    lib.w2l_text_edit_workspace_size.restype = sz
-    lib.w2l_text_edit_workspace_size.argtypes = [vp, i, i, i]
-    lib.w2l_text_edit_counts.argtypes = [vp, vp, i, i, vp, vp, i, vp, vp, vp, sz]
-    lib.w2l_trainer_evaluate.argtypes = [vp, vp, vp, i, i, vp, i, vp, vp, vp, vp, vp]
-    lib.w2l_trainer_create.restype = vp
-    lib.w2l_trainer_create.argtypes = [vp, ctypes.c_char_p, i, i, ctypes.c_char_p, i, f32, f32, f32, f32, f32]
-    lib.w2l_trainer_create_seq2seq.restype = vp
-    lib.w2l_trainer_create_seq2seq.argtypes = [vp, ctypes.c_char_p, i, i, i, i, i, i, i, i, f32, f32, i, f32, i, f32, f32, f32, f32]
-    lib.w2l_trainer_output_width.argtypes = [vp, vp]
-    lib.w2l_trainer_seq2seq_config.argtypes = [vp, vp]
-    lib.w2l_trainer_clear_window.argtypes = [vp]
-    lib.w2l_trainer_seq2seq_seed.argtypes = [vp, vp]
-    lib.w2l_trainer_decode.argtypes = [vp, vp, i, i, vp, vp, vp, ll]
-    lib.w2l_trainer_beam_search.argtypes = [vp, vp, i, i, vp, i, i, vp, vp, vp, vp, ll]
-    lib.w2l_seq2seq_check.argtypes = [i, i]
-    lib.w2l_seq2seq_embed_fwd.argtypes = [vp, i, i, i, i, vp, vp, vp, f32, u64, vp, vp, vp]
-    lib.w2l_seq2seq_embed_bwd.argtypes = [vp, i, i, i, i, vp, vp, vp, vp]
-    lib.w2l_seq2seq_gru_stash_floats.restype = sz
-    lib.w2l_seq2seq_gru_stash_floats.argtypes = [i, i, i]
-    lib.w2l_seq2seq_gru_fwd.argtypes = [vp, i, i, i, vp, vp, vp, vp, vp, vp]
-    lib.w2l_seq2seq_gru_bwd.argtypes = [vp, i, i, i, vp, vp, vp, vp, vp, vp]
-    lib.w2l_seq2seq_attn_fwd.argtypes = [vp, i, i, i, i, vp, vp, i, f32, vp, vp]
-    lib.w2l_seq2seq_attn_bwd.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, vp, vp, vp]
-    lib.w2l_seq2seq_sizes.argtypes = [vp, i, i, i, vp, i, vp, vp, vp, vp]
-    lib.w2l_seq2seq_attn_fwd_sized.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, i, f32, vp, vp]
-    lib.w2l_seq2seq_attn_bwd_sized.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, vp, vp, vp, vp]
-    lib.w2l_trainer_step_sized.argtypes = [vp, vp, i, i, vp, i, vp, vp, vp, vp, i, f32]
-    lib.w2l_trainer_decode_sized.argtypes = [vp, vp, i, i, vp, vp, vp, vp, ll]
-    lib.w2l_trainer_beam_search_sized.argtypes = [vp, vp, i, i, vp, vp, i, i, vp, vp, vp, vp, ll]
-    lib.w2l_seq2seq_loss.argtypes = [vp, i, i, i, i, vp, vp, f32, vp, i, vp, vp, vp]
-    lib.w2l_seq2seq_scale_rows.argtypes = [vp, i, i, i, vp, f32, vp]
-    lib.w2l_seq2seq_decode_init.argtypes = [vp, i, i, i, i, vp, vp, vp, vp, vp]
-    lib.w2l_seq2seq_decode_step.argtypes = [vp, i, i, i, i, i, vp, vp, vp, vp, i, vp, vp]
-    lib.w2l_seq2seq_beam_workspace_size.restype = sz
-    lib.w2l_seq2seq_beam_workspace_size.argtypes = [i, i, i]
-    lib.w2l_seq2seq_beam_init.argtypes = [vp, i, i, i, i, vp, vp, vp, sz]
-    lib.w2l_seq2seq_beam_step.argtypes = [vp, i, i, i, i, i, i, i, i, vp, vp, vp, vp, vp, vp, sz]
-    lib.w2l_seq2seq_beam_finish.argtypes = [vp, i, i, i, i, i, vp, sz, vp, vp, vp, vp]
-    lib.w2l_trainer_destroy.argtypes = [vp]
-    lib.w2l_trainer_destroy.restype = None
-    lib.w2l_trainer_step.argtypes = [vp, vp, i, i, vp, i, vp, vp, i, f32]
-    lib.w2l_trainer_forward.argtypes = [vp, vp, i, i, vp, vp, ll, vp]
-    lib.w2l_soft_label_loss.argtypes = [vp, ll, i, vp, vp, f32, vp, vp, vp]
-    lib.w2l_ema_update.argtypes = [vp, ll, vp, vp, ctypes.c_double]
-    lib.w2l_trainer_set_ema.argtypes = [vp, vp, i, ctypes.c_double]
-    lib.w2l_trainer_ema.argtypes = [vp, vp, vp]
-    lib.w2l_trainer_forward_teacher.argtypes = [vp, vp, i, i, vp, i, vp, ll, vp]
-    lib.w2l_trainer_viterbi_path.argtypes = [vp, vp, i, i, vp, vp, i, vp, ll, vp]
-    lib.w2l_trainer_step_soft.argtypes = [vp, vp, i, i, vp, vp, i, f32, vp, f32]
-    lib.w2l_trainer_align.argtypes = [vp, vp, i, i, vp, i, vp, vp, vp, ll, vp]
-    lib.w2l_trainer_time_stride.argtypes = [vp]
-    lib.w2l_trainer_num_params.restype = ll
-    lib.w2l_trainer_num_params.argtypes = [vp, i]
-    lib.w2l_trainer_param_layout.argtypes = [vp, i, i, vp, vp]
-    lib.w2l_trainer_get_flat.argtypes = [vp, vp, i, i, vp]
-    lib.w2l_trainer_set_flat.argtypes = [vp, vp, i, vp]
-    lib.w2l_trainer_sync_parameters.argtypes = [vp, vp]
-    lib.w2l_trainer_describe.restype = ctypes.c_char_p
-    lib.w2l_trainer_describe.argtypes = [vp]
-    lib.w2l_nccl_unique_id.argtypes = [vp]
-    lib.w2l_init_distributed.argtypes = [i, i, vp]
-    lib.w2l_mfsc_num_frames.argtypes = [i, i, i, i]
-    lib.w2l_mfsc_workspace_size.restype = sz
-    lib.w2l_mfsc_workspace_size.argtypes = [i, i, i, i, i, i]
-    lib.w2l_mfsc.argtypes = [vp, i, i, vp, vp, i, i, i, i, i, vp, i, vp, sz]
-    lib.w2l_stream_create.restype = vp
-    lib.w2l_stream_create.argtypes = [vp, vp, i, i]
-    lib.w2l_stream_destroy.argtypes = [vp]
-    lib.w2l_stream_destroy.restype = None
-    lib.w2l_stream_state_bytes.restype = ctypes.c_longlong
-    lib.w2l_stream_state_bytes.argtypes = [vp]
-    lib.w2l_stream_max_frames_out.argtypes = [vp]
-    lib.w2l_stream_start.argtypes = [vp, vp, i, vp]
-    lib.w2l_stream_run.argtypes = [vp, vp, i, vp, vp, vp, i, i, vp, ctypes.c_longlong, vp]
-    lib.w2l_stream_run_path.argtypes = [vp, vp, i, vp, vp, vp, i, i, vp, ctypes.c_longlong, vp, vp, ctypes.c_longlong, vp]
-    lib.w2l_stream_max_path_out.argtypes = [vp]
-    lib.w2l_stream_plan.argtypes = [ctypes.c_char_p, i, i, i, vp, i, i, vp, vp, vp, vp]
-    lib.w2l_mfsc_stream_create.restype = vp
-    lib.w2l_mfsc_stream_create.argtypes = [vp, i, i, i, i, i, i, i]
-    lib.w2l_mfsc_stream_destroy.argtypes = [vp]
-    lib.w2l_mfsc_stream_destroy.restype = None
-    lib.w2l_mfsc_stream_state_bytes.restype = ctypes.c_longlong
-    lib.w2l_mfsc_stream_state_bytes.argtypes = [vp]
-    lib.w2l_mfsc_stream_max_frames_out.argtypes = [vp]
-    lib.w2l_mfsc_stream_start.argtypes = [vp, vp, i, vp]
-    lib.w2l_mfsc_stream_run.argtypes = [vp, vp, i, vp, vp, vp, i, i, vp, ctypes.c_longlong, vp]
-    return lib
+    with open(HEADER_PATH) as f:
+        prototypes, constants = _read_header(f.read())
+    for name, (restype, argtypes) in prototypes.items():
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
+    return lib, prototypes, constants
 
 
-lib = _load()
+lib, PROTOTYPES, _constants = _load()
+globals().update(_constants)  # W2L_OK, W2L_TERM_ASG, W2L_LN_MAX_PARTS, ...: the names below come from the header
+
+SCALE_MODES = {"none": W2L_SCALE_NONE, "input_sz": W2L_SCALE_INPUT_SZ, "input_sz_sqrt": W2L_SCALE_INPUT_SZ_SQRT,
+               "target_sz": W2L_SCALE_TARGET_SZ, "target_sz_sqrt": W2L_SCALE_TARGET_SZ_SQRT}
+TERM_FCC, TERM_FAC, TERM_ASG = W2L_TERM_FCC, W2L_TERM_FAC, W2L_TERM_ASG
 
 
 def _check(rc: int) -> None:
@@ -497,8 +313,10 @@ def trace_list() -> list:
     return [(ln.split("\t")[0], float(ln.split("\t")[1])) for ln in buf.value.decode().splitlines()]
 
 
-PRECISIONS = {"tf32": 0, "f32": 1, "fp32": 1, "bf16": 2, "fp16": 3}
-GEMM_KINDS = {"tf32": 0, "f32x3": 1, "bf16": 2, "f32x3_split_b": 3, "fp16": 4}
+PRECISIONS = {"tf32": W2L_PRECISION_TF32, "f32": W2L_PRECISION_F32, "fp32": W2L_PRECISION_F32, "bf16": W2L_PRECISION_BF16,
+              "fp16": W2L_PRECISION_FP16}
+GEMM_KINDS = {"tf32": W2L_GEMM_TF32, "f32x3": W2L_GEMM_F32X3, "bf16": W2L_GEMM_BF16, "f32x3_split_b": W2L_GEMM_F32X3_SPLIT_B,
+              "fp16": W2L_GEMM_FP16}
 
 
 def set_precision(p) -> None:
@@ -667,12 +485,17 @@ def conv_time_wgrad(x, dy, K, stride, pad_left, dwt=None, dbias=None):
     return dwt, dbias
 
 
+def layernorm_scratch(B: int, device) -> torch.Tensor:
+    """the scratch of w2l_layernorm_fwd / w2l_layernorm_bwd over B groups: W2L_LN_SCRATCH_DOUBLES(B) float64"""
+    return torch.empty(2 * W2L_LN_MAX_PARTS * B, dtype=torch.float64, device=device)
+
+
 def layernorm_fwd(a, r, gain, bias, eps=1e-5):
     B = a.shape[0]
     R = a[0].numel()
     y = torch.empty_like(a)
     mr = torch.empty((B, 2), dtype=torch.float32, device=a.device)
-    scratch = torch.empty(160 * B, dtype=torch.float64, device=a.device)
+    scratch = layernorm_scratch(B, a.device)
     _check(lib.w2l_layernorm_fwd(_stream(), B, R, float(eps), _ptr(a), _ptr(r), _ptr(gain), _ptr(bias), _ptr(y), _ptr(mr),
                                  _ptr(scratch)))
     return y, mr
@@ -685,7 +508,7 @@ def layernorm_bwd(a, r, dy, gain, mr, branch_mode=0, branch_scale=1.0):
     d_res = torch.empty_like(a)
     dgain = torch.zeros(1, dtype=torch.float32, device=a.device)
     dbias = torch.zeros(1, dtype=torch.float32, device=a.device)
-    scratch = torch.empty(160 * B, dtype=torch.float64, device=a.device)
+    scratch = layernorm_scratch(B, a.device)
     _check(lib.w2l_layernorm_bwd(_stream(), B, R, _ptr(a), _ptr(r), _ptr(dy), _ptr(gain), _ptr(mr), _ptr(d_branch),
                                  _ptr(d_res), int(branch_mode), float(branch_scale), _ptr(dgain), _ptr(dbias),
                                  _ptr(scratch)))
