@@ -512,7 +512,8 @@ W2L_API int w2l_mfsc(void* stream, int B, int max_samples, const float* audio, c
  * criterion + network SGD steps.  `arch_text` is a wav2letter arch file (opcodes V RO PD C2 R DO LN TDS L
  * SAUG), `criterion` "ctc", "asg" or "linseg".  All pointers below are DEVICE pointers:
  * features [T,F,1,B] (ArrayFire layout, T fastest), target [L,B] int32 (-1 padded), loss_out [B].
- * Returns NULL / a status code; w2l_last_error() has the text.
+ * Returns NULL / a status code; w2l_last_error() has the text.  A NULL trainer is W2L_ERR_INVALID_ARGUMENT, with the
+ * call named in the text; num_params, param_layout and time_stride then return -1, describe "", and destroy does nothing.
  * ---------------------------------------------------------------------------------------- */
 W2L_API void* w2l_trainer_create(void* stream, const char* arch_text, int n_feat, int n_label, const char* criterion,
                                  int scale_mode, float transdiag, float lr, float lrcrit, float momentum, float maxgradnorm);
@@ -564,7 +565,8 @@ W2L_API int w2l_trainer_decode_sized(void* trainer, void* stream, int B, int T, 
 W2L_API int w2l_trainer_beam_search_sized(void* trainer, void* stream, int B, int T, const float* features, const int32_t* input_sizes, int beam,
                                           int max_len, int32_t* tokens, int32_t* lengths, float* scores, int32_t* counts, long long capacity);
 /* eval-mode network output [B][T'][width] into emissions_out (capacity floats); T' through t_out.  A buffer smaller than
- * B T' width returns W2L_ERR_INVALID_ARGUMENT with nothing written to it, and t_out still set: call again with that size. */
+ * B T' width returns W2L_ERR_INVALID_ARGUMENT with nothing written to it, and t_out still set: call again with that size.
+ * w2l_trainer_forward_teacher, w2l_trainer_viterbi_path and w2l_trainer_align treat their buffers the same way. */
 W2L_API int w2l_trainer_forward(void* trainer, void* stream, int B, int T, const float* features, float* emissions_out,
                                 long long capacity, int* t_out);
 /* slimIPL (recipes/slimIPL/src/Train.cpp; DESIGN.md §7).
@@ -641,6 +643,7 @@ W2L_API int w2l_trainer_amp_state(void* trainer, void* stream, double* scale, in
 /* steps whose update was skipped on the device because the loss or a gradient was NaN / Inf (Train.cpp:1686-1698,
  * :1753-1771); synchronises `stream` */
 W2L_API int w2l_trainer_status(void* trainer, void* stream, long long* skipped_steps);
+/* the flat parameter arenas: another `which` or get_flat `what` is W2L_ERR_INVALID_ARGUMENT (num_params, param_layout: -1) */
 W2L_API long long w2l_trainer_num_params(void* trainer, int which /*0 network, 1 criterion, 2 teacher*/);
 W2L_API int w2l_trainer_param_layout(void* trainer, int which, int max_params, long long* elements, long long* dims4);
 W2L_API int w2l_trainer_get_flat(void* trainer, void* stream, int which, int what /*0 values, 1 gradients*/, float* out);

@@ -137,6 +137,8 @@ class Trainer:
         el = (ctypes.c_longlong * n)()
         dims = (ctypes.c_longlong * (4 * n))()
         cnt = lib.w2l_trainer_param_layout(self.h, which, n, el, dims)
+        if cnt < 0:
+            raise capi.W2LError(capi.W2L_ERR_INVALID_ARGUMENT, lib.w2l_last_error().decode())
         out, off = [], 0
         for i in range(cnt):
             out.append((off, int(el[i]), tuple(int(dims[4 * i + d]) for d in range(4))))
@@ -184,22 +186,14 @@ class Trainer:
         slimIPL's soft pseudo-labels"""
         B, _, F, T = features.shape
         width = self.output_width()
-        cap = B * (2 * T + 64) * width  # SAME-padded even kernels grow the frame count by one each
-        tout = ctypes.c_int(0)
 
-        def run(cap):
-            out = torch.empty(cap, dtype=torch.float32, device=features.device)
+        def call(out, cap, tout):
             if teacher:
-                rc = lib.w2l_trainer_forward_teacher(self.h, _stream(), B, T, _ptr(features), 1, _ptr(out), cap, ctypes.byref(tout))
-            else:
-                rc = lib.w2l_trainer_forward(self.h, _stream(), B, T, _ptr(features), _ptr(out), cap, ctypes.byref(tout))
-            return rc, out
+                return lib.w2l_trainer_forward_teacher(self.h, _stream(), B, T, _ptr(features), 1, _ptr(out), cap, tout)
+            return lib.w2l_trainer_forward(self.h, _stream(), B, T, _ptr(features), _ptr(out), cap, tout)
 
-        rc, out = run(cap)
-        if rc != 0 and B * tout.value * width > cap:  # explicit padding (e.g. 170 frames a side) outgrew the guess: the exact size
-            rc, out = run(B * tout.value * width)
-        _check(rc)
-        return out[: B * tout.value * width].view(B, tout.value, width)
+        (out,), t = _frame_results(call, features, width, torch.float32)
+        return out.view(B, t, width)
 
     def set_ema(self, decay: float | None = 0.999):
         """slimIPL's teacher (--slimIPL_ema --slimIPL_ema_decay): a second copy of the network, started from the network as
@@ -222,12 +216,12 @@ class Trainer:
             maxlen = self.seq2seq_config()["maxdecoderoutputlen"]
         except capi.W2LError:  # not seq2seq: one token per output frame
             maxlen = 0
-        cap = B * max(2 * T + 64, maxlen)
-        path = torch.empty(cap, dtype=torch.int32, device=features.device)
-        tout = ctypes.c_int(0)
-        _check(lib.w2l_trainer_viterbi_path(self.h, _stream(), B, T, _ptr(features), _ptr(isz), int(bool(teacher)), _ptr(path), cap,
-                                            ctypes.byref(tout)))
-        return path[: B * tout.value].view(B, tout.value)
+
+        def call(path, cap, tout):
+            return lib.w2l_trainer_viterbi_path(self.h, _stream(), B, T, _ptr(features), _ptr(isz), int(bool(teacher)), _ptr(path), cap, tout)
+
+        (path,), t = _frame_results(call, features, frames=maxlen)
+        return path.view(B, t)
 
     def evaluate(self, features: torch.Tensor, target: torch.Tensor, text, input_sizes=None, target_sizes=None):
         """Train.cpp's test() on one batch: the eval-mode forward, the criterion's loss (the bits of step(train=False)), its
@@ -327,14 +321,12 @@ class Trainer:
         aligned)."""
         B, _, F, T = features.shape
         L = target.shape[1]
-        cap = B * (2 * T + 64)  # as in forward: SAME-padded even kernels grow the frame count by one each
-        path = torch.empty(cap, dtype=torch.int32, device=features.device)
-        idx = torch.empty(cap, dtype=torch.int32, device=features.device)
-        tout = ctypes.c_int(0)
-        _check(lib.w2l_trainer_align(self.h, _stream(), B, T, _ptr(features), L, _ptr(target), _ptr(path), _ptr(idx), cap,
-                                     ctypes.byref(tout)))
-        n = B * tout.value
-        return path[:n].view(B, tout.value), idx[:n].view(B, tout.value)
+
+        def call(path, idx, cap, tout):
+            return lib.w2l_trainer_align(self.h, _stream(), B, T, _ptr(features), L, _ptr(target), _ptr(path), _ptr(idx), cap, tout)
+
+        (path, idx), t = _frame_results(call, features, buffers=2)
+        return path.view(B, t), idx.view(B, t)
 
     def time_stride(self) -> int:
         """input frames per output frame (the product of the network's time strides)"""
@@ -342,6 +334,27 @@ class Trainer:
 
     def sync_parameters(self):
         _check(lib.w2l_trainer_sync_parameters(self.h, _stream()))
+
+
+def _frame_results(call, features: torch.Tensor, width: int = 1, dtype=torch.int32, buffers: int = 1, frames: int = 0):
+    """The [B][T'][width] results of the eval entry points that report T' through t_out (forward, viterbi_path, align):
+    call(*buffers, capacity, t_out) fills `buffers` tensors of capacity elements each and returns the status.  They are
+    first sized for max(2T + 64, frames) frames (SAME-padded even kernels grow the frame count by one each) and, when
+    explicit padding (e.g. 170 frames a side) makes T' larger, once more at the T' the first call reported.
+    Returns (the buffers cut to B T' width elements, T')."""
+    B, T = features.shape[0], features.shape[3]
+    tout = ctypes.c_int(0)
+
+    def run(n):
+        bufs = [torch.empty(B * n * width, dtype=dtype, device=features.device) for _ in range(buffers)]
+        return call(*bufs, B * n * width, ctypes.byref(tout)), bufs
+
+    n = max(2 * T + 64, frames)
+    rc, bufs = run(n)
+    if rc != 0 and tout.value > n:
+        rc, bufs = run(tout.value)
+    _check(rc)
+    return [b[: B * tout.value * width] for b in bufs], tout.value
 
 
 def size_arg(sizes, B: int, name: str):
