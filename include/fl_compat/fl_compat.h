@@ -597,11 +597,16 @@ class ConnectionistTemporalClassificationCriterion : public SequenceCriterion {
  public:
   explicit ConnectionistTemporalClassificationCriterion(CriterionScaleMode scalemode = CriterionScaleMode::NONE);
   std::vector<Variable> forward(const std::vector<Variable>& inputs) override;
+  // forward that also hands over viterbiPath(emissions) in `path` ([T,B] int32), written by the loss's own pass over the
+  // emissions (w2l_ctc_forward_backward_path): what evalOutput scores after the criterion (Train.cpp:1699-1714, :965-980)
+  // without a second read of them.  The loss and its gradient are forward's, bit for bit.
+  std::vector<Variable> forwardWithPath(const std::vector<Variable>& inputs, af::array& path);
   af::array viterbiPath(const af::array& input, const af::array& inputSize = af::array()) override;
   af::array viterbiPathWithTarget(const af::array& input, const af::array& target, af::array* index = nullptr) override;
   std::string prettyString() const override;
 
  private:
+  std::vector<Variable> forwardPath(const std::vector<Variable>& inputs, int32_t* path);
   CriterionScaleMode scaleMode_;
   af::array ws_;
 };

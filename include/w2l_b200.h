@@ -154,11 +154,17 @@ W2L_API int w2l_fac_viterbi(void* stream, int B, int T, int N, int L, const floa
  * Train.cpp:1473-1477).  d_emis may be NULL (forward only).  Targets of at most 1023 labels
  * after the clamp to T (2 * min(L, T) + 1 <= 2048 extended states); W2L_ERR_UNSUPPORTED beyond.
  * w2l_argmax_path = CTCLoss::viterbiPath (per-frame argmax, first maximum wins).
+ * w2l_ctc_forward_backward_path: the same call that also writes that argmax into path[B][T] (nullable) from the pass
+ * that reads every row for the log-partition: path equals w2l_argmax_path bit for bit (ties, -inf and NaN rows
+ * included), and loss and d_emis are the bits of the call without it.
  * ---------------------------------------------------------------------------------------- */
 W2L_API size_t w2l_ctc_workspace_size(int B, int T, int N, int L);
 W2L_API int w2l_ctc_forward_backward(void* stream, int B, int T, int N, int L, int scale_mode, const float* emis,
                                      const int32_t* target, const float* dloss, float* loss, float* d_emis,
                                      void* workspace, size_t workspace_bytes);
+W2L_API int w2l_ctc_forward_backward_path(void* stream, int B, int T, int N, int L, int scale_mode, const float* emis,
+                                          const int32_t* target, const float* dloss, float* loss, float* d_emis, int32_t* path,
+                                          void* workspace, size_t workspace_bytes);
 W2L_API int w2l_argmax_path(void* stream, int B, int T, int N, const float* emis, int32_t* path);
 
 /* ----------------------------------------------------------------------------------------
@@ -834,6 +840,20 @@ W2L_API int w2l_text_edit_counts(void* dev_text, void* stream, int B, int n_path
  * input_sizes / target_sizes as in w2l_trainer_step_sized (seq2seq only).  The only host read is the greedy decode's. */
 W2L_API int w2l_trainer_evaluate(void* trainer, void* stream, void* dev_text, int B, int T, const float* features, int L, const int32_t* target,
                                  const int32_t* input_sizes, const int32_t* target_sizes, float* loss, int32_t* counts);
+/* A training step (w2l_trainer_step with train = 1) that also scores itself as Train.cpp's train meters do (:1699-1714,
+ * evalOutput into meters.train.tknEdit / wrdEdit): the criterion's viterbiPath of THIS step's training-mode network
+ * output (dropout and SpecAugment included) scored against target into counts[B][8], laid out as w2l_text_edit_counts.
+ * CTC takes the argmax from its forward's prep pass (w2l_ctc_forward_backward_path); ASG / LinSeg run the FCC Viterbi on
+ * the same emissions.  The Viterbi and the scoring run on a stream of the trainer beside the backward, and the step's
+ * stream waits for them before the update; no host read is added.  Loss, gradients and update are the bits of the
+ * unscored step.  Under mixed precision a retried attempt replays its random draws, so every attempt's path and counts are
+ * the same; Train.cpp adds them once per attempt (1 + the step's increase of w2l_trainer_amp_state's retries).  Refused
+ * with W2L_ERR_INVALID_ARGUMENT before anything runs: a seq2seq trainer, a text pipeline of another criterion (ctc for
+ * ctc, asg for asg and linseg), a null pointer, total_batch not finite and > 0, a target width outside
+ * w2l_text_edit_counts's limit.  A network output wider than that limit is refused after the network forward, before
+ * the criterion: parameters, position and loss scale are left as they were.  Counts stay per rank. */
+W2L_API int w2l_trainer_step_scored(void* trainer, void* stream, void* dev_text, int B, int T, const float* features, int L, const int32_t* target,
+                                    float* loss_out, float total_batch, int32_t* counts);
 
 #ifdef __cplusplus
 }

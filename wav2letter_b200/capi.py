@@ -231,12 +231,16 @@ def fac_viterbi(emis, target, trans, return_index=False):
     return (path, idx) if return_index else path
 
 
-def ctc_forward_backward(emis, target, scale_mode="none", dloss=None, need_grad=True, out=None, ws=None):
-    """CTC on raw activations (blank = N-1).  Returns (loss[B], d_emis | None)."""
+def ctc_forward_backward(emis, target, scale_mode="none", dloss=None, need_grad=True, out=None, ws=None, path=None):
+    """CTC on raw activations (blank = N-1).  Returns (loss[B], d_emis | None).  path: None, or a CUDA int32 [B, T] tensor
+    that receives the per-frame argmax (argmax_path's bits) from the loss's own pass over the activations."""
     emis = _req(emis, torch.float32, "emis")
     target = _req(target, torch.int32, "target")
     dloss = _req(dloss, torch.float32, "dloss")
+    path = _req(path, torch.int32, "path")
     B, T, N = emis.shape
+    if path is not None and tuple(path.shape) != (B, T):
+        raise ValueError(f"path: expected [{B}, {T}], got {tuple(path.shape)}")
     L = 0 if target is None else target.shape[1]
     if out is None:
         loss = torch.empty(B, dtype=torch.float32, device=emis.device)
@@ -246,8 +250,12 @@ def ctc_forward_backward(emis, target, scale_mode="none", dloss=None, need_grad=
     need = lib.w2l_ctc_workspace_size(B, T, N, L)
     if ws is None:
         ws = workspace(need, emis.device)
-    _check(lib.w2l_ctc_forward_backward(_stream(), B, T, N, L, _mode(scale_mode), _ptr(emis), _ptr(target),
-                                        _ptr(dloss), _ptr(loss), _ptr(d_emis), _ptr(ws), ws.numel()))
+    if path is None:
+        _check(lib.w2l_ctc_forward_backward(_stream(), B, T, N, L, _mode(scale_mode), _ptr(emis), _ptr(target),
+                                            _ptr(dloss), _ptr(loss), _ptr(d_emis), _ptr(ws), ws.numel()))
+    else:
+        _check(lib.w2l_ctc_forward_backward_path(_stream(), B, T, N, L, _mode(scale_mode), _ptr(emis), _ptr(target),
+                                                 _ptr(dloss), _ptr(loss), _ptr(d_emis), _ptr(path), _ptr(ws), ws.numel()))
     return loss, d_emis
 
 

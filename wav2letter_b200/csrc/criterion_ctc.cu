@@ -8,7 +8,8 @@
 // Pipeline:
 //   1. ctc_prep_kernel   HBM-bound: lz[b][t] = logsumexp_k e[b][t][k] (one pass over the activations) and, while the row is
 //                        hot, the frame's scores of the extended-target labels gathered into a compact [T][Sp] array;
-//                        per-sample target size / scale.
+//                        per-sample target size / scale.  With a path buffer (the kPath variant) it also writes the
+//                        frame's argmax, CTCLoss::viterbiPath, from the same row reads: no second pass over B T N.
 //   2. ctc_chains_kernel latency-bound.  ONE WARP PER RECURSION (alpha and beta of an utterance run concurrently in two
 //                        32-thread CTAs), no barrier anywhere: lane j owns the P = Sp/32 consecutive extended-target
 //                        states P*j .. P*j+P-1 in registers, the s-1 / s-2 neighbours are registers except for two SHFL
@@ -54,6 +55,7 @@ struct CtcParams {
   int* valid;     // [B]
   float* coef;    // [B]
   float* scale;   // [B]
+  int32_t* path;  // [B][T] per-frame argmax (the kPath variant of the prep kernel), else unused
 };
 
 __device__ __forceinline__ float ex2f(float x) {
@@ -75,6 +77,11 @@ __device__ __forceinline__ void twofloat_add(float& hi, float& lo, float m) {
   lo += e;
 }
 
+// kPath: also path[f] = the frame's argmax with argmax_path_kernel's rule (criterion_viterbi.cu), bit for bit: a lane's
+// first element seeds its maximum and later ones replace it only when strictly greater, then the lowest index wins ties
+// across lanes.  The log-sum-exp's own `v > m` from -inf is a different rule (an all -inf or NaN-led lane keeps no
+// index), so the index is tracked beside it.
+template <bool kPath>
 __global__ void __launch_bounds__(256) ctc_prep_kernel(CtcParams p, int frame_blocks) {
   const int lane = threadIdx.x & 31;
   if ((int)blockIdx.x < frame_blocks) {
@@ -83,14 +90,34 @@ __global__ void __launch_bounds__(256) ctc_prep_kernel(CtcParams p, int frame_bl
     for (long long f = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); f < nframes; f += warps) {
       const float* e = p.emis + f * p.N;
       float m = kNegInf, s = 0.f;
+      float bv = kNegInf;
+      int bi = 0x7fffffff;
       for (int k = lane; k < p.N; k += 32) {
         const float v = __ldg(e + k);
+        if constexpr (kPath) {
+          if (bi == 0x7fffffff || v > bv) {
+            bv = v;
+            bi = k;
+          }
+        }
         if (v > m) {
           s = s * __expf(m - v) + 1.0f;
           m = v;
         } else {
           s += __expf(v - m);
         }
+      }
+      if constexpr (kPath) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+          const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+          const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+          if (oi != 0x7fffffff && (bi == 0x7fffffff || ov > bv || (ov == bv && oi < bi))) {
+            bv = ov;
+            bi = oi;
+          }
+        }
+        if (lane == 0) p.path[f] = bi == 0x7fffffff ? 0 : bi;
       }
       const float gm = warp_max(m);
       s = (m == kNegInf) ? 0.f : s * __expf(m - gm);
@@ -439,9 +466,15 @@ extern "C" size_t w2l_ctc_workspace_size(int B, int T, int N, int L) {
   return total;
 }
 
-extern "C" int w2l_ctc_forward_backward(void* stream_, int B, int T, int N, int L, int scale_mode, const float* emis,
+extern "C" int w2l_ctc_forward_backward(void* stream, int B, int T, int N, int L, int scale_mode, const float* emis,
                                         const int32_t* target, const float* dloss, float* loss, float* d_emis,
                                         void* workspace, size_t workspace_bytes) {
+  return w2l_ctc_forward_backward_path(stream, B, T, N, L, scale_mode, emis, target, dloss, loss, d_emis, nullptr, workspace, workspace_bytes);
+}
+
+extern "C" int w2l_ctc_forward_backward_path(void* stream_, int B, int T, int N, int L, int scale_mode, const float* emis,
+                                             const int32_t* target, const float* dloss, float* loss, float* d_emis, int32_t* path,
+                                             void* workspace, size_t workspace_bytes) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (B <= 0 || T <= 0 || N <= 1) return fail(W2L_ERR_INVALID_ARGUMENT, "ctc: B, T must be positive and N >= 2");
   if (!emis || !loss) return fail(W2L_ERR_INVALID_ARGUMENT, "ctc: null emissions/loss");
@@ -462,13 +495,17 @@ extern "C" int w2l_ctc_forward_backward(void* stream_, int B, int T, int N, int 
   p.dloss = dloss;
   p.loss = loss;
   p.d_emis = d_emis;
+  p.path = path;
   size_t need = 0;
   carve(p, workspace, need);
   if (!workspace || workspace_bytes < need)
     return fail(W2L_ERR_WORKSPACE, "ctc: workspace too small (need " + std::to_string(need) + " bytes)");
   const long long nframes = (long long)B * T;
   const int frame_blocks = (int)std::min<long long>((nframes + 7) / 8, sm_count() * 8);
-  ctc_prep_kernel<<<frame_blocks + (B + 255) / 256, 256, 0, stream>>>(p, frame_blocks);
+  if (path)
+    ctc_prep_kernel<true><<<frame_blocks + (B + 255) / 256, 256, 0, stream>>>(p, frame_blocks);
+  else
+    ctc_prep_kernel<false><<<frame_blocks + (B + 255) / 256, 256, 0, stream>>>(p, frame_blocks);
   W2L_LAUNCH_CHECK("ctc_prep_kernel");
   const int grid = p.need_grad ? 2 * B : B;  // alpha chains, then beta chains
   profile_kind(2);

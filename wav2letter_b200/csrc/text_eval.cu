@@ -439,6 +439,8 @@ void* textDeviceUpload(const TextTablesHost& h, void* stream) {
   return t;
 }
 
+int textDeviceCriterion(const void* dev_text) { return static_cast<const TextDevice*>(dev_text)->criterion; }
+
 }  // namespace w2l
 
 using namespace w2l;

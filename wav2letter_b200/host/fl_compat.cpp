@@ -1800,6 +1800,14 @@ af::array AutoSegmentationCriterion::viterbiPathWithTarget(const af::array& inpu
 ConnectionistTemporalClassificationCriterion::ConnectionistTemporalClassificationCriterion(CriterionScaleMode scalemode) : scaleMode_(scalemode) {}
 std::string ConnectionistTemporalClassificationCriterion::prettyString() const { return "ConnectionistTemporalClassificationCriterion"; }
 std::vector<Variable> ConnectionistTemporalClassificationCriterion::forward(const std::vector<Variable>& inputs) {
+  return forwardPath(inputs, nullptr);
+}
+std::vector<Variable> ConnectionistTemporalClassificationCriterion::forwardWithPath(const std::vector<Variable>& inputs, af::array& path) {
+  checkCriterionInputs(inputs, "ConnectionistTemporalClassificationCriterion");
+  path = af::array::empty(af::dim4(inputs[0].dims(1), inputs[0].dims(2)), DType::i32);
+  return forwardPath(inputs, path.i32());
+}
+std::vector<Variable> ConnectionistTemporalClassificationCriterion::forwardPath(const std::vector<Variable>& inputs, int32_t* path) {
   checkCriterionInputs(inputs, "ConnectionistTemporalClassificationCriterion");
   const Variable& emis = inputs[0];
   const af::array target = inputs[1].array();
@@ -1809,15 +1817,14 @@ std::vector<Variable> ConnectionistTemporalClassificationCriterion::forward(cons
   af::array loss = af::array::empty(af::dim4(B));
   const CriterionScaleMode mode = scaleMode_;
   if (!(train_ && emis.isCalcGrad())) {
-    check(w2l_ctc_forward_backward(currentStream(), B, T, N, L, (int)mode, emis.array().f32(), target.i32(), nullptr, loss.f32(), nullptr, ws.ptr(),
-                                   ws.bytes()));
+    check(w2l_ctc_forward_backward_path(currentStream(), B, T, N, L, (int)mode, emis.array().f32(), target.i32(), nullptr, loss.f32(), nullptr, path,
+                                        ws.ptr(), ws.bytes()));
     return {Variable(loss, false)};
   }
   af::array dEmis = af::array::empty(emis.dims());
   const af::array seed = lossGradSeed(B);  // dloss = 1, or the loss scale
-  check(w2l_ctc_forward_backward(currentStream(), B, T, N, L, (int)mode, emis.array().f32(), target.i32(), seed.isEmpty() ? nullptr : seed.f32(),
-                                 loss.f32(), dEmis.f32(), ws.ptr(),
-                                 ws.bytes()));
+  check(w2l_ctc_forward_backward_path(currentStream(), B, T, N, L, (int)mode, emis.array().f32(), target.i32(), seed.isEmpty() ? nullptr : seed.f32(),
+                                      loss.f32(), dEmis.f32(), path, ws.ptr(), ws.bytes()));
   return {Variable(loss, {emis}, [=](std::vector<Variable>& ins, const Variable& g) mutable {
     af::array de = dEmis;
     if (!g.isOnesSeed()) {

@@ -23,5 +23,7 @@ struct TextTablesHost {
 
 // uploads the tables (one allocation); nullptr with the error text set on failure (csrc/text_eval.cu)
 void* textDeviceUpload(const TextTablesHost& h, void* stream);
+// the TextCriterion of an uploaded handle (csrc/text_eval.cu)
+int textDeviceCriterion(const void* dev_text);
 
 }  // namespace w2l

@@ -23,6 +23,7 @@
 
 #include "fl_compat/fl_compat.h"
 #include "stream_internal.h"
+#include "text_tables.h"
 #include "w2l_b200.h"
 
 namespace w2l {
@@ -116,11 +117,20 @@ struct Trainer {
   bool useGradStream = true;
   int gradStreamDelayUs = 0;  // tests (w2l_trainer_set_grad_stream_delay)
   cudaStream_t gradStream = nullptr;
+  // the scoring stream of w2l_trainer_step_scored (StepScoring), created at its first call at the device's greatest
+  // stream priority, so that its few latency-bound CTAs are placed as soon as the backward's kernels leave room
+  cudaStream_t scoreStream = nullptr;
+  cudaEvent_t scoreEvent = nullptr;
   ~Trainer() {
     if (gradStream) {
       cudaStreamSynchronize(gradStream);
       cudaStreamDestroy(gradStream);
     }
+    if (scoreStream) {
+      cudaStreamSynchronize(scoreStream);
+      cudaStreamDestroy(scoreStream);
+    }
+    if (scoreEvent) cudaEventDestroy(scoreEvent);
   }
 };
 
@@ -272,10 +282,66 @@ Seq2SeqCriterion& seq2seqOnly(const Trainer* t, const char* msg) { return t->s2s
 void notSeq2seq(const Trainer* t, const char* msg) { if (t->s2s) throw std::invalid_argument(msg); }
 void sizesSeq2seqOnly(const Trainer* t, bool sized, const char* msg) { if (sized && !t->s2s) throw std::invalid_argument(msg); }
 
+// The self-scoring of a training step (w2l_trainer_step_scored; evalOutput at Train.cpp:1699-1714).  After the criterion
+// forward of each attempt, launch() scores the criterion's viterbiPath of that attempt's output against the target on the
+// trainer's scoring stream, beside the backward: CTC's path is the argmax its forward wrote, ASG / LinSeg run the FCC
+// Viterbi there.  join() makes the step's stream wait for that work: it runs after the backward and before the update,
+// which rewrites the transitions the Viterbi reads, and before the next attempt's forward or the end of the step can
+// rewrite or free the emissions, the path or the workspace.
+struct StepScoring {
+  Trainer* t;
+  void* text;
+  int B, L;
+  const int32_t* target;
+  int32_t* counts;
+  af::array path;  // [T',B]: CTC's is set by its forward (criterionLoss), the others' by launch()
+  af::array ws;
+  bool pending = false;
+
+  void launch(const Variable& output) {
+    const cudaStream_t main = static_cast<cudaStream_t>(w2l::currentStream());
+    if (!t->scoreStream) {
+      int least = 0, greatest = 0;
+      if (cudaDeviceGetStreamPriorityRange(&least, &greatest) != cudaSuccess ||
+          cudaStreamCreateWithPriority(&t->scoreStream, cudaStreamNonBlocking, greatest) != cudaSuccess ||
+          cudaEventCreateWithFlags(&t->scoreEvent, cudaEventDisableTiming) != cudaSuccess)
+        throw std::runtime_error("trainer: cannot create the scoring stream");
+    }
+    if (cudaEventRecord(t->scoreEvent, main) != cudaSuccess || cudaStreamWaitEvent(t->scoreStream, t->scoreEvent, 0) != cudaSuccess)
+      throw std::runtime_error("trainer: cannot fork the scoring stream");
+    pending = true;
+    struct Back {  // the scoring stream is current only inside launch()
+      cudaStream_t s;
+      ~Back() { w2l::setCurrentStream(s); }
+    } back{main};
+    w2l::setCurrentStream(t->scoreStream);
+    if (!t->isCtc) path = t->crit->viterbiPath(output.array());
+    const int nPath = (int)path.dims(0);
+    const size_t bytes = w2l_text_edit_workspace_size(text, B, nPath, L);  // non-zero: checked before the criterion ran
+    ws = af::array::empty(af::dim4((long long)bytes), w2l::DType::u8);
+    w2l::check(w2l_text_edit_counts(text, t->scoreStream, B, nPath, path.i32(), nullptr, L, target, counts, ws.ptr(), bytes));
+  }
+  void join() {
+    if (!pending) return;
+    pending = false;
+    if (cudaEventRecord(t->scoreEvent, t->scoreStream) != cudaSuccess ||
+        cudaStreamWaitEvent(static_cast<cudaStream_t>(w2l::currentStream()), t->scoreEvent, 0) != cudaSuccess)
+      throw std::runtime_error("trainer: cannot join the scoring stream");
+  }
+  ~StepScoring() {  // an error between launch() and join(): path and ws are freed on the step's stream, behind the scoring
+    try {
+      join();
+    } catch (...) {
+    }
+  }
+};
+
 // One step of Train.cpp's loop (:1454-1831) with the loss lossOf(network output): a training step (train != 0) runs
 // backward, all-reduce, clip, the finite guard, mixed precision's retries and the update, then the teacher's EMA.
+// scoring (nullable, training steps): launched after each attempt's criterion forward, joined after its backward.
 template <class LossOf>
-void runStep(Trainer* t, void* stream, int B, int T, const float* features, const LossOf& lossOf, float* loss_out, int train, float total_batch) {
+void runStep(Trainer* t, void* stream, int B, int T, const float* features, const LossOf& lossOf, float* loss_out, int train, float total_batch,
+             StepScoring* scoring = nullptr) {
   w2l::setCurrentStream(stream);
   PrecisionScope scope(t->precision);
   if (train) {
@@ -304,6 +370,8 @@ void runStep(Trainer* t, void* stream, int B, int T, const float* features, cons
     Variable loss = lossOf(output);
     if (loss_out) af::array::wrap(loss_out, af::dim4(loss.elements())).copyFrom(loss.array());
     if (!train) return;
+    // [eval] Train.cpp:1699-1714: evalOutput of this attempt's output, beside the backward
+    if (scoring) scoring->launch(output);
     // [bwd]  zeroGrad; loss.backward()   Train.cpp:1718-1720
     t->netArena.grads.zero();
     for (auto& p : t->net->params()) p.zeroGrad(false);
@@ -329,6 +397,7 @@ void runStep(Trainer* t, void* stream, int B, int T, const float* features, cons
     loss.backward();
     if (t->reducer) t->reducer->finalize();
     grads.join();  // the weight gradients are complete before the norm, the clip and the update read them
+    if (scoring) scoring->join();
     if (fl::isDistributedInit() && t->critArena.elements) fl::allReduce(t->critArena.grads);
     // [opt]  grads /= totalBatch * scaleFactor (Train.cpp:1752,1783), clipGradNorm(net U crit if clampCrit, else net)
     // (:1791-1798), step (:1801-1802).
@@ -557,9 +626,12 @@ af::array sizesArray(const int32_t* p, int B) { return p ? af::array::wrap(const
 
 namespace {
 // the criterion's loss of the network output (Train.cpp:1664-1676), with the seq2seq sizes when given: the one loss both
-// the step and w2l_trainer_evaluate compute
-Variable criterionLoss(Trainer* t, const Variable& output, int B, int L, const int32_t* target, const int32_t* input_sizes, const int32_t* target_sizes) {
+// the step and w2l_trainer_evaluate compute.  ctcPath (nullable; a CTC trainer): receives the criterion's viterbiPath of
+// the output, written by the loss's own pass over it.
+Variable criterionLoss(Trainer* t, const Variable& output, int B, int L, const int32_t* target, const int32_t* input_sizes, const int32_t* target_sizes,
+                       af::array* ctcPath = nullptr) {
   Variable tgt = fl::noGrad(af::array::wrap(const_cast<int32_t*>(target), af::dim4(L, B), w2l::DType::i32));
+  if (ctcPath) return static_cast<CTCLoss&>(*t->crit).forwardWithPath({output, tgt}, *ctcPath).front();
   if (!input_sizes && !target_sizes) return t->crit->forward({output, tgt}).front();
   return t->crit->forward({output, tgt, fl::noGrad(sizesArray(input_sizes, B)), fl::noGrad(sizesArray(target_sizes, B))}).front();
 }
@@ -733,11 +805,12 @@ W2L_API int w2l_trainer_evaluate(void* h, void* stream, void* dev_text, int B, i
     w2l::setCurrentStream(stream);
     PrecisionScope scope(t->precision);
     Variable output;  // the eval step's own forward and loss; the path is decoded from that same output
+    af::array p;      // CTC: the argmax its loss wrote while it read the output
     runStep(t, stream, B, T, features, [&](const Variable& o) {
       output = o;
-      return criterionLoss(t, o, B, L, target, input_sizes, target_sizes);
+      return criterionLoss(t, o, B, L, target, input_sizes, target_sizes, t->isCtc ? &p : nullptr);
     }, loss, 0, 1.f);
-    const af::array p = t->crit->viterbiPath(output.array(), sizesArray(input_sizes, B));
+    if (!t->isCtc) p = t->crit->viterbiPath(output.array(), sizesArray(input_sizes, B));
     const int nPath = (int)p.dims(0);
     const size_t bytes = w2l_text_edit_workspace_size(dev_text, B, nPath, L);
     if (!bytes) {
@@ -748,6 +821,34 @@ W2L_API int w2l_trainer_evaluate(void* h, void* stream, void* dev_text, int B, i
     rc = w2l_text_edit_counts(dev_text, stream, B, nPath, p.i32(), nullptr, L, target, counts, ws.ptr(), bytes);
   });
   return g != W2L_OK ? g : rc;
+}
+
+// A training step scored as Train.cpp's train meters are (:1699-1714): counts[B][8] of the criterion's viterbiPath of this
+// step's training-mode output against target, computed on the scoring stream beside the backward (StepScoring)
+W2L_API int w2l_trainer_step_scored(void* h, void* stream, void* dev_text, int B, int T, const float* features, int L, const int32_t* target,
+                                    float* loss_out, float total_batch, int32_t* counts) {
+  return onTrainer(h, "trainer_step_scored", [&](Trainer* t) {
+    checkBatch(B, T, features, "trainer_step_scored");
+    if (!dev_text || L <= 0 || !target || !loss_out || !counts) throw std::invalid_argument("trainer_step_scored: bad arguments");
+    if (!(std::isfinite(total_batch) && total_batch > 0.f))
+      throw std::invalid_argument("trainer_step_scored: total_batch must be finite and > 0 for a training step");
+    notSeq2seq(t, "trainer_step_scored: the seq2seq criterion's viterbiPath is its greedy decode, which a training step does not run");
+    if (w2l::textDeviceCriterion(dev_text) != (t->isCtc ? w2l::kTextCtc : w2l::kTextAsg))
+      throw std::invalid_argument(std::string("trainer_step_scored: the text pipeline was not made for the trainer's criterion (") +
+                                  (t->isCtc ? "ctc" : "asg") + " expected)");
+    // the scorer's limits, before anything runs: the target width here, the path width (T') after the network forward
+    const auto refuseWidth = [&] { throw std::invalid_argument(std::string("trainer_step_scored: ") + w2l_last_error()); };
+    if (!w2l_text_edit_workspace_size(dev_text, B, 0, L)) refuseWidth();
+    const unsigned short counter = t->amp.counter;
+    StepScoring scoring{t, dev_text, B, L, target, counts};
+    runStep(t, stream, B, T, features, [&](const Variable& output) {
+      if (!w2l_text_edit_workspace_size(dev_text, B, (int)output.dims(1), L)) {
+        t->amp.counter = counter;  // (the attempt has counted itself)
+        refuseWidth();
+      }
+      return criterionLoss(t, output, B, L, target, nullptr, nullptr, t->isCtc ? &scoring.path : nullptr);
+    }, loss_out, 1, total_batch, &scoring);
+  });
 }
 
 // --slimIPL_ema: on = 1 builds the teacher, a second network from the same arch text or plugin with its own value arena,

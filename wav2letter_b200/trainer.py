@@ -155,14 +155,25 @@ class Trainer:
         _check(lib.w2l_trainer_set_flat(self.h, _stream(), which, _ptr(flat.contiguous())))
 
     def step(self, features: torch.Tensor, target: torch.Tensor, train: bool = True, total_batch: float | None = None,
-             loss_out: torch.Tensor | None = None, input_sizes=None, target_sizes=None) -> torch.Tensor:
+             loss_out: torch.Tensor | None = None, input_sizes=None, target_sizes=None, text=None):
         """features: CUDA float [B,1,F,T] contiguous (== ArrayFire [T,F,1,B]); target CUDA int32 [B,L].
         total_batch: the batch summed over ranks (default B); every gradient is divided by it.  A training step raises
         W2LError (code 1) before running anything unless it is finite and > 0; an eval step does not use it.
         input_sizes / target_sizes (seq2seq only; a list or a CUDA int32 tensor of B entries): the input frame counts of a
         padded batch (the counts features.mfsc returns) and the target sizes (tokens plus eos).  Utterance b then attends
-        to its first ceil(d_b T' / max d) encoder frames, and the soft window follows its own diagonal."""
+        to its first ceil(d_b T' / max d) encoder frames, and the soft window follows its own diagonal.
+
+        text: a TextPipeline (ctc for a ctc trainer, asg for asg and linseg) makes this a scored training step, Train.cpp's
+        meters.train (:1699-1714): returns (loss, counts), counts CUDA int32 [B, 8] laid out as TextPipeline.edit_counts,
+        scoring the criterion's viterbi path of THIS step's training-mode output (dropout and SpecAugment included)
+        against target.  Loss, gradients and update are those of the unscored step, bit for bit; the path and scoring run
+        beside the backward and add no host read.  Add counts to an ErrorRates; under mixed precision Train.cpp adds them
+        once per attempt, i.e. 1 + the step's increase of amp_state()[2] times (a retried attempt replays its random draws,
+        so every attempt's counts are the same).  Which batches to score (--pcttraineval, a hash of the sample ids) is the
+        caller's loop, like data loading; counts stay per rank.  Not for seq2seq (its path is the greedy decode)."""
         B, _, F, T = features.shape
+        if text is not None:
+            return self._step_scored(features, target, train, total_batch, loss_out, input_sizes, target_sizes, text)
         L = target.shape[1]
         isz, tsz = size_arg(input_sizes, B, "input_sizes"), size_arg(target_sizes, B, "target_sizes")
         if loss_out is None:
@@ -174,6 +185,36 @@ class Trainer:
             _check(lib.w2l_trainer_step_sized(self.h, _stream(), B, T, _ptr(features), L, _ptr(target), _ptr(isz), _ptr(tsz), _ptr(loss_out),
                                               int(train), tb))
         return loss_out
+
+    def _step_scored(self, features, target, train, total_batch, loss_out, input_sizes, target_sizes, text):
+        """step(text=...): its arguments are checked here, before anything runs"""
+        from .text import TextPipeline
+
+        if not isinstance(text, TextPipeline):
+            raise TypeError("text: expected a TextPipeline")
+        if not train:
+            raise ValueError("text: a scored step is a training step (train=True); score eval batches with evaluate")
+        if input_sizes is not None or target_sizes is not None:
+            raise ValueError("text: input_sizes / target_sizes are the seq2seq criterion's, which a scored step does not cover")
+        if self.criterion == "seq2seq":
+            raise ValueError("text: the seq2seq criterion's viterbi path is its greedy decode, which a training step does not run")
+        want = {"ctc": "ctc", "asg": "asg", "linseg": "asg"}.get(self.criterion)  # (None for a loaded trainer: the C side checks)
+        if want is not None and text.criterion != want:
+            raise ValueError(f"text: a {self.criterion} trainer is scored with a {want} TextPipeline, got {text.criterion}")
+        B = features.shape[0]
+        if target.dim() != 2 or target.shape[0] != B:
+            raise ValueError(f"target: expected [B={B}, L], got {tuple(target.shape)}")
+        target = capi._req(target, torch.int32, "target")
+        loss_out = capi._req(loss_out, torch.float32, "loss_out")
+        if loss_out is None:
+            loss_out = torch.empty(B, dtype=torch.float32, device=features.device)
+        elif loss_out.numel() != B:
+            raise ValueError(f"loss_out: expected {B} elements, got {loss_out.numel()}")
+        counts = torch.empty((B, 8), dtype=torch.int32, device=features.device)
+        tb = float(total_batch if total_batch is not None else B)
+        _check(lib.w2l_trainer_step_scored(self.h, _stream(), text.to_device(), B, features.shape[3], _ptr(features), target.shape[1],
+                                           _ptr(target), _ptr(loss_out), tb, _ptr(counts)))
+        return loss_out, counts
 
     def output_width(self) -> int:
         """features per frame of the network output: n_label, or 2 * hidden (the encoder) for seq2seq"""
